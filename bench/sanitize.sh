@@ -5,7 +5,10 @@
 set -u
 mkdir -p ${OUT:-prof_out}
 SAN=/usr/local/cuda/bin/compute-sanitizer
-K='gemm_kk and 128-64-64 or conv_fprop and 2-16-16 or conv_wgrad and 2-16-16 or conv_dgrad and 2-32-32 or maxpool or cross_entropy and 64-3 or adam or bias_grad and 64-3 or head_ce or fprop_pool_fused'
+K='gemm_kk and 128-64-64 or gemm_kk and 4096-5-4096 or gemm_mnk and 4096-16-512 or gemm_mnmn_store and 10-4096-5'
+K+=' or gemm_mnmn_bf16 and 10-4096-37 or bias_relu and 300-48-64 or conv_fprop and 2-16-16 or conv_wgrad and 2-16-16'
+K+=' or conv_dgrad and 2-32-32 or conv0_fused and 2-16-16 or fprop_pool_fused and 2-32-32 or fprop_pool_fused and 4-14-14'
+K+=' or maxpool or cross_entropy and 64-3 or adam or bias_grad and 64-3 or head_ce'
 for tool in memcheck synccheck; do
   timeout 900 $SAN --tool $tool --error-exitcode 7 python -m pytest tests/test_kernels_gpu.py -q -x -m gpu -k "$K" \
       > ${OUT:-prof_out}/sanitize_$tool.log 2>&1

@@ -42,7 +42,7 @@ static void conv_fprop(const at::Tensor& x, const at::Tensor& w, c10::optional<a
   TORCH_CHECK(w.numel() == (int64_t)Cout * 9 * Cin && y.numel() == (int64_t)N * H * W * Cout, "conv_fprop: shape mismatch");
   b200::conv3x3_fprop(bfp(x), bfp(w), f32p_opt(bias), bfp_mut(y), N, H, W, Cin, Cout, relu, (int)bn, cur_stream());
 }
-// EXPERIMENTAL (B200_FUSE_POOL=1): pooled activation + int32 mask words [N,H/2,W/2,Cout/32,4]
+// Fused conv + pool (default; B200_FUSE_POOL=0 turns it off): pooled activation + int32 mask words [N,H/2,W/2,Cout/32,4]
 static void conv_fprop_pool(const at::Tensor& x, const at::Tensor& w, c10::optional<at::Tensor> bias,
                             at::Tensor pooled, at::Tensor mask, int64_t bn) {
   c10::cuda::CUDAGuard g(x.device());

@@ -143,7 +143,7 @@ void maxpool2x2_relu_bwd(const bf16* y, const bf16* dp, bf16* dz, float* colsum,
   check_last("maxpool2x2_relu_bwd");
 }
 
-// EXPERIMENTAL: backward of the pool fused into the conv epilogue (ConvPolicy::epilogue_pool).  One
+// Backward of the pool fused into the conv epilogue (ConvPolicy::epilogue_pool).  One
 // thread = one pooled pixel x 8 channels: reads 16 B of dp and the chunk's mask words, writes the
 // four 16-byte pieces of dz.  Reads 3/8 of a full-resolution tensor instead of 1 1/2.
 __global__ void unpool2x2_kernel(const bf16* __restrict__ dp, const uint32_t* __restrict__ mask,

@@ -188,17 +188,24 @@ struct GemmPolicy {
       }
     } else if constexpr (EPI == EPI_BF16_BIAS_RELU) {
       __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + static_cast<long long>(r) * p.ldo + cb;
+      if ((cb + 32 <= p.N) && ((reinterpret_cast<uintptr_t>(o) & 15) == 0)) {
 #pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        float v[8];
+        for (int j = 0; j < 32; j += 8) {
+          float v[8];
 #pragma unroll
-        for (int t = 0; t < 8; ++t) {
-          float b = p.bias ? __ldg(p.bias + cb + j + t) : 0.f;
-          v[t] = fmaxf(__uint_as_float(acc[j + t]) + b, 0.f);
+          for (int t = 0; t < 8; ++t) {
+            float b = p.bias ? __ldg(p.bias + cb + j + t) : 0.f;
+            v[t] = fmaxf(__uint_as_float(acc[j + t]) + b, 0.f);
+          }
+          uint4 pk = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
+                                pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+          *reinterpret_cast<uint4*>(o + j) = pk;
         }
-        uint4 pk = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
-                              pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-        *reinterpret_cast<uint4*>(o + j) = pk;
+      } else {   // ragged last chunk or unaligned row: neither the bias nor the output past N is touched
+        for (int j = 0; j < 32 && cb + j < p.N; ++j) {
+          const float b = p.bias ? __ldg(p.bias + cb + j) : 0.f;
+          o[j] = __float2bfloat16(fmaxf(__uint_as_float(acc[j]) + b, 0.f));
+        }
       }
     }
   }
@@ -219,8 +226,8 @@ enum ConvFlags : int {
   CONV_MASK = 4,          // zero where mask_src <= 0 (ReLU backward fused into dgrad)
   CONV_COLSUM = 8,        // colsum[channel] += sum over pixels of the stored (bf16-rounded) output:
                           // the bias gradient of the previous layer, for free in the dgrad epilogue
-  CONV_POOL = 16,         // fprop only, EXPERIMENTAL (B200_FUSE_POOL=1): 2x2/2 max-pool inside the
-                          // epilogue -- writes pool_out + pool_mask, never the un-pooled tensor
+  CONV_POOL = 16,         // fprop only, on by default (B200_FUSE_POOL=0 turns it off): 2x2/2 max-pool inside
+                          // the epilogue -- writes pool_out + pool_mask, never the un-pooled tensor
 };
 
 struct ConvParams {
@@ -253,8 +260,7 @@ __device__ __forceinline__ void conv_tile_origin(const ConvTile& t, int tile, in
   n0 = static_cast<int>(tn) * t.Nb;
 }
 
-// POOL (fprop only, experimental): a separate instantiation, so the default kernels stay exactly
-// the code that was profiled and validated.
+// POOL (fprop only): a separate instantiation, so the un-pooled fprop kernels carry none of its code.
 template <int BN_, int STAGES_, bool DGRAD, bool POOL = false>
 struct ConvPolicy {
   static_assert(!(DGRAD && POOL), "the fused pool is an fprop epilogue");
@@ -424,7 +430,7 @@ struct ConvPolicy {
     }
   }
 
-  // EXPERIMENTAL (CONV_POOL): bias + ReLU + 2x2/2 max-pool of one 32-channel chunk.  The epilogue row
+  // CONV_POOL: bias + ReLU + 2x2/2 max-pool of one 32-channel chunk.  The epilogue row
   // is the pixel, a warp holds 32 consecutive tile rows = (32 / Wb) image rows of Wb pixels, so the
   // four pixels of a pool window are lanes {l, l^1, l^Wb, l^Wb^1} (Wb <= 16, tile origin and image
   // extent even: the launcher checks).  The top-left lane of each window stores the pooled bf16

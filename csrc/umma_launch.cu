@@ -329,6 +329,8 @@ static void fprop_impl(const bf16* x, const bf16* w, const float* bias, bf16* y,
                        cudaStream_t stream) {
   check_channels(Cin, "conv3x3_fprop Cin");
   check_channels(Cout, "conv3x3_fprop Cout");
+  // the epilogue stages the bias in a 512-float shared-memory scratch (ConvPolicy::EPI_MAXC)
+  if (bias && Cout > 512) throw std::runtime_error("[b200] conv3x3_fprop: a bias supports Cout <= 512");
   ConvParams prm;
   prm.t = make_tile(N, H, W, UMMA_BM);
   prm.Ca = Cin; prm.Cn = Cout; prm.wcols_per_tap = Cin;
@@ -359,7 +361,7 @@ void conv3x3_fprop(const bf16* x, const bf16* w, const float* bias, bf16* y, int
   fprop_impl(x, w, bias, y, nullptr, nullptr, N, H, W, Cin, Cout, relu, bn, stream);
 }
 
-// EXPERIMENTAL: the pool windows must lie inside one epilogue warp (see ConvPolicy::epilogue_pool).
+// The pool windows must lie inside one epilogue warp (see ConvPolicy::epilogue_pool).
 bool conv3x3_pool_fusable(int N, int H, int W) {
   if (H % 2 || W % 2) return false;
   if (halo_applicable(H, W)) return true;               // 8 x 16 tiles

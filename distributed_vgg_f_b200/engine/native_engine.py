@@ -290,7 +290,7 @@ class NativeEngine:
         self.x_nhwc = torch.empty(B, HW, HW, 4, dtype=BF16, device=dev)
         self.acts: List[torch.Tensor] = []      # post-ReLU conv outputs
         self.pools: List[Optional[torch.Tensor]] = []
-        # EXPERIMENTAL, off unless B200_FUSE_POOL=1: the pooled layers' conv epilogue pools in
+        # On by default (B200_FUSE_POOL=0 turns it off): the pooled layers' conv epilogue pools in
         # registers and records argmax / ReLU bit masks; the un-pooled activation is never written
         # (acts[i] of such a layer then holds stale data) and backward is an "unpool" kernel.
         want_fused_pool = os.environ.get("B200_FUSE_POOL", "1") == "1"
@@ -413,7 +413,7 @@ class NativeEngine:
         if c0.pool_after:
             x = ops.maxpool2x2(x, out=self.pools[0][:b])
         for i, c in enumerate(spec.convs[1:], start=1):
-            if self.pool_masks[i] is not None:           # experimental fused conv + ReLU + pool
+            if self.pool_masks[i] is not None:           # fused conv + ReLU + pool
                 x, _ = ops.conv3x3_fprop_pool(x, self._w(c.name), self._b(c.name), out=self.pools[i][:b],
                                               mask=self.pool_masks[i][:b])
                 self._mark("fwd " + c.name)

@@ -70,8 +70,9 @@ def pool_mask_like(n: int, h: int, w: int, c: int, device) -> torch.Tensor:
 
 
 def conv3x3_fprop_pool(x, w, bias, bn: int = 0, out=None, mask=None):
-    """EXPERIMENTAL (B200_FUSE_POOL=1): maxpool2x2(relu(conv(x) + bias)) without materialising the
-    un-pooled tensor.  Returns (pooled bf16 [N,H/2,W/2,Cout], mask int32 [N,H/2,W/2,Cout/32,4])."""
+    """maxpool2x2(relu(conv(x) + bias)) without materialising the un-pooled tensor (the engine's
+    default for pooled layers; B200_FUSE_POOL=0 turns it off).
+    Returns (pooled bf16 [N,H/2,W/2,Cout], mask int32 [N,H/2,W/2,Cout/32,4])."""
     N, H, W, _ = x.shape
     cout = w.shape[0]
     p = out if out is not None else torch.empty(N, H // 2, W // 2, cout, dtype=torch.bfloat16, device=x.device)

@@ -73,18 +73,29 @@ def test_backward_matches_reference_on_same_forward(capsys):
     """Backward pass vs a torch fp32 chain with the engine's bf16 rounding points
     (ops.ref.emulated_step), gated on the engine's own forward activations: ReLU / pool routing is
     then identical on both sides and only accumulation order differs."""
+    _backward_on_same_forward(capsys, classes=3, batch=4, b=4)
+
+
+@pytest.mark.parametrize("classes,batch,b", [(10, 4, 4),     # > 8 classes: unfused head (GEMM + epilogue + CE)
+                                             (3, 4, 3)])     # ragged training batch
+def test_backward_matches_reference_unfused_head_and_ragged_batch(capsys, classes, batch, b):
+    """The same check on the paths the default mini model does not take."""
+    _backward_on_same_forward(capsys, classes=classes, batch=batch, b=b)
+
+
+def _backward_on_same_forward(capsys, classes, batch, b):
     from distributed_vgg_f_b200.models import layout as L
     from distributed_vgg_f_b200.ops import ref as R
 
     # the un-pooled activations this check gates on only exist when the pool is NOT fused into the conv
     # epilogue (the default fuses it: test_fused_pool_step_matches_unfused_step covers that path)
-    spec, oracle, eng = _mk(fuse_pool=False)
+    spec, oracle, eng = _mk(batch=batch, classes=classes, fuse_pool=False)
+    assert eng.fused_head == (classes <= 8)
     eng.train_dropout = False
     eng.apply_updates = False
     torch.manual_seed(3)
-    b = 4
     x = torch.randn(b, 3, 64, 64, device=DEV).to(torch.bfloat16).float()
-    y = torch.randint(0, 3, (b,), device=DEV)
+    y = torch.randint(0, classes, (b,), device=DEV)
     got_loss = float(eng.train_step((x, y)))
     eng.sync()
     override = {

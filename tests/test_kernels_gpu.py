@@ -4,11 +4,13 @@ bf16 operands: inputs are rounded to bf16 first, the reference is evaluated in f
 rounded values, so the only differences are accumulation order and the final bf16 rounding.
 """
 import math
-import os
 
 import pytest
 import torch
 import torch.nn.functional as F
+
+import kernel_check as KC
+from distributed_vgg_f_b200.ops import ref as R
 
 pytestmark = pytest.mark.gpu
 
@@ -30,95 +32,174 @@ def bf(t):
     return t.to(torch.bfloat16)
 
 
+MODES = ["exact", "gauss"]
+
+
+def _rup8(v):
+    return (v + 7) // 8 * 8
+
+
 # ------------------------------------------------------------------------------------------ GEMM
-@pytest.mark.parametrize("M,N,K", [(128, 64, 64), (256, 64, 512), (4096, 64, 4096), (200, 48, 200),
-                                   (4096, 96, 25088 // 8)])
-@pytest.mark.parametrize("ksplit", [1, 4])
+GEMM_KK = pytest.mark.parametrize("M,N,K", [
+    (128, 64, 64), (256, 64, 512), (4096, 64, 4096), (200, 48, 200), (4096, 96, 25088 // 8),
+    # N <= 32: 32-wide tiles (FC forward at batch <= 32, ragged last batches)
+    (4096, 1, 25088), (4096, 5, 4096), (512, 16, 4096), (4096, 32, 25088), (10, 37, 512)])
+KSPLIT = pytest.mark.parametrize("ksplit", [1, 4, 8])
+
+
+@GEMM_KK
+@KSPLIT
 def test_gemm_kk_transposed_out(M, N, K, ksplit):
     """FC forward form (swap-AB): out[b, n] += sum_k W[n, k] X[b, k]."""
+    _gemm_kk(M, N, K, ksplit, "gauss")
+
+
+@GEMM_KK
+@KSPLIT
+def test_gemm_kk_transposed_out_exact(M, N, K, ksplit):
+    _gemm_kk(M, N, K, ksplit, "exact")
+
+
+def _gemm_kk(M, N, K, ksplit, mode):
     ops = _ops()
-    torch.manual_seed(0)
-    Kp = (K + 7) // 8 * 8
-    A = bf(torch.randn(M, Kp, device=DEV))[:, :K]
-    B = bf(torch.randn(N, Kp, device=DEV))[:, :K]
+    g = KC.generator(M * 7 + N * 3 + K + ksplit, DEV)
+    Kp = _rup8(K)
+    A = KC.operand((M, Kp), mode, K, g, DEV)[:, :K]
+    B = KC.operand((N, Kp), mode, K, g, DEV)[:, :K]
     out = torch.zeros(N, M, device=DEV)
-    ops.gemm(A, B, out, M=M, N=N, K=K, epi="f32_atomic_t", ksplit=ksplit)
-    ref = B.float() @ A.float().t()
-    assert rel_err(out, ref) < 2e-3
+    ops.gemm(A, B, out, M=M, N=N, K=K, epi="f32_atomic_t", ksplit=ksplit, ldo=M)
+    ref, mag = R.gemm64(A, B, M=M, N=N, K=K, epi="f32_atomic_t")
+    KC.check(out, ref, mag, chain=KC.gemm_chain(K, ksplit), exact=mode == "exact", family="gemm")
 
 
-@pytest.mark.parametrize("M,N,K", [(128, 64, 64), (25088 // 4, 64, 4096), (300, 40, 130)])
+GEMM_MNK = pytest.mark.parametrize("M,N,K", [(128, 64, 64), (25088 // 4, 64, 4096), (300, 40, 130),
+                                                (4096, 32, 4096), (512, 3, 10)])
+
+
+@GEMM_MNK
 def test_gemm_mnk_store_t(M, N, K):
-    """FC dgrad form: A stored [K][M] (W[n_out][k_in] read as A[m=k_in, k=n_out])."""
+    """FC dgrad form: A stored [K][M] (W[n_out][k_in] read as A[m=k_in, k=n_out]); B = dz [N][K] with
+    ldb = round_up(K, 8)."""
+    _gemm_mnk(M, N, K, 1, "f32_store_t", "gauss")
+
+
+@GEMM_MNK
+def test_gemm_mnk_store_t_exact(M, N, K):
+    _gemm_mnk(M, N, K, 1, "f32_store_t", "exact")
+
+
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("M,N,K,ksplit", [(4096, 64, 4096, 8), (4096, 37, 4096, 8), (4096, 16, 512, 8),
+                                          (25088, 5, 4096, 8), (4096, 64, 4096, 1), (512, 10, 10, 1)])
+def test_gemm_mnk_atomic_t(M, N, K, ksplit, mode):
+    """FC dgrad as the engine runs it: M = fin, N = batch, K = fout, split-K into the atomic epilogue."""
+    _gemm_mnk(M, N, K, ksplit, "f32_atomic_t", mode)
+
+
+def _gemm_mnk(M, N, K, ksplit, epi, mode):
     ops = _ops()
-    torch.manual_seed(1)
-    Mp = (M + 7) // 8 * 8
-    Kp = (K + 7) // 8 * 8
-    A_km = bf(torch.randn(K, Mp, device=DEV))[:, :M]          # [K][M]
-    B = bf(torch.randn(N, Kp, device=DEV))[:, :K]             # [N][K]
+    g = KC.generator(M + N * 5 + K * 3 + ksplit, DEV)
+    A_km = KC.operand((K, _rup8(M)), mode, K, g, DEV)[:, :M]       # [K][M]
+    B = KC.operand((N, _rup8(K)), mode, K, g, DEV)[:, :K]          # [N][K]
     out = torch.zeros(N, M, device=DEV)
-    ops.gemm(A_km, B, out, M=M, N=N, K=K, a_mn=True, epi="f32_store_t")
-    ref = B.float() @ A_km.float()
-    assert rel_err(out, ref) < 2e-3
+    ops.gemm(A_km, B, out, M=M, N=N, K=K, a_mn=True, epi=epi, ksplit=ksplit, ldo=M)
+    ref, mag = R.gemm64(A_km, B, M=M, N=N, K=K, a_mn=True, epi=epi)
+    KC.check(out, ref, mag, chain=KC.gemm_chain(K, ksplit), exact=mode == "exact", family="gemm")
 
 
-@pytest.mark.parametrize("M,N,K", [(128, 64, 64), (4096, 1024, 64), (512, 256, 96), (3 * 8, 512, 64)])
+# FC wgrad: M = fout, N = fin, K = batch; A = dz [K][round_up(fout, 8)] (lda > M when fout % 8 != 0)
+WGRAD_FC = [(128, 64, 64), (4096, 1024, 64), (512, 256, 96), (3 * 8, 512, 64), (256, 72, 64),
+            (10, 4096, 5), (10, 4096, 37), (1000, 4096, 16), (4096, 512, 37), (10, 512, 64), (4096, 4096, 5)]
+
+
+@pytest.mark.parametrize("M,N,K", WGRAD_FC)
 def test_gemm_mnmn_store(M, N, K):
     """FC wgrad form: dW[n_out, k_in] = sum_b dY[b, n_out] X[b, k_in]; both operands [K][*]."""
+    _gemm_mnmn(M, N, K, "gauss")
+
+
+@pytest.mark.parametrize("M,N,K", WGRAD_FC)
+def test_gemm_mnmn_store_exact(M, N, K):
+    _gemm_mnmn(M, N, K, "exact")
+
+
+def _gemm_mnmn(M, N, K, mode):
     ops = _ops()
-    torch.manual_seed(2)
-    A_km = bf(torch.randn(K, M, device=DEV))
-    B_kn = bf(torch.randn(K, N, device=DEV))
+    g = KC.generator(M + N + K, DEV)
+    A_km = KC.operand((K, _rup8(M)), mode, K, g, DEV)
+    B_kn = KC.operand((K, N), mode, K, g, DEV)
     out = torch.empty(M, N, device=DEV)
     ops.gemm(A_km, B_kn, out, M=M, N=N, K=K, a_mn=True, b_mn=True, epi="f32_store", alpha=0.5)
-    ref = 0.5 * (A_km.float().t() @ B_kn.float())
-    assert rel_err(out, ref) < 2e-3
+    ref, mag = R.gemm64(A_km, B_kn, M=M, N=N, K=K, a_mn=True, b_mn=True, alpha=0.5)
+    KC.check(out, ref, mag, chain=KC.gemm_chain(K), exact=mode == "exact", family="gemm")
 
 
-@pytest.mark.parametrize("M,N,K,off", [(128, 64, 64, 0), (4096, 1024, 64, 0), (512, 256, 96, 8), (256, 72, 64, 0),
-                                       (24, 512, 64, 4)])
+GEMM_MNMN_BF16 = pytest.mark.parametrize("M,N,K,off", [
+    (128, 64, 64, 0), (4096, 1024, 64, 0), (512, 256, 96, 8), (256, 72, 64, 0), (24, 512, 64, 4),
+    (10, 4096, 5, 0), (10, 4096, 37, 8), (1000, 4096, 16, 0), (4096, 512, 37, 4)])
+
+
+@GEMM_MNMN_BF16
 def test_gemm_mnmn_bf16_store(M, N, K, off):
     """FC wgrad written straight to the bf16 wire: out = bf16(alpha * dY^T X).  ``off`` shifts the
     output start by a few elements (32-byte vs 16-byte vs scalar store paths), N=72 is ragged."""
+    _gemm_mnmn_bf16(M, N, K, off, "gauss")
+
+
+@GEMM_MNMN_BF16
+def test_gemm_mnmn_bf16_store_exact(M, N, K, off):
+    _gemm_mnmn_bf16(M, N, K, off, "exact")
+
+
+def _gemm_mnmn_bf16(M, N, K, off, mode):
     ops = _ops()
-    torch.manual_seed(4)
-    A_km = bf(torch.randn(K, M, device=DEV))
-    B_kn = bf(torch.randn(K, N, device=DEV))
+    g = KC.generator(M * 3 + N + K + off, DEV)
+    A_km = KC.operand((K, _rup8(M)), mode, K, g, DEV)
+    B_kn = KC.operand((K, N), mode, K, g, DEV)
     buf = torch.full((M * N + 64,), 7.0, dtype=torch.bfloat16, device=DEV)
     out = buf[off:off + M * N].view(M, N)
     ops.gemm(A_km, B_kn, out, M=M, N=N, K=K, a_mn=True, b_mn=True, epi="bf16_store", alpha=0.125)
-    ref = 0.125 * (A_km.float().t() @ B_kn.float())
-    assert rel_err(out, ref) < 1e-2
+    ref, mag = R.gemm64(A_km, B_kn, M=M, N=N, K=K, a_mn=True, b_mn=True, alpha=0.125)
+    KC.check(out, ref, mag, chain=KC.gemm_chain(K), exact=mode == "exact", family="gemm")
     assert bool((buf[:off] == 7.0).all()) and bool((buf[off + M * N:] == 7.0).all())
 
 
 def test_gemm_bf16_bias_relu():
     """Layer-0 im2col GEMM: bf16(relu(A W^T + b))."""
+    _gemm_bias_relu(1000, 64, 64, "gauss")
+
+
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("M,N,K", [(1000, 64, 64), (300, 48, 64), (129, 96, 128)])
+def test_gemm_bf16_bias_relu_ragged_n(M, N, K, mode):
+    """A ragged N (48, 96) must write nothing past column N of a row nor past the end of the output,
+    and read no bias past N (the bias is a slice of a NaN-filled buffer)."""
+    _gemm_bias_relu(M, N, K, mode)
+
+
+def _gemm_bias_relu(M, N, K, mode):
     ops = _ops()
-    torch.manual_seed(3)
-    M, N, K = 1000, 64, 64
-    A = bf(torch.randn(M, K, device=DEV))
-    W = bf(torch.randn(N, K, device=DEV) * 0.2)
-    bias = torch.randn(N, device=DEV)
-    out = torch.empty(M, N, dtype=torch.bfloat16, device=DEV)
+    g = KC.generator(M + N + K, DEV)
+    A = KC.operand((M, K), mode, K, g, DEV)
+    W = KC.operand((N, K), mode, K, g, DEV, scale=0.2)
+    bias_buf = torch.full((N + 64,), float("nan"), device=DEV)
+    bias_buf[16:16 + N] = KC.bias(N, mode, g, DEV)
+    bias = bias_buf[16:16 + N]
+    buf = torch.full((M * N + 256,), 7.0, dtype=torch.bfloat16, device=DEV)
+    out = buf[:M * N].view(M, N)
     ops.gemm(A, W, out, M=M, N=N, K=K, epi="bf16_bias_relu", bias=bias)
-    ref = torch.relu(A.float() @ W.float().t() + bias)
-    assert rel_err(out, ref) < 1e-2
+    ref, mag = R.gemm64(A, W, M=M, N=N, K=K, epi="bf16_bias_relu", bias=bias)
+    KC.check(out, ref, mag, chain=KC.gemm_chain(K), exact=mode == "exact", family="gemm")
+    assert bool((buf[M * N:] == 7.0).all())
 
 
 # ------------------------------------------------------------------------------------------ conv
-def _conv_case(N, H, W, Cin, Cout, seed=0):
-    torch.manual_seed(seed)
-    x = bf(torch.randn(N, H, W, Cin, device=DEV))
-    w = bf(torch.randn(Cout, 3, 3, Cin, device=DEV) * (1.0 / math.sqrt(9 * Cin)))
-    b = torch.randn(Cout, device=DEV) * 0.1
-    return x, w, b
-
-
-def _conv_ref(x, w, b):
-    xr = x.float().permute(0, 3, 1, 2)
-    wr = w.float().permute(0, 3, 1, 2)
-    return F.conv2d(xr, wr, b, padding=1)
+def _conv_case(N, H, W, Cin, Cout, seed=0, mode="gauss"):
+    g = KC.generator(seed * 1000003 + N * 7919 + H * 131 + Cin + Cout, DEV)
+    x = KC.operand((N, H, W, Cin), mode, 9 * Cin, g, DEV)
+    w = KC.operand((Cout, 3, 3, Cin), mode, 9 * Cin, g, DEV, scale=1.0 / math.sqrt(9 * Cin))
+    b = KC.bias(Cout, mode, g, DEV)
+    return x, w, b, g
 
 
 CONV_SHAPES = [(2, 16, 16, 64, 64), (1, 28, 28, 128, 256), (4, 14, 14, 512, 512), (2, 56, 56, 64, 128),
@@ -126,102 +207,184 @@ CONV_SHAPES = [(2, 16, 16, 64, 64), (1, 28, 28, 128, 256), (4, 14, 14, 512, 512)
                # halo-tile kernel (H % 16 == 0, W % 8 == 0, W >= 32): resident / streaming weights
                (2, 32, 32, 64, 64), (1, 32, 32, 64, 128), (1, 48, 64, 128, 128), (1, 32, 32, 256, 256),
                (3, 16, 40, 128, 64)]
+# one layer per VGG resolution, at batch 64 and at a ragged last batch of 37
+VGG_SHAPES = [(n, h, h, c, c) for n in (64, 37) for h, c in ((224, 64), (112, 128), (56, 256), (28, 512), (14, 512))]
+CONV_ALL = pytest.mark.parametrize("N,H,W,Cin,Cout", CONV_SHAPES + VGG_SHAPES)
 
 
-@pytest.mark.parametrize("N,H,W,Cin,Cout", CONV_SHAPES)
+@CONV_ALL
 def test_conv_fprop(N, H, W, Cin, Cout):
+    _conv_fprop(N, H, W, Cin, Cout, "gauss")
+
+
+@CONV_ALL
+def test_conv_fprop_exact(N, H, W, Cin, Cout):
+    _conv_fprop(N, H, W, Cin, Cout, "exact")
+
+
+def _conv_fprop(N, H, W, Cin, Cout, mode):
     ops = _ops()
-    x, w, b = _conv_case(N, H, W, Cin, Cout)
+    x, w, b, _ = _conv_case(N, H, W, Cin, Cout, mode=mode)
     y = ops.conv3x3_fprop(x, w, b, relu=True)
-    ref = torch.relu(_conv_ref(x, w, b)).permute(0, 2, 3, 1)
-    assert rel_err(y, ref) < 1e-2
+    ref, mag = R.conv3x3_fprop64(x, w, b, relu=True)
+    KC.check(y, ref, mag, chain=KC.conv_chain(Cin), exact=mode == "exact", family="conv_fprop")
 
 
-@pytest.mark.parametrize("N,H,W,Cin,Cout", CONV_SHAPES)
+def test_conv_fprop_rejects_a_bias_wider_than_its_scratch():
+    """The fprop epilogue stages the bias in 512 floats of shared memory: Cout > 512 with a bias is
+    refused on the host (without a bias the layer is fine)."""
+    ops = _ops()
+    x = torch.zeros(1, 8, 8, 64, dtype=torch.bfloat16, device=DEV)
+    w = torch.zeros(576, 3, 3, 64, dtype=torch.bfloat16, device=DEV)
+    with pytest.raises(RuntimeError, match="Cout <= 512"):
+        ops.conv3x3_fprop(x, w, torch.zeros(576, device=DEV))
+    with pytest.raises(RuntimeError, match="Cout <= 512"):
+        ops.conv3x3_fprop_pool(x, w, torch.zeros(576, device=DEV))
+    torch.cuda.synchronize()
+
+
+@CONV_ALL
 def test_conv_dgrad(N, H, W, Cin, Cout):
+    _conv_dgrad(N, H, W, Cin, Cout, "gauss")
+
+
+@CONV_ALL
+def test_conv_dgrad_exact(N, H, W, Cin, Cout):
+    _conv_dgrad(N, H, W, Cin, Cout, "exact")
+
+
+def _conv_dgrad(N, H, W, Cin, Cout, mode):
     ops = _ops()
-    x, w, _ = _conv_case(N, H, W, Cin, Cout, seed=1)
-    dz = bf(torch.randn(N, H, W, Cout, device=DEV))
+    x, w, _, g = _conv_case(N, H, W, Cin, Cout, seed=1, mode=mode)
+    exact = mode == "exact"
+    dz = KC.operand((N, H, W, Cout), mode, 9 * Cout, g, DEV)
     dx = ops.conv3x3_dgrad(dz, w, Cin)
-    ref = F.conv_transpose2d(dz.float().permute(0, 3, 1, 2), w.float().permute(0, 3, 1, 2),
-                             padding=1).permute(0, 2, 3, 1)
-    assert rel_err(dx, ref) < 1e-2
+    ref, mag = R.conv3x3_dgrad64(dz, w)
+    chain = KC.conv_chain(Cout)
+    KC.check(dx, ref, mag, chain=chain, exact=exact, family="conv_dgrad")
     # fused ReLU mask
-    mask_src = bf(torch.randn(N, H, W, Cin, device=DEV))
+    mask_src = KC.operand((N, H, W, Cin), "gauss", 1, g, DEV)
     dx2 = ops.conv3x3_dgrad(dz, w, Cin, mask_src=mask_src)
-    assert rel_err(dx2, ref * (mask_src.float() > 0)) < 1e-2
+    ref, mag = R.conv3x3_dgrad64(dz, w, mask_src=mask_src)
+    KC.check(dx2, ref, mag, chain=chain, exact=exact, family="conv_dgrad", what="masked")
     # fused column sum (= bias gradient of the previous layer): sums exactly what was stored
-    cs = torch.zeros(Cin, device=DEV)
-    dx3 = ops.conv3x3_dgrad(dz, w, Cin, mask_src=mask_src, colsum=cs)
-    assert torch.equal(dx3, dx2)
-    assert rel_err(cs, dx2.float().sum((0, 1, 2))) < 1e-3
+    if Cin <= 512:
+        cs = torch.zeros(Cin, device=DEV)
+        dx3 = ops.conv3x3_dgrad(dz, w, Cin, mask_src=mask_src, colsum=cs)
+        assert torch.equal(dx3, dx2)
+        stored = dx2.to(torch.float64).reshape(-1, Cin)
+        KC.check(cs, stored.sum(0), stored.abs().sum(0), chain=KC.conv_colsum_chain(N * H * W, Cin, KC.sm_count()),
+                 exact=False, family="conv_colsum")
 
 
-@pytest.mark.parametrize("N,H,W,Cin,Cout", CONV_SHAPES)
+@CONV_ALL
 def test_conv_wgrad(N, H, W, Cin, Cout):
+    _conv_wgrad(N, H, W, Cin, Cout, "gauss")
+
+
+@CONV_ALL
+def test_conv_wgrad_exact(N, H, W, Cin, Cout):
+    _conv_wgrad(N, H, W, Cin, Cout, "exact")
+
+
+def _conv_wgrad(N, H, W, Cin, Cout, mode):
     ops = _ops()
-    x, w, _ = _conv_case(N, H, W, Cin, Cout, seed=2)
-    dz = bf(torch.randn(N, H, W, Cout, device=DEV))
+    g = KC.generator(N * 7 + H + Cin * 3 + Cout, DEV)
+    P = N * H * W
+    x = KC.operand((N, H, W, Cin), mode, P, g, DEV)
+    dz = KC.operand((N, H, W, Cout), mode, P, g, DEV)
     dw = torch.zeros(Cout, 3, 3, Cin, device=DEV)
     ops.conv3x3_wgrad(dz, x, dw)
-    xr = x.float().permute(0, 3, 1, 2).requires_grad_(False)
-    wr = w.float().permute(0, 3, 1, 2).clone().requires_grad_(True)
-    F.conv2d(xr, wr, None, padding=1).backward(dz.float().permute(0, 3, 1, 2))
-    ref = wr.grad.permute(0, 2, 3, 1)
-    assert rel_err(dw, ref) < 5e-3
+    ref, mag = R.conv3x3_wgrad64(dz, x)
+    KC.check(dw, ref, mag, chain=KC.wgrad_chain(N, H, W, Cin, Cout, KC.sm_count()), exact=mode == "exact",
+             family="conv_wgrad")
 
 
-@pytest.mark.parametrize("N,H,W", [(2, 16, 16), (1, 30, 22), (3, 64, 64)])
+CONV0 = pytest.mark.parametrize("N,H,W", [(2, 16, 16), (1, 30, 22), (3, 64, 64), (64, 224, 224), (37, 224, 224)])
+
+
+@CONV0
 def test_conv0_fused(N, H, W):
-    """First conv straight from NHWC4 pixels (im2col tile built in shared memory): fprop + wgrad."""
+    """First conv straight from NHWC4 pixels (im2col tile built in shared memory): fprop + wgrad.
+    64 x 224 x 224 gives every CTA many tiles, so the stage ring and the builder groups wrap."""
+    _conv0(N, H, W, "gauss")
+
+
+@CONV0
+def test_conv0_fused_exact(N, H, W):
+    _conv0(N, H, W, "exact")
+
+
+def _conv0(N, H, W, mode):
     ops = _ops()
     C = ops.require()
-    torch.manual_seed(0)
-    x = bf(torch.randn(N, H, W, 3, device=DEV))
+    exact = mode == "exact"
+    g = KC.generator(N * 31 + H + W, DEV)
     x4 = torch.zeros(N, H, W, 4, dtype=torch.bfloat16, device=DEV)
-    x4[..., :3] = x
-    w = bf(torch.randn(64, 3, 3, 3, device=DEV) * 0.2)           # [co][kh][kw][c]
+    x4[..., :3] = KC.operand((N, H, W, 3), mode, 27, g, DEV)
     w0 = torch.zeros(64, 64, dtype=torch.bfloat16, device=DEV)
-    w0[:, :27] = w.reshape(64, 27)
-    bias = torch.randn(64, device=DEV)
+    w0[:, :27] = KC.operand((64, 27), mode, 27, g, DEV, scale=0.2)
+    bias = KC.bias(64, mode, g, DEV)
     y = torch.empty(N, H, W, 64, dtype=torch.bfloat16, device=DEV)
     C.conv0_fprop(x4, w0, bias, y)
-    xr = x.float().permute(0, 3, 1, 2)
-    wr = w.float().permute(0, 3, 1, 2).clone().requires_grad_(True)
-    ref = torch.relu(F.conv2d(xr, wr, bias, padding=1))
-    assert rel_err(y, ref.permute(0, 2, 3, 1)) < 1e-2
-    dz = bf(torch.randn(N, H, W, 64, device=DEV))
+    ref, mag = R.conv0_fprop64(x4, w0, bias)
+    KC.check(y, ref, mag, chain=KC.gemm_chain(64), exact=exact, family="conv0_fprop")
+    P = N * H * W
+    x4w = torch.zeros_like(x4)
+    x4w[..., :3] = KC.operand((N, H, W, 3), mode, P, g, DEV)
+    dz = KC.operand((N, H, W, 64), mode, P, g, DEV)
     dw0 = torch.zeros(64, 64, device=DEV)
-    C.conv0_wgrad(dz, x4, dw0)
-    F.conv2d(xr, wr, None, padding=1).backward(dz.float().permute(0, 3, 1, 2))
-    assert rel_err(dw0[:, :27], wr.grad.permute(0, 2, 3, 1).reshape(64, 27)) < 5e-3
-    assert torch.count_nonzero(dw0[:, 27:]) == 0
+    C.conv0_wgrad(dz, x4w, dw0)
+    ref, mag = R.conv0_wgrad64(dz, x4w)
+    KC.check(dw0, ref, mag, chain=KC.conv0_wgrad_chain(P, KC.sm_count()), exact=exact, family="conv0_wgrad")
 
 
 # ------------------------------------------------------------------------------------- pointwise
-EXPERIMENTAL = pytest.mark.skipif(os.environ.get("B200_EXPERIMENTAL", "0") != "1",
-                                  reason="experimental kernels: set B200_EXPERIMENTAL=1")
+POOL_SHAPES = [(2, 32, 32, 64, 64), (1, 48, 64, 128, 128), (2, 56, 56, 64, 128), (3, 28, 28, 128, 256),
+               (4, 14, 14, 512, 512), (1, 224, 224, 64, 64),
+               # the pooled VGG layers at batch 64 and at a ragged batch of 37
+               (64, 224, 224, 64, 64), (37, 112, 112, 128, 128), (64, 56, 56, 256, 256), (37, 28, 28, 512, 512),
+               (64, 14, 14, 512, 512), (37, 14, 14, 512, 512)]
 
 
-@EXPERIMENTAL
-@pytest.mark.parametrize("N,H,W,Cin,Cout", [(2, 32, 32, 64, 64), (1, 48, 64, 128, 128), (2, 56, 56, 64, 128),
-                                            (3, 28, 28, 128, 256), (4, 14, 14, 512, 512), (1, 224, 224, 64, 64)])
+@pytest.mark.parametrize("N,H,W,Cin,Cout", POOL_SHAPES)
 def test_conv_fprop_pool_fused(N, H, W, Cin, Cout):
-    """conv + bias + ReLU + 2x2 max-pool in the conv epilogue, and its unpool backward, against the
-    separate kernels (bit-identical by construction: same rounding point, same first-maximum rule)."""
+    """conv + bias + ReLU + 2x2 max-pool in the conv epilogue (the default for pooled layers) against
+    the float64 reference, and bit-identical to the separate kernels (same rounding point, same
+    first-maximum rule); then its unpool backward."""
+    _conv_pool(N, H, W, Cin, Cout, "gauss")
+
+
+@pytest.mark.parametrize("N,H,W,Cin,Cout", POOL_SHAPES)
+def test_conv_fprop_pool_fused_exact(N, H, W, Cin, Cout):
+    _conv_pool(N, H, W, Cin, Cout, "exact")
+
+
+def _conv_pool(N, H, W, Cin, Cout, mode):
     ops = _ops()
-    x, w, b = _conv_case(N, H, W, Cin, Cout, seed=5)
-    y = ops.conv3x3_fprop(x, w, b, relu=True)
-    p_ref = ops.maxpool2x2(y)
+    exact = mode == "exact"
+    x, w, b, g = _conv_case(N, H, W, Cin, Cout, seed=5, mode=mode)
     p, mask = ops.conv3x3_fprop_pool(x, w, b)
-    assert torch.equal(p, p_ref)
-    dp = bf(torch.randn(N, H // 2, W // 2, Cout, device=DEV))
+    ref, mag = R.conv3x3_fprop64(x, w, b, relu=True)
+    KC.check_pool(p, mask, ref, mag, chain=KC.conv_chain(Cin), exact=exact)
+    del ref, mag
+    y = ops.conv3x3_fprop(x, w, b, relu=True)
+    assert torch.equal(p, ops.maxpool2x2(y))
+    idx, pos = R.pool_mask_decode(mask, Cout)
+    _, ridx, rpos = R.pool2x2_select(y.float())
+    assert torch.equal(pos, rpos) and torch.equal(torch.where(pos, idx, 0), torch.where(rpos, ridx, 0))
+    dp = KC.operand((N, H // 2, W // 2, Cout), mode, 1, g, DEV)
     cs_ref = torch.zeros(Cout, device=DEV)
     dz_ref = ops.maxpool2x2_relu_bwd(y, dp, colsum=cs_ref)
+    del y
     cs = torch.zeros(Cout, device=DEV)
     dz = ops.unpool2x2(dp, mask, colsum=cs)
     assert torch.equal(dz, dz_ref)
-    assert rel_err(cs, cs_ref) < 1e-3
+    want, want_cs, cs_mag = R.unpool2x2_64(dp, idx, pos)
+    KC.check(dz, want, want, chain=0, exact=True, family="unpool2x2")
+    chain = KC.unpool_colsum_chain(N * (H // 2) * (W // 2), Cout, KC.sm_count())
+    KC.check(cs, want_cs, cs_mag, chain=chain, exact=False, family="unpool_colsum")
+    KC.check(cs_ref, want_cs, cs_mag, chain=chain, exact=False, family="unpool_colsum", what="maxpool2x2_relu_bwd")
 
 
 def test_maxpool_fwd_bwd():
