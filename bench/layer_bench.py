@@ -2,7 +2,10 @@
 fprop / dgrad / wgrad, the FC GEMMs and the memory-bound kernels, with achieved TFLOP/s or GB/s
 against MEASURED_PEAKS.json, and torch (cuDNN/cuBLAS, bf16 channels_last) numbers for context.
 Writes gpurun_out/layer_bench.json and prints a table."""
-import json, os, sys, time
+# Without MEASURED_PEAKS.json the peaks are the H100 SXM data sheet's: 989 dense bf16 TFLOP/s and
+# 3,350 GB/s.  Every native conv call uses the training step's kernel choice (bn = 0, ksplit = 0).
+# The table is headed by the card's name, power limit and maximum SM clock.
+import json, os, subprocess, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import torch.nn.functional as F
@@ -13,8 +16,20 @@ dev = "cuda"
 B = int(os.environ.get("LB_BATCH", "64"))
 HW = 224
 PEAK = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json"))) \
-    if os.path.exists(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")) else {"bf16_tflops": 1590.0, "hbm_gbs": 6650.0}
+    if os.path.exists(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")) else {"bf16_tflops": 989.0, "hbm_gbs": 3350.0}
 flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
+
+
+def card_info():
+    info = {"name": torch.cuda.get_device_name(), "power_limit": None, "sm_max_clock": None}
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()),
+                            "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        info["power_limit"], info["sm_max_clock"] = q[0].strip(), q[1].strip()
+    except (OSError, IndexError, subprocess.SubprocessError):
+        pass
+    return info
 
 
 def timeit(fn, iters=5, warm=2):
@@ -67,21 +82,20 @@ for i, c in enumerate(spec.convs):
         dw = torch.zeros(c.cout, 3, 3, c.cin, device=dev)
         fl = 2.0 * B * h * h * c.cout * 9 * c.cin / 1e12
         C = ops.require()
-        for bn in ([64] if c.cout == 64 else [128]):
-            t = timeit(lambda: C.conv_fprop(x, w, bias, y, True, bn))
-            rows.append(("%s fprop %dx%d %d->%d bn%d" % (c.name, h, h, c.cin, c.cout, bn), t, fl, 0))
-        for bn in ([64] if c.cin == 64 else [128]):
-            t = timeit(lambda: C.conv_dgrad(dz, w, x, dx, None, bn))
-            rows.append(("%s dgrad bn%d" % (c.name, bn), t, fl, 0))
-            cs = torch.zeros(c.cin, device=dev)
-            t = timeit(lambda: C.conv_dgrad(dz, w, x, dx, cs, bn))
-            rows.append(("%s dgrad+colsum bn%d" % (c.name, bn), t, fl, 0))
-        for bn in ([64] if c.cin == 64 else [128]):
-            t = timeit(lambda: C.conv_wgrad(dz, x, dw, 1.0, 0, bn))
-            rows.append(("%s wgrad bn%d" % (c.name, bn), t, fl, 0))
-        if c.cin == 64:
-            t = timeit(lambda: C.conv_wgrad(dz, x, dw, 1.0, 0, 0))
-            rows.append(("%s wgrad halo64" % c.name, t, fl, 0))
+        t = timeit(lambda: C.conv_fprop(x, w, bias, y, True, 0))
+        rows.append(("%s fprop %dx%d %d->%d" % (c.name, h, h, c.cin, c.cout), t, fl, 0))
+        if c.pool_after:                         # what the step runs for a pooled layer
+            pooled = torch.empty(B, h // 2, h // 2, c.cout, dtype=torch.bfloat16, device=dev)
+            pmask = ops.pool_mask_like(B, h, h, c.cout, dev)
+            t = timeit(lambda: C.conv_fprop_pool(x, w, bias, pooled, pmask, 0))
+            rows.append(("%s fprop+pool" % c.name, t, fl, 0))
+        t = timeit(lambda: C.conv_dgrad(dz, w, x, dx, None, 0))
+        rows.append(("%s dgrad" % c.name, t, fl, 0))
+        cs = torch.zeros(c.cin, device=dev)
+        t = timeit(lambda: C.conv_dgrad(dz, w, x, dx, cs, 0))
+        rows.append(("%s dgrad+colsum" % c.name, t, fl, 0))
+        t = timeit(lambda: C.conv_wgrad(dz, x, dw, 1.0, 0, 0))    # Cin = 64 on 8-divisible maps: the halo kernel
+        rows.append(("%s wgrad" % c.name, t, fl, 0))
         if with_torch:
             xt = x.permute(0, 3, 1, 2)            # NCHW view, channels_last memory
             wt = w.permute(0, 3, 1, 2)
@@ -146,7 +160,9 @@ t = timeit(lambda: ops.require().im2col_c3(x4, col, 64))
 rows.append(("NHWC4 -> im2col", t, 0, col.numel() * 2 / 1e9))
 
 out = []
-tot_native = 0.0
+card = card_info()
+print("card: %s, power limit %s, max SM clock %s; peaks %.0f TFLOP/s, %.0f GB/s"
+      % (card["name"], card["power_limit"], card["sm_max_clock"], PEAK["bf16_tflops"], PEAK["hbm_gbs"]))
 print("%-46s %9s %9s %9s %7s" % ("kernel", "ms", "TFLOP/s", "GB/s", "%peak"))
 for name, ms, tf, gb in rows:
     tfs = tf / (ms / 1e3) if tf else 0.0

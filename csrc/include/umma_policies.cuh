@@ -486,13 +486,18 @@ struct ConvPolicy {
   // Transpose-reduce across the warp with shuffles (recursive halving, 31 SHFL): afterwards lane l
   // holds the sum over the warp's 32 pixels of column l, added to the per-CTA sums in shared
   // memory.  No shared-memory traffic for the reduction itself -- operand staging saturates it.
+  // Both loops have constant trip counts so that they unroll completely: with `i < s` as the bound
+  // ptxas kept a partly unrolled loop that indexed cs[] at run time, which put cs[] -- and the
+  // epilogue's column sums -- in local memory (a 128-byte stack frame, ~100 local loads and stores).
   __device__ static void colsum_flush(const Params& p, int ch0, int lane, float (&cs)[32], float* sm) {
     __syncwarp();
 #pragma unroll
-    for (int s = 16; s >= 1; s >>= 1) {
+    for (int level = 0; level < 5; ++level) {
+      const int s = 16 >> level;
       const bool upper = (lane & s) != 0;
 #pragma unroll
-      for (int i = 0; i < s; ++i) {
+      for (int i = 0; i < 16; ++i) {
+        if (i >= s) continue;
         const float keep = upper ? cs[i + s] : cs[i];
         const float send = upper ? cs[i] : cs[i + s];
         cs[i] = keep + __shfl_xor_sync(0xffffffffu, send, s);
