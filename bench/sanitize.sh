@@ -14,6 +14,16 @@ for tool in memcheck synccheck; do
       > ${OUT:-prof_out}/sanitize_$tool.log 2>&1
   echo "== compute-sanitizer $tool exit $?"; grep -E "ERROR SUMMARY|passed|failed" ${OUT:-prof_out}/sanitize_$tool.log | tail -3
 done
+# one small case of each family of the float64 element-wise tests, under memcheck and racecheck
+E='maxpool_fwd_relu_bwd_colsum and 3-16-8 or avgpool_fwd_bwd and 5-64-1 or bias_grad and 37-3-8 or bias_grad and 64-64-64'
+E+=' or fc_bias_act_and_dropout and 37-10-0.6 or fc_grad_act and 1-5-True or test_cross_entropy and 7-10 or head_ce and 37-3'
+E+=' or adam_steps or sgd_steps and 0.0 or casts and 4099 or nchw_to_nhwc_zero_pads and 1-3-5'
+for tool in memcheck racecheck; do
+  timeout 900 $SAN --tool $tool --error-exitcode 7 python -m pytest tests/test_elementwise_gpu.py -q -x -m gpu -k "$E" \
+      > ${OUT:-prof_out}/sanitize_elementwise_$tool.log 2>&1
+  echo "== compute-sanitizer $tool (elementwise) exit $?"
+  grep -E "RACECHECK SUMMARY|ERROR SUMMARY|passed|failed" ${OUT:-prof_out}/sanitize_elementwise_$tool.log | tail -3
+done
 timeout 900 $SAN --tool racecheck --error-exitcode 7 python -m pytest tests/test_kernels_gpu.py -q -x -m gpu \
     -k "maxpool or cross_entropy and 64-3 or bias_grad and 64-3 or adam or head_ce" > ${OUT:-prof_out}/sanitize_racecheck.log 2>&1
 echo "== compute-sanitizer racecheck exit $?"; grep -E "RACECHECK SUMMARY|ERROR SUMMARY|passed|failed" ${OUT:-prof_out}/sanitize_racecheck.log | tail -3

@@ -23,6 +23,18 @@ static float* f32p(const at::Tensor& t) {
 }
 static const bf16* bfp_opt(const c10::optional<at::Tensor>& t) { return t.has_value() ? bfp(*t) : nullptr; }
 static float* f32p_opt(const c10::optional<at::Tensor>& t) { return t.has_value() ? f32p(*t) : nullptr; }
+// The element-wise kernels move 16-byte (8 x bf16 / 4 x fp32) or 8-byte vectors: refuse a tensor they
+// would read or write out of bounds or misaligned before anything is launched.
+static void check_vec(const at::Tensor& t, at::ScalarType dt, int64_t align, const char* op, const char* name) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == dt && t.is_contiguous(), op, ": ", name, " must be a contiguous CUDA ",
+              dt == at::kFloat ? "fp32" : "bf16", " tensor");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % align == 0, op, ": ", name, " must be ", align,
+              "-byte aligned");
+}
+static void check_nhwc(const at::Tensor& t, int64_t N, int64_t H, int64_t W, int64_t C, const char* op, const char* name) {
+  TORCH_CHECK(t.dim() == 4 && t.size(0) == N && t.size(1) == H && t.size(2) == W && t.size(3) == C, op, ": ", name,
+              " must be [", N, ", ", H, ", ", W, ", ", C, "], got ", t.sizes());
+}
 
 // ------------------------------------------------------------------------------------- GEMM / conv
 static void gemm(const at::Tensor& A, bool a_mn, const at::Tensor& B, bool b_mn, int64_t M, int64_t N,
@@ -104,24 +116,49 @@ static void conv0_wgrad(const at::Tensor& dz, const at::Tensor& x4, at::Tensor d
 // ------------------------------------------------------------------------------------ element-wise
 static void maxpool_fwd(const at::Tensor& x, at::Tensor y) {
   c10::cuda::CUDAGuard g(x.device());
+  check_vec(x, at::kBFloat16, 16, "maxpool_fwd", "x");
+  check_vec(y, at::kBFloat16, 16, "maxpool_fwd", "y");
+  TORCH_CHECK(x.dim() == 4, "maxpool_fwd: x must be NHWC");
+  check_nhwc(y, x.size(0), x.size(1) / 2, x.size(2) / 2, x.size(3), "maxpool_fwd", "y");
   b200::maxpool2x2_fwd(bfp(x), bfp_mut(y), x.size(0), x.size(1), x.size(2), x.size(3), cur_stream());
 }
 static void maxpool_relu_bwd(const at::Tensor& y, const at::Tensor& dp, at::Tensor dz,
                              c10::optional<at::Tensor> colsum) {
   c10::cuda::CUDAGuard g(y.device());
+  check_vec(y, at::kBFloat16, 16, "maxpool_relu_bwd", "y");
+  check_vec(dp, at::kBFloat16, 16, "maxpool_relu_bwd", "dp");
+  check_vec(dz, at::kBFloat16, 16, "maxpool_relu_bwd", "dz");
+  TORCH_CHECK(y.dim() == 4, "maxpool_relu_bwd: y must be NHWC");
+  check_nhwc(dp, y.size(0), y.size(1) / 2, y.size(2) / 2, y.size(3), "maxpool_relu_bwd", "dp");
+  check_nhwc(dz, y.size(0), y.size(1), y.size(2), y.size(3), "maxpool_relu_bwd", "dz");
+  if (colsum.has_value())
+    TORCH_CHECK(colsum->scalar_type() == at::kFloat && colsum->numel() >= y.size(3), "maxpool_relu_bwd: colsum fp32 [C]");
   b200::maxpool2x2_relu_bwd(bfp(y), bfp(dp), bfp_mut(dz), f32p_opt(colsum), y.size(0), y.size(1), y.size(2), y.size(3),
                             cur_stream());
 }
 static void avgpool_fwd(const at::Tensor& x, at::Tensor y) {
   c10::cuda::CUDAGuard g(x.device());
+  check_vec(x, at::kBFloat16, 16, "avgpool_fwd", "x");
+  check_vec(y, at::kBFloat16, 16, "avgpool_fwd", "y");
+  TORCH_CHECK(x.dim() == 4 && y.dim() == 4, "avgpool_fwd: NHWC x and y");
+  check_nhwc(y, x.size(0), y.size(1), y.size(2), x.size(3), "avgpool_fwd", "y");
   b200::adaptive_avgpool_fwd(bfp(x), bfp_mut(y), x.size(0), x.size(1), x.size(2), x.size(3), y.size(1), y.size(2), cur_stream());
 }
 static void avgpool_bwd(const at::Tensor& dy, at::Tensor dx) {
   c10::cuda::CUDAGuard g(dy.device());
+  check_vec(dy, at::kBFloat16, 16, "avgpool_bwd", "dy");
+  check_vec(dx, at::kBFloat16, 16, "avgpool_bwd", "dx");
+  TORCH_CHECK(dy.dim() == 4 && dx.dim() == 4, "avgpool_bwd: NHWC dy and dx");
+  check_nhwc(dy, dx.size(0), dy.size(1), dy.size(2), dx.size(3), "avgpool_bwd", "dy");
   b200::adaptive_avgpool_bwd(bfp(dy), bfp_mut(dx), dx.size(0), dx.size(1), dx.size(2), dx.size(3), dy.size(1), dy.size(2), cur_stream());
 }
 static void bias_grad(const at::Tensor& dz, at::Tensor db, int64_t rows, int64_t C, int64_t ld, double scale) {
   c10::cuda::CUDAGuard g(dz.device());
+  TORCH_CHECK(dz.is_cuda() && dz.scalar_type() == at::kBFloat16 && dz.is_contiguous() && ld >= C && C > 0 &&
+                  dz.numel() >= (rows - 1) * ld + C,
+              "bias_grad: contiguous bf16 dz of at least rows x ld elements, ld >= C");
+  TORCH_CHECK(db.scalar_type() == at::kFloat && db.numel() >= C, "bias_grad: db must be fp32 with C elements");
+  if (C % 8 == 0 && ld == C) check_vec(dz, at::kBFloat16, 16, "bias_grad", "dz");
   if (C % 8 == 0 && ld == C) b200::bias_grad(bfp(dz), f32p(db), rows, (int)C, (float)scale, cur_stream());
   else b200::bias_grad_ld(bfp(dz), f32p(db), rows, (int)C, (int)ld, (float)scale, cur_stream());
 }
@@ -129,6 +166,11 @@ static void fc_bias_act(at::Tensor acc, c10::optional<at::Tensor> bias, c10::opt
                         c10::optional<at::Tensor> y_f32, int64_t B, int64_t N, bool relu, double drop_p,
                         int64_t seed, int64_t offset, bool clear) {
   c10::cuda::CUDAGuard g(acc.device());
+  TORCH_CHECK(acc.is_contiguous() && acc.numel() >= B * N, "fc_bias_act: contiguous acc of B x N");
+  TORCH_CHECK(!bias.has_value() || bias->numel() >= N, "fc_bias_act: bias of N");
+  TORCH_CHECK(!y.has_value() || (y->is_contiguous() && y->numel() >= B * N), "fc_bias_act: contiguous y of B x N");
+  TORCH_CHECK(!y_f32.has_value() || (y_f32->is_contiguous() && y_f32->numel() >= B * N),
+              "fc_bias_act: contiguous y_f32 of B x N");
   b200::fc_bias_act(f32p(acc), f32p_opt(bias), y.has_value() ? bfp_mut(*y) : nullptr, f32p_opt(y_f32), (int)B,
                     (int)N, relu, (float)drop_p, (unsigned long long)seed, (unsigned long long)offset, clear,
                     cur_stream());
@@ -136,14 +178,24 @@ static void fc_bias_act(at::Tensor acc, c10::optional<at::Tensor> bias, c10::opt
 static void fc_grad_act(at::Tensor acc, c10::optional<at::Tensor> act, at::Tensor dz, int64_t B, int64_t N,
                         bool relu, double drop_p, bool clear) {
   c10::cuda::CUDAGuard g(acc.device());
+  // the dropout mask is read back from act > 0, which only a ReLU layer's output encodes
+  TORCH_CHECK(relu || drop_p == 0.0, "fc_grad_act: dropout without ReLU is not supported");
+  TORCH_CHECK(acc.is_contiguous() && acc.numel() >= B * N && dz.is_contiguous() && dz.numel() >= B * N,
+              "fc_grad_act: contiguous acc and dz of B x N");
+  TORCH_CHECK(!relu || (act.has_value() && act->is_contiguous() && act->numel() >= B * N),
+              "fc_grad_act: relu needs a contiguous act of B x N");
   b200::fc_grad_act(f32p(acc), bfp_opt(act), bfp_mut(dz), (int)B, (int)N, relu, (float)drop_p, 0, 0, clear, cur_stream());
 }
 static void cast_to_bf16(const at::Tensor& x, at::Tensor y) {
   c10::cuda::CUDAGuard g(x.device());
+  check_vec(x, at::kFloat, 16, "cast_to_bf16", "x");
+  check_vec(y, at::kBFloat16, 8, "cast_to_bf16", "y");
+  TORCH_CHECK(y.numel() == x.numel(), "cast_to_bf16: x and y differ in size");
   b200::cast_f32_to_bf16(f32p(x), bfp_mut(y), x.numel(), cur_stream());
 }
 static void cast_to_f32(const at::Tensor& x, at::Tensor y) {
   c10::cuda::CUDAGuard g(x.device());
+  TORCH_CHECK(x.is_contiguous() && y.is_contiguous() && y.numel() == x.numel(), "cast_to_f32: contiguous, same size");
   b200::cast_bf16_to_f32(bfp(x), f32p(y), x.numel(), cur_stream());
 }
 
@@ -162,6 +214,16 @@ static void adam(at::Tensor p, at::Tensor m, at::Tensor v, c10::optional<at::Ten
                  c10::optional<at::Tensor> g16, c10::optional<at::Tensor> shadow, double lr, double b1, double b2,
                  double eps, double wd, int64_t step, double grad_scale, c10::optional<at::Tensor> gzero) {
   c10::cuda::CUDAGuard g(p.device());
+  const int64_t n = p.numel();
+  for (auto* t : {&p, &m, &v}) check_vec(*t, at::kFloat, 16, "adam", "p, m and v");
+  if (g32.has_value()) check_vec(*g32, at::kFloat, 16, "adam", "g32");
+  if (gzero.has_value()) check_vec(*gzero, at::kFloat, 16, "adam", "gzero");
+  if (g16.has_value()) check_vec(*g16, at::kBFloat16, 8, "adam", "g16");
+  if (shadow.has_value()) check_vec(*shadow, at::kBFloat16, 8, "adam", "shadow");
+  TORCH_CHECK(g32.has_value() != g16.has_value(), "adam: exactly one of g32 and g16");
+  for (const auto* t : {&g32, &g16, &shadow, &gzero})
+    TORCH_CHECK(!t->has_value() || (*t)->numel() == n, "adam: every tensor has p's size");
+  TORCH_CHECK(m.numel() == n && v.numel() == n, "adam: every tensor has p's size");
   b200::adam_fused(f32p(p), f32p(m), f32p(v), f32p_opt(g32), bfp_opt(g16),
                    shadow.has_value() ? bfp_mut(*shadow) : nullptr, p.numel(), (float)lr, (float)b1, (float)b2,
                    (float)eps, (float)wd, (int)step, (float)grad_scale, false, f32p_opt(gzero), cur_stream());
@@ -170,6 +232,16 @@ static void sgd(at::Tensor p, at::Tensor mom, c10::optional<at::Tensor> g32, c10
                 c10::optional<at::Tensor> shadow, double lr, double momentum, double wd, bool first,
                 double grad_scale, c10::optional<at::Tensor> gzero) {
   c10::cuda::CUDAGuard g(p.device());
+  const int64_t n = p.numel();
+  for (auto* t : {&p, &mom}) check_vec(*t, at::kFloat, 16, "sgd", "p and mom");
+  if (g32.has_value()) check_vec(*g32, at::kFloat, 16, "sgd", "g32");
+  if (gzero.has_value()) check_vec(*gzero, at::kFloat, 16, "sgd", "gzero");
+  if (g16.has_value()) check_vec(*g16, at::kBFloat16, 8, "sgd", "g16");
+  if (shadow.has_value()) check_vec(*shadow, at::kBFloat16, 8, "sgd", "shadow");
+  TORCH_CHECK(g32.has_value() != g16.has_value(), "sgd: exactly one of g32 and g16");
+  for (const auto* t : {&g32, &g16, &shadow, &gzero})
+    TORCH_CHECK(!t->has_value() || (*t)->numel() == n, "sgd: every tensor has p's size");
+  TORCH_CHECK(mom.numel() == n, "sgd: every tensor has p's size");
   b200::sgd_fused(f32p(p), f32p(mom), f32p_opt(g32), bfp_opt(g16), shadow.has_value() ? bfp_mut(*shadow) : nullptr,
                   p.numel(), (float)lr, (float)momentum, (float)wd, first, (float)grad_scale, f32p_opt(gzero),
                   cur_stream());
@@ -192,6 +264,8 @@ static void im2col_c3(const at::Tensor& x, at::Tensor out, int64_t kpad) {
 static void nchw_to_nhwc(const at::Tensor& x, at::Tensor y) {
   c10::cuda::CUDAGuard g(x.device());
   TORCH_CHECK(x.is_contiguous() && x.dim() == 4, "nchw_to_nhwc: contiguous NCHW fp32");
+  TORCH_CHECK(y.is_contiguous() && y.dim() == 4 && y.size(3) >= x.size(1), "nchw_to_nhwc: contiguous NHWC y, cpad >= C");
+  check_nhwc(y, x.size(0), x.size(2), x.size(3), y.size(3), "nchw_to_nhwc", "y");
   b200::nchw_f32_to_nhwc_bf16(f32p(x), bfp_mut(y), x.size(0), x.size(1), x.size(2), x.size(3), y.size(3), cur_stream());
 }
 
@@ -371,6 +445,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(target.scalar_type() == at::kLong && logits.is_contiguous() && logits.size(0) == h.size(0) &&
                 logits.size(1) == W.size(0), "head_ce: int64 targets, logits [B][C]");
     TORCH_CHECK(dW.has_value() == db.has_value(), "head_ce: dW and db come together");
+    // dh keeps only the elements with h > 0: that is the dropout mask only after a ReLU
+    TORCH_CHECK(relu || drop_scale == 1.0, "head_ce: dropout without ReLU is not supported");
     b200::head_ce_fused(bfp(h), bfp(W), f32p(bias), reinterpret_cast<const long long*>(target.data_ptr()), f32p(logits),
                         dlogits.has_value() ? bfp_mut(*dlogits) : nullptr, (int)ldd, f32p_opt(dW), f32p_opt(db),
                         dh.has_value() ? bfp_mut(*dh) : nullptr, (float)drop_scale, relu, f32p_opt(meter),

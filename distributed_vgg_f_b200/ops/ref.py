@@ -274,3 +274,282 @@ def unpool2x2_64(dp: torch.Tensor, idx: torch.Tensor, pos: torch.Tensor):
     win.scatter_(-1, idx.to(torch.int64)[..., None], g[..., None])
     dz = win.view(N, OH, OW, C, 2, 2).permute(0, 1, 4, 2, 5, 3).reshape(N, 2 * OH, 2 * OW, C)
     return dz, g.sum((0, 1, 2)), g.abs().sum((0, 1, 2))
+
+
+# ----------------------------------------------------- float64 references of the memory-bound kernels
+# elementwise.cu and loss_optim.cu.  Where a kernel's fp32 arithmetic is at most one add and one
+# multiply of fp32 operands, the reference reproduces its rounding points (``_r32``): float64 holds
+# such a sum or product exactly (barring a 30-bit exponent gap in a sum), so rounding it once to fp32
+# gives the kernel's value and the tests compare bit for bit.
+
+def _r32(t: torch.Tensor) -> torch.Tensor:
+    """Round float64 values to fp32 and back: one fp32 operation's result."""
+    return t.to(torch.float32).to(torch.float64)
+
+
+def _f32(x: float) -> float:
+    """A Python scalar as the fp32 value the kernel receives."""
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def _first_max(win: torch.Tensor):
+    """(max, index of its first occurrence) over the last dimension."""
+    val = win.amax(-1)
+    pos = torch.arange(win.shape[-1], device=win.device)
+    idx = torch.where(win == val[..., None], pos, win.shape[-1]).amin(-1)
+    return val, idx
+
+
+def maxpool2x2_64(x: torch.Tensor):
+    """maxpool2x2_fwd on NHWC x: (pooled max [N,H/2,W/2,C], first maximum 0..3 in window order)."""
+    return _first_max(pool_windows(_f64(x)))
+
+
+def maxpool2x2_relu_bwd64(y: torch.Tensor, dp: torch.Tensor):
+    """Backward of [ReLU -> maxpool2x2] from the stored post-ReLU map y: dp goes to the first maximum
+    of each window whose maximum is > 0.  Returns (dz, column sum of dz, column sum of |dz|)."""
+    val, idx = maxpool2x2_64(y)
+    return unpool2x2_64(dp, idx, val > 0)
+
+
+def _ap_windows(n_in: int, n_out: int):
+    """torch's adaptive-pool windows: [floor(o*in/out), ceil((o+1)*in/out)) -- they overlap when in < out."""
+    return [((o * n_in) // n_out, -(-((o + 1) * n_in) // n_out)) for o in range(n_out)]
+
+
+def adaptive_avgpool64(x: torch.Tensor, OH: int, OW: int):
+    """adaptive_avgpool_fwd on NHWC x -> (mean of each window [N,OH,OW,C], mean of |x|)."""
+    N, H, W, C = x.shape
+    x64 = _f64(x)
+    ref = torch.zeros(N, OH, OW, C, dtype=torch.float64, device=x.device)
+    mag = torch.zeros_like(ref)
+    for oh, (h0, h1) in enumerate(_ap_windows(H, OH)):
+        for ow, (w0, w1) in enumerate(_ap_windows(W, OW)):
+            win = x64[:, h0:h1, w0:w1]
+            ref[:, oh, ow] = win.mean((1, 2))
+            mag[:, oh, ow] = win.abs().mean((1, 2))
+    return ref, mag
+
+
+def adaptive_avgpool_bwd64(dy: torch.Tensor, H: int, W: int):
+    """adaptive_avgpool_bwd: every input pixel gets dy / (window size) of each window it lies in."""
+    N, OH, OW, C = dy.shape
+    dy64 = _f64(dy)
+    ref = torch.zeros(N, H, W, C, dtype=torch.float64, device=dy.device)
+    mag = torch.zeros_like(ref)
+    for oh, (h0, h1) in enumerate(_ap_windows(H, OH)):
+        for ow, (w0, w1) in enumerate(_ap_windows(W, OW)):
+            g = dy64[:, oh, ow][:, None, None] / ((h1 - h0) * (w1 - w0))
+            ref[:, h0:h1, w0:w1] += g
+            mag[:, h0:h1, w0:w1] += g.abs()
+    return ref, mag
+
+
+def ap_max_window(n_in: int, n_out: int) -> int:
+    """Largest window of adaptive pooling along one dimension."""
+    return max(b - a for a, b in _ap_windows(n_in, n_out))
+
+
+def ap_max_cover(n_in: int, n_out: int) -> int:
+    """Most windows one input position lies in, along one dimension."""
+    return max(sum(a <= i < b for a, b in _ap_windows(n_in, n_out)) for i in range(n_in))
+
+
+def bias_grad64(dz: torch.Tensor, C: int, scale: float = 1.0, rows=None):
+    """bias_grad / bias_grad_ld: scale * sum over rows of dz[:rows, :C] for a row stride ld >= C."""
+    d = _f64(dz.reshape(dz.shape[0], -1)[:rows, :C])
+    return scale * d.sum(0), abs(scale) * d.abs().sum(0)
+
+
+# ---- Philox4x32-10 (Random123), vectorised over int64 tensors holding 32-bit words
+_PHILOX_M = (0xD2511F53, 0xCD9E8D57)
+_PHILOX_W = (0x9E3779B9, 0xBB67AE85)
+_MASK32 = 0xFFFFFFFF
+
+
+def _mulhilo(a: int, b: torch.Tensor):
+    # 32 x 32 -> 64-bit product in int64 without overflow: split b into 16-bit halves
+    lo16, hi16 = b & 0xFFFF, b >> 16
+    p_lo = a * lo16                                   # < 2^48
+    p_hi = a * hi16                                   # < 2^48
+    lo = (p_lo + ((p_hi & 0xFFFF) << 16)) & _MASK32
+    hi = ((p_hi + (p_lo >> 16)) >> 16) & _MASK32
+    return hi, lo
+
+
+def philox4x32_10(key, ctr):
+    """Philox4x32-10 of 32-bit words (Python ints or int64 tensors): key (k0, k1), counter (c0..c3)
+    -> the four output words, as int64 tensors."""
+    k0, k1 = (torch.as_tensor(k, dtype=torch.int64) for k in key)
+    c0, c1, c2, c3 = (torch.as_tensor(c, dtype=torch.int64) for c in ctr)
+    for _ in range(10):
+        hi0, lo0 = _mulhilo(_PHILOX_M[0], c0)
+        hi1, lo1 = _mulhilo(_PHILOX_M[1], c2)
+        c0, c1, c2, c3 = hi1 ^ c1 ^ k0, lo1, hi0 ^ c3 ^ k1, lo0
+        k0, k1 = (k0 + _PHILOX_W[0]) & _MASK32, (k1 + _PHILOX_W[1]) & _MASK32
+    return c0, c1, c2, c3
+
+
+def dropout_mask64(seed: int, offset: int, B: int, N: int, p: float, device=None):
+    """The dropout of fc_bias_act: (keep [B][N] bool, keep_scale).  Word j of Philox quad q, keyed by
+    (seed lo, seed hi) with counter (q lo, q hi, offset lo, offset hi), decides element 4q + j of the
+    flattened [B][N]: u = (word >> 8) * 2^-24 and the element is dropped iff u < fp32(p).
+    keep_scale = fp32(1 / (1 - fp32(p)))."""
+    total = B * N
+    q = torch.arange((total + 3) // 4, dtype=torch.int64, device=device)
+    words = philox4x32_10((seed & _MASK32, (seed >> 32) & _MASK32),
+                          (q & _MASK32, q >> 32, offset & _MASK32, (offset >> 32) & _MASK32))
+    r = torch.stack(words, dim=1).reshape(-1)[:total]
+    u = (r >> 8).to(torch.float64) * 2.0 ** -24
+    p32 = torch.tensor(p, dtype=torch.float32)
+    one = torch.tensor(1.0, dtype=torch.float32)
+    keep_scale = float(one / (one - p32)) if p > 0 else 1.0
+    keep = ~(u < float(p32)) if p > 0 else torch.ones_like(u, dtype=torch.bool)
+    return keep.view(B, N), keep_scale
+
+
+def fc_bias_act64(acc: torch.Tensor, bias, *, relu: bool, drop_p: float = 0.0, seed: int = 0, offset: int = 0):
+    """fc_bias_act on fp32 acc [B][N]: dropout(relu(acc + bias)) with the kernel's rounding points
+    (fp32 add, fp32 multiply by keep_scale).  Returns (y [B][N], mag)."""
+    B, N = acc.shape
+    a = _f64(acc)
+    b = _f64(bias).view(1, N) if bias is not None else torch.zeros(1, N, dtype=torch.float64, device=acc.device)
+    v = _r32(a + b)
+    mag = a.abs() + b.abs()
+    if relu:
+        v = torch.relu(v)
+    if drop_p > 0:
+        keep, ks = dropout_mask64(seed, offset, B, N, drop_p, device=acc.device)
+        v = torch.where(keep, _r32(v * ks), torch.zeros_like(v))
+        mag = mag * keep * ks
+    return v, mag
+
+
+def fc_grad_act64(acc: torch.Tensor, act, *, relu: bool, drop_p: float = 0.0):
+    """fc_grad_act: dz = acc * [act > 0] * fp32(1 / (1 - p)), or acc unchanged without ReLU."""
+    a = _f64(acc)
+    if not relu:
+        return a, a.abs()
+    ks = dropout_mask64(0, 0, 1, 1, drop_p)[1]
+    v = torch.where(act.to(torch.float64) > 0, _r32(a * ks), torch.zeros_like(a))
+    return v, v.abs()
+
+
+def _first_argmax(z: torch.Tensor) -> torch.Tensor:
+    return _first_max(z)[1]
+
+
+def cross_entropy64(logits: torch.Tensor, target: torch.Tensor, *, ldd: int = 0, class_weights=None,
+                    grad_scale=None):
+    """cross_entropy on fp32 logits [B][C] -> dict with
+    loss: mean nll, or sum_i w_i nll_i / sum_i w_i with class weights;
+    dlogits [B][ldd]: (softmax - onehot) * w_i / sum w (or * grad_scale, default 1/B), columns >= C zero;
+    meter: (loss * B, count of first-maximum argmax == target, B)."""
+    z = _f64(logits)
+    B, C = z.shape
+    t = target.to(torch.int64).view(-1)
+    lse = torch.logsumexp(z, dim=1)
+    nll = lse - z.gather(1, t.view(-1, 1)).view(-1)
+    if class_weights is not None:
+        w = _f64(class_weights)[t]
+        norm = 1.0 / w.sum()
+        loss = (w * nll).sum() * norm
+    else:
+        w = torch.ones(B, dtype=torch.float64, device=z.device)
+        norm = _f32(1.0 / B if grad_scale is None else grad_scale)
+        loss = nll.mean()
+    dl = torch.zeros(B, max(ldd, C), dtype=torch.float64, device=z.device)
+    dl[:, :C] = (torch.softmax(z, 1) - torch.nn.functional.one_hot(t, C).to(torch.float64)) * (w * norm)[:, None]
+    correct = float((_first_argmax(z) == t).sum())
+    meter = torch.tensor([float(loss) * B, correct, float(B)], dtype=torch.float64)
+    return {"loss": loss, "dlogits": dl, "meter": meter}
+
+
+def head_ce64(h: torch.Tensor, W: torch.Tensor, bias: torch.Tensor, *, dl_used: torch.Tensor,
+              drop_scale: float = 1.0, relu: bool = True):
+    """head_ce's GEMM parts, each (ref, mag).  logits = h W^T + bias; the backward takes the dlogits
+    the kernel rounded to bf16 (dl_used [B][C]), because that rounding point is part of the kernel:
+    dW = dl^T h, db = sum_r dl, dh = (dl W) * [h > 0 if relu] * drop_scale.  The loss and dlogits are
+    cross_entropy64 of the logits."""
+    h64, W64, b64, dl = _f64(h), _f64(W), _f64(bias), _f64(dl_used)
+    out = {"logits": (h64 @ W64.t() + b64, h64.abs() @ W64.abs().t() + b64.abs()),
+           "dW": (dl.t() @ h64, dl.abs().t() @ h64.abs()),
+           "db": (dl.sum(0), dl.abs().sum(0))}
+    keep = (h64 > 0).to(torch.float64) if relu else torch.ones_like(h64)
+    out["dh"] = ((dl @ W64) * keep * drop_scale, (dl.abs() @ W64.abs()) * keep * abs(drop_scale))
+    return out
+
+
+_U = 2.0 ** -24
+
+
+def _sqrt_err(s, e_v):
+    # |sqrt(a) - sqrt(b)| <= min(|a - b| / (2 sqrt(a)), sqrt(|a - b|))
+    return torch.minimum(e_v / (2 * s).clamp_min(1e-300), e_v.sqrt())
+
+
+def adam_step64(p, m, v, g, *, lr: float, beta1: float, beta2: float, eps: float, weight_decay: float,
+                step: int, grad_scale: float = 1.0):
+    """One step of adam_kernel (torch.optim.Adam with L2 weight decay, bias correction of step ``step``,
+    the gradient scaled by grad_scale) from the given state.  Hyperparameters are taken as given: pass
+    their fp32 values to compare with the kernel.  Returns {"p", "m", "v": (ref, err)}: err is a
+    first-order running bound, in absolute units, of what the kernel's fp32 operations may add to
+    each result (u per operation, the inputs taken as exact, the fp32 rounding of the bias
+    corrections included)."""
+    u = _U
+    p, m, v, g = _f64(p), _f64(m), _f64(v), _f64(g)
+    b1, b2 = beta1, beta2
+    bc1i, bc2i = 1.0 / (1.0 - b1 ** step), 1.0 / (1.0 - b2 ** step) ** 0.5
+    gs, wdp = g * grad_scale, weight_decay * p
+    gk = gs + wdp
+    e_gk = u * (gs.abs() + wdp.abs() + gk.abs())
+    m1 = b1 * m + (1 - b1) * gk
+    e_m = u * (b1 * m.abs() + m1.abs()) + (1 - b1) * (e_gk + u * gk.abs())
+    t = (1 - b2) * gk
+    e_t = (1 - b2) * e_gk + u * t.abs()
+    t2 = t * gk
+    e_t2 = gk.abs() * e_t + t.abs() * e_gk + u * t2.abs()
+    v1 = b2 * v + t2
+    e_v = u * (b2 * v.abs() + v1.abs()) + e_t2
+    s = v1.sqrt()
+    e_s = _sqrt_err(s, e_v) + u * s
+    d = s * bc2i + eps
+    e_d = bc2i * e_s + 3 * u * s * bc2i + u * d
+    a = lr * bc1i
+    num = a * m1
+    e_num = a * e_m + 3 * u * num.abs()
+    q = num / d
+    e_q = e_num / d + num.abs() * e_d / d ** 2 + u * q.abs()
+    p1 = p - q
+    e_p = e_q + u * p1.abs()
+    return {"p": (p1, e_p), "m": (m1, e_m), "v": (v1, e_v)}
+
+
+def sgd_step64(p, buf, g, *, lr: float, momentum: float, weight_decay: float, first: bool,
+               grad_scale: float = 1.0):
+    """One step of sgd_kernel (torch.optim.SGD with momentum, no dampening, L2 weight decay):
+    d = g * grad_scale + wd * p; buf = d on the first step, else momentum * buf + d; p -= lr * buf.
+    Returns {"p", "buf": (ref, err)} like adam_step64."""
+    u = _U
+    p, buf, g = _f64(p), _f64(buf), _f64(g)
+    gs, wdp = g * grad_scale, weight_decay * p
+    gk = gs + wdp
+    e_gk = u * (gs.abs() + wdp.abs() + gk.abs())
+    if first:
+        b1, e_b = gk, e_gk
+    else:
+        mb = momentum * buf
+        b1 = mb + gk
+        e_b = u * (mb.abs() + b1.abs()) + e_gk
+    q = lr * b1
+    p1 = p - q
+    e_p = lr * e_b + u * (q.abs() + p1.abs())
+    return {"p": (p1, e_p), "buf": (b1, e_b)}
+
+
+def nchw_to_nhwc64(x: torch.Tensor, cpad: int):
+    """nchw_to_nhwc: fp32 NCHW -> NHWC with channels zero-padded to cpad (the kernel rounds to bf16)."""
+    N, C, H, W = x.shape
+    y = torch.zeros(N, H, W, cpad, dtype=torch.float64, device=x.device)
+    y[..., :C] = _f64(x).permute(0, 2, 3, 1)
+    return y, y.abs()

@@ -29,6 +29,10 @@ EPS_BF16 = 2.0 ** -8        # unit roundoff of bf16
 # precision.  Worst err/bound of the gauss-mode tests on one H100 80GB HBM3 (700 W limit), fp32
 # outputs: GEMM 0.11, conv wgrad 0.014, conv0 wgrad 0.007, column sums <= 0.002 -- below 1 / SAFETY.
 # bf16 outputs reach 0.99 because their own rounding may use the whole 2^-8 |ref| term.
+# Memory-bound kernels (test_elementwise_gpu.py and the replay, H100 80GB HBM3 at a 400 W limit),
+# fp32 outputs: Adam p 0.25, m 0.19, v 0.17; SGD p 0.25, momentum 0.24; bias_grad 0.12; head_ce db 0.12,
+# dW 0.02, logits 0.04, loss 0.02; cross_entropy loss 0.04; max-pool column sum 6e-5.  The optimizer
+# bounds are running bounds without slack of their own, so their worst case sits at 1 / SAFETY.
 SAFETY = 4.0
 EXACT_DEPTH = 4608          # deepest reduction that gets |v| <= 4 operands (|sum| <= 16 * 4608 < 2^24)
 
@@ -55,8 +59,10 @@ def bias(n: int, mode: str, gen: torch.Generator, device) -> torch.Tensor:
 
 
 def check(got: torch.Tensor, ref: torch.Tensor, mag: torch.Tensor, *, chain: float, exact: bool,
-          family: str = "", what: str = "") -> float:
-    """Assert the criterion on every element; returns the worst err/bound ratio (0 in exact mode)."""
+          family: str = "", what: str = "", err=None) -> float:
+    """Assert the criterion on every element; returns the worst err/bound ratio (0 in exact mode).
+    ``err`` (optional, absolute units) is a derived error bound of arithmetic that is not a chain of
+    additions (ce_bound, the optimizer references); it is added to the bound times SAFETY."""
     assert got.shape == ref.shape == mag.shape, (what, tuple(got.shape), tuple(ref.shape), tuple(mag.shape))
     bf = got.dtype == torch.bfloat16
     g = got.to(torch.float64)
@@ -71,8 +77,10 @@ def check(got: torch.Tensor, ref: torch.Tensor, mag: torch.Tensor, *, chain: flo
                                  "expected %r" % (family, what, n, got.numel(), idx, float(g.flatten()[i]),
                                                   float(want.flatten()[i])))
         return 0.0
-    err = (g - ref).abs()
     bound = (EPS_BF16 if bf else 0.0) * ref.abs() + gamma(chain) * mag
+    if err is not None:
+        bound = bound + SAFETY * err
+    err = (g - ref).abs()
     ratio = torch.where(err == 0, torch.zeros_like(err), err / bound).nan_to_num(float("inf"))
     i = int(ratio.argmax())
     worst = float(ratio.flatten()[i])
@@ -198,3 +206,105 @@ def sm_count() -> int:
 def generator(seed: int, device) -> torch.Generator:
     return torch.Generator(device=device).manual_seed(seed)
 
+
+
+# ------------------------------------------------- chains and bounds of the memory-bound kernels
+def avgpool_chain(terms: int) -> int:
+    """adaptive_avgpool_fwd / _bwd: ``terms`` is the most window elements one output sums (forward:
+    ops.ref.ap_max_window squared) or the most windows one input lies in (backward: ap_max_cover
+    squared).  Each term costs at most an fp32 1/count, a product and an add."""
+    return 3 * terms
+
+
+def bias_grad_chain(rows: int, C: int, sms: int, ld: int = None) -> int:
+    """bias_grad with the launch geometry of elementwise.cu::bias_grad(): CG column groups of 8
+    channels (<= 256) x RL = 256 / CG row lanes; blocks of RL * 16 rows, capped at 8 blocks per SM per
+    column-group slice; each lane adds every RL-th row of its block's rows_per_block, lane 0 adds the
+    other RL - 1 lanes, multiplies by scale, and each block adds its sum atomically.  C % 8 != 0 or
+    ld != C takes bias_grad_ld: one thread adds all rows."""
+    if C % 8 or (ld is not None and ld != C):
+        return rows + 2
+    c8 = C // 8
+    CG = min(c8, 256)
+    RL = max(256 // CG, 1)
+    nblk = _cdiv(rows, RL * 16)
+    nblk = max(min(nblk, sms * 8 // _cdiv(c8, CG)), 1)
+    rpb = _cdiv(rows, nblk)
+    return _cdiv(rpb, RL) + RL + 1 + _cdiv(rows, rpb)
+
+
+def head_chain(K: int, B: int) -> dict:
+    """head_ce: logits = fmas over one lane's K / 32 inputs, 5 shuffle adds and the bias; dW[c][k] and
+    db[c] are serial sums over the B rows (db added to the buffer's value); dh = at most 8 fmas over the
+    classes, times drop_scale."""
+    return {"logits": _cdiv(K, 32) + 6, "dW": B, "db": B + 1, "dh": 9}
+
+
+# CUDA C++ Programming Guide, table of intrinsic functions (single precision):
+#   __expf(x): at most 2 + floor(|1.173 x|) ulp;
+#   __logf(x): at most 2^-21.41 absolute for x in [0.5, 2], else 3 ulp.
+# One ulp of a normal fp32 value y is at most 2^-23 |y|.
+def _expf_rel(x: torch.Tensor) -> torch.Tensor:
+    return (2 + torch.floor((1.173 * x).abs())) * 2.0 ** -23
+
+
+def _logf_abs(s: torch.Tensor) -> torch.Tensor:
+    L = s.log()
+    inner = (s >= 0.5) & (s <= 2.0)
+    return torch.where(inner, torch.full_like(s, 2.0 ** -21.41), 3 * 2.0 ** -23 * L.abs())
+
+
+def ce_bound(logits: torch.Tensor, target: torch.Tensor, *, class_weights=None, grad_scale=None,
+             se_chain: int, warps: int) -> dict:
+    """First-order bound of what cross_entropy_kernel / head_ce_kernel may get wrong, per output, in
+    absolute units, for the fp32 logits z the kernel saw (u = 2^-24 per fp32 operation):
+
+      x_c = z_c - max            rounded:          |dx_c| <= u |x_c|
+      e_c = __expf(x_c)          relative error    r(x_c) = (2 + floor|1.173 x_c|) 2^-23, plus |dx_c|
+      se  = sum_c e_c            se_chain adds of positive terms (lanes, then 5 shuffles, or serial)
+                                 |dse| <= sum_c e_c (r(x_c) + u|x_c|) + se_chain u se
+      lse = max + __logf(se)     |dlse| <= |dse| / se + logf_abs(se) + u |lse|
+      nll = w (lse - z_t)        |dnll| <= w (|dlse| + 2u |lse - z_t|)
+      loss = sum nll / D         rows / warps per warp, then the warps: |dsum| <= sum|dnll| + chain u sum|nll|;
+                                 D = B exact, or sum w with its own chain; one division
+      a_c = z_c - lse            |da_c| <= |dlse| + u |a_c|
+      g_c = (__expf(a_c) - [c == t]) w norm
+                                 |dg_c| <= w norm (p_c (|da_c| + r(a_c)) + u |p_c - [c == t]|) + 3u |g_c| + |g_c| dnorm
+    The bf16 rounding of dlogits is check()'s own 2^-8 |ref| term; results below 2^-126 may be flushed
+    to zero, hence an absolute 2^-126 more.  Returns {"loss", "dlogits" [B][C],
+    "meter0"}."""
+    u = U32
+    z = logits.to(torch.float64)
+    B, C = z.shape
+    t = target.to(torch.int64).view(-1)
+    mx = z.amax(1, keepdim=True)
+    x = z - mx
+    e = x.exp()
+    se = e.sum(1)
+    dse = (e * (_expf_rel(x) + u * x.abs())).sum(1) + se_chain * u * se
+    L = se.log()
+    lse = mx.view(-1) + L
+    dlse = dse / se + _logf_abs(se) + u * lse.abs()
+    if class_weights is not None:
+        w = class_weights.to(torch.float64)[t]
+        D = w.sum()
+        dD = (_cdiv(B, 1024) + 5 + warps) * u * D
+        norm, dnorm = 1.0 / D, dD / D + u
+    else:
+        w = torch.ones(B, dtype=torch.float64, device=z.device)
+        D, dD = float(B), 0.0
+        norm, dnorm = (1.0 / B if grad_scale is None else grad_scale), 0.0
+    zt = z.gather(1, t.view(-1, 1)).view(-1)
+    nll = w * (lse - zt)
+    dnll = w * (dlse + 2 * u * (lse - zt).abs())
+    tl = nll.sum()
+    dtl = dnll.sum() + (_cdiv(B, warps) + warps) * u * nll.abs().sum()
+    loss = tl / D
+    dloss = dtl / D + tl.abs() * dD / D ** 2 + u * loss.abs()
+    a = z - lse[:, None]
+    p = a.exp()
+    onehot = torch.nn.functional.one_hot(t, C).to(torch.float64)
+    g = (p - onehot) * (w * norm)[:, None]
+    dg = (w * norm)[:, None] * (p * (dlse[:, None] + u * a.abs() + _expf_rel(a)) + u * (p - onehot).abs()) \
+        + g.abs() * (3 * u + dnorm) + (w * norm)[:, None] * 2.0 ** -126 + 2.0 ** -126
+    return {"loss": dloss, "dlogits": dg, "meter0": B * dloss + u * B * loss.abs()}

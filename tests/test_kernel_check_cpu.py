@@ -273,3 +273,328 @@ def test_exact_mode_sums_are_fp32_integers():
     assert set(a.float().unique().tolist()) <= {-1.0, 0.0, 1.0}
     a = KC.operand((4, 4608), "exact", 4608, g, CPU)
     assert float(a.float().abs().max()) <= 4
+
+
+# ========================================================= memory-bound kernels: references vs torch
+def test_philox_known_answers():
+    """Random123's known-answer vectors of Philox4x32-10."""
+    kat = [((0, 0), (0, 0, 0, 0), (0x6627e8d5, 0xe169c58d, 0xbc57ac4c, 0x9b00dbd8)),
+           ((0xffffffff, 0xffffffff), (0xffffffff,) * 4, (0x408f276d, 0x41c83b0e, 0xa20bc7c6, 0x6d5451fd)),
+           ((0xa4093822, 0x299f31d0), (0x243f6a88, 0x85a308d3, 0x13198a2e, 0x03707344),
+            (0xd16cfe09, 0x94fdcceb, 0x5001e420, 0x24126ea1))]
+    for key, ctr, want in kat:
+        got = tuple(int(w) for w in R.philox4x32_10(key, ctr))
+        assert got == want, [hex(v) for v in got]
+
+
+def test_dropout_mask_layout():
+    """Element 4q + j of the flattened [B][N] uses word j of quad q, counter (q, offset); fp32 p."""
+    seed, offset, B, N, p = (1 << 33) + 12345, (1 << 32) + 1, 3, 10, 0.6
+    keep, ks = R.dropout_mask64(seed, offset, B, N, p)
+    for i in (0, 5, 7, 29):
+        q, j = divmod(i, 4)
+        w = R.philox4x32_10((seed & 0xFFFFFFFF, seed >> 32), (q, 0, offset & 0xFFFFFFFF, offset >> 32))[j]
+        u = (int(w) >> 8) / 2 ** 24
+        assert bool(keep.view(-1)[i]) == (not u < float(torch.tensor(p, dtype=torch.float32)))
+    assert ks == float(torch.tensor(1.0) / (torch.tensor(1.0) - torch.tensor(0.6)))
+    assert ks != 2.5                                      # fp32 1 / (1 - 0.6f) is 2.5000002
+    big, _ = R.dropout_mask64(seed, offset, 64, N, p)
+    assert torch.equal(big[:B], keep)                     # a row's mask does not depend on the batch size
+    frac = 1 - float(R.dropout_mask64(7, 1, 64, 4096, 0.5)[0].float().mean())
+    assert 0.49 < frac < 0.51
+
+
+def test_maxpool_references_match_torch():
+    g = _gen(20)
+    y = torch.relu(torch.randint(-2, 3, (2, 6, 8, 16), generator=g).to(F64))      # ties and all-zero windows
+    val, idx = R.maxpool2x2_64(y)
+    p, ind = F.max_pool2d(_nchw(y), 2, 2, return_indices=True)
+    torch.testing.assert_close(val, _nhwc(p))
+    W = y.shape[2]
+    assert torch.equal(idx, _nhwc((ind // W % 2) * 2 + ind % W % 2))
+    dp = torch.randn(val.shape, generator=g, dtype=F64)
+    dz, cs, csmag = R.maxpool2x2_relu_bwd64(y, dp)
+    yr = _nchw(y).clone().requires_grad_(True)
+    F.max_pool2d(yr, 2, 2).backward(_nchw(dp))
+    want = _nhwc(yr.grad * (yr > 0))
+    torch.testing.assert_close(dz, want)
+    torch.testing.assert_close(cs, want.sum((0, 1, 2)))
+    torch.testing.assert_close(csmag, want.abs().sum((0, 1, 2)))
+
+
+@pytest.mark.parametrize("H", [2, 4, 5, 7, 10, 14])
+def test_avgpool_references_match_torch(H):
+    g = _gen(21)
+    x = torch.randn(2, H, H + 1, 8, generator=g, dtype=F64)
+    ref, mag = R.adaptive_avgpool64(x, 7, 7)
+    xr = _nchw(x).clone().requires_grad_(True)
+    y = F.adaptive_avg_pool2d(xr, (7, 7))
+    torch.testing.assert_close(ref, _nhwc(y.detach()))
+    torch.testing.assert_close(mag, _nhwc(F.adaptive_avg_pool2d(_nchw(x).abs(), (7, 7))))
+    dy = torch.randn(ref.shape, generator=g, dtype=F64)
+    y.backward(_nchw(dy))
+    dx, _ = R.adaptive_avgpool_bwd64(dy, H, H + 1)
+    torch.testing.assert_close(dx, _nhwc(xr.grad))
+
+
+@pytest.mark.parametrize("weighted", [False, True])
+def test_cross_entropy_reference_matches_torch(weighted):
+    g = _gen(22)
+    B, C = 9, 5
+    z = torch.randn(B, C, generator=g, dtype=F64) * 3
+    z[0, 1] = z[0, 3] = z[0].max() + 1                      # a tie for the argmax: the lower index wins
+    t = torch.randint(0, C, (B,), generator=g)
+    t[0] = 1
+    w = torch.rand(C, generator=g, dtype=F64) + 0.1 if weighted else None
+    out = R.cross_entropy64(z, t, ldd=8, class_weights=w, grad_scale=0.125 if not weighted else None)
+    zr = z.clone().requires_grad_(True)
+    loss = F.cross_entropy(zr, t, weight=w)
+    loss.backward()
+    torch.testing.assert_close(out["loss"], loss.detach())
+    scale = 1.0 if weighted else 0.125 * B                  # torch's gradient is that of the mean: 1/B
+    torch.testing.assert_close(out["dlogits"][:, :C], zr.grad * scale)
+    assert torch.count_nonzero(out["dlogits"][:, C:]) == 0
+    assert float(out["meter"][1]) == float((torch.argmax(z, 1) == t).sum()) and float(out["meter"][2]) == B
+    assert float(out["meter"][1]) >= 1                       # row 0's tie counted as correct
+
+
+def test_optimizer_references_match_torch():
+    g = _gen(23)
+    n = 64
+    p0 = torch.randn(n, generator=g, dtype=F64)
+    hp = dict(lr=1e-2, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.05)
+    pr = p0.clone().requires_grad_(True)
+    opt = torch.optim.Adam([pr], lr=hp["lr"], betas=(hp["beta1"], hp["beta2"]), eps=hp["eps"],
+                           weight_decay=hp["weight_decay"])
+    p, m, v = p0.clone(), torch.zeros(n, dtype=F64), torch.zeros(n, dtype=F64)
+    for step in range(1, 5):
+        gr = torch.randn(n, generator=g, dtype=F64)
+        out = R.adam_step64(p, m, v, gr * 8, step=step, grad_scale=0.125, **hp)
+        p, m, v = out["p"][0], out["m"][0], out["v"][0]
+        pr.grad = gr.clone()
+        opt.step()
+        torch.testing.assert_close(p, pr.detach(), rtol=1e-12, atol=1e-12)
+        torch.testing.assert_close(m, opt.state[pr]["exp_avg"], rtol=1e-12, atol=1e-12)
+        torch.testing.assert_close(v, opt.state[pr]["exp_avg_sq"], rtol=1e-12, atol=1e-12)
+    for momentum in (0.9, 0.0):
+        pr = p0.clone().requires_grad_(True)
+        opt = torch.optim.SGD([pr], lr=0.1, momentum=momentum, weight_decay=0.01)
+        p, buf = p0.clone(), torch.zeros(n, dtype=F64)
+        for step in range(3):
+            gr = torch.randn(n, generator=g, dtype=F64)
+            out = R.sgd_step64(p, buf, gr, lr=0.1, momentum=momentum, weight_decay=0.01, first=step == 0)
+            p, buf = out["p"][0], out["buf"][0]
+            pr.grad = gr.clone()
+            opt.step()
+            torch.testing.assert_close(p, pr.detach(), rtol=1e-12, atol=1e-12)
+
+
+def test_nchw_to_nhwc_reference():
+    x = torch.randn(2, 3, 4, 5, generator=_gen(24))
+    y, _ = R.nchw_to_nhwc64(x, 8)
+    torch.testing.assert_close(y[..., :3], x.to(F64).permute(0, 2, 3, 1))
+    assert torch.count_nonzero(y[..., 3:]) == 0
+
+
+# ============================================= memory-bound kernels: emulations and planted defects
+def _emu_pool_bwd(y, dp, last=False):
+    """maxpool2x2_relu_bwd: first (or, planted, last) maximum of each window gets dp where max > 0."""
+    win = R.pool_windows(y.float())
+    val = win.amax(-1)
+    idx = 3 - win.flip(-1).argmax(-1) if last else R._first_max(win)[1]
+    dz, _, _ = R.unpool2x2_64(dp, idx, val > 0)
+    return dz.to(torch.bfloat16)
+
+
+def test_pool_bwd_criterion_catches_last_maximum_ties():
+    g = _gen(30)
+    y = torch.relu(torch.randint(-2, 3, (2, 8, 8, 16), generator=g)).to(torch.bfloat16)
+    dp = KC.operand((2, 4, 4, 16), "exact", 1, g, CPU)
+    ref, _, _ = R.maxpool2x2_relu_bwd64(y, dp)
+    KC.check(_emu_pool_bwd(y, dp), ref, ref.abs(), chain=0, exact=True)
+    _rejects(lambda: KC.check(_emu_pool_bwd(y, dp, last=True), ref, ref.abs(), chain=0, exact=True))
+
+
+def _emu_avgpool(x, OH, floor_end=False):
+    N, H, W, C = x.shape
+    out = torch.zeros(N, OH, OH, C)
+    for oh in range(OH):
+        h0, h1 = oh * H // OH, ((oh + 1) * H if floor_end else (oh + 1) * H + OH - 1) // OH
+        for ow in range(OH):
+            w0, w1 = ow * W // OH, ((ow + 1) * W if floor_end else (ow + 1) * W + OH - 1) // OH
+            acc = torch.zeros(N, C)
+            for h in range(h0, h1):
+                for w in range(w0, w1):
+                    acc += x[:, h, w].float()
+            out[:, oh, ow] = acc * (1.0 / float(max((h1 - h0) * (w1 - w0), 1)))
+    return out.to(torch.bfloat16)
+
+
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("H", [5, 10])
+def test_avgpool_criterion_catches_ap_end_without_ceiling(mode, H):
+    g = _gen(31)
+    x = KC.operand((2, H, H, 8), mode, 9, g, CPU)
+    ref, mag = R.adaptive_avgpool64(x, 7, 7)
+    chain = KC.avgpool_chain(R.ap_max_window(H, 7) ** 2)
+    exact = mode == "exact" and H == 5                 # window sizes 1, 2, 4: powers of two
+    KC.check(_emu_avgpool(x, 7), ref, mag, chain=chain, exact=exact)
+    _rejects(lambda: KC.check(_emu_avgpool(x, 7, floor_end=True), ref, mag, chain=chain, exact=exact))
+
+
+def _emu_bias_grad(dz, C, scale, sms, drop_block=None):
+    """bias_grad's block split (elementwise.cu): blocks of rows_per_block rows summed in fp32,
+    added atomically; optionally one block left out."""
+    rows = dz.shape[0]
+    c8 = C // 8
+    CG = min(c8, 256)
+    RL = max(256 // CG, 1)
+    nblk = max(min(-(-rows // (RL * 16)), sms * 8 // -(-c8 // CG)), 1)
+    rpb = -(-rows // nblk)
+    db = torch.zeros(C)
+    for b, r0 in enumerate(range(0, rows, rpb)):
+        if b != drop_block:
+            db += dz[r0:r0 + rpb, :C].float().sum(0) * scale
+    return db
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_bias_grad_criterion_catches_a_dropped_row_block(mode):
+    g = _gen(32)
+    rows, C, sms = 20000, 64, 132
+    dz = KC.operand((rows, C), mode, rows, g, CPU)
+    ref, mag = R.bias_grad64(dz, C, 0.5)
+    chain = KC.bias_grad_chain(rows, C, sms)
+    exact = mode == "exact"
+    KC.check(_emu_bias_grad(dz, C, 0.5, sms), ref, mag, chain=chain, exact=exact)
+    _rejects(lambda: KC.check(_emu_bias_grad(dz, C, 0.5, sms, drop_block=3), ref, mag, chain=chain, exact=exact))
+
+
+def _emu_fc_bias_act(acc, bias, p, seed, offset, counter="quad", scale=None):
+    """fc_bias_act in fp32 with a Philox mask; planted: the counter from the element index."""
+    B, N = acc.shape
+    v = torch.relu(acc + bias)
+    if counter == "quad":
+        keep, ks = R.dropout_mask64(seed, offset, B, N, p)
+    else:
+        i = torch.arange(B * N, dtype=torch.int64)
+        r = R.philox4x32_10((seed & 0xFFFFFFFF, seed >> 32), (i, i >> 32, offset, 0))[0]
+        keep = ~((r >> 8).to(F64) * 2 ** -24 < float(torch.tensor(p, dtype=torch.float32))).view(B, N)
+        ks = R.dropout_mask64(seed, offset, 1, 1, p)[1]
+    ks = torch.tensor(ks if scale is None else scale, dtype=torch.float32)
+    return torch.where(keep, v * ks, torch.zeros_like(v))
+
+
+@pytest.mark.parametrize("mode", MODES)
+def test_dropout_criterion_catches_mask_and_scale_defects(mode):
+    g = _gen(33)
+    B, N, p, seed = 37, 100, 0.6, 1000003 * 5 + 2
+    acc = KC.operand((B, N), mode, 1, g, CPU).float()
+    bias = KC.bias(N, mode, g, CPU)
+    ref, mag = R.fc_bias_act64(acc, bias, relu=True, drop_p=p, seed=seed, offset=7)
+    good = _emu_fc_bias_act(acc, bias, p, seed, 7)
+    KC.check(good, ref, mag, chain=0, exact=True)
+    KC.check(good.to(torch.bfloat16), ref, mag, chain=0, exact=True)
+    _rejects(lambda: KC.check(_emu_fc_bias_act(acc, bias, p, seed, 7, counter="element"), ref, mag, chain=0,
+                              exact=True))
+    _rejects(lambda: KC.check(_emu_fc_bias_act(acc, bias, p, seed, 6), ref, mag, chain=0, exact=True))
+    _rejects(lambda: KC.check(_emu_fc_bias_act(acc, bias, p, seed, 7, scale=2.5), ref, mag, chain=0, exact=True))
+
+
+def _emu_ce(z, t, ldd, w=None, pad=0.0, high_ties=False):
+    """cross_entropy_kernel in fp32 torch ops: (loss, dlogits [B][ldd] bf16, correct count)."""
+    B, C = z.shape
+    mx = z.amax(1, keepdim=True)
+    lse = mx + (z - mx).exp().sum(1, keepdim=True).log()
+    wt = w[t] if w is not None else torch.ones(B)
+    norm = 1.0 / wt.sum() if w is not None else torch.tensor(1.0 / B)
+    dl = torch.full((B, ldd), pad)
+    dl[:, :C] = ((z - lse).exp() - F.one_hot(t, C).float()) * wt[:, None] * norm
+    nll = wt * (lse.view(-1) - z.gather(1, t.view(-1, 1)).view(-1))
+    loss = nll.sum() / (wt.sum() if w is not None else B)
+    am = (C - 1 - z.flip(1).argmax(1)) if high_ties else R._first_max(z)[1]
+    return loss, dl.to(torch.bfloat16), float((am == t).sum())
+
+
+@pytest.mark.parametrize("weighted", [False, True])
+def test_cross_entropy_criterion_catches_padding_and_tie_defects(weighted):
+    g = _gen(34)
+    B, C, ldd = 64, 10, 16
+    z = torch.randn(B, C, generator=g) * 30                 # __expf at large |x|
+    t = torch.randint(0, C, (B,), generator=g)
+    z[:8, 7] = z[:8, 2] = z[:8].amax(1) + 1                 # ties for the argmax in 8 rows, target 2
+    t[:8] = 2
+    w = torch.rand(C, generator=g) + 0.1 if weighted else None
+    ref = R.cross_entropy64(z, t, ldd=ldd, class_weights=w)
+    bnd = KC.ce_bound(z, t, class_weights=w, se_chain=-(-C // 32) + 5, warps=32)
+    err = torch.zeros(B, ldd, dtype=F64)
+    err[:, :C] = bnd["dlogits"]
+    loss, dl, correct = _emu_ce(z, t, ldd, w)
+    KC.check(loss.view(1), ref["loss"].view(1), torch.zeros(1, dtype=F64), chain=0, exact=False,
+             err=bnd["loss"].view(1))
+    KC.check(dl, ref["dlogits"], torch.zeros_like(ref["dlogits"]), chain=0, exact=False, err=err)
+    assert correct == float(ref["meter"][1])
+    _, bad, _ = _emu_ce(z, t, ldd, w, pad=7.0)
+    _rejects(lambda: KC.check(bad, ref["dlogits"], torch.zeros_like(err), chain=0, exact=False, err=err))
+    assert _emu_ce(z, t, ldd, w, high_ties=True)[2] != float(ref["meter"][1])
+
+
+def _emu_adam(p, m, v, g, *, lr, b1, b2, eps, wd, step, gs, bc_off=0, eps_in_sqrt=False, drop_wd=False):
+    """adam_kernel in fp32 torch ops; the planted defects are options."""
+    f = torch.float32
+    s = step + bc_off
+    bc1i = torch.tensor(1.0 / (1.0 - b1 ** s), dtype=f)
+    bc2i = torch.tensor(1.0 / (1.0 - b2 ** s) ** 0.5, dtype=f)
+    b1_, b2_ = torch.tensor(b1, dtype=f), torch.tensor(b2, dtype=f)
+    gk = g * gs + (0.0 if drop_wd else torch.tensor(wd, dtype=f) * p)
+    m1 = b1_ * m + (1 - b1_) * gk
+    v1 = b2_ * v + (1 - b2_) * gk * gk
+    d = (v1 + eps).sqrt() * bc2i if eps_in_sqrt else v1.sqrt() * bc2i + eps
+    p1 = p - torch.tensor(lr, dtype=f) * bc1i * m1 / d
+    return p1, m1, v1
+
+
+def test_adam_criterion_catches_optimizer_defects():
+    g = _gen(35)
+    n = 4096
+    f32 = R._f32
+    hp = dict(lr=f32(1e-3), b1=f32(0.9), b2=f32(0.999), eps=f32(1e-8), wd=f32(0.01), gs=0.125)
+    p = torch.randn(n, generator=g)
+    m = torch.randn(n, generator=g) * 1e-3
+    v = torch.rand(n, generator=g) * 1e-6
+    gr = torch.randn(n, generator=g) * 10 ** (torch.rand(n, generator=g) * -6)   # magnitudes 1 .. 1e-6
+    step = 10
+    ref = R.adam_step64(p, m, v, gr, lr=hp["lr"], beta1=hp["b1"], beta2=hp["b2"], eps=hp["eps"],
+                        weight_decay=hp["wd"], step=step, grad_scale=hp["gs"])
+
+    def ok(out):
+        for got, key in zip(out, ("p", "m", "v")):
+            r, e = ref[key]
+            KC.check(got, r, torch.zeros_like(r), chain=0, exact=False, err=e)
+
+    kw = dict(lr=hp["lr"], b1=hp["b1"], b2=hp["b2"], eps=hp["eps"], wd=hp["wd"], step=step, gs=hp["gs"])
+    good = _emu_adam(p, m, v, gr, **kw)
+    ok(good)
+    _rejects(lambda: ok(_emu_adam(p, m, v, gr, bc_off=1, **kw)))
+    _rejects(lambda: ok(_emu_adam(p, m, v, gr, eps_in_sqrt=True, **kw)))
+    _rejects(lambda: ok(_emu_adam(p, m, v, gr, drop_wd=True, **kw)))
+    # the shadow is RNE(p) of the kernel's own p, bit for bit
+    KC.check(good[0].to(torch.bfloat16), good[0].to(F64), good[0].to(F64), chain=0, exact=True)
+    _rejects(lambda: KC.check(_trunc_bf16(good[0]), good[0].to(F64), good[0].to(F64), chain=0, exact=True))
+
+
+def test_sgd_criterion_passes_emulation():
+    g = _gen(36)
+    n = 4096
+    p, buf, gr = (torch.randn(n, generator=g) for _ in range(3))
+    for first in (True, False):
+        ref = R.sgd_step64(p, buf, gr, lr=R._f32(0.01), momentum=R._f32(0.9), weight_decay=R._f32(1e-4),
+                           first=first, grad_scale=0.125)
+        f = torch.float32
+        gk = gr * 0.125 + torch.tensor(R._f32(1e-4), dtype=f) * p
+        b1 = gk if first else torch.tensor(R._f32(0.9), dtype=f) * buf + gk
+        p1 = p - torch.tensor(R._f32(0.01), dtype=f) * b1
+        KC.check(p1, ref["p"][0], torch.zeros(n, dtype=F64), chain=0, exact=False, err=ref["p"][1])
+        KC.check(b1, ref["buf"][0], torch.zeros(n, dtype=F64), chain=0, exact=False, err=ref["buf"][1])
+        _rejects(lambda: KC.check(p + torch.tensor(R._f32(0.01)) * gr * 0.125, ref["p"][0], torch.zeros(n, dtype=F64),
+                                  chain=0, exact=False, err=ref["p"][1]))       # weight decay and momentum dropped
