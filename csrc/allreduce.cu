@@ -30,10 +30,10 @@ namespace b200 {
 
 // Footprint: the comm stream's CTAs run WHILE the persistent wgmma kernels of backward hold every
 // SM.  A 256-thread CTA capped at 40 registers (10 240) and no shared memory fits next to a
-// persistent CTA only where that leaves 10 240 registers free: a 384-thread GEMM / conv CTA
-// (umma_kernel, conv_halo_kernel) compiled to <= 128 registers (49 152) does; one at 136-168
-// registers (52 224 - 64 512: the BN = 128 instantiations) does not, nor do wgrad_halo64_kernel
-// (512 x 128 = 65 536) and conv0_kernel (640 threads).  `cuobjdump --dump-resource-usage` on the
+// persistent CTA only where that leaves 10 240 registers free.  None of the wgmma kernels does:
+// umma_kernel, conv_halo_kernel and wgrad_halo64_kernel are 512-thread CTAs at 128 registers
+// (65 536, redistributed between their warpgroups with setmaxnreg), and conv0_kernel has 640
+// threads.  `cuobjdump --dump-resource-usage` on the
 // library lists each kernel's count.  Where a conv CTA fills the SM, reduction CTAs wait for it to
 // finish; thin CTAs (bytes in flight = CTAs x 256 threads x UNR x 16 B) still keep the footprint of
 // each small.

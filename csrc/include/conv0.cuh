@@ -19,7 +19,8 @@ namespace b200 {
 
 constexpr int C0_STAGES = 4;
 constexpr int C0_PROD_WARPS = 8;                                  // 256 producer threads, in row-groups
-constexpr int C0_THREADS = UMMA_THREADS + 32 * C0_PROD_WARPS;     // TMA / 2 consumer / 2 builder warpgroups
+constexpr int C0_MMA_THREADS = 128 * (1 + UMMA_CONSUMERS);       // TMA warpgroup + 2 consumer warpgroups
+constexpr int C0_THREADS = C0_MMA_THREADS + 32 * C0_PROD_WARPS;   // ... + 2 builder warpgroups
 constexpr int C0_TILE_BYTES = 128 * 128;                          // 128 rows x 64 bf16
 
 struct Conv0Params {
@@ -192,7 +193,7 @@ __global__ void __launch_bounds__(C0_THREADS, 1) conv0_kernel(const __grid_const
     // 256 threads in groups of ROWS (one thread per row); group g builds the stages of iterations
     // it = g, g + NGROUPS, ... so several tiles are under construction at once.
     constexpr int NGROUPS = (32 * C0_PROD_WARPS) / ROWS;
-    const int pt = threadIdx.x - UMMA_THREADS;          // 0..255
+    const int pt = threadIdx.x - C0_MMA_THREADS;        // 0..255
     const int grp = pt / ROWS, r = pt % ROWS;
     if constexpr (!WGRAD) {
       uint32_t it = 0;

@@ -14,8 +14,8 @@
 // When all 9 * chunks weight tiles fit in the B ring and there is a single channel tile, they are
 // loaded once per CTA and stay resident for every tile the persistent CTA processes.
 //
-// Warp roles and the epilogue (bias / ReLU / ReLU-mask / fused column sum, shared with ConvPolicy)
-// are those of umma_core.cuh.
+// Warp roles (producer, two consumers, epilogue warpgroup), the staging hand-off and the epilogue
+// (bias / ReLU / ReLU-mask / fused column sum, shared with ConvPolicy) are those of umma_core.cuh.
 #pragma once
 #include "umma_policies.cuh"
 
@@ -32,11 +32,12 @@ template <int BN>
 struct HaloCfg {
   static constexpr int NA = BN >= 128 ? 2 : 3;
   static constexpr int B_SLOT = BN * 128;
-  static constexpr int BAR_BYTES = 512;
+  static constexpr int BAR_BYTES = 512;       // a_full/a_empty[NA], b_full/b_empty[NB], stage_full, stage_empty
   static constexpr int EPI_MAX = 2048;        // ConvPolicy::EPI_SMEM
   static constexpr int ROOM = UMMA_MAX_SMEM - NA * HALO_SLOT - UMMA_CONSUMERS * STAGE_BYTES - 1024 - BAR_BYTES - EPI_MAX;
   static constexpr int NB = ROOM / B_SLOT > 18 ? 18 : ROOM / B_SLOT;
   static constexpr int SMEM = NA * HALO_SLOT + NB * B_SLOT + UMMA_CONSUMERS * STAGE_BYTES + 1024 + BAR_BYTES;
+  static_assert((2 * NA + 2 * NB + 2) * 8 <= BAR_BYTES, "mbarriers");
 };
 
 template <int BN, bool DGRAD, bool POOL = false>
@@ -45,6 +46,7 @@ conv_halo_kernel(const __grid_constant__ ConvParams prm) {
   using Cfg = HaloCfg<BN>;
   using Epi = ConvPolicy<BN, 1, DGRAD, POOL>;
   constexpr int NA = Cfg::NA, NB = Cfg::NB, B_SLOT = Cfg::B_SLOT;
+  using Regs = RoleRegs<BN>;
   static_assert(Epi::EPI_SMEM <= Cfg::EPI_MAX, "epilogue scratch");
   // A fragments of the next tap are loaded while the previous tap's wgmmas run (two buffers) where
   // the accumulator leaves registers for it.
@@ -60,6 +62,8 @@ conv_halo_kernel(const __grid_constant__ ConvParams prm) {
   uint64_t* a_empty = a_full + NA;
   uint64_t* b_full = a_empty + NA;
   uint64_t* b_empty = b_full + NB;
+  uint64_t* stage_full = b_empty + NB;
+  uint64_t* stage_empty = stage_full + 1;
   float* epi_smem = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a_full) + Cfg::BAR_BYTES);
 
   const int wg = threadIdx.x >> 7;
@@ -69,6 +73,8 @@ conv_halo_kernel(const __grid_constant__ ConvParams prm) {
     tma_prefetch_desc(&prm.mapB);
     for (int s = 0; s < NA; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], UMMA_CONSUMERS); }
     for (int s = 0; s < NB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], UMMA_CONSUMERS); }
+    mbar_init(stage_full, STAGE_FULL_ARRIVALS);
+    mbar_init(stage_empty, STAGE_EMPTY_ARRIVALS);
     fence_mbar_init();
   }
   __syncthreads();
@@ -77,6 +83,7 @@ conv_halo_kernel(const __grid_constant__ ConvParams prm) {
   const bool resident = prm.resident != 0;
 
   if (wg == 0) {
+    set_role_regs<Regs::PRODUCER>();
     if (warp == 0) {                             // converged producer warp, elect.sync-predicated issue
       uint32_t a = 0, aph = 0, bs = 0, bph = 0;  // ring positions / phases as counters
       bool first = true;
@@ -119,15 +126,11 @@ conv_halo_kernel(const __grid_constant__ ConvParams prm) {
         first = false;
       }
     }
-  } else {
+  } else if (wg <= UMMA_CONSUMERS) {
+    set_role_regs<Regs::CONSUMER>();
     const int cw = wg - 1;
     const int t = threadIdx.x & 127;
     const int lane = t & 31;
-    float* stage = stage_base + cw * (STAGE_BYTES / 4);
-    if constexpr (Epi::EPI_SMEM > 0) {
-      Epi::epi_begin(prm, epi_smem, threadIdx.x - 128);
-      named_bar_sync(1, UMMA_EPI_THREADS);
-    }
     constexpr uint32_t B_KSTEP = DGRAD ? 16 * 128 : 32;
     constexpr uint32_t B_LBO = DGRAD ? UMMA_SLAB_BYTES : 16;
     const uint64_t bd_base = wgmma_desc_sw128(smem_u32(sB), B_LBO, 1024);
@@ -136,17 +139,9 @@ conv_halo_kernel(const __grid_constant__ ConvParams prm) {
     const int trow = cw * 64 + 16 * (t >> 5) + (lane & 15);
     const int hrow0 = (trow >> 3) * HALO_PITCH + (trow & 7);
     const int khalf = lane >> 4;
-    // Fused bias gradient with a single channel tile (the 64-channel layers): every tile of this
-    // CTA lands on the same columns, so a thread keeps running sums of what it stored and the
-    // warp transpose-reduce runs once per kernel instead of once per tile.
-    float keep[32];
-    const bool keep_on = DGRAD && BN == 64 && (prm.flags & CONV_COLSUM) && prm.Cn <= BN;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) keep[i] = 0.f;
-    uint32_t a = 0, aph = 0, bs = 0, bph = 0;
+    uint32_t a = 0, aph = 0, bs = 0, bph = 0, eph = 0;
     bool first = true;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const typename Epi::Ctx ctx = Epi::make_ctx(prm, tile);
       float d[BN / 2];
       for (int c = 0; c < cchunks; ++c) {
         mbar_wait(&a_full[a], aph, 25);
@@ -188,17 +183,52 @@ conv_halo_kernel(const __grid_constant__ ConvParams prm) {
       }
       first = false;
       wgmma_fence_acc(d);
-      const typename Epi::RowCtx rc = Epi::row_ctx(prm, ctx, cw * 64 + epi_row_local(t));
-      staged_epilogue<BN>(d, stage, t, 2 + cw, [&](int row_local, int col0, const uint32_t (&acc)[32]) {
-        Epi::epilogue(prm, ctx, rc, cw * 64 + row_local, col0, acc, epi_smem, nullptr, keep, keep_on);
-      });
+      stage_put<BN, 23>(d, stage_base, cw, t, stage_full, stage_empty, eph);
+    }
+  } else {
+    set_role_regs<Regs::EPILOGUE>();
+    const int t = threadIdx.x & 127;          // row t of the tile
+    const int lane = t & 31;
+    if constexpr (Epi::EPI_SMEM > 0) {
+      Epi::epi_begin(prm, epi_smem, t);
+      named_bar_sync(1, UMMA_EPI_THREADS);
+    }
+    // Fused bias gradient with a single channel tile (the 64-channel layers): every tile of this
+    // CTA lands on the same columns, so a thread keeps running sums of what it stored and the
+    // warp transpose-reduce runs once per kernel instead of once per tile.
+    float keep[2][32];
+    const bool keep_on = DGRAD && BN == 64 && (prm.flags & CONV_COLSUM) && prm.Cn <= BN;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) keep[0][i] = keep[1][i] = 0.f;
+    const bool masked = Epi::masked(prm);
+    uint32_t fph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const typename Epi::Ctx ctx = Epi::make_ctx(prm, tile);
+      const typename Epi::RowCtx rc = Epi::row_ctx(prm, ctx, t);
+#pragma unroll
+      for (int c0 = 0; c0 < BN; c0 += 64) {
+        // the mask does not depend on the accumulator: fetch it while the MMAs still run
+        uint32_t pm[2][16];
+        if (masked) {
+          Epi::load_mask(prm, ctx, rc, c0, pm[0]);
+          Epi::load_mask(prm, ctx, rc, c0 + 32, pm[1]);
+        }
+        uint32_t acc[2][32];
+        stage_take<BN, 24>(stage_base, c0, t, stage_full, stage_empty, fph, acc);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          Epi::epilogue(prm, ctx, rc, t, c0 + 32 * h, acc[h], epi_smem, pm[h], keep[h], keep_on);
+      }
     }
     if constexpr (DGRAD) {
-      if (keep_on) Epi::colsum_flush(prm, epi_col_half(t), lane, keep, epi_smem);
+      if (keep_on) {
+        Epi::colsum_flush(prm, 0, lane, keep[0], epi_smem);
+        Epi::colsum_flush(prm, 32, lane, keep[1], epi_smem);
+      }
     }
     if constexpr (Epi::EPI_SMEM > 0) {
       named_bar_sync(1, UMMA_EPI_THREADS);
-      Epi::epi_end(prm, epi_smem, threadIdx.x - 128);
+      Epi::epi_end(prm, epi_smem, t);
     }
   }
 }

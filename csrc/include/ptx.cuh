@@ -87,6 +87,26 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int ta
   }
 }
 
+// The same wait for warps that issue no wgmma and run under a raised setmaxnreg budget (the epilogue
+// warpgroup).  A trap inlined into such a region makes ptxas keep the region within the launch
+// allocation, so the timeout report and trap are out of line, after the loop.
+static __device__ __noinline__ void mbar_timeout(int tag, uint32_t parity) {
+  if (atomicCAS(&mbar_timeout_info[0], 0u, static_cast<uint32_t>(tag) | 0x80000000u) == 0u) {
+    mbar_timeout_info[1] = blockIdx.x;
+    mbar_timeout_info[2] = threadIdx.x;
+    mbar_timeout_info[3] = parity;
+    __threadfence();
+  }
+  __trap();
+}
+__device__ __forceinline__ void mbar_wait_outlined_timeout(uint64_t* bar, uint32_t parity, int tag) {
+  unsigned long long spins = 0;
+  bool ok;
+  while (!(ok = mbar_try_wait(bar, parity)) && ++spins <= (B200_SPIN_LIMIT >> 6)) {
+  }
+  if (!ok) mbar_timeout(tag, parity);
+}
+
 // ----------------------------------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
@@ -167,6 +187,18 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t add
 // Barrier over a subset of the CTA's warps (ids 1..15; 0 is __syncthreads).
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// Per-warpgroup register budget (executed by all 128 threads of a warpgroup; N a multiple of 8 in
+// [24, 256]).  The budgets of all warpgroups together must fit the allocation the kernel launched with.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  static_assert(N % 8 == 0 && N >= 24 && N <= 256, "setmaxnreg: multiple of 8 in [24, 256]");
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  static_assert(N % 8 == 0 && N >= 24 && N <= 256, "setmaxnreg: multiple of 8 in [24, 256]");
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
 
 // --------------------------------------------------------------------- cross-GPU memory ops

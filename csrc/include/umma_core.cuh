@@ -8,10 +8,14 @@
 //   warpgroups 1, 2  consumers: warpgroup c owns rows [64c, 64c+64) of the 128 x BN tile and keeps
 //                    its fp32 accumulator in registers.  Per k-block it waits "full[s]", issues four
 //                    wgmma.m64nBNk16, and releases the previous stage once its wgmmas retired (one
-//                    group stays in flight).  After the tile's last k-block the accumulator goes
-//                    through a per-warpgroup staging buffer in shared memory, 64 columns at a time,
-//                    so that the policy sees the row-major fragments it expects: one row and 32
-//                    consecutive columns per thread, a warp holding 32 consecutive rows.
+//                    group stays in flight).  After the tile's last k-block it writes the accumulator
+//                    into the shared staging tile, 64 columns at a time ("stage_empty" ->
+//                    write -> "stage_full"), and goes straight on to the next tile's k-blocks.
+//   warpgroup 3      epilogue: thread t takes row t of each staged 64-column chunk into registers,
+//                    releases the chunk and runs the policy's epilogue on it, so the policy sees
+//                    the row-major fragments it expects: one row and 32 consecutive columns per
+//                    call, a warp holding 32 consecutive rows.  It overlaps the next tile's MMAs.
+// setmaxnreg moves registers from the producer to the consumers and the epilogue (RoleRegs).
 //
 // Tile: 128 (M) x BN (N), BK = 64 bf16 = one 128-byte swizzle row.  Operands are staged in the
 // canonical SWIZZLE_128B layouts, K-major (rows = M/N index) or MN-major (rows = K index,
@@ -31,8 +35,10 @@
 //   __device__ static void epilogue(const Params&, const Ctx&, const RowCtx&, int row, int col0,
 //                                   const uint32_t (&acc)[32], float* epi_smem);
 //                                                                 // row in [0,128), 32 columns
+//   static constexpr bool PREMASK;      // true: where masked(prm), load_mask(prm, ctx, rc, col0, m[16])
+//                                       // fetches what the epilogue's `const uint32_t* premask` takes
 //   static constexpr int EPI_SMEM;                                // bytes of epilogue scratch
-//   __device__ static void epi_begin(const Params&, float* epi_smem, int tid);  // tid in [0,256)
+//   __device__ static void epi_begin(const Params&, float* epi_smem, int tid);  // tid in [0,128)
 //   __device__ static void epi_end(const Params&, float* epi_smem, int tid);    // after all tiles
 #pragma once
 #include "ptx.cuh"
@@ -44,16 +50,18 @@ constexpr int UMMA_BK = 64;                           // elements per k-block (1
 constexpr int UMMA_A_BYTES = UMMA_BM * UMMA_BK * 2;   // 16 KB per stage
 constexpr int UMMA_SLAB_BYTES = 64 * 128;             // one MN-major slab: 64 k-rows x 128 B
 constexpr int UMMA_CONSUMERS = 2;                     // consumer warpgroups, 64 rows each
-constexpr int UMMA_EPI_THREADS = 128 * UMMA_CONSUMERS;
-constexpr int UMMA_THREADS = 128 + UMMA_EPI_THREADS;
+constexpr int UMMA_EPI_THREADS = 128;                 // the epilogue warpgroup
+constexpr int UMMA_THREADS = 128 * (1 + UMMA_CONSUMERS) + UMMA_EPI_THREADS;
+constexpr int UMMA_LAUNCH_REGS = 65536 / UMMA_THREADS;   // __launch_bounds__(UMMA_THREADS, 1): 128
 constexpr int UMMA_MAX_SMEM = 227 * 1024;             // H100: opt-in shared memory per block
 constexpr int STAGE_LD = 68;                          // staging row pitch (floats): conflict-free row reads
-constexpr int STAGE_BYTES = 64 * STAGE_LD * 4;        // one warpgroup's 64 x 64 fp32 staging tile
-constexpr int UMMA_BAR_BYTES = 256;
+constexpr int STAGE_BYTES = 64 * STAGE_LD * 4;        // one consumer's 64 rows of a 64-column fp32 chunk
+constexpr int UMMA_BAR_BYTES = 256;                   // full[STAGES], empty[STAGES], stage_full, stage_empty
 
 template <int BN>
 __host__ __device__ constexpr int umma_b_bytes() { return BN * UMMA_BK * 2; }
-// Pipeline depth: as many stages as fit next to the staging tiles and the epilogue scratch, <= 8.
+// Pipeline depth: as many stages as fit next to the staging tile, the barriers and the epilogue
+// scratch, <= 8.
 template <int BN, int EPI_SMEM>
 __host__ __device__ constexpr int umma_stages() {
   constexpr int room = UMMA_MAX_SMEM - 1024 - UMMA_BAR_BYTES - UMMA_CONSUMERS * STAGE_BYTES - EPI_SMEM;
@@ -62,14 +70,28 @@ __host__ __device__ constexpr int umma_stages() {
 }
 template <int BN, int STAGES>
 __host__ __device__ constexpr int umma_smem_bytes() {
+  static_assert((2 * STAGES + 2) * 8 <= UMMA_BAR_BYTES, "mbarriers");
   return STAGES * (UMMA_A_BYTES + umma_b_bytes<BN>()) + UMMA_CONSUMERS * STAGE_BYTES + 1024 /*alignment slack*/ +
          UMMA_BAR_BYTES;
 }
 
-// Rows and column half a consumer thread handles in the row-major epilogue: warp w of the
-// warpgroup takes rows (w & 1) * 32 + lane and columns [(w >> 1) * 32, +32) of each 64-column chunk.
-__device__ __forceinline__ int epi_row_local(int t) { return ((t >> 5) & 1) * 32 + (t & 31); }
-__device__ __forceinline__ int epi_col_half(int t) { return (t >> 6) * 32; }
+// Registers per thread of each warpgroup role (setmaxnreg; multiples of 8 that add up to the launch
+// allocation of 4 x 128).  The producer is one converged warp with a few counters.  A consumer holds
+// BN / 2 accumulator registers (plus, in the halo kernel, two sets of A fragments) and nothing else.
+// The epilogue warpgroup gets the rest: it holds a 64-column row (64 registers), the prefetched ReLU
+// mask and, in the 64-channel halo dgrad, 64 running column sums.
+template <int BN>
+struct RoleRegs {
+  static constexpr int PRODUCER = 40;
+  static constexpr int CONSUMER = BN >= 128 ? 152 : 128;
+  static constexpr int EPILOGUE = 4 * UMMA_LAUNCH_REGS - PRODUCER - UMMA_CONSUMERS * CONSUMER;
+  static_assert(EPILOGUE % 8 == 0 && EPILOGUE >= 24 && EPILOGUE <= 256, "register budgets");
+};
+template <int N>
+__device__ __forceinline__ void set_role_regs() {
+  if constexpr (N > UMMA_LAUNCH_REGS) setmaxnreg_inc<N>();
+  else if constexpr (N < UMMA_LAUNCH_REGS) setmaxnreg_dec<N>();
+}
 
 // Accumulator columns [c0, c0 + 64) of a warpgroup (wgmma fragment layout) -> stage[64][STAGE_LD].
 // Fragment: d[i] is row 16 * warp + lane / 4 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2 * (lane & 3) + (i & 1).
@@ -97,24 +119,36 @@ __device__ __forceinline__ void stage_read_row(const float* stage, int row_local
   }
 }
 
-// Hands a warpgroup's accumulator to `epi(row_local, col0, acc32)` in 64-column chunks.  `bar` is the
-// warpgroup's named barrier.  Every thread of the warpgroup calls this; `epi` is called by whole warps.
-template <int BN, class F>
-__device__ __forceinline__ void staged_epilogue(const float (&d)[BN / 2], float* stage, int t, int bar, F&& epi) {
-  const int row_local = epi_row_local(t);
-  const int ch = epi_col_half(t);
+// Consumer side of the hand-off: warpgroup `cw`'s accumulator into its half of the staging tile,
+// one 64-column chunk after the other.  `eph` counts the chunks handed over (parity of stage_empty).
+template <int BN, int TAG>
+__device__ __forceinline__ void stage_put(const float (&d)[BN / 2], float* stage_base, int cw, int t,
+                                          uint64_t* stage_full, uint64_t* stage_empty, uint32_t& eph) {
+  float* stage = stage_base + cw * (STAGE_BYTES / 4);
 #pragma unroll
   for (int c0 = 0; c0 < BN; c0 += 64) {
-    named_bar_sync(bar, 128);                 // the previous chunk has been read
+    mbar_wait(stage_empty, eph ^ 1, TAG);     // the epilogue has read the previous chunk
+    eph ^= 1;
     stage_acc_chunk(d, c0, stage, t);
-    named_bar_sync(bar, 128);
-    if (c0 + ch < BN) {
-      uint32_t acc[32];
-      stage_read_row(stage, row_local, ch, acc);
-      epi(row_local, c0 + ch, acc);
-    }
+    __syncwarp();
+    if ((t & 31) == 0) mbar_arrive(stage_full);   // one arrival per consumer warp
   }
 }
+// Epilogue side: row t of the staged chunk, both 32-column halves (the second only when the tile
+// is that wide), into registers; then the chunk is released.  `fph` is stage_full's parity.
+template <int BN, int TAG>
+__device__ __forceinline__ void stage_take(const float* stage_base, int c0, int t, uint64_t* stage_full,
+                                           uint64_t* stage_empty, uint32_t& fph, uint32_t (&acc)[2][32]) {
+  mbar_wait_outlined_timeout(stage_full, fph, TAG);
+  fph ^= 1;
+  const float* stage = stage_base + (t >> 6) * (STAGE_BYTES / 4);
+  stage_read_row(stage, t & 63, 0, acc[0]);
+  if (c0 + 32 < BN) stage_read_row(stage, t & 63, 32, acc[1]);
+  __syncwarp();
+  if ((t & 31) == 0) mbar_arrive(stage_empty);    // one arrival per epilogue warp
+}
+constexpr uint32_t STAGE_FULL_ARRIVALS = UMMA_CONSUMERS * 4;
+constexpr uint32_t STAGE_EMPTY_ARRIVALS = UMMA_EPI_THREADS / 32;
 
 template <class P>
 __global__ void __launch_bounds__(UMMA_THREADS, 1)
@@ -123,6 +157,7 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
   constexpr int STAGES = P::STAGES;
   constexpr int B_BYTES = umma_b_bytes<BN>();
   constexpr uint32_t STAGE_TX = UMMA_A_BYTES + B_BYTES;
+  using Regs = RoleRegs<BN>;
   static_assert(BN % 32 == 0 && BN >= 32 && BN <= 256, "tile N must be a multiple of 32 in [32,256]");
   static_assert(!P::B_MN || BN % 64 == 0, "MN-major B is staged in 64-wide slabs");
 
@@ -134,6 +169,8 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
   float* stage_base = reinterpret_cast<float*>(sB + STAGES * B_BYTES);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stage_base) + UMMA_CONSUMERS * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* stage_full = empty_bar + STAGES;
+  uint64_t* stage_empty = stage_full + 1;
   float* epi_smem = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + UMMA_BAR_BYTES);
 
   const int wg = threadIdx.x >> 7;
@@ -145,12 +182,15 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], UMMA_CONSUMERS);   // one arrival per consumer warpgroup
     }
+    mbar_init(stage_full, STAGE_FULL_ARRIVALS);
+    mbar_init(stage_empty, STAGE_EMPTY_ARRIVALS);
     fence_mbar_init();
   }
   __syncthreads();
   const int num_tiles = prm.num_tiles;
 
   if (wg == 0) {
+    set_role_regs<Regs::PRODUCER>();
     // The producer warp runs CONVERGED (all 32 lanes execute the loop and poll the barriers); only
     // the TMA instructions themselves are predicated on elect.sync, so addresses stay warp-uniform.
     if (warp == 0) {
@@ -169,14 +209,10 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
         }
       }
     }
-  } else {
+  } else if (wg <= UMMA_CONSUMERS) {
+    set_role_regs<Regs::CONSUMER>();
     const int cw = wg - 1;                    // consumer index: rows [64 cw, 64 cw + 64) of the tile
     const int t = threadIdx.x & 127;
-    float* stage = stage_base + cw * (STAGE_BYTES / 4);
-    if constexpr (P::EPI_SMEM > 0) {
-      P::epi_begin(prm, epi_smem, threadIdx.x - 128);
-      named_bar_sync(1, UMMA_EPI_THREADS);    // the consumer warpgroups only
-    }
     // byte step per k16: K-major -> 32 B inside the swizzle row; MN-major -> 16 k-rows.
     constexpr uint32_t A_KSTEP = P::A_MN ? 16 * 128 : 32;
     constexpr uint32_t B_KSTEP = P::B_MN ? 16 * 128 : 32;
@@ -186,7 +222,7 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
     // memory is < 256 KB, so the add never carries out of the 14-bit field.
     const uint64_t ad_base = wgmma_desc_sw128(smem_u32(sA) + cw * 8192, A_LBO, 1024);
     const uint64_t bd_base = wgmma_desc_sw128(smem_u32(sB), B_LBO, 1024);
-    uint32_t s = 0, ph = 0, prev = 0;
+    uint32_t s = 0, ph = 0, prev = 0, eph = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const typename P::Ctx ctx = P::make_ctx(prm, tile);
       const int nk = P::num_k_iters(prm, ctx);
@@ -210,15 +246,47 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
       wgmma_fence_acc(d);
       if (nk > 0) {
         if (t == 0) mbar_arrive(&empty_bar[prev]);
-        const typename P::RowCtx rc = P::row_ctx(prm, ctx, cw * 64 + epi_row_local(t));
-        staged_epilogue<BN>(d, stage, t, 2 + cw, [&](int row_local, int col0, const uint32_t (&acc)[32]) {
-          P::epilogue(prm, ctx, rc, cw * 64 + row_local, col0, acc, epi_smem);
-        });
+        stage_put<BN, 3>(d, stage_base, cw, t, stage_full, stage_empty, eph);
+      }
+    }
+  } else {
+    set_role_regs<Regs::EPILOGUE>();
+    const int t = threadIdx.x & 127;          // row t of the tile
+    if constexpr (P::EPI_SMEM > 0) {
+      P::epi_begin(prm, epi_smem, t);
+      named_bar_sync(1, UMMA_EPI_THREADS);
+    }
+    uint32_t fph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const typename P::Ctx ctx = P::make_ctx(prm, tile);
+      if (P::num_k_iters(prm, ctx) == 0) continue;
+      const typename P::RowCtx rc = P::row_ctx(prm, ctx, t);
+#pragma unroll
+      for (int c0 = 0; c0 < BN; c0 += 64) {
+        uint32_t acc[2][32];
+        if constexpr (P::PREMASK) {
+          // the mask does not depend on the accumulator: fetch it while the MMAs still run
+          uint32_t pm[2][16];
+          const bool masked = P::masked(prm);
+          if (masked) {
+            P::load_mask(prm, ctx, rc, c0, pm[0]);
+            if (c0 + 32 < BN) P::load_mask(prm, ctx, rc, c0 + 32, pm[1]);
+          }
+          stage_take<BN, 4>(stage_base, c0, t, stage_full, stage_empty, fph, acc);
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            if (c0 + 32 * h < BN) P::epilogue(prm, ctx, rc, t, c0 + 32 * h, acc[h], epi_smem, pm[h]);
+        } else {
+          stage_take<BN, 4>(stage_base, c0, t, stage_full, stage_empty, fph, acc);
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            if (c0 + 32 * h < BN) P::epilogue(prm, ctx, rc, t, c0 + 32 * h, acc[h], epi_smem);
+        }
       }
     }
     if constexpr (P::EPI_SMEM > 0) {
       named_bar_sync(1, UMMA_EPI_THREADS);
-      P::epi_end(prm, epi_smem, threadIdx.x - 128);
+      P::epi_end(prm, epi_smem, t);
     }
   }
 }

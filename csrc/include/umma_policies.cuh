@@ -69,6 +69,7 @@ struct GemmPolicy {
   static constexpr bool A_MN = A_MN_;
   static constexpr bool B_MN = B_MN_;
   using Params = GemmParams;
+  static constexpr bool PREMASK = false;
   static constexpr int EPI_SMEM = 0;
   __device__ static void epi_begin(const Params&, float*, int) {}
   __device__ static void epi_end(const Params&, float*, int) {}
@@ -273,19 +274,20 @@ struct ConvPolicy {
   // fprop = the bias vector, staged once per CTA and read back as broadcast float4 loads
   static constexpr int EPI_MAXC = 512;
   static constexpr int EPI_SMEM = EPI_MAXC * 4;
+  static constexpr bool PREMASK = DGRAD;
   __device__ static void epi_begin(const Params& p, float* sm, int tid) {
     if constexpr (DGRAD) {
       if (p.flags & CONV_COLSUM)
-        for (int i = tid; i < EPI_MAXC; i += 256) sm[i] = 0.f;
+        for (int i = tid; i < EPI_MAXC; i += UMMA_EPI_THREADS) sm[i] = 0.f;
     } else {
       if (p.flags & CONV_BIAS)
-        for (int i = tid; i < p.Cn && i < EPI_MAXC; i += 256) sm[i] = p.bias[i];
+        for (int i = tid; i < p.Cn && i < EPI_MAXC; i += UMMA_EPI_THREADS) sm[i] = p.bias[i];
     }
   }
   __device__ static void epi_end(const Params& p, float* sm, int tid) {
     if constexpr (DGRAD) {
       if (p.flags & CONV_COLSUM)
-        for (int i = tid; i < p.Cn; i += 256) {
+        for (int i = tid; i < p.Cn; i += UMMA_EPI_THREADS) {
           const float v = sm[i];
           if (v != 0.f) atomicAdd(p.colsum + i, v);
         }
@@ -342,8 +344,9 @@ struct ConvPolicy {
   }
 
   // The ReLU mask of a dgrad chunk (the previous layer's activations at this thread's pixel)
-  // depends only on the tile, not on the accumulator: kernels whose epilogue is on the critical
-  // path fetch it BEFORE they wait for the MMAs, so the global-load latency is off that path.
+  // depends only on the tile, not on the accumulator: the epilogue warpgroup fetches it BEFORE it
+  // waits for the staged accumulator, so the global-load latency overlaps the MMAs.
+  __device__ static bool masked(const Params& p) { return DGRAD && (p.flags & CONV_MASK) != 0; }
   __device__ static void load_mask(const Params& p, const Ctx& c, const RowCtx& rc, int col0, uint32_t (&m)[16]) {
     const int ch = c.c0 + col0;
     if (rc.valid && ch < p.Cn) {
@@ -388,17 +391,10 @@ struct ConvPolicy {
 #pragma unroll
           for (int u = 0; u < 16; ++u) v[u] = fmaxf(v[u], 0.f);
         }
-        if (p.flags & CONV_MASK) {
-          uint32_t mw[8];
-          if (premask) {
-#pragma unroll
-            for (int u = 0; u < 8; ++u) mw[u] = premask[(j >> 1) + u];
-          } else {
-            ld_global_nc_v8(p.mask_src + off + j, mw);
-          }
+        if (DGRAD && (p.flags & CONV_MASK)) {    // premask: load_mask of this chunk
 #pragma unroll
           for (int u = 0; u < 8; ++u) {
-            const float2 f = unpack_bf16x2(mw[u]);
+            const float2 f = unpack_bf16x2(premask[(j >> 1) + u]);
             if (!(f.x > 0.f)) v[2 * u] = 0.f;
             if (!(f.y > 0.f)) v[2 * u + 1] = 0.f;
           }
@@ -530,6 +526,7 @@ struct WgradPolicy {
   static constexpr bool A_MN = true;
   static constexpr bool B_MN = true;
   using Params = WgradParams;
+  static constexpr bool PREMASK = false;
   static constexpr int EPI_SMEM = 0;
   __device__ static void epi_begin(const Params&, float*, int) {}
   __device__ static void epi_end(const Params&, float*, int) {}

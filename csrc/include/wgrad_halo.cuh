@@ -33,6 +33,11 @@ constexpr int WH_STAGES = 8;
 constexpr int WH_CONSUMERS = 3;                           // one per filter row kh
 constexpr int WH_THREADS = 128 * (1 + WH_CONSUMERS);
 constexpr int WH_SMEM = WH_STAGES * WH_STAGE + 1024 + 512;
+// Registers per thread (setmaxnreg; launch allocation 4 x 128): the producer warpgroup gives up what
+// the consumers need for three 64 x 64 fp32 accumulators (96) and two sets of A fragments (32).
+constexpr int WH_PRODUCER_REGS = 24;
+constexpr int WH_CONSUMER_REGS = 160;
+static_assert(WH_PRODUCER_REGS + WH_CONSUMERS * WH_CONSUMER_REGS <= 4 * (65536 / WH_THREADS), "register budgets");
 
 struct WgradHaloParams {
   CUtensorMap mapX;        // X  {64, W, H, N}, box {64, 10, 10, 1}
@@ -74,6 +79,7 @@ wgrad_halo64_kernel(const __grid_constant__ WgradHaloParams prm) {
   };
 
   if (wg == 0) {
+    setmaxnreg_dec<WH_PRODUCER_REGS>();
     if (warp == 0) {
       uint32_t it = 0;
       for (int item = blockIdx.x; item < prm.num_items; item += gridDim.x) {
@@ -98,6 +104,7 @@ wgrad_halo64_kernel(const __grid_constant__ WgradHaloParams prm) {
       }
     }
   } else {
+    setmaxnreg_inc<WH_CONSUMER_REGS>();
     const int kh = wg - 1;                    // this warpgroup's taps: (kh, 0), (kh, 1), (kh, 2)
     const int t = threadIdx.x & 127;
     const int lane = t & 31, w = t >> 5;
@@ -113,12 +120,15 @@ wgrad_halo64_kernel(const __grid_constant__ WgradHaloParams prm) {
       float d[3][32];
       for (int i = 0; i < nk; ++i, ++it) {
         const uint32_t s = it % WH_STAGES;
-        mbar_wait(&full_bar[s], (it / WH_STAGES) & 1, 33);
+        mbar_wait_outlined_timeout(&full_bar[s], (it / WH_STAGES) & 1, 33);   // no wgmma in flight here
         const uint32_t x0 = smem_u32(smem + s * WH_STAGE);
         const uint64_t zd0 = wgmma_desc_sw128(x0 + WH_X_SLOT, UMMA_SLAB_BYTES, 1024);
+        // Two sets of A fragments: kw = 2 reloads the first set once kw = 0's wgmmas have retired.
+        uint32_t af[2][4][4];
 #pragma unroll
         for (int kw = 0; kw < 3; ++kw) {
-          uint32_t f[4][4];
+          uint32_t (&f)[4][4] = af[kw & 1];
+          if (kw == 2) wgmma_wait<1>();
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) {   // k16 step = pixel rows 2 ks, 2 ks + 1 of the 8 x 8 tile
             const int hr = (2 * ks + prow + kh) * WH_PITCH + px + kw;

@@ -275,7 +275,7 @@ void gemm_bf16(const bf16* A, long long lda, bool a_mn, const bf16* B, long long
                int M, int N, int K, void* out, long long ldo, int epi, const float* bias,
                float alpha, int ksplit, int bn, cudaStream_t stream) {
   // Tiles are at most 128 wide: a 64 x 256 fp32 accumulator (128 registers per thread) does not fit
-  // next to the epilogue under the 168-register limit of a 384-thread CTA, and spills.
+  // a consumer warpgroup's register budget (RoleRegs in umma_core.cuh) next to its descriptors.
   if (bn == 0) bn = N <= 32 && !b_mn ? 32 : (N <= 64 ? 64 : 128);
   if (ksplit < 1) ksplit = 1;
   GemmParams prm;
