@@ -3,7 +3,9 @@ fprop / dgrad / wgrad, the FC GEMMs and the memory-bound kernels, with achieved 
 against MEASURED_PEAKS.json, and torch (cuDNN/cuBLAS, bf16 channels_last) numbers for context.
 Writes gpurun_out/layer_bench.json and prints a table."""
 # Without MEASURED_PEAKS.json the peaks are the H100 SXM data sheet's: 989 dense bf16 TFLOP/s and
-# 3,350 GB/s.  Every native conv call uses the training step's kernel choice (bn = 0, ksplit = 0).
+# 3,350 GB/s.  Every native conv call uses the training step's kernel choice (bn = 0, ksplit = 0);
+# where the output side of a conv has >= 256 channels (the only place the width rule can pick a
+# 256-wide tile) the same call is also timed at bn = 128 and bn = 256, rows tagged "[bn=...]".
 # The table is headed by the card's name, power limit and maximum SM clock.
 import json, os, subprocess, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -82,20 +84,24 @@ for i, c in enumerate(spec.convs):
         dw = torch.zeros(c.cout, 3, 3, c.cin, device=dev)
         fl = 2.0 * B * h * h * c.cout * 9 * c.cin / 1e12
         C = ops.require()
-        t = timeit(lambda: C.conv_fprop(x, w, bias, y, True, 0))
-        rows.append(("%s fprop %dx%d %d->%d" % (c.name, h, h, c.cin, c.cout), t, fl, 0))
+
+        def timed(name, wide, fn):               # fn(bn)
+            rows.append((name, timeit(lambda: fn(0)), fl, 0))
+            if wide:
+                for bn in (128, 256):
+                    rows.append(("%s [bn=%d]" % (name, bn), timeit(lambda: fn(bn)), fl, 0))
+
+        timed("%s fprop %dx%d %d->%d" % (c.name, h, h, c.cin, c.cout), c.cout >= 256,
+              lambda bn: C.conv_fprop(x, w, bias, y, True, bn))
         if c.pool_after:                         # what the step runs for a pooled layer
             pooled = torch.empty(B, h // 2, h // 2, c.cout, dtype=torch.bfloat16, device=dev)
             pmask = ops.pool_mask_like(B, h, h, c.cout, dev)
-            t = timeit(lambda: C.conv_fprop_pool(x, w, bias, pooled, pmask, 0))
-            rows.append(("%s fprop+pool" % c.name, t, fl, 0))
-        t = timeit(lambda: C.conv_dgrad(dz, w, x, dx, None, 0))
-        rows.append(("%s dgrad" % c.name, t, fl, 0))
+            timed("%s fprop+pool" % c.name, c.cout >= 256, lambda bn: C.conv_fprop_pool(x, w, bias, pooled, pmask, bn))
+        timed("%s dgrad" % c.name, c.cin >= 256, lambda bn: C.conv_dgrad(dz, w, x, dx, None, bn))
         cs = torch.zeros(c.cin, device=dev)
-        t = timeit(lambda: C.conv_dgrad(dz, w, x, dx, cs, 0))
-        rows.append(("%s dgrad+colsum" % c.name, t, fl, 0))
-        t = timeit(lambda: C.conv_wgrad(dz, x, dw, 1.0, 0, 0))    # Cin = 64 on 8-divisible maps: the halo kernel
-        rows.append(("%s wgrad" % c.name, t, fl, 0))
+        timed("%s dgrad+colsum" % c.name, c.cin >= 256, lambda bn: C.conv_dgrad(dz, w, x, dx, cs, bn))
+        # Cin = 64 on 8-divisible maps: the halo kernel
+        timed("%s wgrad" % c.name, c.cin >= 256, lambda bn: C.conv_wgrad(dz, x, dw, 1.0, 0, bn))
         if with_torch:
             xt = x.permute(0, 3, 1, 2)            # NCHW view, channels_last memory
             wt = w.permute(0, 3, 1, 2)

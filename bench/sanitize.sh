@@ -14,6 +14,12 @@ for tool in memcheck synccheck; do
       > ${OUT:-prof_out}/sanitize_$tool.log 2>&1
   echo "== compute-sanitizer $tool exit $?"; grep -E "ERROR SUMMARY|passed|failed" ${OUT:-prof_out}/sanitize_$tool.log | tail -3
 done
+# the 256-wide conv tiles: fprop, fprop + pool, dgrad (plain / masked / column sum) and wgrad, one small case each
+for tool in memcheck synccheck; do
+  timeout 900 $SAN --tool $tool --error-exitcode 7 python -m pytest tests/test_wide_tiles_gpu.py -q -x -m gpu \
+      -k "exact and 2-28-28-256-256" > ${OUT:-prof_out}/sanitize_wide_$tool.log 2>&1
+  echo "== compute-sanitizer $tool (256-wide tiles) exit $?"; grep -E "ERROR SUMMARY|passed|failed" ${OUT:-prof_out}/sanitize_wide_$tool.log | tail -3
+done
 # one small case of each family of the float64 element-wise tests, under memcheck and racecheck
 E='maxpool_fwd_relu_bwd_colsum and 3-16-8 or avgpool_fwd_bwd and 5-64-1 or bias_grad and 37-3-8 or bias_grad and 64-64-64'
 E+=' or fc_bias_act_and_dropout and 37-10-0.6 or fc_grad_act and 1-5-True or test_cross_entropy and 7-10 or head_ce and 37-3'

@@ -34,9 +34,9 @@ struct HaloCfg {
   static constexpr int B_SLOT = BN * 128;
   static constexpr int BAR_BYTES = 512;       // a_full/a_empty[NA], b_full/b_empty[NB], stage_full, stage_empty
   static constexpr int EPI_MAX = 2048;        // ConvPolicy::EPI_SMEM
-  static constexpr int ROOM = UMMA_MAX_SMEM - NA * HALO_SLOT - UMMA_CONSUMERS * STAGE_BYTES - 1024 - BAR_BYTES - EPI_MAX;
+  static constexpr int ROOM = UMMA_MAX_SMEM - NA * HALO_SLOT - UMMA_CONSUMERS * stage_bytes<BN>() - 1024 - BAR_BYTES - EPI_MAX;
   static constexpr int NB = ROOM / B_SLOT > 18 ? 18 : ROOM / B_SLOT;
-  static constexpr int SMEM = NA * HALO_SLOT + NB * B_SLOT + UMMA_CONSUMERS * STAGE_BYTES + 1024 + BAR_BYTES;
+  static constexpr int SMEM = NA * HALO_SLOT + NB * B_SLOT + UMMA_CONSUMERS * stage_bytes<BN>() + 1024 + BAR_BYTES;
   static_assert((2 * NA + 2 * NB + 2) * 8 <= BAR_BYTES, "mbarriers");
 };
 
@@ -58,7 +58,7 @@ conv_halo_kernel(const __grid_constant__ ConvParams prm) {
   uint8_t* sA = smem;
   uint8_t* sB = smem + NA * HALO_SLOT;
   float* stage_base = reinterpret_cast<float*>(sB + NB * B_SLOT);
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stage_base) + UMMA_CONSUMERS * STAGE_BYTES);
+  uint64_t* a_full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stage_base) + UMMA_CONSUMERS * stage_bytes<BN>());
   uint64_t* a_empty = a_full + NA;
   uint64_t* b_full = a_empty + NA;
   uint64_t* b_empty = b_full + NB;

@@ -7,11 +7,12 @@
 //                    cp.async.bulk.tensor loads.
 //   warpgroups 1, 2  consumers: warpgroup c owns rows [64c, 64c+64) of the 128 x BN tile and keeps
 //                    its fp32 accumulator in registers.  Per k-block it waits "full[s]", issues four
-//                    wgmma.m64nBNk16, and releases the previous stage once its wgmmas retired (one
-//                    group stays in flight).  After the tile's last k-block it writes the accumulator
-//                    into the shared staging tile, 64 columns at a time ("stage_empty" ->
+//                    wgmma.m64nBNk16 (two m64n128k16 per k16 step at BN = 256), and releases the
+//                    previous stage once its wgmmas retired (one group stays in flight).  After
+//                    the tile's last k-block it writes the accumulator into the shared staging
+//                    tile, one chunk of stage_cols<BN>() columns at a time ("stage_empty" ->
 //                    write -> "stage_full"), and goes straight on to the next tile's k-blocks.
-//   warpgroup 3      epilogue: thread t takes row t of each staged 64-column chunk into registers,
+//   warpgroup 3      epilogue: thread t takes row t of each staged chunk into registers,
 //                    releases the chunk and runs the policy's epilogue on it, so the policy sees
 //                    the row-major fragments it expects: one row and 32 consecutive columns per
 //                    call, a warp holding 32 consecutive rows.  It overlaps the next tile's MMAs.
@@ -54,9 +55,19 @@ constexpr int UMMA_EPI_THREADS = 128;                 // the epilogue warpgroup
 constexpr int UMMA_THREADS = 128 * (1 + UMMA_CONSUMERS) + UMMA_EPI_THREADS;
 constexpr int UMMA_LAUNCH_REGS = 65536 / UMMA_THREADS;   // __launch_bounds__(UMMA_THREADS, 1): 128
 constexpr int UMMA_MAX_SMEM = 227 * 1024;             // H100: opt-in shared memory per block
-constexpr int STAGE_LD = 68;                          // staging row pitch (floats): conflict-free row reads
-constexpr int STAGE_BYTES = 64 * STAGE_LD * 4;        // one consumer's 64 rows of a 64-column fp32 chunk
 constexpr int UMMA_BAR_BYTES = 256;                   // full[STAGES], empty[STAGES], stage_full, stage_empty
+
+// Staging tile: each consumer hands its 64 accumulator rows to the epilogue warpgroup one chunk of
+// stage_cols columns at a time.  64 columns up to BN = 128.  At BN = 256 the chunk is 32 columns:
+// the two 17 KB staging halves of a 64-column chunk would leave room for only three 48 KB stages,
+// and the epilogue's 120 registers (RoleRegs<256>) hold one 32-column row, not a 64-column one.
+// The row pitch of 4 extra floats makes the epilogue's float4 row reads conflict-free.
+template <int BN>
+__host__ __device__ constexpr int stage_cols() { return BN >= 256 ? 32 : 64; }
+template <int BN>
+__host__ __device__ constexpr int stage_ld() { return stage_cols<BN>() + 4; }
+template <int BN>
+__host__ __device__ constexpr int stage_bytes() { return 64 * stage_ld<BN>() * 4; }   // one consumer's rows
 
 template <int BN>
 __host__ __device__ constexpr int umma_b_bytes() { return BN * UMMA_BK * 2; }
@@ -64,26 +75,29 @@ __host__ __device__ constexpr int umma_b_bytes() { return BN * UMMA_BK * 2; }
 // scratch, <= 8.
 template <int BN, int EPI_SMEM>
 __host__ __device__ constexpr int umma_stages() {
-  constexpr int room = UMMA_MAX_SMEM - 1024 - UMMA_BAR_BYTES - UMMA_CONSUMERS * STAGE_BYTES - EPI_SMEM;
+  constexpr int room = UMMA_MAX_SMEM - 1024 - UMMA_BAR_BYTES - UMMA_CONSUMERS * stage_bytes<BN>() - EPI_SMEM;
   constexpr int s = room / (UMMA_A_BYTES + umma_b_bytes<BN>());
   return s > 8 ? 8 : s;
 }
 template <int BN, int STAGES>
 __host__ __device__ constexpr int umma_smem_bytes() {
   static_assert((2 * STAGES + 2) * 8 <= UMMA_BAR_BYTES, "mbarriers");
-  return STAGES * (UMMA_A_BYTES + umma_b_bytes<BN>()) + UMMA_CONSUMERS * STAGE_BYTES + 1024 /*alignment slack*/ +
-         UMMA_BAR_BYTES;
+  static_assert(STAGES >= 4, "the operand ring keeps at least four stages at every tile width");
+  return STAGES * (UMMA_A_BYTES + umma_b_bytes<BN>()) + UMMA_CONSUMERS * stage_bytes<BN>() +
+         1024 /*alignment slack*/ + UMMA_BAR_BYTES;
 }
 
 // Registers per thread of each warpgroup role (setmaxnreg; multiples of 8 that add up to the launch
 // allocation of 4 x 128).  The producer is one converged warp with a few counters.  A consumer holds
 // BN / 2 accumulator registers (plus, in the halo kernel, two sets of A fragments) and nothing else.
-// The epilogue warpgroup gets the rest: it holds a 64-column row (64 registers), the prefetched ReLU
-// mask and, in the 64-channel halo dgrad, 64 running column sums.
+// The epilogue warpgroup gets the rest: it holds one staged row (64 registers up to BN = 128, 32 at
+// BN = 256), the prefetched ReLU mask and, in the 64-channel halo dgrad, 64 running column sums.
+// At BN = 256 the producer drops to the minimum so that a consumer can hold its 128 accumulator
+// registers with room for descriptors and counters.
 template <int BN>
 struct RoleRegs {
-  static constexpr int PRODUCER = 40;
-  static constexpr int CONSUMER = BN >= 128 ? 152 : 128;
+  static constexpr int PRODUCER = BN >= 256 ? 24 : 40;
+  static constexpr int CONSUMER = BN >= 256 ? 184 : (BN >= 128 ? 152 : 128);
   static constexpr int EPILOGUE = 4 * UMMA_LAUNCH_REGS - PRODUCER - UMMA_CONSUMERS * CONSUMER;
   static_assert(EPILOGUE % 8 == 0 && EPILOGUE >= 24 && EPILOGUE <= 256, "register budgets");
 };
@@ -93,24 +107,26 @@ __device__ __forceinline__ void set_role_regs() {
   else if constexpr (N < UMMA_LAUNCH_REGS) setmaxnreg_dec<N>();
 }
 
-// Accumulator columns [c0, c0 + 64) of a warpgroup (wgmma fragment layout) -> stage[64][STAGE_LD].
+// Accumulator columns [c0, c0 + COLS) of a warpgroup (wgmma fragment layout) -> stage[64][COLS + 4].
 // Fragment: d[i] is row 16 * warp + lane / 4 + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + 2 * (lane & 3) + (i & 1).
-template <int NACC>
+template <int NACC, int COLS>
 __device__ __forceinline__ void stage_acc_chunk(const float (&d)[NACC], int c0, float* stage, int t) {
+  constexpr int LD = COLS + 4;
   const int w = t >> 5, l = t & 31;
   const int r = 16 * w + (l >> 2);
   const int cq = 2 * (l & 3);
 #pragma unroll
   for (int i = 0; i < NACC; i += 4) {
     const int col = 8 * (i >> 2);
-    if (col >= c0 && col < c0 + 64) {
-      *reinterpret_cast<float2*>(stage + r * STAGE_LD + col - c0 + cq) = make_float2(d[i], d[i + 1]);
-      *reinterpret_cast<float2*>(stage + (r + 8) * STAGE_LD + col - c0 + cq) = make_float2(d[i + 2], d[i + 3]);
+    if (col >= c0 && col < c0 + COLS) {
+      *reinterpret_cast<float2*>(stage + r * LD + col - c0 + cq) = make_float2(d[i], d[i + 1]);
+      *reinterpret_cast<float2*>(stage + (r + 8) * LD + col - c0 + cq) = make_float2(d[i + 2], d[i + 3]);
     }
   }
 }
+template <int LD>
 __device__ __forceinline__ void stage_read_row(const float* stage, int row_local, int col, uint32_t (&acc)[32]) {
-  const float4* src = reinterpret_cast<const float4*>(stage + row_local * STAGE_LD + col);
+  const float4* src = reinterpret_cast<const float4*>(stage + row_local * LD + col);
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const float4 v = src[j];
@@ -120,30 +136,35 @@ __device__ __forceinline__ void stage_read_row(const float* stage, int row_local
 }
 
 // Consumer side of the hand-off: warpgroup `cw`'s accumulator into its half of the staging tile,
-// one 64-column chunk after the other.  `eph` counts the chunks handed over (parity of stage_empty).
+// one chunk after the other.  `eph` counts the chunks handed over (parity of stage_empty).
 template <int BN, int TAG>
 __device__ __forceinline__ void stage_put(const float (&d)[BN / 2], float* stage_base, int cw, int t,
                                           uint64_t* stage_full, uint64_t* stage_empty, uint32_t& eph) {
-  float* stage = stage_base + cw * (STAGE_BYTES / 4);
+  constexpr int COLS = stage_cols<BN>();
+  float* stage = stage_base + cw * (stage_bytes<BN>() / 4);
 #pragma unroll
-  for (int c0 = 0; c0 < BN; c0 += 64) {
+  for (int c0 = 0; c0 < BN; c0 += COLS) {
     mbar_wait(stage_empty, eph ^ 1, TAG);     // the epilogue has read the previous chunk
     eph ^= 1;
-    stage_acc_chunk(d, c0, stage, t);
+    stage_acc_chunk<BN / 2, COLS>(d, c0, stage, t);
     __syncwarp();
     if ((t & 31) == 0) mbar_arrive(stage_full);   // one arrival per consumer warp
   }
 }
-// Epilogue side: row t of the staged chunk, both 32-column halves (the second only when the tile
-// is that wide), into registers; then the chunk is released.  `fph` is stage_full's parity.
+// Epilogue side: row t of the staged chunk, in 32-column halves (a 64-column chunk's second half
+// only when the tile is that wide), into registers; then the chunk is released.  `fph` is
+// stage_full's parity.
 template <int BN, int TAG>
 __device__ __forceinline__ void stage_take(const float* stage_base, int c0, int t, uint64_t* stage_full,
-                                           uint64_t* stage_empty, uint32_t& fph, uint32_t (&acc)[2][32]) {
+                                           uint64_t* stage_empty, uint32_t& fph,
+                                           uint32_t (&acc)[stage_cols<BN>() / 32][32]) {
+  constexpr int LD = stage_ld<BN>();
   mbar_wait_outlined_timeout(stage_full, fph, TAG);
   fph ^= 1;
-  const float* stage = stage_base + (t >> 6) * (STAGE_BYTES / 4);
-  stage_read_row(stage, t & 63, 0, acc[0]);
-  if (c0 + 32 < BN) stage_read_row(stage, t & 63, 32, acc[1]);
+  const float* stage = stage_base + (t >> 6) * (stage_bytes<BN>() / 4);
+#pragma unroll
+  for (int h = 0; h < stage_cols<BN>() / 32; ++h)
+    if (c0 + 32 * h < BN) stage_read_row<LD>(stage, t & 63, 32 * h, acc[h]);
   __syncwarp();
   if ((t & 31) == 0) mbar_arrive(stage_empty);    // one arrival per epilogue warp
 }
@@ -167,7 +188,7 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * UMMA_A_BYTES;
   float* stage_base = reinterpret_cast<float*>(sB + STAGES * B_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stage_base) + UMMA_CONSUMERS * STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stage_base) + UMMA_CONSUMERS * stage_bytes<BN>());
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* stage_full = empty_bar + STAGES;
   uint64_t* stage_empty = stage_full + 1;
@@ -233,9 +254,21 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
         const uint64_t bd0 = bd_base + s * (B_BYTES >> 4);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < UMMA_BK / 16; ++k)     // start-address field is in 16-byte units
-          wgmma_ss<P::A_MN ? 1 : 0, P::B_MN ? 1 : 0>(d, ad0 + k * (A_KSTEP >> 4), bd0 + k * (B_KSTEP >> 4),
-                                                     (i | k) != 0 ? 1 : 0);
+        for (int k = 0; k < UMMA_BK / 16; ++k) {   // start-address field is in 16-byte units
+          const uint64_t ad = ad0 + k * (A_KSTEP >> 4), bd = bd0 + k * (B_KSTEP >> 4);
+          const int acc = (i | k) != 0 ? 1 : 0;
+          if constexpr (BN == 256) {
+            // Two m64n128 halves: ptxas needs 154 registers for one m64n256 instruction and checks
+            // that against the 128-register launch allocation, whatever setmaxnreg raised it to.
+            // Columns 128..255 of B start 16 KB in, both K-major (rows) and MN-major (slabs 2, 3);
+            // d[64 + i] is then column 128 + the column of d[i], the m64n256 fragment layout.
+            constexpr uint32_t B_HALF = (128 * 128) >> 4;
+            wgmma_ss<P::A_MN ? 1 : 0, P::B_MN ? 1 : 0>(*reinterpret_cast<float(*)[64]>(d), ad, bd, acc);
+            wgmma_ss<P::A_MN ? 1 : 0, P::B_MN ? 1 : 0>(*reinterpret_cast<float(*)[64]>(d + 64), ad, bd + B_HALF, acc);
+          } else {
+            wgmma_ss<P::A_MN ? 1 : 0, P::B_MN ? 1 : 0>(d, ad, bd, acc);
+          }
+        }
         wgmma_commit();
         wgmma_wait<1>();                      // the previous k-block's wgmmas have retired
         if (i > 0 && t == 0) mbar_arrive(&empty_bar[prev]);
@@ -256,30 +289,33 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
       P::epi_begin(prm, epi_smem, t);
       named_bar_sync(1, UMMA_EPI_THREADS);
     }
+    constexpr int COLS = stage_cols<BN>();
+    constexpr int HALVES = COLS / 32;
     uint32_t fph = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const typename P::Ctx ctx = P::make_ctx(prm, tile);
       if (P::num_k_iters(prm, ctx) == 0) continue;
       const typename P::RowCtx rc = P::row_ctx(prm, ctx, t);
 #pragma unroll
-      for (int c0 = 0; c0 < BN; c0 += 64) {
-        uint32_t acc[2][32];
+      for (int c0 = 0; c0 < BN; c0 += COLS) {
+        uint32_t acc[HALVES][32];
         if constexpr (P::PREMASK) {
           // the mask does not depend on the accumulator: fetch it while the MMAs still run
-          uint32_t pm[2][16];
+          uint32_t pm[HALVES][16];
           const bool masked = P::masked(prm);
           if (masked) {
-            P::load_mask(prm, ctx, rc, c0, pm[0]);
-            if (c0 + 32 < BN) P::load_mask(prm, ctx, rc, c0 + 32, pm[1]);
+#pragma unroll
+            for (int h = 0; h < HALVES; ++h)
+              if (c0 + 32 * h < BN) P::load_mask(prm, ctx, rc, c0 + 32 * h, pm[h]);
           }
           stage_take<BN, 4>(stage_base, c0, t, stage_full, stage_empty, fph, acc);
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+          for (int h = 0; h < HALVES; ++h)
             if (c0 + 32 * h < BN) P::epilogue(prm, ctx, rc, t, c0 + 32 * h, acc[h], epi_smem, pm[h]);
         } else {
           stage_take<BN, 4>(stage_base, c0, t, stage_full, stage_empty, fph, acc);
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+          for (int h = 0; h < HALVES; ++h)
             if (c0 + 32 * h < BN) P::epilogue(prm, ctx, rc, t, c0 + 32 * h, acc[h], epi_smem);
         }
       }

@@ -274,8 +274,9 @@ static void gemm_launch(GemmParams& prm, const bf16* A, long long lda, const bf1
 void gemm_bf16(const bf16* A, long long lda, bool a_mn, const bf16* B, long long ldb, bool b_mn,
                int M, int N, int K, void* out, long long ldo, int epi, const float* bias,
                float alpha, int ksplit, int bn, cudaStream_t stream) {
-  // Tiles are at most 128 wide: a 64 x 256 fp32 accumulator (128 registers per thread) does not fit
-  // a consumer warpgroup's register budget (RoleRegs in umma_core.cuh) next to its descriptors.
+  // Tiles are at most 128 wide here: the FC forward and dgrad have the batch as N (swap-AB), and
+  // the FC wgrad has it as K -- one k-block per tile, bound by storing its output, which a wider
+  // tile does not shorten.  256-wide tiles are built for the convolutions only (conv_bn).
   if (bn == 0) bn = N <= 32 && !b_mn ? 32 : (N <= 64 ? 64 : 128);
   if (ksplit < 1) ksplit = 1;
   GemmParams prm;
@@ -318,10 +319,22 @@ static void conv_launch(ConvParams& prm, cudaStream_t stream) {
   launch<P>(prm, stream);
 }
 
-// Channel tiles are at most 128 wide (see gemm_bf16).
-static int auto_bn(int cn, int bn) {
-  if (bn) return bn;
-  return cn <= 64 ? 64 : 128;
+// Channel-tile width of a convolution with `cn` output channels, from the tile counts at 128 and
+// 256 columns.  A 256-wide tile does twice the work of a 128-wide one but reads the activation tile
+// once instead of twice, and takes 1.67-1.77x as long (the 56^2, 28^2 and 14^2 layers at batch 64,
+// per wave; H100 80GB HBM3, 700 W): 7/4.  It is taken where the number of waves over the SMs times
+// that cost is no worse than at 128 -- at batch 64 on 132 SMs every 56^2 and 28^2 layer, not the
+// 14^2 ones, whose 196 wide tiles take 2 waves x 7/4 against 392 narrow tiles in 3 waves x 1.
+static int conv_bn(int cn, long long tiles128, long long tiles256) {
+  if (cn <= 64) return 64;
+  if (cn < 256) return 128;
+  const long long sms = num_sms();
+  return ((tiles256 + sms - 1) / sms) * 7 <= ((tiles128 + sms - 1) / sms) * 4 ? 256 : 128;
+}
+// The same for fprop / dgrad: the pixel tiles are the same at both widths.
+static int conv_bn_pixels(const ConvTile& t, int cn) {
+  const long long tiles_m = static_cast<long long>(t.tiles_w) * t.tiles_h * ((t.N + t.Nb - 1) / t.Nb);
+  return conv_bn(cn, tiles_m * ((cn + 127) / 128), tiles_m * ((cn + 255) / 256));
 }
 
 static void fprop_impl(const bf16* x, const bf16* w, const float* bias, bf16* y, bf16* pool_out,
@@ -337,22 +350,25 @@ static void fprop_impl(const bf16* x, const bf16* w, const float* bias, bf16* y,
   prm.out = y; prm.bias = bias; prm.mask_src = nullptr; prm.colsum = nullptr;
   prm.pool_out = pool_out; prm.pool_mask = pool_mask;
   prm.flags = (bias ? CONV_BIAS : 0) | (relu ? CONV_RELU : 0) | (pool_out ? CONV_POOL : 0);
-  bn = auto_bn(Cout, bn);
-  prm.resident = 0;
-  map_2d(&prm.mapB, w, Cout, 9LL * Cin, 9LL * Cin, 64, bn);
   const bool pool = pool_out != nullptr;
+  prm.resident = 0;
   if (halo_applicable(H, W)) {
+    if (bn == 0) bn = Cout <= 64 ? 64 : 128;
+    map_2d(&prm.mapB, w, Cout, 9LL * Cin, 9LL * Cin, 64, bn);
     switch (bn) {
       case 64: pool ? conv_halo_launch<64, false, true>(prm, x, stream) : conv_halo_launch<64, false>(prm, x, stream); return;
       case 128: pool ? conv_halo_launch<128, false, true>(prm, x, stream) : conv_halo_launch<128, false>(prm, x, stream); return;
       default: throw std::runtime_error("[b200] conv3x3_fprop: bn must be 64 or 128");
     }
   }
+  if (bn == 0) bn = conv_bn_pixels(prm.t, Cout);
+  map_2d(&prm.mapB, w, Cout, 9LL * Cin, 9LL * Cin, 64, bn);
   map_nhwc(&prm.mapA, x, N, H, W, Cin, prm.t.Wb, prm.t.Hb, prm.t.Nb);
   switch (bn) {
     case 64: pool ? conv_launch<64, false, true>(prm, stream) : conv_launch<64, false>(prm, stream); break;
     case 128: pool ? conv_launch<128, false, true>(prm, stream) : conv_launch<128, false>(prm, stream); break;
-    default: throw std::runtime_error("[b200] conv3x3_fprop: bn must be 64 or 128");
+    case 256: pool ? conv_launch<256, false, true>(prm, stream) : conv_launch<256, false>(prm, stream); break;
+    default: throw std::runtime_error("[b200] conv3x3_fprop: bn must be 64, 128 or 256");
   }
 }
 
@@ -388,21 +404,23 @@ void conv3x3_dgrad(const bf16* dz, const bf16* w, const bf16* mask_src, bf16* dx
   prm.pool_out = nullptr; prm.pool_mask = nullptr;
   prm.flags = (mask_src ? CONV_MASK : 0) | (colsum ? CONV_COLSUM : 0);
   if (colsum && Cin > 512) throw std::runtime_error("[b200] conv3x3_dgrad: fused column sum supports Cin <= 512");
-  bn = auto_bn(Cin, bn);
   prm.resident = 0;
   map_2d(&prm.mapB, w, Cout, 9LL * Cin, 9LL * Cin, 64, 64);   // MN-major: 64 ci x 64 co boxes
   if (halo_applicable(H, W)) {
+    if (bn == 0) bn = Cin <= 64 ? 64 : 128;
     switch (bn) {
       case 64: conv_halo_launch<64, true>(prm, dz, stream); return;
       case 128: conv_halo_launch<128, true>(prm, dz, stream); return;
       default: throw std::runtime_error("[b200] conv3x3_dgrad: bn must be 64 or 128");
     }
   }
+  if (bn == 0) bn = conv_bn_pixels(prm.t, Cin);
   map_nhwc(&prm.mapA, dz, N, H, W, Cout, prm.t.Wb, prm.t.Hb, prm.t.Nb);
   switch (bn) {
     case 64: conv_launch<64, true>(prm, stream); break;
     case 128: conv_launch<128, true>(prm, stream); break;
-    default: throw std::runtime_error("[b200] conv3x3_dgrad: bn must be 64 or 128");
+    case 256: conv_launch<256, true>(prm, stream); break;
+    default: throw std::runtime_error("[b200] conv3x3_dgrad: bn must be 64, 128 or 256");
   }
 }
 
@@ -457,9 +475,11 @@ void conv3x3_wgrad(const bf16* dz, const bf16* x, float* dw, int N, int H, int W
   const int tiles_n = (N + prm.t.Nb - 1) / prm.t.Nb;
   prm.Cout = Cout; prm.Cin = Cin;
   prm.total_tiles = prm.t.tiles_w * prm.t.tiles_h * tiles_n;
-  bn = auto_bn(Cin, bn);
+  // The split is chosen for the width asked for, or for the narrow tile when the width is chosen
+  // here; a 256-wide tile then keeps that split, so it has half as many work items of the same depth.
+  const int split_bn = bn ? bn : (Cin <= 64 ? 64 : 128);
   if (ksplit <= 0) {     // work items of <= ~64 k-blocks (4096 pixels), and at least ~4 per SM
-    const int base = ((Cout + UMMA_BM - 1) / UMMA_BM) * ((Cin + bn - 1) / bn) * 9;
+    const int base = ((Cout + UMMA_BM - 1) / UMMA_BM) * ((Cin + split_bn - 1) / split_bn) * 9;
     ksplit = (prm.total_tiles + 63) / 64;
     const int min_split = (4 * num_sms() + base - 1) / base;
     if (ksplit < min_split) ksplit = min_split;
@@ -467,13 +487,18 @@ void conv3x3_wgrad(const bf16* dz, const bf16* x, float* dw, int N, int H, int W
   if (ksplit > prm.total_tiles) ksplit = prm.total_tiles;
   prm.tiles_per_split = (prm.total_tiles + ksplit - 1) / ksplit;
   prm.ksplit = (prm.total_tiles + prm.tiles_per_split - 1) / prm.tiles_per_split;
+  if (bn == 0) {
+    const long long items = static_cast<long long>((Cout + UMMA_BM - 1) / UMMA_BM) * 9 * prm.ksplit;
+    bn = conv_bn(Cin, items * ((Cin + 127) / 128), items * ((Cin + 255) / 256));
+  }
   prm.dW = dw; prm.scale = scale;
   map_nhwc(&prm.mapA, dz, N, H, W, Cout, prm.t.Wb, prm.t.Hb, prm.t.Nb);
   map_nhwc(&prm.mapB, x, N, H, W, Cin, prm.t.Wb, prm.t.Hb, prm.t.Nb);
   switch (bn) {
     case 64: wgrad_launch<64>(prm, stream); break;
     case 128: wgrad_launch<128>(prm, stream); break;
-    default: throw std::runtime_error("[b200] conv3x3_wgrad: bn must be 64 or 128");
+    case 256: wgrad_launch<256>(prm, stream); break;
+    default: throw std::runtime_error("[b200] conv3x3_wgrad: bn must be 64, 128 or 256");
   }
 }
 
