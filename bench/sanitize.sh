@@ -3,6 +3,9 @@
 # TMA kernels are checked with memcheck + synccheck, the element-wise kernels additionally with
 # racecheck (racecheck does not model async-proxy (TMA / wgmma) shared-memory traffic).
 set -u
+# every test tensor its own allocation: with the caching allocator an overrun lands inside a cached
+# segment that memcheck counts as valid memory
+export PYTORCH_NO_CUDA_MEMORY_CACHING=1
 mkdir -p ${OUT:-prof_out}
 SAN=/usr/local/cuda/bin/compute-sanitizer
 K='gemm_kk and 128-64-64 or gemm_kk and 4096-5-4096 or gemm_mnk and 4096-16-512 or gemm_mnmn_store and 10-4096-5'

@@ -42,6 +42,22 @@ static void gemm(const at::Tensor& A, bool a_mn, const at::Tensor& B, bool b_mn,
                  double alpha, int64_t ksplit, int64_t bn) {
   c10::cuda::CUDAGuard g(A.device());
   TORCH_CHECK(A.dim() == 2 && B.dim() == 2 && A.stride(1) == 1 && B.stride(1) == 1, "gemm: 2-D row-major operands");
+  TORCH_CHECK(epi >= 0 && epi <= 5, "gemm: unknown epilogue ", epi);
+  TORCH_CHECK(M > 0 && N > 0 && K > 0, "gemm: M, N and K must be positive");
+  // the tensor maps span the operand's own rows and columns: A is [M][K] or [K][M] (a_mn), B [N][K] or [K][N]
+  TORCH_CHECK(A.size(0) >= (a_mn ? K : M) && A.size(1) >= (a_mn ? M : K), "gemm: A must be at least ",
+              a_mn ? "[K, M]" : "[M, K]", ", got ", A.sizes());
+  TORCH_CHECK(B.size(0) >= (b_mn ? K : N) && B.size(1) >= (b_mn ? N : K), "gemm: B must be at least ",
+              b_mn ? "[K, N]" : "[N, K]", ", got ", B.sizes());
+  // the epilogue writes rows x cols elements at row stride ldo: [M][N], or [N][M] for the transposed ones
+  const bool bf_out = epi == 3 || epi == 5, t_out = epi == 2 || epi == 4;
+  const int64_t rows = t_out ? N : M, cols = t_out ? M : N;
+  TORCH_CHECK(out.is_cuda() && out.is_contiguous() && out.scalar_type() == (bf_out ? at::kBFloat16 : at::kFloat),
+              "gemm: out must be a contiguous ", bf_out ? "bf16" : "fp32", " tensor for this epilogue");
+  TORCH_CHECK(ldo >= cols && out.numel() >= (rows - 1) * ldo + cols, "gemm: out must hold ", rows, " rows of ",
+              cols, " elements at ldo = ", ldo, ", got ", out.numel(), " elements");
+  TORCH_CHECK(epi != 3 || bias.has_value(), "gemm: the bias + ReLU epilogue needs a bias");
+  TORCH_CHECK(!bias.has_value() || bias->numel() >= N, "gemm: bias must have N = ", N, " elements");
   b200::gemm_bf16(bfp(A), A.stride(0), a_mn, bfp(B), B.stride(0), b_mn, (int)M, (int)N, (int)K, out.data_ptr(),
                   ldo, (int)epi, f32p_opt(bias), (float)alpha, (int)ksplit, (int)bn, cur_stream());
 }
@@ -52,6 +68,7 @@ static void conv_fprop(const at::Tensor& x, const at::Tensor& w, c10::optional<a
   TORCH_CHECK(x.dim() == 4 && x.is_contiguous() && w.is_contiguous() && y.is_contiguous(), "conv_fprop: contiguous NHWC");
   const int N = x.size(0), H = x.size(1), W = x.size(2), Cin = x.size(3), Cout = w.size(0);
   TORCH_CHECK(w.numel() == (int64_t)Cout * 9 * Cin && y.numel() == (int64_t)N * H * W * Cout, "conv_fprop: shape mismatch");
+  TORCH_CHECK(!bias.has_value() || bias->numel() >= Cout, "conv_fprop: bias must have Cout = ", Cout, " elements");
   b200::conv3x3_fprop(bfp(x), bfp(w), f32p_opt(bias), bfp_mut(y), N, H, W, Cin, Cout, relu, (int)bn, cur_stream());
 }
 // Fused conv + pool (default; B200_FUSE_POOL=0 turns it off): pooled activation + int32 mask words [N,H/2,W/2,Cout/32,4]
@@ -66,6 +83,7 @@ static void conv_fprop_pool(const at::Tensor& x, const at::Tensor& w, c10::optio
               "conv_fprop_pool: shape mismatch");
   TORCH_CHECK(mask.scalar_type() == at::kInt && mask.numel() == (int64_t)N * (H / 2) * (W / 2) * (Cout / 32) * 4,
               "conv_fprop_pool: mask must be int32 [N,H/2,W/2,Cout/32,4]");
+  TORCH_CHECK(!bias.has_value() || bias->numel() >= Cout, "conv_fprop_pool: bias must have Cout = ", Cout, " elements");
   b200::conv3x3_fprop_pool(bfp(x), bfp(w), f32p_opt(bias), bfp_mut(pooled),
                            reinterpret_cast<uint32_t*>(mask.data_ptr<int>()), N, H, W, Cin, Cout, (int)bn, cur_stream());
 }
@@ -89,6 +107,12 @@ static void conv_dgrad(const at::Tensor& dz, const at::Tensor& w, c10::optional<
   TORCH_CHECK(dz.dim() == 4 && dz.is_contiguous() && w.is_contiguous() && dx.is_contiguous(), "conv_dgrad: contiguous NHWC");
   const int N = dz.size(0), H = dz.size(1), W = dz.size(2), Cout = dz.size(3), Cin = dx.size(3);
   TORCH_CHECK(w.numel() == (int64_t)Cout * 9 * Cin, "conv_dgrad: weight shape mismatch");
+  check_nhwc(dx, N, H, W, Cin, "conv_dgrad", "dx");
+  if (mask.has_value()) {
+    TORCH_CHECK(mask->is_contiguous(), "conv_dgrad: mask_src must be contiguous");
+    check_nhwc(*mask, N, H, W, Cin, "conv_dgrad", "mask_src");
+  }
+  TORCH_CHECK(!colsum.has_value() || colsum->numel() >= Cin, "conv_dgrad: colsum must have Cin = ", Cin, " elements");
   b200::conv3x3_dgrad(bfp(dz), bfp(w), bfp_opt(mask), bfp_mut(dx), f32p_opt(colsum), N, H, W, Cin, Cout, (int)bn, cur_stream());
 }
 static void conv_wgrad(const at::Tensor& dz, const at::Tensor& x, at::Tensor dw, double scale, int64_t ksplit,
@@ -96,7 +120,8 @@ static void conv_wgrad(const at::Tensor& dz, const at::Tensor& x, at::Tensor dw,
   c10::cuda::CUDAGuard g(dz.device());
   TORCH_CHECK(dz.dim() == 4 && dz.is_contiguous() && x.is_contiguous(), "conv_wgrad: contiguous NHWC");
   const int N = dz.size(0), H = dz.size(1), W = dz.size(2), Cout = dz.size(3), Cin = x.size(3);
-  TORCH_CHECK(dw.numel() == (int64_t)Cout * 9 * Cin, "conv_wgrad: dw shape mismatch");
+  TORCH_CHECK(dw.numel() == (int64_t)Cout * 9 * Cin && dw.is_contiguous(), "conv_wgrad: dw shape mismatch");
+  check_nhwc(x, N, H, W, Cin, "conv_wgrad", "x");
   b200::conv3x3_wgrad(bfp(dz), bfp(x), f32p(dw), N, H, W, Cin, Cout, (float)scale, (int)ksplit, (int)bn, cur_stream());
 }
 
@@ -104,12 +129,17 @@ static void conv0_fprop(const at::Tensor& x4, const at::Tensor& w0, const at::Te
   c10::cuda::CUDAGuard g(x4.device());
   TORCH_CHECK(x4.dim() == 4 && x4.size(3) == 4 && x4.is_contiguous() && w0.numel() == 64 * 64 && y.is_contiguous(),
               "conv0_fprop: x4 [N,H,W,4], w0 [64,64]");
+  TORCH_CHECK(w0.is_contiguous(), "conv0_fprop: w0 must be contiguous");
+  check_nhwc(y, x4.size(0), x4.size(1), x4.size(2), 64, "conv0_fprop", "y");
+  TORCH_CHECK(bias.numel() >= 64, "conv0_fprop: bias must have 64 elements");
   b200::conv0_fprop(bfp(x4), bfp(w0), f32p(bias), bfp_mut(y), x4.size(0), x4.size(1), x4.size(2), cur_stream());
 }
 static void conv0_wgrad(const at::Tensor& dz, const at::Tensor& x4, at::Tensor dw0) {
   c10::cuda::CUDAGuard g(x4.device());
   TORCH_CHECK(x4.dim() == 4 && x4.size(3) == 4 && x4.is_contiguous() && dz.is_contiguous() && dw0.numel() == 64 * 64,
               "conv0_wgrad: x4 [N,H,W,4], dw0 [64,64]");
+  TORCH_CHECK(dw0.is_contiguous(), "conv0_wgrad: dw0 must be contiguous");
+  check_nhwc(dz, x4.size(0), x4.size(1), x4.size(2), 64, "conv0_wgrad", "dz");
   b200::conv0_wgrad(bfp(dz), bfp(x4), f32p(dw0), x4.size(0), x4.size(1), x4.size(2), cur_stream());
 }
 
@@ -204,6 +234,15 @@ static void cross_entropy(const at::Tensor& logits, const at::Tensor& target, c1
                           double grad_scale, c10::optional<at::Tensor> class_weights) {
   c10::cuda::CUDAGuard g(logits.device());
   TORCH_CHECK(target.scalar_type() == at::kLong && logits.is_contiguous(), "cross_entropy: int64 targets, contiguous logits");
+  TORCH_CHECK(logits.dim() == 2, "cross_entropy: logits must be [B, C]");
+  const int64_t B = logits.size(0), C = logits.size(1);
+  TORCH_CHECK(target.is_contiguous() && target.numel() >= B, "cross_entropy: contiguous targets of B = ", B);
+  if (dlogits.has_value())
+    TORCH_CHECK(ldd >= C && dlogits->is_contiguous() && dlogits->numel() >= B * ldd,
+                "cross_entropy: dlogits must be contiguous, ldd >= C and at least B x ldd elements");
+  TORCH_CHECK(!meter.has_value() || meter->numel() >= 3, "cross_entropy: meter must have 3 elements");
+  TORCH_CHECK(!loss_out.has_value() || loss_out->numel() >= 1, "cross_entropy: loss_out must have 1 element");
+  TORCH_CHECK(!class_weights.has_value() || class_weights->numel() >= C, "cross_entropy: class_weights of C = ", C);
   b200::cross_entropy_fused(f32p(logits), reinterpret_cast<const long long*>(target.data_ptr()),
                             dlogits.has_value() ? bfp_mut(*dlogits) : nullptr, (int)ldd, f32p_opt(meter),
                             f32p_opt(loss_out), (int)logits.size(0), (int)logits.size(1), (float)grad_scale,
@@ -253,12 +292,26 @@ static void augment(const at::Tensor& src, const at::Tensor& params, at::Tensor 
   c10::cuda::CUDAGuard g(src.device());
   TORCH_CHECK(src.is_cuda() && src.scalar_type() == at::kByte && src.is_contiguous() && src.dim() == 4 && src.size(3) == 3,
               "augment: uint8 [N,H,W,3] CUDA tensor");
+  const int64_t N = src.size(0);
+  TORCH_CHECK(params.is_contiguous() && params.dim() == 2 && params.size(0) >= N && params.size(1) == 8,
+              "augment: params must be contiguous [N, 8]");
+  TORCH_CHECK(mode == 0 || mode == 1, "augment: mode is 0 (NHWC) or 1 (im2col)");
+  TORCH_CHECK(OH > 0 && OW > 0 && mean.size() == 3 && stdv.size() == 3, "augment: OH, OW > 0, 3 means and deviations");
+  // mode 0 writes 3 channels and zeros up to pad (one 8-byte store at pad = 4); mode 1 16-byte stores of pad-wide rows
+  TORCH_CHECK(mode == 1 || pad >= 3, "augment: NHWC pad must be >= 3");
+  check_vec(out, at::kBFloat16, mode == 1 ? 16 : (pad == 4 ? 8 : 2), "augment", "out");
+  TORCH_CHECK(out.numel() >= N * OH * OW * pad, "augment: out must hold N x OH x OW x pad elements");
   float m[3] = {(float)mean[0], (float)mean[1], (float)mean[2]}, s[3] = {(float)stdv[0], (float)stdv[1], (float)stdv[2]};
   b200::augment_fused(src.data_ptr<uint8_t>(), f32p(params), bfp_mut(out), src.size(0), src.size(1), src.size(2),
                       (int)RH, (int)RW, (int)OH, (int)OW, (int)mode, (int)pad, m, s, cur_stream());
 }
 static void im2col_c3(const at::Tensor& x, at::Tensor out, int64_t kpad) {
   c10::cuda::CUDAGuard g(x.device());
+  check_vec(x, at::kBFloat16, 8, "im2col_c3", "x");
+  check_vec(out, at::kBFloat16, 16, "im2col_c3", "out");
+  TORCH_CHECK(x.dim() == 4 && x.size(3) == 4, "im2col_c3: x must be [N, H, W, 4]");
+  TORCH_CHECK(kpad >= 32 && kpad % 8 == 0 && out.numel() >= x.size(0) * x.size(1) * x.size(2) * kpad,
+              "im2col_c3: kpad a multiple of 8 >= 32, out of N x H x W x kpad elements");
   b200::im2col3x3_c3(bfp(x), bfp_mut(out), x.size(0), x.size(1), x.size(2), x.size(3), (int)kpad, cur_stream());
 }
 static void nchw_to_nhwc(const at::Tensor& x, at::Tensor y) {
@@ -447,6 +500,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(dW.has_value() == db.has_value(), "head_ce: dW and db come together");
     // dh keeps only the elements with h > 0: that is the dropout mask only after a ReLU
     TORCH_CHECK(relu || drop_scale == 1.0, "head_ce: dropout without ReLU is not supported");
+    const int64_t B = h.size(0), C = W.size(0), K = h.size(1);
+    TORCH_CHECK(target.is_contiguous() && target.numel() >= B, "head_ce: contiguous targets of B = ", B);
+    TORCH_CHECK(bias.numel() >= C, "head_ce: bias must have C = ", C, " elements");
+    if (dlogits.has_value())
+      TORCH_CHECK(ldd >= C && dlogits->is_contiguous() && dlogits->numel() >= B * ldd,
+                  "head_ce: dlogits must be contiguous, ldd >= C and at least B x ldd elements");
+    TORCH_CHECK(!dW.has_value() || (dW->is_contiguous() && dW->numel() >= C * K), "head_ce: contiguous dW of C x K");
+    TORCH_CHECK(!db.has_value() || db->numel() >= C, "head_ce: db must have C elements");
+    TORCH_CHECK(!dh.has_value() || (dh->is_contiguous() && dh->numel() >= B * K), "head_ce: contiguous dh of B x K");
+    TORCH_CHECK(!meter.has_value() || meter->numel() >= 3, "head_ce: meter must have 3 elements");
+    TORCH_CHECK(!loss_out.has_value() || loss_out->numel() >= 1, "head_ce: loss_out must have 1 element");
+    TORCH_CHECK(!class_weights.has_value() || class_weights->numel() >= C, "head_ce: class_weights of C = ", C);
     b200::head_ce_fused(bfp(h), bfp(W), f32p(bias), reinterpret_cast<const long long*>(target.data_ptr()), f32p(logits),
                         dlogits.has_value() ? bfp_mut(*dlogits) : nullptr, (int)ldd, f32p_opt(dW), f32p_opt(db),
                         dh.has_value() ? bfp_mut(*dh) : nullptr, (float)drop_scale, relu, f32p_opt(meter),

@@ -396,7 +396,21 @@ def _misaligned(shape, dtype, by=1):
 def _refusals():
     bf, f = torch.bfloat16, torch.float32
     z = lambda *s, dt=bf: torch.zeros(*s, dtype=dt, device=DEV)       # noqa: E731
+    lz = lambda n: torch.zeros(n, dtype=torch.long, device=DEV)       # noqa: E731
     C = _C()
+
+    def head(target=None, bias=None, ldd=8, dl=None, dW=None, db=None, dh=None, meter=None, cw=None):
+        """A valid head_ce call (B 4, C 3, K 32) with one argument replaced."""
+        return C.head_ce(z(4, 32), z(3, 32), z(3, dt=f) if bias is None else bias, lz(4) if target is None else target,
+                         z(4, 3, dt=f), z(4, 8) if dl is None else dl, ldd, z(3, 32, dt=f) if dW is None else dW,
+                         z(3, dt=f) if db is None else db, z(4, 32) if dh is None else dh, 1.0, True,
+                         z(4, dt=f) if meter is None else meter, None, cw)
+
+    def aug(params=None, out=None, pad=4):
+        """A valid NHWC augment call (2 images of 16 x 16 to 8 x 8) with one argument replaced."""
+        return C.augment(torch.zeros(2, 16, 16, 3, dtype=torch.uint8, device=DEV),
+                         z(2, 8, dt=f) if params is None else params, z(2, 8, 8, 4) if out is None else out,
+                         16, 16, 8, 8, 0, pad, [0.5] * 3, [0.5] * 3)
     return {
         "fc_grad_act dropout without relu": lambda: C.fc_grad_act(z(4, 8, dt=f), None, z(4, 8), 4, 8, False, 0.5, True),
         "head_ce dropout without relu": lambda: C.head_ce(z(4, 32), z(3, 32), z(3, dt=f),
@@ -428,6 +442,60 @@ def _refusals():
         "cast_to_bf16 misaligned": lambda: C.cast_to_bf16(_misaligned((64,), f), z(64)),
         "cast_to_bf16 size": lambda: C.cast_to_bf16(z(64, dt=f), z(60)),
         "nchw_to_nhwc shape": lambda: C.nchw_to_nhwc(z(2, 3, 8, 8, dt=f), z(2, 8, 4, 4)),
+        # wgmma entry points: operand extents against M / N / K, ldo and the epilogue
+        "gemm short A": lambda: C.gemm(z(8, 64), False, z(16, 64), False, 16, 16, 64, z(16, 16, dt=f), 16, 0, None,
+                                       1.0, 1, 0),
+        "gemm short B": lambda: C.gemm(z(16, 64), False, z(8, 64), False, 16, 16, 64, z(16, 16, dt=f), 16, 0, None,
+                                       1.0, 1, 0),
+        "gemm out dtype": lambda: C.gemm(z(16, 64), False, z(16, 64), False, 16, 16, 64, z(16, 16), 16, 0, None,
+                                         1.0, 1, 0),
+        "gemm short out": lambda: C.gemm(z(16, 64), False, z(16, 64), False, 16, 16, 64, z(15, 16, dt=f), 16, 0,
+                                         None, 1.0, 1, 0),
+        "gemm ldo": lambda: C.gemm(z(16, 64), False, z(16, 64), False, 16, 16, 64, z(16, 16, dt=f), 8, 0, None,
+                                   1.0, 1, 0),
+        "gemm short bias": lambda: C.gemm(z(16, 64), False, z(16, 64), False, 16, 16, 64, z(16, 16), 16, 3,
+                                          z(8, dt=f), 1.0, 1, 0),
+        "gemm missing bias": lambda: C.gemm(z(16, 64), False, z(16, 64), False, 16, 16, 64, z(16, 16), 16, 3, None,
+                                            1.0, 1, 0),
+        "conv_fprop short bias": lambda: C.conv_fprop(z(1, 8, 8, 64), z(64, 3, 3, 64), z(32, dt=f), z(1, 8, 8, 64),
+                                                      True, 0),
+        "conv_fprop_pool short bias": lambda: C.conv_fprop_pool(z(1, 8, 8, 64), z(64, 3, 3, 64), z(32, dt=f),
+                                                                z(1, 4, 4, 64), z(1, 4, 4, 2, 4, dt=torch.int32), 0),
+        "conv_dgrad dx shape": lambda: C.conv_dgrad(z(1, 8, 8, 64), z(64, 3, 3, 64), None, z(1, 8, 4, 64), None, 0),
+        "conv_dgrad mask shape": lambda: C.conv_dgrad(z(1, 8, 8, 64), z(64, 3, 3, 64), z(1, 4, 8, 64),
+                                                      z(1, 8, 8, 64), None, 0),
+        "conv_dgrad short colsum": lambda: C.conv_dgrad(z(1, 8, 8, 64), z(64, 3, 3, 64), None, z(1, 8, 8, 64),
+                                                        z(32, dt=f), 0),
+        "conv_wgrad x shape": lambda: C.conv_wgrad(z(1, 8, 8, 64), z(1, 4, 8, 64), z(64, 3, 3, 64, dt=f), 1.0, 0, 0),
+        "conv0_fprop y shape": lambda: C.conv0_fprop(z(1, 8, 8, 4), z(64, 64), z(64, dt=f), z(1, 8, 4, 64)),
+        "conv0_fprop short bias": lambda: C.conv0_fprop(z(1, 8, 8, 4), z(64, 64), z(32, dt=f), z(1, 8, 8, 64)),
+        "conv0_wgrad dz shape": lambda: C.conv0_wgrad(z(1, 8, 4, 64), z(1, 8, 8, 4), z(64, 64, dt=f)),
+        # loss kernels: targets, dlogits and the optional outputs against B, C and ldd
+        "cross_entropy short targets": lambda: C.cross_entropy(z(4, 3, dt=f), lz(2), z(4, 8), 8, None, None, 0.25,
+                                                               None),
+        "cross_entropy ldd < C": lambda: C.cross_entropy(z(4, 3, dt=f), lz(4), z(4, 8), 2, None, None, 0.25, None),
+        "cross_entropy short dlogits": lambda: C.cross_entropy(z(4, 3, dt=f), lz(4), z(2, 8), 8, None, None, 0.25,
+                                                               None),
+        "cross_entropy short meter": lambda: C.cross_entropy(z(4, 3, dt=f), lz(4), None, 0, z(2, dt=f), None, 0.25,
+                                                             None),
+        "cross_entropy short class_weights": lambda: C.cross_entropy(z(4, 3, dt=f), lz(4), None, 0, None, None,
+                                                                     0.25, z(2, dt=f)),
+        "head_ce short targets": lambda: head(target=lz(2)),
+        "head_ce short bias": lambda: head(bias=z(2, dt=f)),
+        "head_ce ldd < C": lambda: head(ldd=2),
+        "head_ce short dlogits": lambda: head(dl=z(2, 8)),
+        "head_ce short dW": lambda: head(dW=z(2, 32, dt=f)),
+        "head_ce short db": lambda: head(db=z(2, dt=f)),
+        "head_ce short dh": lambda: head(dh=z(2, 32)),
+        "head_ce short meter": lambda: head(meter=z(2, dt=f)),
+        "head_ce short class_weights": lambda: head(cw=z(2, dt=f)),
+        # input kernels
+        "augment params shape": lambda: aug(params=z(2, 7, dt=f)),
+        "augment short params": lambda: aug(params=z(1, 8, dt=f)),
+        "augment short out": lambda: aug(out=z(1, 8, 8, 4)),
+        "augment pad < 3": lambda: aug(out=z(2, 8, 8, 2), pad=2),
+        "im2col_c3 short out": lambda: C.im2col_c3(z(2, 8, 8, 4), z(64, 64), 64),
+        "im2col_c3 x channels": lambda: C.im2col_c3(z(2, 8, 8, 3), z(128, 64), 64),
     }
 
 
@@ -436,7 +504,16 @@ REFUSALS = ["fc_grad_act dropout without relu", "head_ce dropout without relu", 
             "maxpool_relu_bwd dtype", "avgpool_fwd batch", "avgpool_bwd mismatch", "avgpool_bwd non-contiguous",
             "bias_grad misaligned", "bias_grad short dz", "adam misaligned", "adam size", "adam dtype",
             "adam non-contiguous", "sgd misaligned shadow", "sgd size", "cast_to_bf16 misaligned",
-            "cast_to_bf16 size", "nchw_to_nhwc shape"]
+            "cast_to_bf16 size", "nchw_to_nhwc shape",
+            "gemm short A", "gemm short B", "gemm out dtype", "gemm short out", "gemm ldo", "gemm short bias",
+            "gemm missing bias", "conv_fprop short bias", "conv_fprop_pool short bias", "conv_dgrad dx shape",
+            "conv_dgrad mask shape", "conv_dgrad short colsum", "conv_wgrad x shape", "conv0_fprop y shape",
+            "conv0_fprop short bias", "conv0_wgrad dz shape", "cross_entropy short targets", "cross_entropy ldd < C",
+            "cross_entropy short dlogits", "cross_entropy short meter", "cross_entropy short class_weights",
+            "head_ce short targets", "head_ce short bias", "head_ce ldd < C", "head_ce short dlogits",
+            "head_ce short dW", "head_ce short db", "head_ce short dh", "head_ce short meter",
+            "head_ce short class_weights", "augment params shape", "augment short params", "augment short out",
+            "augment pad < 3", "im2col_c3 short out", "im2col_c3 x channels"]
 
 
 @pytest.mark.parametrize("case", REFUSALS)

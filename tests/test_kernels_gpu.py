@@ -40,11 +40,13 @@ def _rup8(v):
 
 
 # ------------------------------------------------------------------------------------------ GEMM
-GEMM_KK = pytest.mark.parametrize("M,N,K", [
+GEMM_KK_SHAPES = [
     (128, 64, 64), (256, 64, 512), (4096, 64, 4096), (200, 48, 200), (4096, 96, 25088 // 8),
     # N <= 32: 32-wide tiles (FC forward at batch <= 32, ragged last batches)
-    (4096, 1, 25088), (4096, 5, 4096), (512, 16, 4096), (4096, 32, 25088), (10, 37, 512)])
-KSPLIT = pytest.mark.parametrize("ksplit", [1, 4, 8])
+    (4096, 1, 25088), (4096, 5, 4096), (512, 16, 4096), (4096, 32, 25088), (10, 37, 512)]
+GEMM_KK = pytest.mark.parametrize("M,N,K", GEMM_KK_SHAPES)
+KSPLITS = [1, 4, 8]
+KSPLIT = pytest.mark.parametrize("ksplit", KSPLITS)
 
 
 @GEMM_KK
@@ -72,8 +74,8 @@ def _gemm_kk(M, N, K, ksplit, mode):
     KC.check(out, ref, mag, chain=KC.gemm_chain(K, ksplit), exact=mode == "exact", family="gemm")
 
 
-GEMM_MNK = pytest.mark.parametrize("M,N,K", [(128, 64, 64), (25088 // 4, 64, 4096), (300, 40, 130),
-                                                (4096, 32, 4096), (512, 3, 10)])
+GEMM_MNK_SHAPES = [(128, 64, 64), (25088 // 4, 64, 4096), (300, 40, 130), (4096, 32, 4096), (512, 3, 10)]
+GEMM_MNK = pytest.mark.parametrize("M,N,K", GEMM_MNK_SHAPES)
 
 
 @GEMM_MNK
@@ -88,9 +90,12 @@ def test_gemm_mnk_store_t_exact(M, N, K):
     _gemm_mnk(M, N, K, 1, "f32_store_t", "exact")
 
 
+GEMM_MNK_ATOMIC = [(4096, 64, 4096, 8), (4096, 37, 4096, 8), (4096, 16, 512, 8), (25088, 5, 4096, 8),
+                   (4096, 64, 4096, 1), (512, 10, 10, 1)]
+
+
 @pytest.mark.parametrize("mode", MODES)
-@pytest.mark.parametrize("M,N,K,ksplit", [(4096, 64, 4096, 8), (4096, 37, 4096, 8), (4096, 16, 512, 8),
-                                          (25088, 5, 4096, 8), (4096, 64, 4096, 1), (512, 10, 10, 1)])
+@pytest.mark.parametrize("M,N,K,ksplit", GEMM_MNK_ATOMIC)
 def test_gemm_mnk_atomic_t(M, N, K, ksplit, mode):
     """FC dgrad as the engine runs it: M = fin, N = batch, K = fout, split-K into the atomic epilogue."""
     _gemm_mnk(M, N, K, ksplit, "f32_atomic_t", mode)
@@ -134,9 +139,10 @@ def _gemm_mnmn(M, N, K, mode):
     KC.check(out, ref, mag, chain=KC.gemm_chain(K), exact=mode == "exact", family="gemm")
 
 
-GEMM_MNMN_BF16 = pytest.mark.parametrize("M,N,K,off", [
+GEMM_MNMN_BF16_SHAPES = [
     (128, 64, 64, 0), (4096, 1024, 64, 0), (512, 256, 96, 8), (256, 72, 64, 0), (24, 512, 64, 4),
-    (10, 4096, 5, 0), (10, 4096, 37, 8), (1000, 4096, 16, 0), (4096, 512, 37, 4)])
+    (10, 4096, 5, 0), (10, 4096, 37, 8), (1000, 4096, 16, 0), (4096, 512, 37, 4)]
+GEMM_MNMN_BF16 = pytest.mark.parametrize("M,N,K,off", GEMM_MNMN_BF16_SHAPES)
 
 
 @GEMM_MNMN_BF16
@@ -169,8 +175,11 @@ def test_gemm_bf16_bias_relu():
     _gemm_bias_relu(1000, 64, 64, "gauss")
 
 
+BIAS_RELU_SHAPES = [(1000, 64, 64), (300, 48, 64), (129, 96, 128)]
+
+
 @pytest.mark.parametrize("mode", MODES)
-@pytest.mark.parametrize("M,N,K", [(1000, 64, 64), (300, 48, 64), (129, 96, 128)])
+@pytest.mark.parametrize("M,N,K", BIAS_RELU_SHAPES)
 def test_gemm_bf16_bias_relu_ragged_n(M, N, K, mode):
     """A ragged N (48, 96) must write nothing past column N of a row nor past the end of the output,
     and read no bias past N (the bias is a slice of a NaN-filled buffer)."""
@@ -300,7 +309,8 @@ def _conv_wgrad(N, H, W, Cin, Cout, mode):
              family="conv_wgrad")
 
 
-CONV0 = pytest.mark.parametrize("N,H,W", [(2, 16, 16), (1, 30, 22), (3, 64, 64), (64, 224, 224), (37, 224, 224)])
+CONV0_SHAPES = [(2, 16, 16), (1, 30, 22), (3, 64, 64), (64, 224, 224), (37, 224, 224)]
+CONV0 = pytest.mark.parametrize("N,H,W", CONV0_SHAPES)
 
 
 @CONV0
