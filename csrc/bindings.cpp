@@ -491,7 +491,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                       at::Tensor logits, c10::optional<at::Tensor> dlogits, int64_t ldd, c10::optional<at::Tensor> dW,
                       c10::optional<at::Tensor> db, c10::optional<at::Tensor> dh, double drop_scale, bool relu,
                       c10::optional<at::Tensor> meter, c10::optional<at::Tensor> loss_out,
-                      c10::optional<at::Tensor> class_weights) {
+                      c10::optional<at::Tensor> class_weights, bool accumulate) {
     c10::cuda::CUDAGuard g(h.device());
     TORCH_CHECK(h.dim() == 2 && W.dim() == 2 && h.size(1) == W.size(1) && h.is_contiguous() && W.is_contiguous(),
                 "head_ce: h [B][K], W [C][K], contiguous");
@@ -516,8 +516,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                         dlogits.has_value() ? bfp_mut(*dlogits) : nullptr, (int)ldd, f32p_opt(dW), f32p_opt(db),
                         dh.has_value() ? bfp_mut(*dh) : nullptr, (float)drop_scale, relu, f32p_opt(meter),
                         f32p_opt(loss_out), (int)h.size(0), (int)W.size(0), (int)h.size(1), f32p_opt(class_weights),
-                        cur_stream());
-  });
+                        accumulate, cur_stream());
+  },
+  // accumulate: dW += the batch's gradient instead of dW = (later micro-batches of an accumulation group)
+  py::arg("h"), py::arg("W"), py::arg("bias"), py::arg("target"), py::arg("logits"), py::arg("dlogits"), py::arg("ldd"),
+  py::arg("dW"), py::arg("db"), py::arg("dh"), py::arg("drop_scale"), py::arg("relu"), py::arg("meter"),
+  py::arg("loss_out"), py::arg("class_weights"), py::arg("accumulate") = false);
   m.def("adam", &adam);
   m.def("sgd", &sgd);
   m.def("augment", &augment);

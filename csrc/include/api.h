@@ -95,12 +95,13 @@ void cross_entropy_fused(const float* logits, const long long* target, bf16* dlo
 // K-FUN2+CE: last Linear(K -> C) + cross-entropy + metrics + the layer's whole backward in one launch
 // (C <= 8, K <= 1024, B <= 256).  h [B][K] bf16 (the previous FC layer's output), W [C][K] bf16.
 // Writes logits [B][C] fp32, meter / loss_out as cross_entropy_fused, optional dlogits (bf16, ld ldd);
-// with dW != nullptr also dW [C][K] (fp32, stored), db [C] (fp32, accumulated) and
+// with dW != nullptr also dW [C][K] (fp32, stored; added to with `accumulate`), db [C] (fp32, accumulated) and
 // dh [B][K] = (h > 0 or !relu) * drop_scale * dlogits W  (bf16: the previous layer's dz).
 bool head_ce_supported(int B, int C, int K);
 void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long long* target, float* logits,
                    bf16* dlogits, int ldd, float* dW, float* db, bf16* dh, float drop_scale, bool relu, float* meter,
-                   float* loss_out, int B, int C, int K, const float* class_weights, cudaStream_t s);
+                   float* loss_out, int B, int C, int K, const float* class_weights, bool accumulate,
+                   cudaStream_t s);
 
 // Fused optimizers over flat arenas.  grad is fp32 (local) or bf16 (the reduced wire buffer).
 void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16, bf16* shadow,

@@ -104,7 +104,7 @@ void cross_entropy_fused(const float* logits, const long long* target, bf16* dlo
 // in shared memory / registers:
 //   logits[r][c] = bias[c] + sum_k h[r][k] W[c][k]            (warp per row, fp32 accumulation)
 //   loss, argmax == target count, B  -> device meter;  dlogits = (softmax - onehot) * w / norm -> bf16
-//   db[c] += sum_r dl[r][c];  dW[c][k] = sum_r dl[r][c] h[r][k];                (thread per k)
+//   db[c] += sum_r dl[r][c];  dW[c][k] = sum_r dl[r][c] h[r][k]  (+= with accumulate) (thread per k)
 //   dh[r][k] = (h[r][k] > 0) * drop_scale * sum_c dl[r][c] W[c][k]  -> bf16     (previous layer's dz)
 // Rounding points are those of the unfused path: dlogits are rounded to bf16 before they are used.
 constexpr int HEAD_MAXC = 8, HEAD_MAXK = 1024, HEAD_MAXB = 256, HEAD_THREADS = 512;
@@ -114,7 +114,7 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
                const long long* __restrict__ target, float* __restrict__ logits, bf16* __restrict__ dlogits, int ldd,
                float* __restrict__ dW, float* __restrict__ db, bf16* __restrict__ dh, float drop_scale, int relu,
                float* __restrict__ meter, float* __restrict__ loss_out, int B, int C, int K,
-               const float* __restrict__ cw) {
+               const float* __restrict__ cw, int accumulate) {
   __shared__ float sW[HEAD_MAXC * HEAD_MAXK];
   __shared__ float sdl[HEAD_MAXB * HEAD_MAXC];
   __shared__ float s_loss[32], s_correct[32], s_wsum[32];
@@ -227,9 +227,13 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
         }
       if (dh) dh[static_cast<long long>(r) * K + k] = __float2bfloat16((!relu || hv > 0.f) ? dx * drop_scale : 0.f);
     }
+    // accumulate: a later micro-batch of a gradient-accumulation group adds to the group's dW
 #pragma unroll
     for (int c = 0; c < HEAD_MAXC; ++c)
-      if (c < C) dW[static_cast<long long>(c) * K + k] = gw[c];
+      if (c < C) {
+        float* o = dW + static_cast<long long>(c) * K + k;
+        *o = accumulate ? *o + gw[c] : gw[c];
+      }
   }
 }
 
@@ -237,11 +241,13 @@ bool head_ce_supported(int B, int C, int K) { return C <= HEAD_MAXC && K <= HEAD
 
 void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long long* target, float* logits,
                    bf16* dlogits, int ldd, float* dW, float* db, bf16* dh, float drop_scale, bool relu, float* meter,
-                   float* loss_out, int B, int C, int K, const float* class_weights, cudaStream_t s) {
+                   float* loss_out, int B, int C, int K, const float* class_weights, bool accumulate,
+                   cudaStream_t s) {
   if (!head_ce_supported(B, C, K)) throw std::runtime_error("[b200] head_ce_fused: needs C <= 8, K <= 1024, B <= 256");
   if (ldd > 32) throw std::runtime_error("[b200] head_ce_fused: dlogits row stride must be <= 32");
   head_ce_kernel<<<1, HEAD_THREADS, 0, s>>>(h, W, bias, target, logits, dlogits, ldd, dW, db, dh, drop_scale,
-                                            relu ? 1 : 0, meter, loss_out, B, C, K, class_weights);
+                                            relu ? 1 : 0, meter, loss_out, B, C, K, class_weights,
+                                            accumulate ? 1 : 0);
   count_launch();
   check_last("head_ce_fused");
 }

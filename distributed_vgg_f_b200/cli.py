@@ -117,6 +117,9 @@ def build_parser() -> argparse.ArgumentParser:
                           "the last training step of every epoch, when each layer's kernels and each bucket's reduction / "
                           "update finished (CUDA events, ms since the start of the step; native engine)")
     ext.add_argument("--log-jsonl", default=None, help="append one JSON record per epoch")
+    ext.add_argument("--accum-steps", type=int, default=1,
+                     help="gradient accumulation: one optimizer update (and one gradient all-reduce) per K "
+                          "mini-batches and after the last one of an epoch, with the mean of their gradients")
     return parser
 
 
@@ -125,6 +128,8 @@ def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
     args = build_parser().parse_args(argv)
     if args.root_dir is None:
         build_parser().error("the following arguments are required: -rd/--root_dir")
+    if args.accum_steps < 1:
+        build_parser().error("--accum-steps must be >= 1")
     print(args)
     if args.socket_ifname:
         os.environ["GLOO_SOCKET_IFNAME"] = args.socket_ifname

@@ -103,7 +103,10 @@ class NativeEngine:
         self.beta1, self.beta2, self.eps = TRAIN.adam_beta1, TRAIN.adam_beta2, TRAIN.adam_eps
         self.seed, self.HW = int(seed), int(input_hw)
         self.same_dropout_all_ranks = bool(same_dropout_all_ranks)
-        self.step_count = 0
+        self.step_count = 0              # optimizer updates (Adam / SGD step, LR schedule, checkpoint "step")
+        self.micro_count = 0             # training micro-batches: the Philox dropout offset
+        self._accum = 0                  # micro-batches whose gradients sit in g32 awaiting an update
+        self._update = self._wire_direct = True      # per train_step: see train_step
         self.train_dropout = True        # tests switch dropout off to compare gradients exactly
         self.apply_updates = True        # False: leave raw gradients in g32 (gradient inspection)
         self.meter: Optional[DeviceMeter] = None
@@ -174,6 +177,8 @@ class NativeEngine:
         fc_w = {f.name + ".weight" for f in spec.fcs}
         self._bucket_store_only = [all(t in fc_w for t in bk.tensors) for bk in self.plan.buckets]
         # FC weights that span whole buckets by themselves can be produced directly as bf16 on the wire
+        # (when the updating micro-batch is also the first of its accumulation group: see _wire_direct);
+        # those buckets are also the ones ZeRO-1 may shard
         self._prepacked = set()
         self._bucket_prepacked = [False] * len(self.plan.buckets)
         if self.arena is not None and self.arena.wire_dtype == BF16:
@@ -223,6 +228,7 @@ class NativeEngine:
     def prepare_export(self) -> None:
         """Collective.  Under --zero1 every rank holds the current fp32 master / moments only for the
         cells it owns: sum the owned pieces over ranks so that every rank has the full state again."""
+        self._refuse_pending("prepare_export")
         if not self._zero1_buckets:
             return
         self.sync()
@@ -236,12 +242,18 @@ class NativeEngine:
                 arena[bk.start:bk.end] = tmp
         torch.cuda.synchronize(self.device)
 
+    def _refuse_pending(self, what: str) -> None:
+        if self._accum:
+            raise RuntimeError("%s: %d accumulated micro-batch(es) await an update; finish the group with "
+                               "train_step(batch, update=True) first" % (what, self._accum))
+
     def export_state(self) -> Dict[str, torch.Tensor]:
+        self._refuse_pending("export_state")
         return {name: L.to_torch(self.spec, name, self._view(self.p32, name)).detach().cpu()
                 for name in self.spec.param_names}
 
     def export_optimizer_state(self) -> dict:
-        st = {"name": self.opt_name, "step": self.step_count, "lr": self.lr}
+        st = {"name": self.opt_name, "step": self.step_count, "micro_step": self.micro_count, "lr": self.lr}
         if self.opt_name == "adam":
             st["exp_avg"] = {n: L.to_torch(self.spec, n, self._view(self.m32, n)).cpu() for n in self.spec.param_names}
             st["exp_avg_sq"] = {n: L.to_torch(self.spec, n, self._view(self.v32, n)).cpu() for n in self.spec.param_names}
@@ -252,6 +264,7 @@ class NativeEngine:
 
     def import_optimizer_state(self, st: dict) -> None:
         self.step_count = int(st.get("step", 0))
+        self.micro_count = int(st.get("micro_step", self.step_count))    # one micro-batch per update before
         if "lr" in st:                       # a run resumed behind an LR-step boundary keeps the decayed rate
             self.lr = float(st["lr"])
         with torch.no_grad():
@@ -442,7 +455,7 @@ class NativeEngine:
             else:
                 p = f.dropout if (train and self.train_dropout) else 0.0
                 ops.fc_bias_act(acc, self._b(f.name), self.fc_y[i][:b], None, B=b, N=f.fout, relu=f.relu,
-                                drop_p=p, seed=self._drop_key(i), offset=self.step_count)
+                                drop_p=p, seed=self._drop_key(i), offset=self.micro_count)
                 h = self.fc_y[i][:b]
 
     def _loss(self, b: int, train: bool) -> None:
@@ -458,10 +471,14 @@ class NativeEngine:
         C = ops.require()
         if train:
             p = prev.dropout if self.train_dropout else 0.0
-            C.head_ce(self._head_in, self._w(f.name), self._b(f.name), self.labels_dev[:b], self.logits[:b],
-                      self.fc_dz[-1][:b], self.fc_dz[-1].shape[1], self._grad(f.name + ".weight"),
-                      self._grad(f.name + ".bias"), self.fc_dz[-2][:b], 1.0 / (1.0 - p), bool(prev.relu), meter,
-                      self.loss_buf, self.class_weights)
+            args = (self._head_in, self._w(f.name), self._b(f.name), self.labels_dev[:b], self.logits[:b],
+                    self.fc_dz[-1][:b], self.fc_dz[-1].shape[1], self._grad(f.name + ".weight"),
+                    self._grad(f.name + ".bias"), self.fc_dz[-2][:b], 1.0 / (1.0 - p), bool(prev.relu), meter,
+                    self.loss_buf, self.class_weights)
+            if self._accum:                  # a later micro-batch of the group: dW += (db always accumulates)
+                C.head_ce(*args, True)
+            else:
+                C.head_ce(*args)
         else:
             C.head_ce(self._head_in, self._w(f.name), self._b(f.name), self.labels_dev[:b], self.logits[:b],
                       None, 0, None, None, None, 1.0, False, meter, self.loss_buf, None)
@@ -489,7 +506,7 @@ class NativeEngine:
             ops.bias_grad(dz, self._grad(f.name + ".bias"), b, f.fout, ld=ld)
             self._bucket_done(f.name + ".bias")
             # wgrad: dW[fout][fin] = dz^T x_in   (both operands MN-major: stored [K=b][*])
-            if (f.name + ".weight") in self._prepacked:
+            if self._wire_direct and (f.name + ".weight") in self._prepacked:
                 # big FC weights own whole buckets: write bf16(dW / ws) straight into the symmetric
                 # wire buffer -- no fp32 gradient, no pack pass before the reduction
                 off = self.plan.offsets[f.name + ".weight"]
@@ -497,8 +514,10 @@ class NativeEngine:
                 ops.gemm(dz, x_in, wire_w, M=f.fout, N=f.fin, K=b, a_mn=True, b_mn=True, epi="bf16_store",
                          ldo=f.fin, alpha=1.0 / self.world)
             else:
+                # the first micro-batch of a group stores, later ones add (ksplit 1: each tile owns its
+                # elements, so the red.add epilogue adds every element exactly once)
                 ops.gemm(dz, x_in, self._grad(f.name + ".weight"), M=f.fout, N=f.fin, K=b, a_mn=True,
-                         b_mn=True, epi="f32_store", ldo=f.fin)
+                         b_mn=True, epi="f32_atomic" if self._accum else "f32_store", ldo=f.fin)
             # dgrad: dX[b][fin] = dz W ; swap-AB with W read MN-major (stored [K=fout][M=fin])
             m_tiles = (f.fin + 127) // 128
             ks = self._ksplit(m_tiles, (f.fout + 63) // 64)
@@ -578,24 +597,28 @@ class NativeEngine:
         """Called right after the kernels producing ``name``'s gradient were enqueued."""
         for bi in self._tensor_buckets[name]:
             self._missing[bi] -= 1
-            if self._missing[bi] == 0:
+            if self._missing[bi] == 0 and self._update:
                 self._reduce_and_update(bi)
 
-    def _apply_update(self, s: int, e: int, g16: Optional[torch.Tensor], zero: bool = True) -> None:
+    def _apply_update(self, s: int, e: int, g16: Optional[torch.Tensor], zero: bool = True,
+                      grad_scale: float = 1.0) -> None:
         g32 = None if g16 is not None else self.g32[s:e]
         z = self.g32[s:e] if zero else None      # ranges written with plain stores need no re-zeroing
         if self.opt_name == "adam":
             ops.adam_step(self.p32[s:e], self.m32[s:e], self.v32[s:e], g32=g32, g16=g16, shadow=self.w16[s:e],
                           lr=self.lr, beta1=self.beta1, beta2=self.beta2, eps=self.eps,
-                          weight_decay=self.weight_decay, step=self.step_count, zero=z)
+                          weight_decay=self.weight_decay, step=self.step_count, grad_scale=grad_scale, zero=z)
         else:
             ops.sgd_step(self.p32[s:e], self.m32[s:e], g32=g32, g16=g16, shadow=self.w16[s:e], lr=self.lr,
                          momentum=self.momentum, weight_decay=self.weight_decay,
-                         first=(self.step_count == 1), zero=z)
+                         first=(self.step_count == 1), grad_scale=grad_scale, zero=z)
 
     def _reduce_and_update(self, bi: int) -> None:
         bk = self.plan.buckets[bi]
         s, e = bk.start, bk.end
+        # g32 holds the sum of the group's k' micro-batch means: the update uses their mean (1/k' where
+        # 1/world is applied, on the optimizer's grad_scale at world 1)
+        k = self._accum + 1
         if self.world == 1:
             if self.apply_updates:
                 # The optimizer is HBM-bound, the convolutions still to come are tensor-bound: run the
@@ -606,7 +629,7 @@ class NativeEngine:
                 self.comm_stream.wait_event(ev)
                 with torch.cuda.stream(self.comm_stream):
                     self._mark("opt%d start" % bi, "comm")
-                    self._apply_update(s, e, None, zero=not self._bucket_store_only[bi])
+                    self._apply_update(s, e, None, zero=not self._bucket_store_only[bi], grad_scale=1.0 / k)
                     self._mark("opt%d end" % bi, "comm")
             return
         ev = torch.cuda.Event()
@@ -614,20 +637,20 @@ class NativeEngine:
         self.comm_stream.wait_event(ev)
         with torch.cuda.stream(self.comm_stream):
             if self.use_nccl:                    # library baseline (comparison only)
-                self.g32[s:e].mul_(1.0 / self.world)
+                self.g32[s:e].mul_(1.0 / (self.world * k))
                 dist.all_reduce(self.g32[s:e])
                 if self.apply_updates:
                     self._apply_update(s, e, None)
                 return
             algo = self.arena.pick_algo(e - s, self.ar_algo)
-            prepacked = self._bucket_prepacked[bi]
-            if prepacked and algo == "oneshot":
+            prepacked = self._wire_direct and self._bucket_prepacked[bi]
+            if self._bucket_prepacked[bi] and algo == "oneshot":
                 algo = "twoshot"                 # one-shot cannot leave its result on the wire
             # ZeRO-1 only for buckets that hold nothing but one big FC weight (88 % of the parameters):
             # the forward pass reads those through the all-gathered bf16 shadow.  Buckets with biases
             # stay replicated -- biases are read from the fp32 master, which under ZeRO-1 is current on
             # the owner rank only.
-            if self.zero1 and self.apply_updates and prepacked and algo != "oneshot":
+            if self.zero1 and self.apply_updates and self._bucket_prepacked[bi] and algo != "oneshot":
                 self._mark("z1_%d start" % bi, "comm")
                 zev0 = None
                 if self._comm_events is not None:
@@ -635,8 +658,9 @@ class NativeEngine:
                     zev0.record()
                 self.arena.zero1_step(None if prepacked else self.g32, self.p32, self.m32, self.v32, self.w16,
                                       s, e - s, algo=algo, slot=bi % self.arena.slots, max_ctas=self.zero1_ctas,
-                                      inv_world=1.0 / self.world, lr=self.lr, beta1=self.beta1, beta2=self.beta2,
-                                      eps=self.eps, weight_decay=self.weight_decay, step=self.step_count)
+                                      inv_world=1.0 / (self.world * k), lr=self.lr, beta1=self.beta1,
+                                      beta2=self.beta2, eps=self.eps, weight_decay=self.weight_decay,
+                                      step=self.step_count)
                 self._zero1_buckets.add(bi)
                 if zev0 is not None:             # reduce-scatter + optimizer + all-gather: same wire bytes
                     zev1 = torch.cuda.Event(enable_timing=True)
@@ -653,12 +677,12 @@ class NativeEngine:
                 ev0.record()
             self.arena.allreduce(None if prepacked else self.g32, self.g32 if to_f32 else None, s, e - s,
                                  algo=algo, slot=bi % self.arena.slots, max_ctas=self.comm_ctas,
-                                 inv_world=1.0 / self.world)
+                                 inv_world=1.0 / (self.world * k))
             if ev0 is not None:
                 ev1 = torch.cuda.Event(enable_timing=True)
                 ev1.record()
                 self._comm_events.append((ev0, ev1, (e - s) * self.arena.wire.element_size()))
-            if self.cross_group is not None:     # node sums (already x 1/world) -> job sum, over NCCL
+            if self.cross_group is not None:     # node sums (already x 1/(world k')) -> job sum, over NCCL
                 dist.all_reduce(self.g32[s:e] if to_f32 else self.arena.wire[s:e], group=self.cross_group)
             self._mark("ar%d end" % bi, "comm")
             if self.apply_updates:
@@ -685,9 +709,16 @@ class NativeEngine:
         """Per-class loss weights (the reference's optional weighted cross-entropy)."""
         self.class_weights = None if weights is None else weights.to(self.device, F32).contiguous()
 
-    def train_step(self, batch) -> torch.Tensor:
-        """One optimisation step.  Returns the device scalar holding this batch's mean loss."""
-        self.step_count += 1
+    def train_step(self, batch, update: bool = True) -> torch.Tensor:
+        """One micro-batch: forward, loss and backward into the gradient arena, and with ``update`` the
+        reduction and optimizer step over the group of micro-batches accumulated since the last update
+        (mean of their gradients).  Returns the device scalar holding this batch's mean loss."""
+        self.micro_count += 1
+        if update:
+            self.step_count += 1
+        self._update = bool(update)
+        # FC-1 / FC-2 gradients go straight to the wire as bf16 only when nothing else is to be added
+        self._wire_direct = self._update and self._accum == 0
         t = self.timer
         if self.nvtx:
             torch.cuda.nvtx.range_push("step")
@@ -706,6 +737,7 @@ class NativeEngine:
         self._begin_step()
         self._backward(b)
         self._end_step()
+        self._accum = 0 if update else self._accum + 1
         self._mark("step end (joined comm)")
         t.stop("backward+reduce+update")
         if self.nvtx:

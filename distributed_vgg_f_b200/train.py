@@ -157,7 +157,8 @@ def manage_training(args) -> Trainer:
         if cw.numel() != num_classes:
             raise ValueError("--class-weights needs %d comma-separated values" % num_classes)
     trainer = Trainer(model, optimizer, train_loader, valid_loader, device, class_weights=cw,
-                      on_epoch_end=on_epoch_end, shard_eval=getattr(args, "shard_eval", False))
+                      on_epoch_end=on_epoch_end, shard_eval=getattr(args, "shard_eval", False),
+                      accum_steps=getattr(args, "accum_steps", 1))
     trainer.profile_timeline = getattr(args, "profile", None) == "timeline"
     if getattr(args, "eval_only", False):        # score a checkpoint: one validation pass, no training
         test_loss, test_acc = trainer._evaluate()

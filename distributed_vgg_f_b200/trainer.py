@@ -12,6 +12,11 @@ device).fit(epochs)`` -- per batch: H2D, forward, cross-entropy, zero_grad, back
 Differences kept on purpose: metrics accumulate on the device and are read once per epoch
 (``DeviceMeter``), ``set_epoch`` is called so shuffling changes between epochs, and throughput is
 reported on an extra line.
+
+``accum_steps=K`` (gradient accumulation): one optimizer update per group of K consecutive training
+mini-batches, and after the epoch's last one, so the last group of an epoch may be shorter (k' < K) and
+no group crosses an epoch boundary.  Each mini-batch's loss is its own mean; the update uses the sum of
+the group's gradients divided by k'.  Metrics count every mini-batch.
 """
 from __future__ import annotations
 
@@ -54,7 +59,13 @@ def _is_native(model) -> bool:
 class Trainer:
     def __init__(self, model, optimizer, train_loader, test_loader, device,
                  class_weights: Optional[torch.Tensor] = None, verbose_throughput: bool = True,
-                 on_epoch_end=None, shard_eval: bool = False) -> None:
+                 on_epoch_end=None, shard_eval: bool = False, accum_steps: int = 1) -> None:
+        if accum_steps < 1:
+            raise ValueError("accum_steps must be >= 1 (got %d)" % accum_steps)
+        if accum_steps > 1 and not hasattr(train_loader, "__len__"):
+            raise ValueError("accum_steps > 1 needs a training loader with __len__: the last group of an epoch "
+                             "ends at its last batch")
+        self.accum_steps = int(accum_steps)
         self.model = model
         self.optimizer = optimizer
         self.train_loader = train_loader
@@ -122,12 +133,14 @@ class Trainer:
         (SURVEY 5.5).  Needs ``engine.comm_timing(True)`` (the CLI's --profile comm)."""
         rep = getattr(self.model, "comm_report", None)
         steps = len(self.train_loader) if hasattr(self.train_loader, "__len__") else 0
-        r = rep(max(steps, 1)) if rep is not None else None
+        updates = -(-steps // self.accum_steps)          # the all-reduces run once per update
+        r = rep(max(updates, 1)) if rep is not None else None
         self.epoch_allreduce = r
         if not r:
             return ""
-        return ", grad all-reduce {:.0f} MB/step in {:.2f} ms = {:.0f} GB/s bus ({:.0f}% of 450 nominal)".format(
-            r["wire_MB_per_step"], r["ms_per_step"], r["bus_GBs"], 100 * r["frac_of_450_nominal"])
+        return ", grad all-reduce {:.0f} MB/{} in {:.2f} ms = {:.0f} GB/s bus ({:.0f}% of 450 nominal)".format(
+            r["wire_MB_per_step"], "step" if self.accum_steps == 1 else "update", r["ms_per_step"], r["bus_GBs"],
+            100 * r["frac_of_450_nominal"])
 
     def _utilisation(self, images: int, seconds: float) -> str:
         """Native engine only: achieved training TFLOP/s (3 x forward FLOPs of the layer table) and
@@ -145,6 +158,10 @@ class Trainer:
         inputs, targets = batch
         return inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
 
+    def _updates_after(self, k: int, n_steps: int) -> bool:
+        """Does the (k+1)-th training batch of an epoch of ``n_steps`` end its accumulation group?"""
+        return (k + 1) % self.accum_steps == 0 or k + 1 == n_steps
+
     def _train(self):
         meter = DeviceMeter(self.device)
         if _is_native(self.model):
@@ -159,7 +176,10 @@ class Trainer:
                 if want_tl and k == n_steps - 1:           # trace the epoch's last step
                     self.model.sync()
                     self.model.timeline(True)
-                self.model.train_step(batch)
+                if self.accum_steps == 1 or self._updates_after(k, n_steps):
+                    self.model.train_step(batch)
+                else:
+                    self.model.train_step(batch, update=False)
             t1 = time.perf_counter()
             self.model.sync()
             if want_tl:
@@ -171,18 +191,32 @@ class Trainer:
 
         self.model.train()
         wrapper = self.model if hasattr(self.model, "finish_backward") else None
-        for batch in self.train_loader:
+        n_steps = len(self.train_loader) if self.accum_steps > 1 else 0
+        pending = 0                                      # mini-batches accumulated since the last update
+        for k, batch in enumerate(self.train_loader):
+            update = self.accum_steps == 1 or self._updates_after(k, n_steps)
             inputs, targets = self._to_device(batch)
             outputs = self.model(inputs)
             loss = F.cross_entropy(outputs, targets, weight=self.class_weights)
+            if pending == 0:                             # zeroed once per group, before its first backward
+                if wrapper is not None:
+                    wrapper.zero_grad()
+                else:
+                    self.optimizer.zero_grad()
             if wrapper is not None:
-                wrapper.zero_grad()
-            else:
-                self.optimizer.zero_grad()
+                wrapper._require_sync = update           # all-reduce each bucket once, on the updating batch
             loss.backward()
+            pending += 1
             if wrapper is not None:
                 wrapper.finish_backward()
-            self.optimizer.step()
+            if update:
+                if pending > 1:                          # the mean of the group's gradients
+                    with torch.no_grad():
+                        for p in self.model.parameters():
+                            if p.grad is not None:
+                                p.grad.mul_(1.0 / pending)
+                self.optimizer.step()
+                pending = 0
             meter.add_reference(outputs.detach(), targets, self.class_weights)
         return meter.snapshot()
 
