@@ -140,6 +140,182 @@ void augment_fused(const uint8_t* src, const float* params, bf16* out, int N, in
   check_last("augment_fused");
 }
 
+// ------------------------------------------------------------------ ragged batches, Pillow resampling
+// Images of any size.  The crop box is resized with Pillow's BILINEAR filter (libImaging/Resample.c),
+// which widens to the whole footprint when it shrinks: per axis scale = in/out, support = max(scale, 1),
+// fp64 triangle weights normalised by their sum, then 22-bit fixed point.  Like Pillow, the horizontal
+// pass rounds to uint8 before the vertical pass, so both passes are exact integer arithmetic and the
+// fp64 operations below are spelled with _rn intrinsics so that nvcc contracts none of them.
+// data/transforms.py::ragged_reference is the oracle.
+struct RaggedGeom {
+  int N, OH, OW;
+  float mean[3], stdv[3];
+};
+
+constexpr int kPilBits = 22;
+
+struct PilAxis {
+  double scale, support, ss;
+  int in;
+};
+
+__device__ __forceinline__ PilAxis pil_axis(int in, int out) {
+  PilAxis a;
+  a.scale = __ddiv_rn(static_cast<double>(in), static_cast<double>(out));
+  a.support = a.scale < 1.0 ? 1.0 : a.scale;
+  a.ss = __ddiv_rn(1.0, a.support);
+  a.in = in;
+  return a;
+}
+
+// Input window [lo, lo + n) of output index i, and the sum of its unnormalised weights.
+struct PilWindow {
+  double center, ww;
+  int lo, n;
+};
+
+__device__ __forceinline__ double pil_weight(const PilAxis& a, const PilWindow& w, int x) {
+  const double t = fabs(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(x + w.lo), w.center), 0.5), a.ss));
+  return t < 1.0 ? __dsub_rn(1.0, t) : 0.0;
+}
+
+__device__ __forceinline__ PilWindow pil_window(const PilAxis& a, int i) {
+  PilWindow w;
+  w.center = __dmul_rn(static_cast<double>(i) + 0.5, a.scale);
+  w.lo = max(static_cast<int>(__dadd_rn(__dsub_rn(w.center, a.support), 0.5)), 0);
+  w.n = min(static_cast<int>(__dadd_rn(__dadd_rn(w.center, a.support), 0.5)), a.in) - w.lo;
+  w.ww = 0.0;
+  for (int x = 0; x < w.n; ++x) w.ww = __dadd_rn(w.ww, pil_weight(a, w, x));
+  return w;
+}
+
+__device__ __forceinline__ int pil_fixed(const PilAxis& a, const PilWindow& w, int x) {
+  double k = pil_weight(a, w, x);
+  if (w.ww != 0.0) k = __ddiv_rn(k, w.ww);
+  return static_cast<int>(__dadd_rn(0.5, __dmul_rn(k, static_cast<double>(1 << kPilBits))));
+}
+
+__device__ __forceinline__ uint8_t pil_clip8(int acc) { return static_cast<uint8_t>(min(max(acc >> kPilBits, 0), 255)); }
+
+// (rx, ry) in the RH x RW resized image of output pixel (oy, ox): centre crop, flip, nearest rotation,
+// each float operation rounded on its own, as augment_reference evaluates it with torch ops.
+__device__ __forceinline__ void ragged_chain(const float* prm, int RH, int RW, int OH, int OW, int oy, int ox,
+                                             float& rx, float& ry) {
+  const float cs = prm[4], sn = prm[5];
+  const float ay = static_cast<float>(oy + __float2int_rn((RH - OH) * 0.5f));
+  float ax = static_cast<float>(ox + __float2int_rn((RW - OW) * 0.5f));
+  if (prm[6] > 0.5f) ax = static_cast<float>(RW - 1) - ax;
+  const float cx = RW * 0.5f, cy = RH * 0.5f;
+  const float dx = __fsub_rn(__fadd_rn(ax, 0.5f), cx), dy = __fsub_rn(__fadd_rn(ay, 0.5f), cy);
+  rx = floorf(__fadd_rn(__fsub_rn(__fmul_rn(cs, dx), __fmul_rn(sn, dy)), cx));
+  ry = floorf(__fadd_rn(__fadd_rn(__fmul_rn(sn, dx), __fmul_rn(cs, dy)), cy));
+}
+
+// Per-image state shared by a block: every block of both passes works on one image (blockIdx.y).
+struct RaggedImage {
+  long long off, inter;       // byte offsets of the source and of its intermediate
+  int H, W, RH, RW, top, left, ch, cw;
+  int rx0, rx1, ry0, ry1;     // resized pixels the output reads (rx0 > rx1: none)
+};
+
+__device__ void load_ragged_image(const long long* __restrict__ geom, const float* __restrict__ params, int n,
+                                  int OH, int OW, RaggedImage& im) {
+  const long long* g = geom + n * 5;
+  im.off = g[0];
+  im.H = static_cast<int>(g[1]); im.W = static_cast<int>(g[2]);
+  im.RH = static_cast<int>(g[3]); im.RW = static_cast<int>(g[4]);
+  long long inter = 0;       // the intermediates of the batch's images lie back to back, H x RW x 3 each
+  for (int i = 0; i < n; ++i) inter += geom[i * 5 + 1] * geom[i * 5 + 4] * 3;
+  im.inter = inter;
+  const float* p = params + n * 8;
+  im.top = static_cast<int>(p[0]); im.left = static_cast<int>(p[1]);
+  im.ch = static_cast<int>(p[2]); im.cw = static_cast<int>(p[3]);
+  // the chain is monotone in ox and in oy (each rounded operation is), so the corners bound it
+  float x0 = 3.4e38f, x1 = -3.4e38f, y0 = 3.4e38f, y1 = -3.4e38f;
+  for (int c = 0; c < 4; ++c) {
+    float rx, ry;
+    ragged_chain(p, im.RH, im.RW, OH, OW, (c >> 1) * (OH - 1), (c & 1) * (OW - 1), rx, ry);
+    x0 = fminf(x0, rx); x1 = fmaxf(x1, rx); y0 = fminf(y0, ry); y1 = fmaxf(y1, ry);
+  }
+  im.rx0 = static_cast<int>(fmaxf(x0, 0.f)); im.rx1 = static_cast<int>(fminf(x1, im.RW - 1.f));
+  im.ry0 = static_cast<int>(fmaxf(y0, 0.f)); im.ry1 = static_cast<int>(fminf(y1, im.RH - 1.f));
+  if (im.ry0 > im.ry1) im.rx1 = im.rx0 - 1;
+}
+
+// Pass 1: rows of the crop box that the vertical filter reads x the resized columns the output reads,
+// filtered horizontally into inter[crop row][RW][3] (uint8).
+__global__ void augment_ragged_h_kernel(const uint8_t* __restrict__ src, const long long* __restrict__ geom,
+                                        const float* __restrict__ params, uint8_t* __restrict__ inter, RaggedGeom g) {
+  __shared__ RaggedImage im;
+  if (threadIdx.x == 0) load_ragged_image(geom, params, blockIdx.y, g.OH, g.OW, im);
+  __syncthreads();
+  if (im.rx0 > im.rx1) return;
+  const PilAxis va = pil_axis(im.ch, im.RH), ha = pil_axis(im.cw, im.RW);
+  const PilWindow first = pil_window(va, im.ry0), last = pil_window(va, im.ry1);
+  const int r0 = first.lo, rows = last.lo + last.n - first.lo, cols = im.rx1 - im.rx0 + 1;
+  const long long total = static_cast<long long>(rows) * cols;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int r = r0 + static_cast<int>(i / cols), x = im.rx0 + static_cast<int>(i % cols);
+    const PilWindow w = pil_window(ha, x);
+    const uint8_t* s = src + im.off + (static_cast<long long>(im.top + r) * im.W + im.left + w.lo) * 3;
+    int a0 = 1 << (kPilBits - 1), a1 = a0, a2 = a0;
+    for (int t = 0; t < w.n; ++t) {
+      const int k = pil_fixed(ha, w, t);
+      a0 += s[t * 3] * k; a1 += s[t * 3 + 1] * k; a2 += s[t * 3 + 2] * k;
+    }
+    uint8_t* o = inter + im.inter + (static_cast<long long>(r) * im.RW + x) * 3;
+    o[0] = pil_clip8(a0); o[1] = pil_clip8(a1); o[2] = pil_clip8(a2);
+  }
+}
+
+// Pass 2: one thread per output pixel: chain -> (rx, ry), vertical filter down column rx of the
+// intermediate -> uint8 -> normalise -> bf16, one 8-byte NHWC4 store.
+__global__ void augment_ragged_v_kernel(const long long* __restrict__ geom, const float* __restrict__ params,
+                                        const uint8_t* __restrict__ inter, bf16* __restrict__ out, RaggedGeom g) {
+  __shared__ RaggedImage im;
+  const int n = blockIdx.y;
+  if (threadIdx.x == 0) load_ragged_image(geom, params, n, g.OH, g.OW, im);
+  __syncthreads();
+  const PilAxis va = pil_axis(im.ch, im.RH);
+  const float* prm = params + n * 8;
+  const int pixels = g.OH * g.OW;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < pixels; i += gridDim.x * blockDim.x) {
+    const int oy = i / g.OW, ox = i % g.OW;
+    float rx, ry;
+    ragged_chain(prm, im.RH, im.RW, g.OH, g.OW, oy, ox, rx, ry);
+    float v[3] = {0.f, 0.f, 0.f};
+    if (rx >= 0.f && rx < im.RW && ry >= 0.f && ry < im.RH) {     // rotation fill = 0 (pre-normalise)
+      const PilWindow w = pil_window(va, static_cast<int>(ry));
+      const long long stride = static_cast<long long>(im.RW) * 3;
+      const uint8_t* s = inter + im.inter + w.lo * stride + static_cast<int>(rx) * 3;
+      int a0 = 1 << (kPilBits - 1), a1 = a0, a2 = a0;
+      for (int t = 0; t < w.n; ++t) {
+        const int k = pil_fixed(va, w, t);
+        a0 += s[t * stride] * k; a1 += s[t * stride + 1] * k; a2 += s[t * stride + 2] * k;
+      }
+      v[0] = pil_clip8(a0); v[1] = pil_clip8(a1); v[2] = pil_clip8(a2);
+    }
+    float o[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = __fdiv_rn(__fsub_rn(__fdiv_rn(v[c], 255.f), g.mean[c]), g.stdv[c]);
+    *reinterpret_cast<uint2*>(out + (static_cast<long long>(n) * pixels + i) * 4) =
+        make_uint2(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], 0.f));
+  }
+}
+
+void augment_ragged(const uint8_t* src, const long long* geom, const float* params, uint8_t* inter, bf16* out,
+                    int N, int OH, int OW, int grid_x, const float* mean, const float* stdv, cudaStream_t s) {
+  RaggedGeom g;
+  g.N = N; g.OH = OH; g.OW = OW;
+  for (int c = 0; c < 3; ++c) { g.mean[c] = mean[c]; g.stdv[c] = stdv[c]; }
+  const dim3 grid(grid_x, N);
+  augment_ragged_h_kernel<<<grid, 256, 0, s>>>(src, geom, params, inter, g);
+  augment_ragged_v_kernel<<<grid, 256, 0, s>>>(geom, params, inter, out, g);
+  count_launch(2);
+  check_last("augment_ragged");
+}
+
 // im2col of an already-normalised NHWC (3 channels padded to cpad = 4) bf16 image: the second half
 // of the two-pass input path (augment -> 8-byte pixels, 25 MB, stays in L2 -> im2col rows).  One
 // thread per (pixel, 8-element chunk): up to four 8-byte pixel loads, one 16-byte store.

@@ -1,5 +1,6 @@
 // pybind11 surface of the native library: adapts torch tensors to the raw-pointer API of api.h.
 // Every op runs on torch's current CUDA stream of the tensor's device.
+#include <algorithm>
 #include <cstdlib>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -305,6 +306,65 @@ static void augment(const at::Tensor& src, const at::Tensor& params, at::Tensor 
   b200::augment_fused(src.data_ptr<uint8_t>(), f32p(params), bfp_mut(out), src.size(0), src.size(1), src.size(2),
                       (int)RH, (int)RW, (int)OH, (int)OW, (int)mode, (int)pad, m, s, cur_stream());
 }
+// Bytes of the intermediate augment_ragged needs for these geometry rows: H x RW x 3 per image.
+static int64_t ragged_inter_bytes(const at::Tensor& geom) {
+  TORCH_CHECK(!geom.is_cuda() && geom.scalar_type() == at::kLong && geom.dim() == 2 && geom.size(1) == 5 &&
+                  geom.is_contiguous(), "ragged_inter_bytes: geom must be a CPU int64 [N, 5] tensor");
+  const int64_t* g = geom.data_ptr<int64_t>();
+  int64_t total = 0;
+  for (int64_t i = 0; i < geom.size(0); ++i) total += g[i * 5 + 1] * g[i * 5 + 4] * 3;
+  return total;
+}
+
+// The kernels read geom and params on the device; the host copies they were made from are checked
+// here, so that no row can send a launch outside src, inter or out.
+static void augment_ragged(const at::Tensor& src, const at::Tensor& geom, const at::Tensor& params, at::Tensor inter,
+                           at::Tensor out, const at::Tensor& geom_host, const at::Tensor& params_host, int64_t OH,
+                           int64_t OW, std::vector<double> mean, std::vector<double> stdv) {
+  c10::cuda::CUDAGuard g(src.device());
+  TORCH_CHECK(src.is_cuda() && src.scalar_type() == at::kByte && src.is_contiguous(),
+              "augment_ragged: src must be a contiguous CUDA uint8 tensor");
+  TORCH_CHECK(inter.is_cuda() && inter.scalar_type() == at::kByte && inter.is_contiguous(),
+              "augment_ragged: inter must be a contiguous CUDA uint8 tensor");
+  TORCH_CHECK(geom.is_cuda() && geom.scalar_type() == at::kLong && geom.is_contiguous() && geom.dim() == 2 &&
+                  geom.size(1) == 5, "augment_ragged: geom must be a contiguous CUDA int64 [N, 5] tensor");
+  const int64_t N = geom.size(0);
+  TORCH_CHECK(N > 0 && N <= 65535, "augment_ragged: 1 to 65535 images");
+  TORCH_CHECK(params.is_cuda() && params.scalar_type() == at::kFloat && params.is_contiguous() && params.dim() == 2 &&
+                  params.size(0) == N && params.size(1) == 8, "augment_ragged: params must be a contiguous CUDA fp32 [N, 8] tensor");
+  TORCH_CHECK(!geom_host.is_cuda() && geom_host.scalar_type() == at::kLong && geom_host.is_contiguous() &&
+                  geom_host.sizes() == geom.sizes(), "augment_ragged: geom_host must be the CPU int64 copy of geom");
+  TORCH_CHECK(!params_host.is_cuda() && params_host.scalar_type() == at::kFloat && params_host.is_contiguous() &&
+                  params_host.sizes() == params.sizes(), "augment_ragged: params_host must be the CPU fp32 copy of params");
+  TORCH_CHECK(OH > 0 && OW > 0 && mean.size() == 3 && stdv.size() == 3, "augment_ragged: OH, OW > 0, 3 means and deviations");
+  check_vec(out, at::kBFloat16, 8, "augment_ragged", "out");
+  TORCH_CHECK(out.numel() >= N * OH * OW * 4, "augment_ragged: out must hold N x OH x OW x 4 elements");
+  const int64_t* gh = geom_host.data_ptr<int64_t>();
+  const float* ph = params_host.data_ptr<float>();
+  int64_t most = 1;
+  for (int64_t i = 0; i < N; ++i) {
+    const int64_t off = gh[i * 5], H = gh[i * 5 + 1], W = gh[i * 5 + 2], RH = gh[i * 5 + 3], RW = gh[i * 5 + 4];
+    TORCH_CHECK(H >= 1 && W >= 1 && H <= 65535 && W <= 65535 && off >= 0 && off + H * W * 3 <= src.numel(),
+                "augment_ragged: image ", i, " (offset ", off, ", ", H, " x ", W, ") lies outside src of ",
+                src.numel(), " bytes");
+    TORCH_CHECK(RH >= 1 && RW >= 1 && RH <= (1 << 24) && RW <= (1 << 24), "augment_ragged: image ", i,
+                " has a resized size of ", RH, " x ", RW);
+    const int64_t top = (int64_t)ph[i * 8], left = (int64_t)ph[i * 8 + 1];
+    const int64_t ch = (int64_t)ph[i * 8 + 2], cw = (int64_t)ph[i * 8 + 3];
+    TORCH_CHECK(top >= 0 && left >= 0 && ch >= 1 && cw >= 1 && top + ch <= H && left + cw <= W, "augment_ragged: image ",
+                i, " has a crop box (", top, ", ", left, ", ", ch, ", ", cw, ") outside its ", H, " x ", W, " pixels");
+    most = std::max(most, H * RW);
+  }
+  const int64_t need = ragged_inter_bytes(geom_host);
+  TORCH_CHECK(inter.numel() >= need, "augment_ragged: inter must hold ", need, " bytes, got ", inter.numel());
+  // blocks per image: enough for the largest image, at most 16 blocks per SM over the batch
+  const int64_t cap = std::max<int64_t>(1, 16 * b200::sm_count() / N);
+  const int grid_x = (int)std::min(cap, std::max((most + 255) / 256, (OH * OW + 255) / 256));
+  float m[3] = {(float)mean[0], (float)mean[1], (float)mean[2]}, s[3] = {(float)stdv[0], (float)stdv[1], (float)stdv[2]};
+  b200::augment_ragged(src.data_ptr<uint8_t>(), reinterpret_cast<const long long*>(geom.data_ptr<int64_t>()),
+                       f32p(params), inter.data_ptr<uint8_t>(), bfp_mut(out), (int)N, (int)OH, (int)OW, grid_x, m, s,
+                       cur_stream());
+}
 static void im2col_c3(const at::Tensor& x, at::Tensor out, int64_t kpad) {
   c10::cuda::CUDAGuard g(x.device());
   check_vec(x, at::kBFloat16, 8, "im2col_c3", "x");
@@ -330,7 +390,34 @@ struct PngImage {
   bool ok = false;
 };
 void decode_png_files(const std::vector<std::string>& paths, int threads, std::vector<PngImage>& out);
+void decode_png_files_into(const std::vector<std::string>& paths, int threads, uint8_t* dst, const int64_t* offsets,
+                           const int64_t* hw, uint8_t* ok);
 }  // namespace b200
+
+// Ragged splits: decode each file into flat[offsets[i] :] when it is a plain 8-bit PNG of size hw[i].
+// Returns a bool [N] tensor of the files written; the caller decodes the rest with PIL.
+static at::Tensor decode_pngs_into(const std::vector<std::string>& paths, at::Tensor flat, const at::Tensor& offsets,
+                                   const at::Tensor& hw, int64_t threads) {
+  const int64_t N = (int64_t)paths.size();
+  TORCH_CHECK(!flat.is_cuda() && flat.scalar_type() == at::kByte && flat.is_contiguous(),
+              "decode_pngs_into: flat must be a contiguous CPU uint8 tensor");
+  TORCH_CHECK(!offsets.is_cuda() && offsets.scalar_type() == at::kLong && offsets.is_contiguous() && offsets.numel() == N,
+              "decode_pngs_into: offsets must be a CPU int64 [N] tensor");
+  TORCH_CHECK(!hw.is_cuda() && hw.scalar_type() == at::kLong && hw.is_contiguous() && hw.numel() == 2 * N,
+              "decode_pngs_into: hw must be a CPU int64 [N, 2] tensor");
+  const int64_t* o = offsets.data_ptr<int64_t>();
+  const int64_t* s = hw.data_ptr<int64_t>();
+  for (int64_t i = 0; i < N; ++i)
+    TORCH_CHECK(o[i] >= 0 && s[2 * i] >= 0 && s[2 * i + 1] >= 0 && o[i] + s[2 * i] * s[2 * i + 1] * 3 <= flat.numel(),
+                "decode_pngs_into: image ", i, " lies outside flat");
+  at::Tensor ok = at::zeros({N}, at::kBool);
+  {
+    py::gil_scoped_release nogil;
+    b200::decode_png_files_into(paths, (int)threads, flat.data_ptr<uint8_t>(), o, s,
+                                reinterpret_cast<uint8_t*>(ok.data_ptr<bool>()));
+  }
+  return ok;
+}
 
 // All files decoded natively into one uint8 [N,H,W,3] tensor; throws if a file is not a plain 8-bit
 // PNG or the sizes differ (the caller then falls back to PIL).
@@ -362,6 +449,11 @@ struct PrefetchConfig {
   int64_t* ring_lab;
   bool train;
   float scale_lo, scale_hi, ratio_lo, ratio_hi, degrees;
+  const int64_t* offsets = nullptr;
+  const int64_t* hw = nullptr;
+  int64_t* ring_geom = nullptr;
+  int64_t slot_bytes = 0;
+  int resize = 256;
 };
 class BatchPrefetcher;
 BatchPrefetcher* prefetcher_create(const PrefetchConfig& c);
@@ -374,19 +466,62 @@ void prefetcher_stop(BatchPrefetcher* p);
 
 struct PyPrefetcher {
   b200::BatchPrefetcher* p = nullptr;
-  at::Tensor cache, labels, ring_img, ring_par, ring_lab;     // keep the storage alive
+  at::Tensor cache, labels, ring_img, ring_par, ring_lab, offsets, hw, ring_geom;     // keep the storage alive
+  // Uniform splits: cache [N,H,W,3], ring_img [slots][mb][H][W][3].  Ragged splits also pass offsets [N]
+  // and hw [N,2] into a flat cache, ring_img [slots][slot bytes] and ring_geom [slots][mb][5].
   PyPrefetcher(at::Tensor cache_, at::Tensor labels_, at::Tensor ring_img_, at::Tensor ring_par_, at::Tensor ring_lab_,
-               bool train, double scale_lo, double scale_hi, double ratio_lo, double ratio_hi, double degrees)
+               bool train, double scale_lo, double scale_hi, double ratio_lo, double ratio_hi, double degrees,
+               c10::optional<at::Tensor> offsets_, c10::optional<at::Tensor> hw_, c10::optional<at::Tensor> ring_geom_,
+               int64_t resize)
       : cache(cache_), labels(labels_), ring_img(ring_img_), ring_par(ring_par_), ring_lab(ring_lab_) {
-    TORCH_CHECK(cache.dim() == 4 && cache.size(3) == 3 && cache.scalar_type() == at::kByte && cache.is_contiguous() &&
-                !cache.is_cuda(), "Prefetcher: cache must be a CPU uint8 [N,H,W,3] tensor");
-    TORCH_CHECK(ring_img.dim() == 5 && ring_img.is_contiguous() && ring_par.is_contiguous() && ring_lab.is_contiguous() &&
-                labels.scalar_type() == at::kLong && ring_lab.scalar_type() == at::kLong && ring_par.scalar_type() == at::kFloat,
+    const bool ragged = offsets_.has_value();
+    TORCH_CHECK(ragged == hw_.has_value() && ragged == ring_geom_.has_value(),
+                "Prefetcher: offsets, hw and ring_geom come together");
+    TORCH_CHECK(cache.scalar_type() == at::kByte && cache.is_contiguous() && !cache.is_cuda() &&
+                    (ragged ? cache.dim() == 1 : cache.dim() == 4 && cache.size(3) == 3),
+                "Prefetcher: cache must be a CPU uint8 [N,H,W,3] tensor, or flat for a ragged split");
+    TORCH_CHECK(ring_img.dim() == (ragged ? 2 : 5) && ring_img.is_contiguous() && ring_par.is_contiguous() &&
+                    ring_lab.is_contiguous() && labels.scalar_type() == at::kLong &&
+                    ring_lab.scalar_type() == at::kLong && ring_par.scalar_type() == at::kFloat,
                 "Prefetcher: bad ring tensors");
+    const int64_t N = labels.numel();
+    TORCH_CHECK(ring_par.dim() == 3 && ring_par.size(2) == 8 && ring_lab.dim() == 2 &&
+                    ring_par.size(0) == ring_img.size(0) && ring_lab.size(0) == ring_img.size(0) &&
+                    ring_par.size(1) == ring_lab.size(1),
+                "Prefetcher: ring_par [slots][mb][8] and ring_lab [slots][mb]");
     b200::PrefetchConfig c;
     c.cache = cache.data_ptr<uint8_t>(); c.labels = labels.data_ptr<int64_t>();
-    c.H = (int)cache.size(1); c.W = (int)cache.size(2);
-    c.slots = (int)ring_img.size(0); c.mb = (int)ring_img.size(1);
+    c.slots = (int)ring_img.size(0); c.mb = (int)ring_par.size(1);
+    if (ragged) {
+      offsets = *offsets_; hw = *hw_; ring_geom = *ring_geom_;
+      TORCH_CHECK(offsets.scalar_type() == at::kLong && offsets.is_contiguous() && offsets.numel() == N &&
+                      hw.scalar_type() == at::kLong && hw.is_contiguous() && hw.numel() == 2 * N,
+                  "Prefetcher: offsets int64 [N] and hw int64 [N, 2]");
+      TORCH_CHECK(ring_geom.scalar_type() == at::kLong && ring_geom.is_contiguous() && ring_geom.dim() == 3 &&
+                      ring_geom.size(0) == c.slots && ring_geom.size(1) == c.mb && ring_geom.size(2) == 5,
+                  "Prefetcher: ring_geom must be int64 [slots][mb][5]");
+      // a slot must hold the mb largest images, the cache every image
+      const int64_t* o = offsets.data_ptr<int64_t>();
+      const int64_t* s = hw.data_ptr<int64_t>();
+      std::vector<int64_t> sizes(N);
+      for (int64_t i = 0; i < N; ++i) {
+        sizes[i] = s[2 * i] * s[2 * i + 1] * 3;
+        TORCH_CHECK(s[2 * i] >= 1 && s[2 * i + 1] >= 1 && o[i] >= 0 && o[i] + sizes[i] <= cache.numel(),
+                    "Prefetcher: image ", i, " lies outside the cache");
+      }
+      std::sort(sizes.begin(), sizes.end(), std::greater<int64_t>());
+      int64_t need = 0;
+      for (int64_t i = 0; i < std::min<int64_t>(N, c.mb); ++i) need += sizes[i];
+      TORCH_CHECK(ring_img.size(1) >= need, "Prefetcher: a slot of ", ring_img.size(1), " bytes cannot hold ", c.mb,
+                  " images of up to ", need, " bytes");
+      c.offsets = o; c.hw = s; c.ring_geom = ring_geom.data_ptr<int64_t>();
+      c.slot_bytes = ring_img.size(1); c.resize = (int)resize;
+      c.H = 0; c.W = 0;
+    } else {
+      c.H = (int)cache.size(1); c.W = (int)cache.size(2);
+      TORCH_CHECK(ring_img.size(1) == c.mb && ring_img.size(2) == c.H && ring_img.size(3) == c.W,
+                  "Prefetcher: ring_img must be [slots][mb][H][W][3]");
+    }
     c.ring_img = ring_img.data_ptr<uint8_t>(); c.ring_par = ring_par.data_ptr<float>(); c.ring_lab = ring_lab.data_ptr<int64_t>();
     c.train = train; c.scale_lo = (float)scale_lo; c.scale_hi = (float)scale_hi;
     c.ratio_lo = (float)ratio_lo; c.ratio_hi = (float)ratio_hi; c.degrees = (float)degrees;
@@ -467,6 +602,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "distributed-vgg-f_b200 native sm_90a kernels";
   m.def("launch_count", &b200::launch_count);
   m.def("decode_pngs", &decode_pngs);
+  m.def("decode_pngs_into", &decode_pngs_into);
   m.def("gemm", &gemm);
   m.def("conv0_fprop", &conv0_fprop);
   m.def("conv0_wgrad", &conv0_wgrad);
@@ -525,10 +661,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("adam", &adam);
   m.def("sgd", &sgd);
   m.def("augment", &augment);
+  m.def("augment_ragged", &augment_ragged);
+  m.def("ragged_inter_bytes", &ragged_inter_bytes);
   m.def("im2col_c3", &im2col_c3);
   m.def("nchw_to_nhwc", &nchw_to_nhwc);
   py::class_<PyPrefetcher>(m, "Prefetcher")
-      .def(py::init<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, bool, double, double, double, double, double>())
+      .def(py::init<at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, bool, double, double, double, double, double,
+                    c10::optional<at::Tensor>, c10::optional<at::Tensor>, c10::optional<at::Tensor>, int64_t>(),
+           py::arg("cache"), py::arg("labels"), py::arg("ring_img"), py::arg("ring_par"), py::arg("ring_lab"),
+           py::arg("train"), py::arg("scale_lo"), py::arg("scale_hi"), py::arg("ratio_lo"), py::arg("ratio_hi"),
+           py::arg("degrees"), py::arg("offsets") = py::none(), py::arg("hw") = py::none(),
+           py::arg("ring_geom") = py::none(), py::arg("resize") = 256)
       .def("start", &PyPrefetcher::start)
       .def("next", &PyPrefetcher::next)
       .def("release", &PyPrefetcher::release)

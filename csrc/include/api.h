@@ -116,6 +116,15 @@ void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* sh
 void augment_fused(const uint8_t* src, const float* params, bf16* out, int N, int SH, int SW,
                    int RH, int RW, int OH, int OW, int mode, int pad, const float* mean,
                    const float* stdv, cudaStream_t s);
+// The same transform for a batch of images of any sizes, resampled exactly as Pillow's BILINEAR
+// resize does.  src: the images back to back; geom [N][5] int64 rows (byte offset, H, W, RH, RW);
+// params [N][8] as for augment_fused; inter: uint8 scratch of at least ragged_inter_bytes; out:
+// NHWC bf16 with 4 channels (the 4th written as 0).  grid_x: blocks per image of each launch.
+// Pass 1 filters the crop box horizontally into inter; pass 2 filters vertically, follows the
+// rotation / flip / centre-crop chain and normalises.
+void augment_ragged(const uint8_t* src, const long long* geom, const float* params, uint8_t* inter,
+                    bf16* out, int N, int OH, int OW, int grid_x, const float* mean,
+                    const float* stdv, cudaStream_t s);
 // im2col of an NHWC(3, padded to cpad) bf16 image for layer 0 (used when the input is given as a
 // float tensor instead of uint8 + params).
 void im2col3x3_c3(const bf16* x, bf16* out, int N, int H, int W, int cpad, int kpad,

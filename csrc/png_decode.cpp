@@ -138,4 +138,30 @@ void decode_png_files(const std::vector<std::string>& paths, int threads, std::v
   for (auto& t : pool) t.join();
 }
 
+// Decode file i straight into dst + offsets[i] when it is a PNG this decoder handles and its size is
+// hw[i] = (H, W); ok[i] says which files were written.  Only one decoded image per thread is alive.
+void decode_png_files_into(const std::vector<std::string>& paths, int threads, uint8_t* dst, const int64_t* offsets,
+                           const int64_t* hw, uint8_t* ok) {
+  std::atomic<size_t> next{0};
+  auto work = [&]() {
+    for (;;) {
+      const size_t i = next.fetch_add(1);
+      if (i >= paths.size()) return;
+      ok[i] = 0;
+      try {
+        PngImage img;
+        if (decode_one(paths[i], img) && img.h == hw[i * 2] && img.w == hw[i * 2 + 1]) {
+          memcpy(dst + offsets[i], img.rgb.data(), img.rgb.size());
+          ok[i] = 1;
+        }
+      } catch (...) {            // not handled here: PIL decodes this file
+      }
+    }
+  };
+  if (threads < 1) threads = 1;
+  std::vector<std::thread> pool;
+  for (int t = 0; t < threads; ++t) pool.emplace_back(work);
+  for (auto& t : pool) t.join();
+}
+
 }  // namespace b200

@@ -14,6 +14,7 @@
 #include <condition_variable>
 #include <cstdint>
 #include <cstring>
+#include <algorithm>
 #include <deque>
 #include <mutex>
 #include <random>
@@ -31,6 +32,14 @@ struct PrefetchConfig {
   int64_t* ring_lab;         // [slots][mb]
   bool train;
   float scale_lo, scale_hi, ratio_lo, ratio_hi, degrees;
+  // ragged splits (offsets != nullptr): the cache is one flat buffer, image i at offsets[i] with size
+  // hw[i] = (H, W); a slot holds the batch's images back to back in slot_bytes, and ring_geom
+  // [slots][mb][5] gets each sample's (offset in the slot, H, W, RH, RW)
+  const int64_t* offsets = nullptr;
+  const int64_t* hw = nullptr;
+  int64_t* ring_geom = nullptr;
+  int64_t slot_bytes = 0;
+  int resize = 256;
 };
 
 class BatchPrefetcher {
@@ -87,32 +96,33 @@ class BatchPrefetcher {
  private:
   double uni() { return std::generate_canonical<double, 53>(rng_); }
 
-  void sample_params(float* p) {
+  // Parameters of one sample of an H x W source: the same draws, in the same order, for every size.
+  void sample_params(float* p, int H, int W) {
     const PrefetchConfig& c = cfg_;
     if (!c.train) {
-      p[0] = 0; p[1] = 0; p[2] = (float)c.H; p[3] = (float)c.W; p[4] = 1.f; p[5] = 0.f; p[6] = 0.f; p[7] = 0.f;
+      p[0] = 0; p[1] = 0; p[2] = (float)H; p[3] = (float)W; p[4] = 1.f; p[5] = 0.f; p[6] = 0.f; p[7] = 0.f;
       return;
     }
-    const double area = (double)c.H * c.W, llo = std::log(c.ratio_lo), lhi = std::log(c.ratio_hi);
+    const double area = (double)H * W, llo = std::log(c.ratio_lo), lhi = std::log(c.ratio_hi);
     double cw = 0, ch = 0;
     bool ok = false;
     for (int t = 0; t < 10; ++t) {                      // every draw consumed: fixed RNG stride
       const double ta = area * (c.scale_lo + (c.scale_hi - c.scale_lo) * uni());
       const double ar = std::exp(llo + (lhi - llo) * uni());
       const double w = std::nearbyint(std::sqrt(ta * ar)), h = std::nearbyint(std::sqrt(ta / ar));
-      if (!ok && w > 0 && w <= c.W && h > 0 && h <= c.H) { cw = w; ch = h; ok = true; }
+      if (!ok && w > 0 && w <= W && h > 0 && h <= H) { cw = w; ch = h; ok = true; }
     }
     const double u0 = uni(), u1 = uni(), ua = uni(), uf = uni();
     double top, left;
     if (ok) {
-      top = std::fmin(std::floor(u0 * (c.H - ch + 1)), c.H - ch);
-      left = std::fmin(std::floor(u1 * (c.W - cw + 1)), c.W - cw);
+      top = std::fmin(std::floor(u0 * (H - ch + 1)), H - ch);
+      left = std::fmin(std::floor(u1 * (W - cw + 1)), W - cw);
     } else {                                            // torchvision's centre-crop fallback
-      const double in_ratio = (double)c.W / c.H;
-      if (in_ratio < c.ratio_lo) { cw = c.W; ch = std::nearbyint(cw / c.ratio_lo); }
-      else if (in_ratio > c.ratio_hi) { ch = c.H; cw = std::nearbyint(ch * c.ratio_hi); }
-      else { cw = c.W; ch = c.H; }
-      top = std::floor((c.H - ch) / 2); left = std::floor((c.W - cw) / 2);
+      const double in_ratio = (double)W / H;
+      if (in_ratio < c.ratio_lo) { cw = W; ch = std::nearbyint(cw / c.ratio_lo); }
+      else if (in_ratio > c.ratio_hi) { ch = H; cw = std::nearbyint(ch * c.ratio_hi); }
+      else { cw = W; ch = H; }
+      top = std::floor((H - ch) / 2); left = std::floor((W - cw) / 2);
     }
     const double theta = (-c.degrees + 2.0 * c.degrees * ua) * 3.14159265358979323846 / 180.0;
     p[0] = (float)top; p[1] = (float)left; p[2] = (float)ch; p[3] = (float)cw;
@@ -145,11 +155,31 @@ class BatchPrefetcher {
       uint8_t* img = c.ring_img + (size_t)slot * c.mb * img_bytes;
       float* par = c.ring_par + (size_t)slot * c.mb * 8;
       int64_t* lab = c.ring_lab + (size_t)slot * c.mb;
-      for (int i = 0; i < k; ++i) {
-        const int64_t src = indices_[b0 + i];
-        std::memcpy(img + (size_t)i * img_bytes, c.cache + (size_t)src * img_bytes, img_bytes);
-        lab[i] = c.labels[src];
-        sample_params(par + (size_t)i * 8);
+      if (c.offsets) {
+        uint8_t* bytes = c.ring_img + (size_t)slot * c.slot_bytes;
+        int64_t* geom = c.ring_geom + (size_t)slot * c.mb * 5;
+        int64_t at = 0;
+        for (int i = 0; i < k; ++i) {
+          const int64_t src = indices_[b0 + i];
+          const int H = (int)c.hw[src * 2], W = (int)c.hw[src * 2 + 1];
+          const size_t n = (size_t)H * W * 3;
+          std::memcpy(bytes + at, c.cache + c.offsets[src], n);
+          int64_t* g = geom + (size_t)i * 5;
+          g[0] = at; g[1] = H; g[2] = W;
+          if (c.train) { g[3] = c.resize; g[4] = c.resize; }         // data/transforms.py::resized_dims
+          else if (H <= W) { g[3] = c.resize; g[4] = std::max((int64_t)((double)c.resize * W / H), (int64_t)1); }
+          else { g[3] = std::max((int64_t)((double)c.resize * H / W), (int64_t)1); g[4] = c.resize; }
+          at += (int64_t)n;
+          lab[i] = c.labels[src];
+          sample_params(par + (size_t)i * 8, H, W);
+        }
+      } else {
+        for (int i = 0; i < k; ++i) {
+          const int64_t src = indices_[b0 + i];
+          std::memcpy(img + (size_t)i * img_bytes, c.cache + (size_t)src * img_bytes, img_bytes);
+          lab[i] = c.labels[src];
+          sample_params(par + (size_t)i * 8, c.H, c.W);
+        }
       }
       {
         std::lock_guard<std::mutex> lk(mu_);

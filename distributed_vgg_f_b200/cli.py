@@ -85,9 +85,9 @@ def build_parser() -> argparse.ArgumentParser:
     ext.add_argument("--wire-dtype", default="bf16", choices=["bf16", "fp32"])
     ext.add_argument("--bucket-mb", type=float, default=32.0)
     ext.add_argument("--pipeline", default="auto", choices=["auto", "fused", "reference"],
-                     help="input pipeline: fused GPU augment over a decoded uint8 cache, the reference's "
-                          "per-sample PIL transforms, or auto (fused when the split has one image size "
-                          "and fits in host memory)")
+                     help="input pipeline: fused GPU augment over a decoded uint8 cache (any image sizes, "
+                          "resampled as PIL does), the reference's per-sample PIL transforms, or auto "
+                          "(fused when the split has one image size and fits in host memory)")
     ext.add_argument("--pretrained", default=None,
                      help="path to a torchvision vgg16 state dict (offline pretrained=True)")
     ext.add_argument("--save", default=None, help="checkpoint path written by rank 0 every epoch")

@@ -10,10 +10,12 @@ Same surface here, two pipelines:
     ``(float32 [mb,3,224,224], int64 [mb])``.  Bit-level semantics of the reference; ~400 img/s.
   * ``pipeline="fused"`` (default) -- every image is decoded ONCE into a uint8 cache (thread pool),
     a background thread gathers each batch into a pinned staging ring together with the sampled
-    transform parameters, and the consumer runs the fused augment op on the device.  Yields
-    ``FusedBatch``.  Requires a uniform source size (true for COIL-100 / the synthetic set) and a
-    split that fits in host memory; ``pipeline="auto"`` (the CLI default) switches to the
-    reference pipeline when either does not hold.
+    transform parameters, and the consumer runs the fused augment op on the device.  A split whose
+    images all share one size of at most 256 x 256 (COIL-100, the synthetic set) yields
+    ``FusedBatch``; any other split yields ``RaggedBatch``: the images of a batch back to back, one
+    geometry row each, resampled on the device exactly as Pillow does.  The split must fit in host
+    memory.  ``pipeline="auto"`` (the CLI default) switches to the reference pipeline for mixed
+    image sizes or a split too big for host memory.
 Ragged final batches are preserved (``drop_last=False`` in the reference).
 """
 from __future__ import annotations
@@ -46,6 +48,21 @@ class FusedBatch(NamedTuple):
         return x, self.labels.to(device)
 
 
+class RaggedBatch(NamedTuple):
+    """A batch of images of any sizes: ``data_u8`` holds them back to back, row i of ``geom`` is
+    image i's (byte offset, H, W, RH, RW) with (RH, RW) the size it is resized to."""
+    data_u8: torch.Tensor       # uint8 [bytes]        (pinned when CUDA is present)
+    geom: torch.Tensor          # int64 [mb, 5]        (same)
+    params: torch.Tensor        # float32 [mb, 8]      (same)
+    labels: torch.Tensor        # int64 [mb]           (same)
+    state: Optional[dict] = None    # consumer may set state["event"]: slot is reusable after it fires
+
+    def to_float(self, device="cpu") -> Tuple[torch.Tensor, torch.Tensor]:
+        """Evaluate the transform with Pillow's resampling on the CPU (CPU / oracle path)."""
+        x = T.ragged_reference(self.data_u8, self.geom, self.params)
+        return x.to(device), self.labels.to(device)
+
+
 def _decode(path: str) -> np.ndarray:
     from PIL import Image
 
@@ -54,7 +71,7 @@ def _decode(path: str) -> np.ndarray:
 
 
 class CacheUnavailable(ValueError):
-    """The split cannot be held as one uint8 tensor (mixed image sizes, or too big for host RAM)."""
+    """The split cannot be cached (too big for host RAM, or mixed image sizes where they are refused)."""
 
 
 def _cache_budget_bytes() -> int:
@@ -72,17 +89,40 @@ def _cache_budget_bytes() -> int:
     return 16 << 30
 
 
-class DecodedCache:
-    """All images of a split, decoded once to uint8 HWC (optionally by the native PNG decoder)."""
+def _header_hw(path: str) -> Tuple[int, int]:
+    from PIL import Image
 
-    def __init__(self, samples: List[Tuple[str, int]], threads: int = 8, max_bytes: Optional[int] = None) -> None:
+    with Image.open(path) as im:
+        w, h = im.size
+    return h, w
+
+
+class DecodedCache:
+    """All images of a split, decoded once to uint8 HWC (PNGs by the native decoder where it can).
+
+    One image size of at most ``DATA.resize`` on both sides: ``images`` is [N,H,W,3].  Otherwise
+    (``ragged``): ``flat`` holds the images back to back, image i at ``offsets[i]`` with size
+    ``hw[i]``.  ``allow_mixed=False`` refuses a split of mixed sizes.  The budget is checked from
+    the file headers before anything is decoded."""
+
+    def __init__(self, samples: List[Tuple[str, int]], threads: int = 8, max_bytes: Optional[int] = None,
+                 allow_mixed: bool = True) -> None:
         paths = [p for p, _ in samples]
-        if paths:          # size the cache from the first image before decoding everything
-            h, w, _ = _decode(paths[0]).shape
-            need, budget = len(paths) * h * w * 3, (_cache_budget_bytes() if max_bytes is None else max_bytes)
-            if need > budget:
-                raise CacheUnavailable("decoded cache needs %.1f GB for %d images of %dx%d, budget %.1f GB "
-                                       "(B200_MAX_CACHE_GB)" % (need / 2**30, len(paths), h, w, budget / 2**30))
+        with ThreadPoolExecutor(max_workers=threads) as ex:
+            hw = list(ex.map(_header_hw, paths))
+        sizes = set(hw)
+        if len(sizes) > 1 and not allow_mixed:
+            raise CacheUnavailable("mixed image sizes (%s ...)" % sorted(sizes)[:4])
+        need = sum(h * w * 3 for h, w in hw)
+        budget = _cache_budget_bytes() if max_bytes is None else max_bytes
+        if need > budget:
+            raise CacheUnavailable("decoded cache needs %.1f GB for %d images, budget %.1f GB "
+                                   "(B200_MAX_CACHE_GB)" % (need / 2**30, len(paths), budget / 2**30))
+        self.labels = torch.tensor([l for _, l in samples], dtype=torch.int64)
+        self.ragged = bool(paths) and (len(sizes) > 1 or max(hw[0]) > DATA.resize)
+        if self.ragged:
+            self._decode_ragged(paths, hw, threads)
+            return
         images = None
         try:   # native multi-threaded PNG decode (csrc/png_decode.cpp), falls back to PIL
             from ..ops import native_decode_pngs
@@ -93,14 +133,37 @@ class DecodedCache:
         if images is None:
             with ThreadPoolExecutor(max_workers=threads) as ex:
                 arrays = list(ex.map(_decode, paths))
-            shapes = {a.shape for a in arrays}
-            if len(shapes) != 1:
-                raise CacheUnavailable("fused pipeline needs a uniform image size, found %s; "
-                                       "use pipeline='reference'" % sorted(shapes)[:4])
             images = torch.from_numpy(np.stack(arrays))
         self.images = images                                          # [N,H,W,3] uint8
-        self.labels = torch.tensor([l for _, l in samples], dtype=torch.int64)
         self.src_hw = (int(self.images.shape[1]), int(self.images.shape[2]))
+
+    def _decode_ragged(self, paths: List[str], hw: List[Tuple[int, int]], threads: int) -> None:
+        self.images, self.src_hw = None, None
+        self.hw = torch.tensor(hw, dtype=torch.int64).view(-1, 2)
+        nbytes = self.hw[:, 0] * self.hw[:, 1] * 3
+        self.offsets = torch.cumsum(nbytes, 0) - nbytes
+        self.flat = torch.empty(int(nbytes.sum()), dtype=torch.uint8)
+        done = torch.zeros(len(paths), dtype=torch.bool)
+        png = [i for i, p in enumerate(paths) if p.lower().endswith(".png")]
+        from .. import ops
+        if png and ops.available():
+            sel = torch.tensor(png, dtype=torch.int64)
+            ok = ops.require().decode_pngs_into([paths[i] for i in png], self.flat, self.offsets[sel].contiguous(),
+                                                self.hw[sel].contiguous(), threads)
+            done[sel] = ok
+        self.native_decode = int(done.sum())          # images the native decoder wrote
+
+        def pil(i: int) -> None:
+            a = _decode(paths[i])
+            h, w = int(self.hw[i, 0]), int(self.hw[i, 1])
+            if a.shape != (h, w, 3):
+                raise ValueError("%s decodes to %s, its header says %dx%d" % (paths[i], a.shape, h, w))
+            off = int(self.offsets[i])
+            self.flat[off:off + h * w * 3].numpy().reshape(h, w, 3)[...] = a
+
+        rest = [i for i in range(len(paths)) if not bool(done[i])]
+        with ThreadPoolExecutor(max_workers=threads) as ex:
+            list(ex.map(pil, rest))
 
 
 class _FusedLoader:
@@ -116,12 +179,21 @@ class _FusedLoader:
         self.prefetch = prefetch
         self.pin = torch.cuda.is_available() if pin is None else pin
         self.epoch = 0
-        H, W = cache.src_hw
-        self.resized_hw = T.resized_dims(train, H, W)
+        self.ragged = cache.ragged
         slots = prefetch + 1
-        self._img = self._buf((slots, mb, H, W, 3), torch.uint8)
         self._par = self._buf((slots, mb, T.PARAM_DIM), torch.float32)
         self._lab = self._buf((slots, mb), torch.int64)
+        if self.ragged:
+            # a slot holds any batch: the mb largest images of the split
+            sizes = (cache.hw[:, 0] * cache.hw[:, 1] * 3).sort(descending=True).values
+            self.resized_hw = None
+            self._img = self._buf((slots, max(int(sizes[:mb].sum()), 1)), torch.uint8)
+            self._geom = self._buf((slots, mb, T.GEOM_DIM), torch.int64)
+        else:
+            H, W = cache.src_hw
+            self.resized_hw = T.resized_dims(train, H, W)
+            self._img = self._buf((slots, mb, H, W, 3), torch.uint8)
+            self._geom = None
         self._ring = [(self._img[s], self._par[s], self._lab[s]) for s in range(slots)]
         self._state = [{} for _ in range(slots)]
         self._pf = None
@@ -129,10 +201,13 @@ class _FusedLoader:
             try:
                 from .. import ops
                 if ops.available() and hasattr(ops.require(), "Prefetcher"):
+                    extra = {}
+                    if self.ragged:
+                        extra = dict(offsets=cache.offsets, hw=cache.hw, ring_geom=self._geom, resize=DATA.resize)
                     self._pf = ops.require().Prefetcher(
-                        cache.images, cache.labels, self._img, self._par, self._lab, train,
-                        DATA.crop_scale[0], DATA.crop_scale[1], DATA.crop_ratio[0], DATA.crop_ratio[1],
-                        DATA.rotation_deg)
+                        cache.flat if self.ragged else cache.images, cache.labels, self._img, self._par, self._lab,
+                        train, DATA.crop_scale[0], DATA.crop_scale[1], DATA.crop_ratio[0], DATA.crop_ratio[1],
+                        DATA.rotation_deg, **extra)
             except Exception:
                 if native:
                     raise
@@ -163,6 +238,14 @@ class _FusedLoader:
     def _epoch_seed(self) -> int:
         return 1_000_003 * (self.seed + 1) + self.epoch * 7919 + (self.sampler.rank if self.sampler else 0)
 
+    def _batch(self, slot: int, k: int):
+        img, par, lab = self._ring[slot]
+        if not self.ragged:
+            return FusedBatch(img[:k], par[:k], lab[:k], self.resized_hw, self._state[slot])
+        geom = self._geom[slot][:k]
+        used = int(geom[k - 1, 0] + geom[k - 1, 1] * geom[k - 1, 2] * 3)
+        return RaggedBatch(img[:used], geom, par[:k], lab[:k], self._state[slot])
+
     def __iter__(self) -> Iterator[FusedBatch]:
         if self._pf is not None:
             return self._iter_native()
@@ -183,9 +266,8 @@ class _FusedLoader:
                 if item is None:
                     break
                 slot, k = item
-                img, par, lab = self._ring[slot]
                 prev = slot
-                yield FusedBatch(img[:k], par[:k], lab[:k], self.resized_hw, self._state[slot])
+                yield self._batch(slot, k)
         finally:
             self._pf.stop()
 
@@ -193,7 +275,7 @@ class _FusedLoader:
     def _iter_python(self) -> Iterator[FusedBatch]:
         idx = self._indices()
         gen = torch.Generator().manual_seed(self._epoch_seed())
-        H, W = self.cache.src_hw
+        H, W = self.cache.src_hw or (0, 0)
         q: "queue.Queue" = queue.Queue(maxsize=self.prefetch)
         free: "queue.Queue" = queue.Queue()
         for slot in range(len(self._ring)):
@@ -208,10 +290,19 @@ class _FusedLoader:
                 if ev is not None:
                     ev.synchronize()        # async H2D of the previous occupant has finished
                 img, par, lab = self._ring[slot]
-                torch.index_select(self.cache.images, 0, sel, out=img[:k])
                 torch.index_select(self.cache.labels, 0, sel, out=lab[:k])
-                par[:k] = (T.sample_train_params(k, H, W, gen) if self.train
-                           else T.val_params(k, H, W))
+                if self.ragged:
+                    hw = self.cache.hw[sel]
+                    geom = self._geom[slot][:k]
+                    geom.copy_(T.ragged_geometry(hw.tolist(), self.train))
+                    for i, (h, w) in enumerate(hw.tolist()):
+                        off, o, n = int(self.cache.offsets[sel[i]]), int(geom[i, 0]), h * w * 3
+                        img[o:o + n].copy_(self.cache.flat[off:off + n])
+                        par[i] = (T.sample_train_params(1, h, w, gen) if self.train else T.val_params(1, h, w))[0]
+                else:
+                    torch.index_select(self.cache.images, 0, sel, out=img[:k])
+                    par[:k] = (T.sample_train_params(k, H, W, gen) if self.train
+                               else T.val_params(k, H, W))
                 q.put((slot, k))
             q.put(None)
 
@@ -225,9 +316,8 @@ class _FusedLoader:
             if item is None:
                 break
             slot, k = item
-            img, par, lab = self._ring[slot]
             prev = slot
-            yield FusedBatch(img[:k], par[:k], lab[:k], self.resized_hw, self._state[slot])
+            yield self._batch(slot, k)
         th.join()
 
 
@@ -289,7 +379,7 @@ class DataManager:
             sampler = ShardedSampler(self.data_size, world_size, rank, shuffle=False, pad=False)
         if pipeline in ("fused", "auto"):
             try:
-                self.cache = DecodedCache(self.samples, decode_threads)
+                self.cache = DecodedCache(self.samples, decode_threads, allow_mixed=pipeline == "fused")
             except CacheUnavailable as e:
                 if pipeline == "fused":
                     raise

@@ -136,6 +136,107 @@ def augment_reference(src: torch.Tensor, params: torch.Tensor, resized_hw: Tuple
     return ((val - m) / sd).permute(0, 3, 1, 2).contiguous()
 
 
+# ------------------------------------------------------------------------------ ragged (any size)
+# Pillow's 8-bit resampler (libImaging/Resample.c) keeps 22 fractional bits in its fixed-point weights.
+PIL_PRECISION_BITS = 22
+# geometry row of a ragged batch: [byte offset into the batch's flat uint8 buffer, H, W, RH, RW]
+GEOM_DIM = 5
+
+
+def _pil_bilinear_coeffs(in_size: int, out_size: int):
+    """Pillow's BILINEAR coefficients for one axis: (lo [out], k int64 [out, taps]) with k = 0 past
+    each row's window.  Every operation is the fp64 one of precompute_coeffs / normalize_coeffs_8bpc."""
+    import numpy as np
+
+    scale = in_size / out_size
+    fs = max(scale, 1.0)
+    support, ss = fs, 1.0 / fs
+    taps = int(math.ceil(support)) * 2 + 1
+    lo = np.zeros(out_size, np.int64)
+    k = np.zeros((out_size, taps), np.int64)
+    for i in range(out_size):
+        center = (i + 0.5) * scale
+        xmin = max(int(center - support + 0.5), 0)
+        xmax = min(int(center + support + 0.5), in_size) - xmin
+        w = [max(0.0, 1.0 - abs((x + xmin - center + 0.5) * ss)) for x in range(xmax)]
+        ww = 0.0
+        for v in w:
+            ww += v
+        for x, v in enumerate(w):
+            v = v / ww if ww != 0.0 else v
+            k[i, x] = int(-0.5 + v * (1 << PIL_PRECISION_BITS)) if v < 0 else int(0.5 + v * (1 << PIL_PRECISION_BITS))
+        lo[i] = xmin
+    return lo, k
+
+
+def pil_resize_reference(img_u8, out_h: int, out_w: int):
+    """``Image.fromarray(img).resize((out_w, out_h), Image.BILINEAR)`` bit for bit, for uint8 HWC RGB:
+    the horizontal pass first, rounded to uint8, then the vertical pass; an unchanged axis is skipped.
+    Accepts and returns a numpy array (a torch tensor in gives a torch tensor out)."""
+    import numpy as np
+
+    as_torch = isinstance(img_u8, torch.Tensor)
+    src = (img_u8.numpy() if as_torch else np.asarray(img_u8)).astype(np.int64)
+    half, shift = 1 << (PIL_PRECISION_BITS - 1), PIL_PRECISION_BITS
+    H, W = src.shape[:2]
+    if out_w != W:
+        lo, k = _pil_bilinear_coeffs(W, out_w)
+        idx = np.minimum(lo[:, None] + np.arange(k.shape[1])[None, :], W - 1)       # k = 0 past the window
+        src = np.clip((half + (src[:, idx, :] * k[None, :, :, None]).sum(2)) >> shift, 0, 255)
+    if out_h != H:
+        lo, k = _pil_bilinear_coeffs(H, out_h)
+        idx = np.minimum(lo[:, None] + np.arange(k.shape[1])[None, :], H - 1)
+        src = np.clip((half + (src[idx, :, :] * k[:, :, None, None]).sum(1)) >> shift, 0, 255)
+    out = src.astype(np.uint8)
+    return torch.from_numpy(out) if as_torch else out
+
+
+def ragged_geometry(hw, train: bool, resize: int = DATA.resize) -> torch.Tensor:
+    """Geometry rows [k, GEOM_DIM] of images of sizes ``hw`` ([k, 2]) gathered back to back."""
+    g = torch.zeros(len(hw), GEOM_DIM, dtype=torch.int64)
+    off = 0
+    for i, (h, w) in enumerate(hw):
+        h, w = int(h), int(w)
+        g[i, 0], g[i, 1], g[i, 2] = off, h, w
+        g[i, 3], g[i, 4] = resized_dims(train, h, w, resize)
+        off += h * w * 3
+    return g
+
+
+def ragged_reference(data_u8: torch.Tensor, geom: torch.Tensor, params: torch.Tensor,
+                     out_hw: int = DATA.crop, mean=DATA.mean, std=DATA.std) -> torch.Tensor:
+    """The reference chain for images of any size, with Pillow's resampling.  data_u8: the flat uint8
+    buffer the geometry rows point into; params rows as ``sample_train_params`` / ``val_params``.
+    Per image: crop box -> Pillow BILINEAR resize to (RH, RW) -> nearest rotation with zero fill ->
+    flip -> centre crop -> normalise (float32, as ToTensor + Normalize).  Val rows (box = the whole
+    image, no rotation, no flip) are Resize + CenterCrop.  -> float32 [k, 3, out_hw, out_hw]."""
+    n = int(geom.shape[0])
+    data = data_u8.cpu()
+    out = torch.empty(n, 3, out_hw, out_hw, dtype=torch.float32)
+    ys, xs = torch.meshgrid(torch.arange(out_hw, dtype=torch.float32),
+                            torch.arange(out_hw, dtype=torch.float32), indexing="ij")
+    m = torch.tensor(mean, dtype=torch.float32).view(3, 1, 1)
+    sd = torch.tensor(std, dtype=torch.float32).view(3, 1, 1)
+    for i in range(n):
+        off, H, W, RH, RW = [int(v) for v in geom[i]]
+        p = params[i].to(torch.float32)
+        top, left, ch, cw = [int(v) for v in p[:4]]
+        img = data[off:off + H * W * 3].view(H, W, 3)[top:top + ch, left:left + cw]
+        res = pil_resize_reference(img.contiguous(), RH, RW)                       # uint8 [RH, RW, 3]
+        # the coordinate chain of augment_reference, evaluated in the same float32 operations
+        ay = ys + int(round((RH - out_hw) / 2.0))
+        ax = xs + int(round((RW - out_hw) / 2.0))
+        bx = (RW - 1) - ax if float(p[6]) > 0.5 else ax
+        dx, dy = bx + 0.5 - RW / 2.0, ay + 0.5 - RH / 2.0
+        rx = torch.floor(p[4] * dx - p[5] * dy + RW / 2.0)
+        ry = torch.floor(p[5] * dx + p[4] * dy + RH / 2.0)
+        inside = (rx >= 0) & (rx < RW) & (ry >= 0) & (ry < RH)
+        v = res[ry.long().clamp(0, RH - 1), rx.long().clamp(0, RW - 1)].permute(2, 0, 1).to(torch.float32)
+        v = torch.where(inside.unsqueeze(0), v, torch.zeros_like(v))
+        out[i] = (v / 255.0 - m) / sd
+    return out
+
+
 def reference_transforms(train: bool):
     """The literal torchvision pipeline of the reference (distributedVggf.py:88-95 / :103-108)."""
     from torchvision import transforms as T

@@ -29,7 +29,7 @@ import torch.distributed as dist
 
 from .. import ops
 from ..config import DATA, TRAIN
-from ..data.loader import FusedBatch
+from ..data.loader import FusedBatch, RaggedBatch
 from ..models import layout as L
 from ..models.vggf import VGGSpec, build_oracle
 from ..parallel.buckets import BucketPlan, engine_bucket_plan
@@ -294,6 +294,8 @@ class NativeEngine:
         self._src_u8 = [None, None]
         self._params_dev = [torch.zeros(B, 8, dtype=F32, device=dev) for _ in range(2)]
         self._labels_dev = [torch.zeros(B, dtype=torch.int64, device=dev) for _ in range(2)]
+        self._geom_dev = [torch.zeros(B, 5, dtype=torch.int64, device=dev) for _ in range(2)]   # RaggedBatch rows
+        self._inter_u8 = None        # RaggedBatch: horizontally filtered rows, written and read on one stream
         self._in_free = [None, None]           # event: the step that used this slot is done with it
         self.labels_dev = self._labels_dev[0]
         # first conv: fused kernels build the im2col operand in shared memory from NHWC4 pixels
@@ -374,6 +376,32 @@ class NativeEngine:
             # resident), then expand to the first conv's im2col rows with coalesced 16-byte stores
             ops.augment(self._src_u8[j][:b], self._params_dev[j][:b], self.x_nhwc[:b], batch.resized_hw,
                         out_hw=HW, mode="nhwc", pad=4)
+            if not self.fused_conv0:
+                C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
+            return b
+        if isinstance(batch, RaggedBatch):
+            b = int(batch.labels.shape[0])
+            nbytes = int(batch.data_u8.numel())
+            if self._src_u8[j] is None or self._src_u8[j].dim() != 1 or self._src_u8[j].numel() < nbytes:
+                # grows to the loader's slot capacity (the mb largest images) and then stays
+                self._src_u8[j] = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            need = ops.ragged_inter_bytes(batch.geom)
+            if self._inter_u8 is None or self._inter_u8.numel() < need:
+                self._inter_u8 = torch.empty(need, dtype=torch.uint8, device=self.device)
+            with torch.cuda.stream(self.copy_stream):
+                if self._in_free[j] is not None:
+                    self.copy_stream.wait_event(self._in_free[j])
+                self._src_u8[j][:nbytes].copy_(batch.data_u8, non_blocking=True)
+                self._geom_dev[j][:b].copy_(batch.geom, non_blocking=True)
+                self._params_dev[j][:b].copy_(batch.params, non_blocking=True)
+                self._labels_dev[j][:b].copy_(batch.labels, non_blocking=True)
+                h2d = torch.cuda.Event()
+                h2d.record(self.copy_stream)
+            if batch.state is not None:
+                batch.state["event"] = h2d
+            cur.wait_event(h2d)
+            ops.augment_ragged(self._src_u8[j][:nbytes], self._geom_dev[j][:b], self._params_dev[j][:b],
+                               self._inter_u8, self.x_nhwc[:b], batch.geom, batch.params, out_hw=HW)
             if not self.fused_conv0:
                 C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
             return b

@@ -171,6 +171,20 @@ def augment(src_u8, params, out, resized_hw: Tuple[int, int], out_hw: int = DATA
     return out
 
 
+def augment_ragged(data_u8, geom, params, inter, out, geom_host, params_host, out_hw: int = DATA.crop):
+    """Images of any sizes (data/loader.py::RaggedBatch on the device) -> normalised bf16 NHWC4
+    ``out``, resampled as Pillow does.  ``geom_host`` / ``params_host``: the CPU tensors the device
+    ``geom`` / ``params`` were copied from; ``inter`` holds ``ragged_inter_bytes(geom_host)``."""
+    require().augment_ragged(data_u8, geom, params, inter, out, geom_host, params_host, out_hw, out_hw,
+                             list(DATA.mean), list(DATA.std))
+    return out
+
+
+def ragged_inter_bytes(geom_host) -> int:
+    """Bytes of the intermediate ``augment_ragged`` needs for these geometry rows."""
+    return int(require().ragged_inter_bytes(geom_host))
+
+
 def native_decode_pngs(paths, threads: int = 8):
     """Multi-threaded native PNG decode (csrc/png_decode.cpp) -> uint8 tensor [N,H,W,3], or None when
     a file is not a plain 8-bit PNG / sizes differ / the extension is absent (caller uses PIL)."""

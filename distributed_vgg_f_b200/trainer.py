@@ -26,7 +26,7 @@ from typing import Optional
 import torch
 import torch.nn.functional as F
 
-from .data.loader import FusedBatch
+from .data.loader import FusedBatch, RaggedBatch
 from .utils.metrics import DeviceMeter
 
 
@@ -153,7 +153,7 @@ class Trainer:
 
     # ------------------------------------------------------------------------------------------
     def _to_device(self, batch):
-        if isinstance(batch, FusedBatch):
+        if isinstance(batch, (FusedBatch, RaggedBatch)):
             return batch.to_float(self.device)
         inputs, targets = batch
         return inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
