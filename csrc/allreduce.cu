@@ -23,6 +23,7 @@
 #include <cmath>
 #include <stdexcept>
 
+#include "adam.cuh"
 #include "api.h"
 #include "ptx.cuh"
 
@@ -38,7 +39,6 @@ namespace b200 {
 // finish; thin CTAs (bytes in flight = CTAs x 256 threads x UNR x 16 B) still keep the footprint of
 // each small.
 constexpr int AR_MAX_CTAS = 128;
-constexpr int AR_MAX_WORLD = 16;
 constexpr int AR_THREADS = 256;
 constexpr int AR_MIN_BLOCKS = 6;                                // __launch_bounds__ -> <= 40 registers
 constexpr int AR_SLOT_WORDS = 2 * AR_MAX_CTAS * AR_MAX_WORLD;   // two phases per slot
@@ -335,7 +335,10 @@ void allreduce_fused(const CommCtx& ctx, const float* grad_f32, float* grad_out_
 }
 
 // ------------------------------------------------------------ fused reduce-scatter + Adam + all-gather
-// EXPERIMENTAL (--zero1; written after the round-1 GPU budget was spent, not yet run on hardware).
+// EXPERIMENTAL (--zero1).  The two-shot variant has run on one H100 80GB HBM3 with emulated ranks
+// (tests/test_collectives_gpu.py, world 1 .. 16): owned cells, Adam state, wires and shadows bit for
+// bit, nothing written outside its range.  The handshake between real peers and the NVLS variant run
+// only in test_multigpu.py, on a host with several GPUs.
 //
 // ZeRO-1 in ONE kernel per bucket, over peer memory: the compute step (the optimizer) sits between
 // the two halves of the collective instead of after it.
@@ -352,8 +355,9 @@ void allreduce_fused(const CommCtx& ctx, const float* grad_f32, float* grad_out_
 // world size (by a factor of ws), the wire carries new weights instead
 // of averaged gradients (same bytes), and every replica ends with bit-identical bf16 weights by
 // construction.  The fp32 master and moments of a cell live on its owner only (gathered for
-// checkpoints by NativeEngine._zero1_gather).  The reduced gradient is rounded to bf16 once, exactly
-// like the wire of allreduce_kernel, so both paths produce the same update.
+// checkpoints by NativeEngine.prepare_export).  The reduced gradient is rounded to bf16 once, exactly
+// like the wire of allreduce_kernel, and both paths apply adam_update (adam.cuh), so they produce the
+// same update bit for bit.
 struct Zero1Args {
   CommCtx c;
   float* grad;             // local fp32 arena (nullptr: wire already holds the packed data)
@@ -385,13 +389,8 @@ __device__ __forceinline__ uint4 zero1_adam8(const Zero1Args& a, long long elem,
     vv[4 * h] = v4.x; vv[4 * h + 1] = v4.y; vv[4 * h + 2] = v4.z; vv[4 * h + 3] = v4.w;
   }
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {          // same arithmetic as adam_kernel (loss_optim.cu)
-    const float gk = g[k] + a.wd * pp[k];
-    mm[k] = a.b1 * mm[k] + (1.f - a.b1) * gk;
-    vv[k] = a.b2 * vv[k] + (1.f - a.b2) * gk * gk;
-    const float denom = sqrtf(vv[k]) * a.bc2_inv_sqrt + a.eps;
-    pp[k] -= a.lr * a.bc1_inv * mm[k] / denom;
-  }
+  for (int k = 0; k < 8; ++k)            // the update of adam_kernel at grad_scale 1, bit for bit
+    adam_update(g[k], 1.f, pp[k], mm[k], vv[k], a.lr * a.bc1_inv, a.b1, a.b2, a.eps, a.wd, a.bc2_inv_sqrt);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     __stcs(reinterpret_cast<float4*>(a.p + elem + 4 * h), make_float4(pp[4 * h], pp[4 * h + 1], pp[4 * h + 2], pp[4 * h + 3]));

@@ -550,12 +550,22 @@ struct PyPrefetcher {
 };
 
 // ------------------------------------------------------------------------------------------- comm
+// The collectives write into every peer's wire buffer and signal pad: a range past the wire or a slot
+// past the pad lands in another GPU's memory.  Every binding below refuses such operands before it
+// launches anything.
 struct PyComm {
   b200::CommCtx c;
+  int64_t wire_bytes;   // size of each rank's wire buffer
+  int64_t slots;        // barrier groups of each rank's signal pad (allreduce_signal_words(slots) words)
 };
 static PyComm make_comm(int64_t rank, int64_t world, int64_t wire_ptrs_dev, int64_t signal_ptrs_dev,
-                        int64_t wire_mc, int64_t signal_mc) {
+                        int64_t wire_mc, int64_t signal_mc, int64_t wire_bytes, int64_t slots) {
+  TORCH_CHECK(world >= 1 && world <= b200::AR_MAX_WORLD, "make_comm: world must be in [1, ", b200::AR_MAX_WORLD,
+              "], got ", world);
+  TORCH_CHECK(rank >= 0 && rank < world, "make_comm: rank ", rank, " is not in [0, ", world, ")");
+  TORCH_CHECK(wire_bytes >= 0 && slots >= 1, "make_comm: a wire of >= 0 bytes and at least one slot");
   PyComm p;
+  p.wire_bytes = wire_bytes; p.slots = slots;
   p.c.rank = (int)rank; p.c.world = (int)world;
   p.c.wire_ptrs = reinterpret_cast<void* const*>(wire_ptrs_dev);
   p.c.signal_ptrs = reinterpret_cast<uint32_t* const*>(signal_ptrs_dev);
@@ -568,9 +578,27 @@ static PyComm make_comm(int64_t rank, int64_t world, int64_t wire_ptrs_dev, int6
   p.c.timeout_ns = static_cast<unsigned long long>(secs * 1e9);
   return p;
 }
+// [start, start+n) of elements of `elem_bytes` inside the wire, and a slot inside the signal pad
+static void check_comm_range(const PyComm& comm, int64_t start, int64_t n, int64_t elem_bytes, int64_t slot,
+                             const char* op) {
+  TORCH_CHECK(start >= 0 && n >= 0, op, ": start and n must be >= 0");
+  TORCH_CHECK((start + n) * elem_bytes <= comm.wire_bytes, op, ": [", start, ", ", start + n, ") of ", elem_bytes,
+              "-byte elements runs past the ", comm.wire_bytes, "-byte wire");
+  TORCH_CHECK(slot >= 0 && slot < comm.slots, op, ": slot ", slot, " is not in [0, ", comm.slots, ")");
+}
+// an arena (gradient, optimizer state or shadow) the kernels address at [start, start+n) with 16-byte vectors
+static void check_arena(const at::Tensor& t, at::ScalarType dt, int64_t start, int64_t n, const char* op,
+                        const char* name) {
+  check_vec(t, dt, 16, op, name);
+  TORCH_CHECK(t.numel() >= start + n, op, ": ", name, " must hold start + n = ", start + n, " elements, got ",
+              t.numel());
+}
 static void allreduce(const PyComm& comm, c10::optional<at::Tensor> grad, c10::optional<at::Tensor> grad_out,
                       int64_t start, int64_t n, double inv_world, int64_t algo, bool wire_fp32, int64_t slot,
                       int64_t epoch, int64_t max_ctas) {
+  check_comm_range(comm, start, n, wire_fp32 ? 4 : 2, slot, "allreduce");
+  if (grad.has_value()) check_arena(*grad, at::kFloat, start, n, "allreduce", "grad");
+  if (grad_out.has_value()) check_arena(*grad_out, at::kFloat, start, n, "allreduce", "grad_out");
   b200::allreduce_fused(comm.c, f32p_opt(grad), f32p_opt(grad_out), start, n, (float)inv_world, (int)algo,
                         wire_fp32, (int)slot, (uint32_t)epoch, (int)max_ctas, cur_stream());
 }
@@ -583,6 +611,10 @@ static void zero1_step(const PyComm& comm, c10::optional<at::Tensor> grad, at::T
                   shadow.scalar_type() == at::kBFloat16 && p.numel() == m.numel() && p.numel() == v.numel() &&
                   p.numel() == shadow.numel() && start + n <= p.numel(),
               "zero1_step: full fp32 arenas (p, m, v) and the bf16 shadow of the same length");
+  check_comm_range(comm, start, n, 2, slot, "zero1_step");
+  if (grad.has_value()) check_arena(*grad, at::kFloat, start, n, "zero1_step", "grad");
+  for (auto* t : {&p, &m, &v}) check_arena(*t, at::kFloat, start, n, "zero1_step", "p, m and v");
+  check_arena(shadow, at::kBFloat16, start, n, "zero1_step", "shadow");
   b200::zero1_step(comm.c, grad.has_value() ? grad->data_ptr<float>() : nullptr, p.data_ptr<float>(),
                    m.data_ptr<float>(), v.data_ptr<float>(), bfp_mut(shadow), start, n, (float)inv_world, (int)algo,
                    (int)slot, (uint32_t)epoch, (int)max_ctas, (float)lr, (float)beta1, (float)beta2, (float)eps,
@@ -592,9 +624,13 @@ static int64_t allreduce_grid(int64_t n, int64_t world, int64_t max_ctas, bool w
   return b200::allreduce_grid(n, (int)world, (int)max_ctas, wire_fp32);
 }
 static void broadcast(const PyComm& comm, at::Tensor data, int64_t root, int64_t slot, int64_t epoch) {
+  check_vec(data, at::kFloat, 16, "broadcast", "data");
+  check_comm_range(comm, 0, data.numel(), 4, slot, "broadcast");
+  TORCH_CHECK(root >= 0 && root < comm.c.world, "broadcast: root ", root, " is not in [0, ", comm.c.world, ")");
   b200::broadcast_fused(comm.c, f32p(data), data.numel(), (int)root, (int)slot, (uint32_t)epoch, cur_stream());
 }
 static void barrier(const PyComm& comm, int64_t slot, int64_t epoch) {
+  check_comm_range(comm, 0, 0, 1, slot, "barrier");
   b200::device_barrier(comm.c, (int)slot, (uint32_t)epoch, cur_stream());
 }
 

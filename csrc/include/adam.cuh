@@ -1,0 +1,22 @@
+// One Adam step of one parameter (torch.optim.Adam with L2 weight decay, bias-corrected), shared by
+// adam_kernel (loss_optim.cu) and zero1_kernel (allreduce.cu) so that the fused ZeRO-1 step and the
+// replicated optimizer give the same update bit for bit.  Every rounding is spelled out: left to
+// itself, nvcc contracted `g * gscale + wd * p` to fma(g, gscale, wd * p) in one kernel and
+// `g + wd * p` to fma(wd, p, g) in the other, and the two differ in the last bit of the moments
+// (tests/test_collectives_gpu.py).
+#pragma once
+#include <cuda_runtime.h>
+
+namespace b200 {
+
+// lr_bc1 = lr / (1 - beta1^step), bc2_inv_sqrt = 1 / sqrt(1 - beta2^step), both rounded to fp32 once
+__device__ __forceinline__ void adam_update(float g, float gscale, float& p, float& m, float& v, float lr_bc1,
+                                            float b1, float b2, float eps, float wd, float bc2_inv_sqrt) {
+  const float gk = __fmaf_rn(g, gscale, __fmul_rn(wd, p));
+  m = __fmaf_rn(b1, m, __fmul_rn(1.f - b1, gk));
+  v = __fmaf_rn(b2, v, __fmul_rn(__fmul_rn(1.f - b2, gk), gk));
+  const float denom = __fmaf_rn(__fsqrt_rn(v), bc2_inv_sqrt, eps);
+  p = __fsub_rn(p, __fdiv_rn(__fmul_rn(lr_bc1, m), denom));
+}
+
+}  // namespace b200

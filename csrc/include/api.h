@@ -133,6 +133,7 @@ void nchw_f32_to_nhwc_bf16(const float* x, bf16* y, int N, int C, int H, int W, 
                            cudaStream_t s);
 
 // ---- cross-GPU (allreduce.cu) ------------------------------------------------------------------
+constexpr int AR_MAX_WORLD = 16;   // ranks of one CommCtx (the signal pad has a word per source rank)
 struct CommCtx {
   int rank, world;
   void* const* wire_ptrs;        // device array [world]: peers' wire buffers (bf16 or fp32)

@@ -8,6 +8,7 @@
 #include <cstdlib>
 #include <stdexcept>
 
+#include "adam.cuh"
 #include "api.h"
 #include "ptx.cuh"
 
@@ -287,13 +288,7 @@ __global__ void __launch_bounds__(256, 6) adam_kernel(float* __restrict__ p, flo
     float mm[4] = {mv.x, mv.y, mv.z, mv.w};
     float vs[4] = {vv.x, vv.y, vv.z, vv.w};
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      float gk = g[k] * gscale + wd * pp[k];
-      mm[k] = b1 * mm[k] + (1.f - b1) * gk;
-      vs[k] = b2 * vs[k] + (1.f - b2) * gk * gk;
-      const float denom = sqrtf(vs[k]) * bc2_inv_sqrt + eps;
-      pp[k] -= lr * bc1_inv * mm[k] / denom;
-    }
+    for (int k = 0; k < 4; ++k) adam_update(g[k], gscale, pp[k], mm[k], vs[k], lr * bc1_inv, b1, b2, eps, wd, bc2_inv_sqrt);
     __stcs(reinterpret_cast<float4*>(p) + i, make_float4(pp[0], pp[1], pp[2], pp[3]));
     __stcs(reinterpret_cast<float4*>(m) + i, make_float4(mm[0], mm[1], mm[2], mm[3]));
     __stcs(reinterpret_cast<float4*>(v) + i, make_float4(vs[0], vs[1], vs[2], vs[3]));

@@ -66,7 +66,8 @@ class SymmetricArena:
             int(getattr(self.wire_hdl, "multicast_ptr", 0) or 0) != 0
         mc = int(self.wire_hdl.multicast_ptr) if self.has_multicast else 0
         self.comm = C.make_comm(self.rank, self.world, int(self.wire_hdl.buffer_ptrs_dev),
-                                int(self.flags_hdl.buffer_ptrs_dev), mc, 0)
+                                int(self.flags_hdl.buffer_ptrs_dev), mc, 0,
+                                self.wire.numel() * self.wire.element_size(), slots)
         self.slots = slots
         self._epoch: Dict[int, int] = {}
         self._algo = {"oneshot": C.AR_ONESHOT, "twoshot": C.AR_TWOSHOT, "nvls": C.AR_NVLS}
