@@ -43,7 +43,9 @@ def _rup8(v):
 GEMM_KK_SHAPES = [
     (128, 64, 64), (256, 64, 512), (4096, 64, 4096), (200, 48, 200), (4096, 96, 25088 // 8),
     # N <= 32: 32-wide tiles (FC forward at batch <= 32, ragged last batches)
-    (4096, 1, 25088), (4096, 5, 4096), (512, 16, 4096), (4096, 32, 25088), (10, 37, 512)]
+    (4096, 1, 25088), (4096, 5, 4096), (512, 16, 4096), (4096, 32, 25088), (10, 37, 512),
+    # N > 128: batches above 128 run two or more N tiles of the swap-AB forward
+    (4096, 256, 4096), (1000, 130, 512), (512, 200, 25088 // 8)]
 GEMM_KK = pytest.mark.parametrize("M,N,K", GEMM_KK_SHAPES)
 KSPLITS = [1, 4, 8]
 KSPLIT = pytest.mark.parametrize("ksplit", KSPLITS)
@@ -74,7 +76,8 @@ def _gemm_kk(M, N, K, ksplit, mode):
     KC.check(out, ref, mag, chain=KC.gemm_chain(K, ksplit), exact=mode == "exact", family="gemm")
 
 
-GEMM_MNK_SHAPES = [(128, 64, 64), (25088 // 4, 64, 4096), (300, 40, 130), (4096, 32, 4096), (512, 3, 10)]
+GEMM_MNK_SHAPES = [(128, 64, 64), (25088 // 4, 64, 4096), (300, 40, 130), (4096, 32, 4096), (512, 3, 10),
+                   (4096, 256, 4096), (300, 129, 130)]                  # N > 128: two N tiles
 GEMM_MNK = pytest.mark.parametrize("M,N,K", GEMM_MNK_SHAPES)
 
 
@@ -91,7 +94,8 @@ def test_gemm_mnk_store_t_exact(M, N, K):
 
 
 GEMM_MNK_ATOMIC = [(4096, 64, 4096, 8), (4096, 37, 4096, 8), (4096, 16, 512, 8), (25088, 5, 4096, 8),
-                   (4096, 64, 4096, 1), (512, 10, 10, 1)]
+                   (4096, 64, 4096, 1), (512, 10, 10, 1), (25088, 256, 4096, 8), (4096, 144, 512, 1),
+                   (4096, 192, 4096, 4)]
 
 
 @pytest.mark.parametrize("mode", MODES)
