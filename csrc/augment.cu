@@ -59,16 +59,32 @@ __device__ __forceinline__ void aug_sample(const uint8_t* __restrict__ src, cons
 }
 
 // mode 0: NHWC bf16, C padded to `pad` (pad in {4, 8}); one thread per output pixel.
+// MIX (augment_mixed): MixNone is the plain transform.  The partner of sample n is n-1 mod N.
+//   MixCutMix: a pixel inside the box evaluates the partner's chain (its source and params), one
+//              evaluation per pixel either way.
+//   MixMixUp:  both chains, blended in fp32 as lam * x_n + (1 - lam) * x_partner, rounded to bf16 once.
+template <int MIX>
 __global__ void augment_nhwc_kernel(const uint8_t* __restrict__ src, const float* __restrict__ params,
-                                    bf16* __restrict__ out, AugGeom g, int pad) {
+                                    bf16* __restrict__ out, AugGeom g, int pad, MixParams mix) {
   const long long total = static_cast<long long>(g.N) * g.OH * g.OW;
+  const long long img = static_cast<long long>(g.SH) * g.SW * 3;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int ox = i % g.OW;
     const int oy = (i / g.OW) % g.OH;
-    const int n = static_cast<int>(i / (static_cast<long long>(g.OW) * g.OH));
+    int n = static_cast<int>(i / (static_cast<long long>(g.OW) * g.OH));
     float v[3];
-    aug_sample(src + static_cast<long long>(n) * g.SH * g.SW * 3, params + n * 8, g, oy, ox, v);
+    if constexpr (MIX == MixCutMix) {
+      if (ox >= mix.x1 && ox < mix.x2 && oy >= mix.y1 && oy < mix.y2) n = n == 0 ? g.N - 1 : n - 1;
+    }
+    aug_sample(src + n * img, params + n * 8, g, oy, ox, v);
+    if constexpr (MIX == MixMixUp) {
+      const int p = n == 0 ? g.N - 1 : n - 1;
+      float w[3];
+      aug_sample(src + p * img, params + p * 8, g, oy, ox, w);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) v[c] = __fadd_rn(__fmul_rn(mix.lam, v[c]), __fmul_rn(mix.lam_b, w[c]));
+    }
     bf16* o = out + i * pad;
     if (pad == 4) {          // one 8-byte store per pixel
       *reinterpret_cast<uint2*>(o) = make_uint2(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], 0.f));
@@ -129,7 +145,7 @@ void augment_fused(const uint8_t* src, const float* params, bf16* out, int N, in
   const long long pixels = static_cast<long long>(N) * OH * OW;
   if (mode == 0) {
     const int blocks = static_cast<int>((pixels + 255) / 256 < sm_count() * 16 ? (pixels + 255) / 256 : sm_count() * 16);
-    augment_nhwc_kernel<<<blocks, 256, 0, s>>>(src, params, out, g, pad);
+    augment_nhwc_kernel<MixNone><<<blocks, 256, 0, s>>>(src, params, out, g, pad, MixParams{});
   } else {
     if (pad < 32 || pad % 8) throw std::runtime_error("[b200] augment_fused: kpad must be a multiple of 8, >= 32");
     const long long total = pixels * (pad / 8);
@@ -138,6 +154,23 @@ void augment_fused(const uint8_t* src, const float* params, bf16* out, int N, in
   }
   count_launch();
   check_last("augment_fused");
+}
+
+void augment_mixed(const uint8_t* src, const float* params, bf16* out, int N, int SH, int SW, int RH, int RW,
+                   int OH, int OW, int pad, const float* mean, const float* stdv, const MixParams& mix,
+                   cudaStream_t s) {
+  if (mix.kind != MixMixUp && mix.kind != MixCutMix) throw std::runtime_error("[b200] augment_mixed: kind is MixUp or CutMix");
+  AugGeom g;
+  g.N = N; g.SH = SH; g.SW = SW; g.RH = RH; g.RW = RW; g.OH = OH; g.OW = OW;
+  for (int c = 0; c < 3; ++c) { g.mean[c] = mean[c]; g.inv_std[c] = 1.f / stdv[c]; }
+  const long long pixels = static_cast<long long>(N) * OH * OW;
+  const int blocks = static_cast<int>((pixels + 255) / 256 < sm_count() * 16 ? (pixels + 255) / 256 : sm_count() * 16);
+  if (mix.kind == MixMixUp)
+    augment_nhwc_kernel<MixMixUp><<<blocks, 256, 0, s>>>(src, params, out, g, pad, mix);
+  else
+    augment_nhwc_kernel<MixCutMix><<<blocks, 256, 0, s>>>(src, params, out, g, pad, mix);
+  count_launch();
+  check_last("augment_mixed");
 }
 
 // ------------------------------------------------------------------ ragged batches, Pillow resampling
@@ -269,49 +302,81 @@ __global__ void augment_ragged_h_kernel(const uint8_t* __restrict__ src, const l
   }
 }
 
-// Pass 2: one thread per output pixel: chain -> (rx, ry), vertical filter down column rx of the
-// intermediate -> uint8 -> normalise -> bf16, one 8-byte NHWC4 store.
+// Normalised value of output pixel (oy, ox) of a ragged image: chain -> (rx, ry), vertical filter down
+// column rx of the intermediate -> uint8 -> normalise.
+__device__ __forceinline__ void ragged_pixel(const RaggedImage& im, const PilAxis& va, const float* prm,
+                                             const uint8_t* __restrict__ inter, const RaggedGeom& g, int oy, int ox,
+                                             float (&o)[3]) {
+  float rx, ry;
+  ragged_chain(prm, im.RH, im.RW, g.OH, g.OW, oy, ox, rx, ry);
+  float v[3] = {0.f, 0.f, 0.f};
+  if (rx >= 0.f && rx < im.RW && ry >= 0.f && ry < im.RH) {     // rotation fill = 0 (pre-normalise)
+    const PilWindow w = pil_window(va, static_cast<int>(ry));
+    const long long stride = static_cast<long long>(im.RW) * 3;
+    const uint8_t* s = inter + im.inter + w.lo * stride + static_cast<int>(rx) * 3;
+    int a0 = 1 << (kPilBits - 1), a1 = a0, a2 = a0;
+    for (int t = 0; t < w.n; ++t) {
+      const int k = pil_fixed(va, w, t);
+      a0 += s[t * stride] * k; a1 += s[t * stride + 1] * k; a2 += s[t * stride + 2] * k;
+    }
+    v[0] = pil_clip8(a0); v[1] = pil_clip8(a1); v[2] = pil_clip8(a2);
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) o[c] = __fdiv_rn(__fsub_rn(__fdiv_rn(v[c], 255.f), g.mean[c]), g.stdv[c]);
+}
+
+// Pass 2: one thread per output pixel: ragged_pixel, one 8-byte NHWC4 store.  MIX as for
+// augment_nhwc_kernel: the partner's intermediate covers every (oy, ox) of its own output, so pass 1
+// needs no change.
+template <int MIX>
 __global__ void augment_ragged_v_kernel(const long long* __restrict__ geom, const float* __restrict__ params,
-                                        const uint8_t* __restrict__ inter, bf16* __restrict__ out, RaggedGeom g) {
-  __shared__ RaggedImage im;
-  const int n = blockIdx.y;
+                                        const uint8_t* __restrict__ inter, bf16* __restrict__ out, RaggedGeom g,
+                                        MixParams mix) {
+  __shared__ RaggedImage im, pim;
+  const int n = blockIdx.y, p = n == 0 ? g.N - 1 : n - 1;
   if (threadIdx.x == 0) load_ragged_image(geom, params, n, g.OH, g.OW, im);
+  if (MIX != MixNone && threadIdx.x == 32) load_ragged_image(geom, params, p, g.OH, g.OW, pim);
   __syncthreads();
   const PilAxis va = pil_axis(im.ch, im.RH);
-  const float* prm = params + n * 8;
+  PilAxis pva = va;
+  if constexpr (MIX != MixNone) pva = pil_axis(pim.ch, pim.RH);
   const int pixels = g.OH * g.OW;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < pixels; i += gridDim.x * blockDim.x) {
     const int oy = i / g.OW, ox = i % g.OW;
-    float rx, ry;
-    ragged_chain(prm, im.RH, im.RW, g.OH, g.OW, oy, ox, rx, ry);
-    float v[3] = {0.f, 0.f, 0.f};
-    if (rx >= 0.f && rx < im.RW && ry >= 0.f && ry < im.RH) {     // rotation fill = 0 (pre-normalise)
-      const PilWindow w = pil_window(va, static_cast<int>(ry));
-      const long long stride = static_cast<long long>(im.RW) * 3;
-      const uint8_t* s = inter + im.inter + w.lo * stride + static_cast<int>(rx) * 3;
-      int a0 = 1 << (kPilBits - 1), a1 = a0, a2 = a0;
-      for (int t = 0; t < w.n; ++t) {
-        const int k = pil_fixed(va, w, t);
-        a0 += s[t * stride] * k; a1 += s[t * stride + 1] * k; a2 += s[t * stride + 2] * k;
-      }
-      v[0] = pil_clip8(a0); v[1] = pil_clip8(a1); v[2] = pil_clip8(a2);
-    }
     float o[3];
+    if constexpr (MIX == MixCutMix) {
+      if (ox >= mix.x1 && ox < mix.x2 && oy >= mix.y1 && oy < mix.y2)
+        ragged_pixel(pim, pva, params + p * 8, inter, g, oy, ox, o);
+      else
+        ragged_pixel(im, va, params + n * 8, inter, g, oy, ox, o);
+    } else {
+      ragged_pixel(im, va, params + n * 8, inter, g, oy, ox, o);
+    }
+    if constexpr (MIX == MixMixUp) {
+      float w[3];
+      ragged_pixel(pim, pva, params + p * 8, inter, g, oy, ox, w);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) o[c] = __fdiv_rn(__fsub_rn(__fdiv_rn(v[c], 255.f), g.mean[c]), g.stdv[c]);
+      for (int c = 0; c < 3; ++c) o[c] = __fadd_rn(__fmul_rn(mix.lam, o[c]), __fmul_rn(mix.lam_b, w[c]));
+    }
     *reinterpret_cast<uint2*>(out + (static_cast<long long>(n) * pixels + i) * 4) =
         make_uint2(pack_bf16x2(o[0], o[1]), pack_bf16x2(o[2], 0.f));
   }
 }
 
 void augment_ragged(const uint8_t* src, const long long* geom, const float* params, uint8_t* inter, bf16* out,
-                    int N, int OH, int OW, int grid_x, const float* mean, const float* stdv, cudaStream_t s) {
+                    int N, int OH, int OW, int grid_x, const float* mean, const float* stdv, cudaStream_t s,
+                    const MixParams* mix) {
   RaggedGeom g;
   g.N = N; g.OH = OH; g.OW = OW;
   for (int c = 0; c < 3; ++c) { g.mean[c] = mean[c]; g.stdv[c] = stdv[c]; }
   const dim3 grid(grid_x, N);
   augment_ragged_h_kernel<<<grid, 256, 0, s>>>(src, geom, params, inter, g);
-  augment_ragged_v_kernel<<<grid, 256, 0, s>>>(geom, params, inter, out, g);
+  if (!mix || mix->kind == MixNone)
+    augment_ragged_v_kernel<MixNone><<<grid, 256, 0, s>>>(geom, params, inter, out, g, MixParams{});
+  else if (mix->kind == MixMixUp)
+    augment_ragged_v_kernel<MixMixUp><<<grid, 256, 0, s>>>(geom, params, inter, out, g, *mix);
+  else
+    augment_ragged_v_kernel<MixCutMix><<<grid, 256, 0, s>>>(geom, params, inter, out, g, *mix);
   count_launch(2);
   check_last("augment_ragged");
 }

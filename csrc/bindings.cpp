@@ -230,10 +230,10 @@ static void cast_to_f32(const at::Tensor& x, at::Tensor y) {
   b200::cast_bf16_to_f32(bfp(x), f32p(y), x.numel(), cur_stream());
 }
 
-static void cross_entropy(const at::Tensor& logits, const at::Tensor& target, c10::optional<at::Tensor> dlogits,
-                          int64_t ldd, c10::optional<at::Tensor> meter, c10::optional<at::Tensor> loss_out,
-                          double grad_scale, c10::optional<at::Tensor> class_weights) {
-  c10::cuda::CUDAGuard g(logits.device());
+static void check_cross_entropy(const at::Tensor& logits, const at::Tensor& target,
+                                const c10::optional<at::Tensor>& dlogits, int64_t ldd,
+                                const c10::optional<at::Tensor>& meter, const c10::optional<at::Tensor>& loss_out,
+                                const c10::optional<at::Tensor>& class_weights) {
   TORCH_CHECK(target.scalar_type() == at::kLong && logits.is_contiguous(), "cross_entropy: int64 targets, contiguous logits");
   TORCH_CHECK(logits.dim() == 2, "cross_entropy: logits must be [B, C]");
   const int64_t B = logits.size(0), C = logits.size(1);
@@ -244,10 +244,38 @@ static void cross_entropy(const at::Tensor& logits, const at::Tensor& target, c1
   TORCH_CHECK(!meter.has_value() || meter->numel() >= 3, "cross_entropy: meter must have 3 elements");
   TORCH_CHECK(!loss_out.has_value() || loss_out->numel() >= 1, "cross_entropy: loss_out must have 1 element");
   TORCH_CHECK(!class_weights.has_value() || class_weights->numel() >= C, "cross_entropy: class_weights of C = ", C);
+}
+
+// Soft targets (label smoothing eps; with `mix`, row r's target also takes lam_b of row r-1's label):
+// the host values are checked here so that a bad draw cannot reach the kernels.
+static b200::SoftTargets soft_targets(const char* what, double eps, double lam, bool mix) {
+  TORCH_CHECK(eps >= 0.0 && eps < 1.0, what, ": label smoothing must lie in [0, 1), got ", eps);
+  TORCH_CHECK(!mix || (lam >= 0.0 && lam <= 1.0), what, ": the mixing weight must lie in [0, 1], got ", lam);
+  return b200::SoftTargets{(float)eps, mix ? (float)lam : 1.f, mix ? (float)(1.0 - lam) : 0.f, mix ? 1 : 0};
+}
+
+static void cross_entropy(const at::Tensor& logits, const at::Tensor& target, c10::optional<at::Tensor> dlogits,
+                          int64_t ldd, c10::optional<at::Tensor> meter, c10::optional<at::Tensor> loss_out,
+                          double grad_scale, c10::optional<at::Tensor> class_weights) {
+  c10::cuda::CUDAGuard g(logits.device());
+  check_cross_entropy(logits, target, dlogits, ldd, meter, loss_out, class_weights);
   b200::cross_entropy_fused(f32p(logits), reinterpret_cast<const long long*>(target.data_ptr()),
                             dlogits.has_value() ? bfp_mut(*dlogits) : nullptr, (int)ldd, f32p_opt(meter),
                             f32p_opt(loss_out), (int)logits.size(0), (int)logits.size(1), (float)grad_scale,
                             f32p_opt(class_weights), cur_stream());
+}
+
+static void cross_entropy_soft(const at::Tensor& logits, const at::Tensor& target, c10::optional<at::Tensor> dlogits,
+                               int64_t ldd, c10::optional<at::Tensor> meter, c10::optional<at::Tensor> loss_out,
+                               double grad_scale, c10::optional<at::Tensor> class_weights, double eps, double lam,
+                               bool mix) {
+  c10::cuda::CUDAGuard g(logits.device());
+  check_cross_entropy(logits, target, dlogits, ldd, meter, loss_out, class_weights);
+  const b200::SoftTargets st = soft_targets("cross_entropy_soft", eps, lam, mix);
+  b200::cross_entropy_soft(f32p(logits), reinterpret_cast<const long long*>(target.data_ptr()),
+                           dlogits.has_value() ? bfp_mut(*dlogits) : nullptr, (int)ldd, f32p_opt(meter),
+                           f32p_opt(loss_out), (int)logits.size(0), (int)logits.size(1), (float)grad_scale,
+                           f32p_opt(class_weights), st, cur_stream());
 }
 
 static void adam(at::Tensor p, at::Tensor m, at::Tensor v, c10::optional<at::Tensor> g32,
@@ -287,10 +315,9 @@ static void sgd(at::Tensor p, at::Tensor mom, c10::optional<at::Tensor> g32, c10
                   cur_stream());
 }
 
-static void augment(const at::Tensor& src, const at::Tensor& params, at::Tensor out, int64_t RH, int64_t RW,
-                    int64_t OH, int64_t OW, int64_t mode, int64_t pad, std::vector<double> mean,
-                    std::vector<double> stdv) {
-  c10::cuda::CUDAGuard g(src.device());
+static void check_augment(const at::Tensor& src, const at::Tensor& params, const at::Tensor& out, int64_t OH,
+                          int64_t OW, int64_t mode, int64_t pad, const std::vector<double>& mean,
+                          const std::vector<double>& stdv) {
   TORCH_CHECK(src.is_cuda() && src.scalar_type() == at::kByte && src.is_contiguous() && src.dim() == 4 && src.size(3) == 3,
               "augment: uint8 [N,H,W,3] CUDA tensor");
   const int64_t N = src.size(0);
@@ -302,9 +329,40 @@ static void augment(const at::Tensor& src, const at::Tensor& params, at::Tensor 
   TORCH_CHECK(mode == 1 || pad >= 3, "augment: NHWC pad must be >= 3");
   check_vec(out, at::kBFloat16, mode == 1 ? 16 : (pad == 4 ? 8 : 2), "augment", "out");
   TORCH_CHECK(out.numel() >= N * OH * OW * pad, "augment: out must hold N x OH x OW x pad elements");
+}
+
+static void augment(const at::Tensor& src, const at::Tensor& params, at::Tensor out, int64_t RH, int64_t RW,
+                    int64_t OH, int64_t OW, int64_t mode, int64_t pad, std::vector<double> mean,
+                    std::vector<double> stdv) {
+  c10::cuda::CUDAGuard g(src.device());
+  check_augment(src, params, out, OH, OW, mode, pad, mean, stdv);
   float m[3] = {(float)mean[0], (float)mean[1], (float)mean[2]}, s[3] = {(float)stdv[0], (float)stdv[1], (float)stdv[2]};
   b200::augment_fused(src.data_ptr<uint8_t>(), f32p(params), bfp_mut(out), src.size(0), src.size(1), src.size(2),
                       (int)RH, (int)RW, (int)OH, (int)OW, (int)mode, (int)pad, m, s, cur_stream());
+}
+
+// One batch's MixUp (kind 1: lam) or CutMix (kind 2: the box x1, y1, x2, y2 in output pixels) draw.
+static b200::MixParams mix_params(const char* what, int64_t kind, double lam, const std::vector<int64_t>& box,
+                                  int64_t OH, int64_t OW) {
+  TORCH_CHECK(kind == b200::MixMixUp || kind == b200::MixCutMix, what, ": kind is 1 (MixUp) or 2 (CutMix)");
+  TORCH_CHECK(lam >= 0.0 && lam <= 1.0, what, ": lam must lie in [0, 1], got ", lam);
+  TORCH_CHECK(box.size() == 4, what, ": box is (x1, y1, x2, y2)");
+  TORCH_CHECK(kind == b200::MixMixUp || (0 <= box[0] && box[0] <= box[2] && box[2] <= OW && 0 <= box[1] &&
+                                         box[1] <= box[3] && box[3] <= OH),
+              what, ": CutMix box (", box[0], ", ", box[1], ", ", box[2], ", ", box[3], ") outside ", OH, " x ", OW);
+  return b200::MixParams{(int)kind, (float)lam, (float)(1.0 - lam), (int)box[0], (int)box[1], (int)box[2], (int)box[3]};
+}
+
+static void augment_mixed(const at::Tensor& src, const at::Tensor& params, at::Tensor out, int64_t RH, int64_t RW,
+                          int64_t OH, int64_t OW, int64_t pad, std::vector<double> mean, std::vector<double> stdv,
+                          int64_t kind, double lam, std::vector<int64_t> box) {
+  c10::cuda::CUDAGuard g(src.device());
+  check_augment(src, params, out, OH, OW, 0, pad, mean, stdv);
+  TORCH_CHECK(src.size(0) >= 1 && src.size(0) <= (1 << 24), "augment_mixed: 1 to 2^24 images");
+  const b200::MixParams mix = mix_params("augment_mixed", kind, lam, box, OH, OW);
+  float m[3] = {(float)mean[0], (float)mean[1], (float)mean[2]}, s[3] = {(float)stdv[0], (float)stdv[1], (float)stdv[2]};
+  b200::augment_mixed(src.data_ptr<uint8_t>(), f32p(params), bfp_mut(out), src.size(0), src.size(1), src.size(2),
+                      (int)RH, (int)RW, (int)OH, (int)OW, (int)pad, m, s, mix, cur_stream());
 }
 // Bytes of the intermediate augment_ragged needs for these geometry rows: H x RW x 3 per image.
 static int64_t ragged_inter_bytes(const at::Tensor& geom) {
@@ -318,9 +376,10 @@ static int64_t ragged_inter_bytes(const at::Tensor& geom) {
 
 // The kernels read geom and params on the device; the host copies they were made from are checked
 // here, so that no row can send a launch outside src, inter or out.
-static void augment_ragged(const at::Tensor& src, const at::Tensor& geom, const at::Tensor& params, at::Tensor inter,
-                           at::Tensor out, const at::Tensor& geom_host, const at::Tensor& params_host, int64_t OH,
-                           int64_t OW, std::vector<double> mean, std::vector<double> stdv) {
+static void augment_ragged_impl(const at::Tensor& src, const at::Tensor& geom, const at::Tensor& params,
+                                at::Tensor inter, at::Tensor out, const at::Tensor& geom_host,
+                                const at::Tensor& params_host, int64_t OH, int64_t OW, const std::vector<double>& mean,
+                                const std::vector<double>& stdv, const b200::MixParams* mix) {
   c10::cuda::CUDAGuard g(src.device());
   TORCH_CHECK(src.is_cuda() && src.scalar_type() == at::kByte && src.is_contiguous(),
               "augment_ragged: src must be a contiguous CUDA uint8 tensor");
@@ -363,7 +422,21 @@ static void augment_ragged(const at::Tensor& src, const at::Tensor& geom, const 
   float m[3] = {(float)mean[0], (float)mean[1], (float)mean[2]}, s[3] = {(float)stdv[0], (float)stdv[1], (float)stdv[2]};
   b200::augment_ragged(src.data_ptr<uint8_t>(), reinterpret_cast<const long long*>(geom.data_ptr<int64_t>()),
                        f32p(params), inter.data_ptr<uint8_t>(), bfp_mut(out), (int)N, (int)OH, (int)OW, grid_x, m, s,
-                       cur_stream());
+                       cur_stream(), mix);
+}
+
+static void augment_ragged(const at::Tensor& src, const at::Tensor& geom, const at::Tensor& params, at::Tensor inter,
+                           at::Tensor out, const at::Tensor& geom_host, const at::Tensor& params_host, int64_t OH,
+                           int64_t OW, std::vector<double> mean, std::vector<double> stdv) {
+  augment_ragged_impl(src, geom, params, inter, out, geom_host, params_host, OH, OW, mean, stdv, nullptr);
+}
+
+static void augment_ragged_mixed(const at::Tensor& src, const at::Tensor& geom, const at::Tensor& params,
+                                 at::Tensor inter, at::Tensor out, const at::Tensor& geom_host,
+                                 const at::Tensor& params_host, int64_t OH, int64_t OW, std::vector<double> mean,
+                                 std::vector<double> stdv, int64_t kind, double lam, std::vector<int64_t> box) {
+  const b200::MixParams mix = mix_params("augment_ragged_mixed", kind, lam, box, OH, OW);
+  augment_ragged_impl(src, geom, params, inter, out, geom_host, params_host, OH, OW, mean, stdv, &mix);
 }
 static void im2col_c3(const at::Tensor& x, at::Tensor out, int64_t kpad) {
   c10::cuda::CUDAGuard g(x.device());
@@ -658,12 +731,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("cast_to_bf16", &cast_to_bf16);
   m.def("cast_to_f32", &cast_to_f32);
   m.def("cross_entropy", &cross_entropy);
+  m.def("cross_entropy_soft", &cross_entropy_soft);
   m.def("head_ce_supported", [](int64_t B, int64_t C, int64_t K) { return b200::head_ce_supported((int)B, (int)C, (int)K); });
   m.def("head_ce", [](const at::Tensor& h, const at::Tensor& W, const at::Tensor& bias, const at::Tensor& target,
                       at::Tensor logits, c10::optional<at::Tensor> dlogits, int64_t ldd, c10::optional<at::Tensor> dW,
                       c10::optional<at::Tensor> db, c10::optional<at::Tensor> dh, double drop_scale, bool relu,
                       c10::optional<at::Tensor> meter, c10::optional<at::Tensor> loss_out,
-                      c10::optional<at::Tensor> class_weights, bool accumulate) {
+                      c10::optional<at::Tensor> class_weights, bool accumulate,
+                      c10::optional<std::vector<double>> soft) {
     c10::cuda::CUDAGuard g(h.device());
     TORCH_CHECK(h.dim() == 2 && W.dim() == 2 && h.size(1) == W.size(1) && h.is_contiguous() && W.is_contiguous(),
                 "head_ce: h [B][K], W [C][K], contiguous");
@@ -684,20 +759,27 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(!meter.has_value() || meter->numel() >= 3, "head_ce: meter must have 3 elements");
     TORCH_CHECK(!loss_out.has_value() || loss_out->numel() >= 1, "head_ce: loss_out must have 1 element");
     TORCH_CHECK(!class_weights.has_value() || class_weights->numel() >= C, "head_ce: class_weights of C = ", C);
+    TORCH_CHECK(!soft.has_value() || soft->size() == 3, "head_ce: soft is (eps, lam, mix)");
+    b200::SoftTargets st{};
+    if (soft.has_value()) st = soft_targets("head_ce", (*soft)[0], (*soft)[1], (*soft)[2] != 0.0);
     b200::head_ce_fused(bfp(h), bfp(W), f32p(bias), reinterpret_cast<const long long*>(target.data_ptr()), f32p(logits),
                         dlogits.has_value() ? bfp_mut(*dlogits) : nullptr, (int)ldd, f32p_opt(dW), f32p_opt(db),
                         dh.has_value() ? bfp_mut(*dh) : nullptr, (float)drop_scale, relu, f32p_opt(meter),
                         f32p_opt(loss_out), (int)h.size(0), (int)W.size(0), (int)h.size(1), f32p_opt(class_weights),
-                        accumulate, cur_stream());
+                        accumulate, cur_stream(), soft.has_value() ? &st : nullptr);
   },
   // accumulate: dW += the batch's gradient instead of dW = (later micro-batches of an accumulation group)
   py::arg("h"), py::arg("W"), py::arg("bias"), py::arg("target"), py::arg("logits"), py::arg("dlogits"), py::arg("ldd"),
   py::arg("dW"), py::arg("db"), py::arg("dh"), py::arg("drop_scale"), py::arg("relu"), py::arg("meter"),
-  py::arg("loss_out"), py::arg("class_weights"), py::arg("accumulate") = false);
+  py::arg("loss_out"), py::arg("class_weights"), py::arg("accumulate") = false,
+  // soft = (eps, lam, mix): label smoothing and MixUp / CutMix targets (cross_entropy_soft); None: integer labels
+  py::arg("soft") = py::none());
   m.def("adam", &adam);
   m.def("sgd", &sgd);
   m.def("augment", &augment);
+  m.def("augment_mixed", &augment_mixed);
   m.def("augment_ragged", &augment_ragged);
+  m.def("augment_ragged_mixed", &augment_ragged_mixed);
   m.def("ragged_inter_bytes", &ragged_inter_bytes);
   m.def("im2col_c3", &im2col_c3);
   m.def("nchw_to_nhwc", &nchw_to_nhwc);

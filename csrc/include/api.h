@@ -92,6 +92,19 @@ void cross_entropy_fused(const float* logits, const long long* target, bf16* dlo
                          float* meter, float* loss_out, int B, int C, float grad_scale,
                          const float* class_weights, cudaStream_t s);
 
+// Soft targets of the loss (label smoothing eps, and MixUp / CutMix's probability targets).
+// Row r's target is t = (lam_a e_{y_r} + lam_b e_{y_(r-1) mod B}) (1 - eps) + eps / C when `mix`, else
+// (1 - eps) e_{y_r} + eps / C; the loss is sum_c w_c t_c (-log p_c) over rows, divided by sum_r w_{y_r}
+// for integer targets (B without class weights) and by B for probability targets (torch's rules).
+// A row is correct when argmax(logits) == argmax(lam_a e_{y_r} + lam_b e_{y_(r-1)}) (first maximum).
+struct SoftTargets {
+  float eps, lam_a, lam_b;
+  int mix;
+};
+void cross_entropy_soft(const float* logits, const long long* target, bf16* dlogits, int ldd, float* meter,
+                        float* loss_out, int B, int C, float grad_scale, const float* class_weights,
+                        const SoftTargets& st, cudaStream_t s);
+
 // K-FUN2+CE: last Linear(K -> C) + cross-entropy + metrics + the layer's whole backward in one launch
 // (C <= 8, K <= 1024, B <= 256).  h [B][K] bf16 (the previous FC layer's output), W [C][K] bf16.
 // Writes logits [B][C] fp32, meter / loss_out as cross_entropy_fused, optional dlogits (bf16, ld ldd);
@@ -101,7 +114,7 @@ bool head_ce_supported(int B, int C, int K);
 void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long long* target, float* logits,
                    bf16* dlogits, int ldd, float* dW, float* db, bf16* dh, float drop_scale, bool relu, float* meter,
                    float* loss_out, int B, int C, int K, const float* class_weights, bool accumulate,
-                   cudaStream_t s);
+                   cudaStream_t s, const SoftTargets* soft = nullptr);
 
 // Fused optimizers over flat arenas.  grad is fp32 (local) or bf16 (the reduced wire buffer).
 void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16, bf16* shadow,
@@ -116,15 +129,28 @@ void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* sh
 void augment_fused(const uint8_t* src, const float* params, bf16* out, int N, int SH, int SW,
                    int RH, int RW, int OH, int OW, int mode, int pad, const float* mean,
                    const float* stdv, cudaStream_t s);
+// MixUp / CutMix of one batch (data/transforms.py::MixDraw).  Sample n's partner is n - 1 mod N.
+// MixUp: lam * x_n + lam_b * x_partner in fp32 (lam_b = 1 - lam, rounded once on the host).  CutMix:
+// output pixels with x1 <= ox < x2 and y1 <= oy < y2 are the partner's.
+enum MixKind { MixNone = 0, MixMixUp = 1, MixCutMix = 2 };
+struct MixParams {
+  int kind;
+  float lam, lam_b;
+  int x1, y1, x2, y2;
+};
+// augment_fused mode 0 (NHWC, C padded to `pad`) with the batch mixed as `mix` says.
+void augment_mixed(const uint8_t* src, const float* params, bf16* out, int N, int SH, int SW, int RH, int RW,
+                   int OH, int OW, int pad, const float* mean, const float* stdv, const MixParams& mix,
+                   cudaStream_t s);
 // The same transform for a batch of images of any sizes, resampled exactly as Pillow's BILINEAR
 // resize does.  src: the images back to back; geom [N][5] int64 rows (byte offset, H, W, RH, RW);
 // params [N][8] as for augment_fused; inter: uint8 scratch of at least ragged_inter_bytes; out:
 // NHWC bf16 with 4 channels (the 4th written as 0).  grid_x: blocks per image of each launch.
 // Pass 1 filters the crop box horizontally into inter; pass 2 filters vertically, follows the
-// rotation / flip / centre-crop chain and normalises.
+// rotation / flip / centre-crop chain and normalises (and mixes the batch when `mix` says so).
 void augment_ragged(const uint8_t* src, const long long* geom, const float* params, uint8_t* inter,
                     bf16* out, int N, int OH, int OW, int grid_x, const float* mean,
-                    const float* stdv, cudaStream_t s);
+                    const float* stdv, cudaStream_t s, const MixParams* mix = nullptr);
 // im2col of an NHWC(3, padded to cpad) bf16 image for layer 0 (used when the input is given as a
 // float tensor instead of uint8 + params).
 void im2col3x3_c3(const bf16* x, bf16* out, int N, int H, int W, int cpad, int kpad,

@@ -14,11 +14,33 @@
 
 namespace b200 {
 
+// Soft-target coefficient of class c in a row (SoftTargets in api.h): loss_r = sum_c q_c (-log p_c),
+// q_c = w_c ((lam_a [c == t] + lam_b [c == tb]) (1 - eps) + eps / C); for integer targets lam_a = 1,
+// lam_b = 0.  Its gradient is (p_c sum_k q_k - q_c) / normaliser.
+__device__ __forceinline__ float soft_q(int c, int t, int tb, float la, float lb, float keep, float eps_c,
+                                        const float* __restrict__ cw) {
+  const float tc = ((c == t ? la : 0.f) + (c == tb ? lb : 0.f)) * keep + eps_c;
+  return cw ? cw[c] * tc : tc;
+}
+
+// Row r's partner label and the two target weights (lam_b = 0 without mixing), and argmax of the
+// unsmoothed target with torch's first-maximum rule.
+__device__ __forceinline__ void soft_row(const long long* __restrict__ target, int r, int B, const SoftTargets& st,
+                                         int& t, int& tb, float& la, float& lb, int& tmax) {
+  t = static_cast<int>(target[r]);
+  tb = st.mix ? static_cast<int>(target[r == 0 ? B - 1 : r - 1]) : t;
+  la = st.mix ? st.lam_a : 1.f;
+  lb = st.mix ? st.lam_b : 0.f;
+  tmax = (tb != t && (lb > la || (lb == la && tb < t))) ? tb : t;
+}
+
 // One block, one warp per row (round-robin).  C is small (3) or moderate (1000).
+// SOFT: label smoothing and / or mixed targets (cross_entropy_soft); !SOFT is the integer-label loss.
+template <bool SOFT>
 __global__ void cross_entropy_kernel(const float* __restrict__ logits, const long long* __restrict__ target,
                                      bf16* __restrict__ dlogits, int ldd, float* __restrict__ meter,
                                      float* __restrict__ loss_out, int B, int C, float grad_scale,
-                                     const float* __restrict__ cw) {
+                                     const float* __restrict__ cw, SoftTargets st) {
   __shared__ float s_loss[32], s_correct[32], s_wsum[32];
   __shared__ float s_total_w;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
@@ -37,12 +59,17 @@ __global__ void cross_entropy_kernel(const float* __restrict__ logits, const lon
     }
     __syncthreads();
   }
-  const float norm = cw ? 1.f / s_total_w : grad_scale;   // grad_scale == 1/B for the mean
+  // probability targets (mixed batches) are divided by B even with class weights, as torch does
+  const bool by_weight = cw && !(SOFT && st.mix);
+  const float norm = by_weight ? 1.f / s_total_w : grad_scale;   // grad_scale == 1/B for the mean
+  const float keep = 1.f - st.eps, eps_c = st.eps / static_cast<float>(C);
 
   float loss_acc = 0.f, correct_acc = 0.f;
   for (int r = warp; r < B; r += nwarps) {
     const float* row = logits + static_cast<long long>(r) * C;
-    const int t = static_cast<int>(target[r]);
+    int t = static_cast<int>(target[r]), tb = t, tmax = t;
+    float la = 1.f, lb = 0.f;
+    if constexpr (SOFT) soft_row(target, r, B, st, t, tb, la, lb, tmax);
     float mx = -INFINITY;
     int amax = 0x7fffffff;
     for (int c = lane; c < C; c += 32) {
@@ -58,17 +85,41 @@ __global__ void cross_entropy_kernel(const float* __restrict__ logits, const lon
     for (int c = lane; c < C; c += 32) se += __expf(row[c] - mx);
     for (int o = 16; o; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
     const float lse = mx + __logf(se);
-    const float w = cw ? cw[t] : 1.f;
-    if (dlogits) {
-      for (int c = lane; c < ldd; c += 32) {
-        float g = 0.f;
-        if (c < C) g = (__expf(row[c] - lse) - (c == t ? 1.f : 0.f)) * w * norm;
-        dlogits[static_cast<long long>(r) * ldd + c] = __float2bfloat16(g);
+    if constexpr (SOFT) {
+      float qs = 0.f, ql = 0.f;          // sum_c q_c and the row's loss sum_c q_c (lse - z_c)
+      for (int c = lane; c < C; c += 32) {
+        const float q = soft_q(c, t, tb, la, lb, keep, eps_c, cw);
+        qs += q;
+        ql += q * (lse - row[c]);
       }
-    }
-    if (lane == 0) {
-      loss_acc += w * (lse - row[t]);
-      correct_acc += (amax == t) ? 1.f : 0.f;
+      for (int o = 16; o; o >>= 1) {
+        qs += __shfl_xor_sync(0xffffffffu, qs, o);
+        ql += __shfl_xor_sync(0xffffffffu, ql, o);
+      }
+      if (dlogits) {
+        for (int c = lane; c < ldd; c += 32) {
+          float g = 0.f;
+          if (c < C) g = (__expf(row[c] - lse) * qs - soft_q(c, t, tb, la, lb, keep, eps_c, cw)) * norm;
+          dlogits[static_cast<long long>(r) * ldd + c] = __float2bfloat16(g);
+        }
+      }
+      if (lane == 0) {
+        loss_acc += ql;
+        correct_acc += (amax == tmax) ? 1.f : 0.f;
+      }
+    } else {
+      const float w = cw ? cw[t] : 1.f;
+      if (dlogits) {
+        for (int c = lane; c < ldd; c += 32) {
+          float g = 0.f;
+          if (c < C) g = (__expf(row[c] - lse) - (c == t ? 1.f : 0.f)) * w * norm;
+          dlogits[static_cast<long long>(r) * ldd + c] = __float2bfloat16(g);
+        }
+      }
+      if (lane == 0) {
+        loss_acc += w * (lse - row[t]);
+        correct_acc += (amax == t) ? 1.f : 0.f;
+      }
     }
   }
   if (lane == 0) { s_loss[warp] = loss_acc; s_correct[warp] = correct_acc; }
@@ -78,7 +129,7 @@ __global__ void cross_entropy_kernel(const float* __restrict__ logits, const lon
     for (int i = 0; i < nwarps; ++i) { tl += s_loss[i]; tc += s_correct[i]; }
     // batch loss as torch reports it: mean over the batch, or sum_i w_i nll_i / sum_i w_i with
     // class weights; the meter accumulates loss * B like Average.update(loss.item(), B)
-    const float mean = cw ? tl / s_total_w : tl / static_cast<float>(B);
+    const float mean = by_weight ? tl / s_total_w : tl / static_cast<float>(B);
     if (meter) {
       atomicAdd(meter + 0, mean * static_cast<float>(B));
       atomicAdd(meter + 1, tc);
@@ -91,10 +142,19 @@ __global__ void cross_entropy_kernel(const float* __restrict__ logits, const lon
 void cross_entropy_fused(const float* logits, const long long* target, bf16* dlogits, int ldd,
                          float* meter, float* loss_out, int B, int C, float grad_scale,
                          const float* class_weights, cudaStream_t s) {
-  cross_entropy_kernel<<<1, 1024, 0, s>>>(logits, target, dlogits, ldd, meter, loss_out, B, C,
-                                          grad_scale, class_weights);
+  cross_entropy_kernel<false><<<1, 1024, 0, s>>>(logits, target, dlogits, ldd, meter, loss_out, B, C,
+                                                 grad_scale, class_weights, SoftTargets{0.f, 1.f, 0.f, 0});
   count_launch();
   check_last("cross_entropy_fused");
+}
+
+void cross_entropy_soft(const float* logits, const long long* target, bf16* dlogits, int ldd, float* meter,
+                        float* loss_out, int B, int C, float grad_scale, const float* class_weights,
+                        const SoftTargets& st, cudaStream_t s) {
+  cross_entropy_kernel<true><<<1, 1024, 0, s>>>(logits, target, dlogits, ldd, meter, loss_out, B, C,
+                                                grad_scale, class_weights, st);
+  count_launch();
+  check_last("cross_entropy_soft");
 }
 
 // ------------------------------------------------------------- fused head: last Linear + CE + bwd
@@ -110,12 +170,14 @@ void cross_entropy_fused(const float* logits, const long long* target, bf16* dlo
 // Rounding points are those of the unfused path: dlogits are rounded to bf16 before they are used.
 constexpr int HEAD_MAXC = 8, HEAD_MAXK = 1024, HEAD_MAXB = 256, HEAD_THREADS = 512;
 
+// SOFT: soft targets as in cross_entropy_kernel<true>; the backward of the layer is unchanged.
+template <bool SOFT>
 __global__ void __launch_bounds__(HEAD_THREADS, 1)
 head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const float* __restrict__ bias,
                const long long* __restrict__ target, float* __restrict__ logits, bf16* __restrict__ dlogits, int ldd,
                float* __restrict__ dW, float* __restrict__ db, bf16* __restrict__ dh, float drop_scale, int relu,
                float* __restrict__ meter, float* __restrict__ loss_out, int B, int C, int K,
-               const float* __restrict__ cw, int accumulate) {
+               const float* __restrict__ cw, int accumulate, SoftTargets st) {
   __shared__ float sW[HEAD_MAXC * HEAD_MAXK];
   __shared__ float sdl[HEAD_MAXB * HEAD_MAXC];
   __shared__ float s_loss[32], s_correct[32], s_wsum[32];
@@ -136,7 +198,9 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
     s_total_w = t;
   }
   __syncthreads();
-  const float norm = cw ? 1.f / s_total_w : 1.f / static_cast<float>(B);
+  const bool by_weight = cw && !(SOFT && st.mix);      // probability targets: divided by B
+  const float norm = by_weight ? 1.f / s_total_w : 1.f / static_cast<float>(B);
+  const float keep = 1.f - st.eps, eps_c = st.eps / static_cast<float>(C);
 
   // ---- forward + loss + dlogits ---------------------------------------------------------------
   float loss_acc = 0.f, correct_acc = 0.f;
@@ -154,7 +218,9 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
 #pragma unroll
     for (int c = 0; c < HEAD_MAXC; ++c)
       for (int o = 16; o; o >>= 1) acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], o);
-    const int t = static_cast<int>(target[r]);
+    int t = static_cast<int>(target[r]), tb = t, tmax = t;
+    float la = 1.f, lb = 0.f;
+    if constexpr (SOFT) soft_row(target, r, B, st, t, tb, la, lb, tmax);
     float mx = -INFINITY;
     int amax = 0;
 #pragma unroll
@@ -171,14 +237,28 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
         if (c == t) zt = acc[c];
       }
     const float lse = mx + __logf(se);
-    const float w = cw ? cw[t] : 1.f;
+    float w = cw ? cw[t] : 1.f;
+    float qs = 0.f, ql = 0.f;        // SOFT: sum_c q_c and the row's loss sum_c q_c (lse - z_c)
+    if constexpr (SOFT) {
+#pragma unroll
+      for (int c = 0; c < HEAD_MAXC; ++c)
+        if (c < C) {
+          const float q = soft_q(c, t, tb, la, lb, keep, eps_c, cw);
+          qs += q;
+          ql += q * (lse - acc[c]);
+        }
+      w = 1.f;
+    }
     if (lane < ldd || lane < C) {
       float g = 0.f, z = 0.f;
 #pragma unroll
       for (int c = 0; c < HEAD_MAXC; ++c)
         if (c == lane && c < C) {
           z = acc[c];
-          g = (__expf(acc[c] - lse) - (c == t ? 1.f : 0.f)) * w * norm;
+          if constexpr (SOFT)
+            g = (__expf(acc[c] - lse) * qs - soft_q(c, t, tb, la, lb, keep, eps_c, cw)) * norm;
+          else
+            g = (__expf(acc[c] - lse) - (c == t ? 1.f : 0.f)) * w * norm;
         }
       if (lane < C) {
         logits[static_cast<long long>(r) * C + lane] = z;
@@ -187,8 +267,13 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
       if (dlogits && lane < ldd) dlogits[static_cast<long long>(r) * ldd + lane] = __float2bfloat16(g);
     }
     if (lane == 0) {
-      loss_acc += w * (lse - zt);
-      correct_acc += (amax == t) ? 1.f : 0.f;
+      if constexpr (SOFT) {
+        loss_acc += ql;
+        correct_acc += (amax == tmax) ? 1.f : 0.f;
+      } else {
+        loss_acc += w * (lse - zt);
+        correct_acc += (amax == t) ? 1.f : 0.f;
+      }
     }
   }
   if (lane == 0) { s_loss[warp] = loss_acc; s_correct[warp] = correct_acc; }
@@ -196,7 +281,7 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
   if (threadIdx.x == 0) {
     float tl = 0.f, tc = 0.f;
     for (int i = 0; i < nwarps; ++i) { tl += s_loss[i]; tc += s_correct[i]; }
-    const float mean = cw ? tl / s_total_w : tl / static_cast<float>(B);
+    const float mean = by_weight ? tl / s_total_w : tl / static_cast<float>(B);
     if (meter) {
       atomicAdd(meter + 0, mean * static_cast<float>(B));
       atomicAdd(meter + 1, tc);
@@ -243,12 +328,17 @@ bool head_ce_supported(int B, int C, int K) { return C <= HEAD_MAXC && K <= HEAD
 void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long long* target, float* logits,
                    bf16* dlogits, int ldd, float* dW, float* db, bf16* dh, float drop_scale, bool relu, float* meter,
                    float* loss_out, int B, int C, int K, const float* class_weights, bool accumulate,
-                   cudaStream_t s) {
+                   cudaStream_t s, const SoftTargets* soft) {
   if (!head_ce_supported(B, C, K)) throw std::runtime_error("[b200] head_ce_fused: needs C <= 8, K <= 1024, B <= 256");
   if (ldd > 32) throw std::runtime_error("[b200] head_ce_fused: dlogits row stride must be <= 32");
-  head_ce_kernel<<<1, HEAD_THREADS, 0, s>>>(h, W, bias, target, logits, dlogits, ldd, dW, db, dh, drop_scale,
-                                            relu ? 1 : 0, meter, loss_out, B, C, K, class_weights,
-                                            accumulate ? 1 : 0);
+  if (soft)
+    head_ce_kernel<true><<<1, HEAD_THREADS, 0, s>>>(h, W, bias, target, logits, dlogits, ldd, dW, db, dh, drop_scale,
+                                                    relu ? 1 : 0, meter, loss_out, B, C, K, class_weights,
+                                                    accumulate ? 1 : 0, *soft);
+  else
+    head_ce_kernel<false><<<1, HEAD_THREADS, 0, s>>>(h, W, bias, target, logits, dlogits, ldd, dW, db, dh, drop_scale,
+                                                     relu ? 1 : 0, meter, loss_out, B, C, K, class_weights,
+                                                     accumulate ? 1 : 0, SoftTargets{0.f, 1.f, 0.f, 0});
   count_launch();
   check_last("head_ce_fused");
 }

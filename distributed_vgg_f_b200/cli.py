@@ -117,6 +117,14 @@ def build_parser() -> argparse.ArgumentParser:
                           "the last training step of every epoch, when each layer's kernels and each bucket's reduction / "
                           "update finished (CUDA events, ms since the start of the step; native engine)")
     ext.add_argument("--log-jsonl", default=None, help="append one JSON record per epoch")
+    ext.add_argument("--label-smoothing", type=float, default=0.0,
+                     help="label smoothing of the training loss, 0 <= eps < 1 (torchvision's --label-smoothing; "
+                          "0 = off).  The test loss stays plain cross-entropy")
+    ext.add_argument("--mixup-alpha", type=float, default=0.0,
+                     help="MixUp every training batch with lam ~ Beta(alpha, alpha) (torchvision's --mixup-alpha; 0 = off)")
+    ext.add_argument("--cutmix-alpha", type=float, default=0.0,
+                     help="CutMix every training batch with lam ~ Beta(alpha, alpha) (torchvision's --cutmix-alpha; "
+                          "0 = off).  With both alphas > 0 each batch takes one of the two with probability 1/2")
     ext.add_argument("--accum-steps", type=int, default=1,
                      help="gradient accumulation: one optimizer update (and one gradient all-reduce) per K "
                           "mini-batches and after the last one of an epoch, with the mean of their gradients")
@@ -130,6 +138,10 @@ def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
         build_parser().error("the following arguments are required: -rd/--root_dir")
     if args.accum_steps < 1:
         build_parser().error("--accum-steps must be >= 1")
+    if not 0.0 <= args.label_smoothing < 1.0:
+        build_parser().error("--label-smoothing must lie in [0, 1)")
+    if args.mixup_alpha < 0.0 or args.cutmix_alpha < 0.0:
+        build_parser().error("--mixup-alpha and --cutmix-alpha must be >= 0")
     print(args)
     if args.socket_ifname:
         os.environ["GLOO_SOCKET_IFNAME"] = args.socket_ifname

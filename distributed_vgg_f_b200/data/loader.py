@@ -17,6 +17,11 @@ Same surface here, two pipelines:
     memory.  ``pipeline="auto"`` (the CLI default) switches to the reference pipeline for mixed
     image sizes or a split too big for host memory.
 Ragged final batches are preserved (``drop_last=False`` in the reference).
+
+With ``mixup_alpha`` / ``cutmix_alpha`` > 0 every training batch carries a MixUp or CutMix draw
+(``transforms.draw_mix``, seeded by (seed, epoch, rank, batch index)): fused batches in their ``mix``
+field, for the augment kernel to apply; the reference pipeline applies it on the host and yields
+``(mixed float batch, labels, draw)``.  Validation batches are never mixed.
 """
 from __future__ import annotations
 
@@ -41,6 +46,7 @@ class FusedBatch(NamedTuple):
     labels: torch.Tensor        # int64 [mb]          (same)
     resized_hw: Tuple[int, int]
     state: Optional[dict] = None    # consumer may set state["event"]: slot is reusable after it fires
+    mix: Optional[T.MixDraw] = None     # MixUp / CutMix of this training batch
 
     def to_float(self, device="cpu") -> Tuple[torch.Tensor, torch.Tensor]:
         """Evaluate the fused transform with torch ops (CPU / oracle path)."""
@@ -56,6 +62,7 @@ class RaggedBatch(NamedTuple):
     params: torch.Tensor        # float32 [mb, 8]      (same)
     labels: torch.Tensor        # int64 [mb]           (same)
     state: Optional[dict] = None    # consumer may set state["event"]: slot is reusable after it fires
+    mix: Optional[T.MixDraw] = None     # MixUp / CutMix of this training batch
 
     def to_float(self, device="cpu") -> Tuple[torch.Tensor, torch.Tensor]:
         """Evaluate the transform with Pillow's resampling on the CPU (CPU / oracle path)."""
@@ -173,8 +180,9 @@ class _FusedLoader:
 
     def __init__(self, cache: DecodedCache, mb: int, train: bool, sampler: Optional[ShardedSampler],
                  shuffle: bool, seed: int, prefetch: int = 3, pin: Optional[bool] = None,
-                 native: Optional[bool] = None) -> None:
+                 native: Optional[bool] = None, mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0) -> None:
         self.cache, self.mb, self.train = cache, mb, train
+        self.mixup_alpha, self.cutmix_alpha = (mixup_alpha, cutmix_alpha) if train else (0.0, 0.0)
         self.sampler, self.shuffle, self.seed = sampler, shuffle, seed
         self.prefetch = prefetch
         self.pin = torch.cuda.is_available() if pin is None else pin
@@ -238,13 +246,18 @@ class _FusedLoader:
     def _epoch_seed(self) -> int:
         return 1_000_003 * (self.seed + 1) + self.epoch * 7919 + (self.sampler.rank if self.sampler else 0)
 
-    def _batch(self, slot: int, k: int):
+    def _draw(self, index: int) -> Optional[T.MixDraw]:
+        return T.draw_mix(self.mixup_alpha, self.cutmix_alpha, self.seed, self.epoch,
+                          self.sampler.rank if self.sampler else 0, index)
+
+    def _batch(self, slot: int, k: int, index: int = 0):
         img, par, lab = self._ring[slot]
+        mix = self._draw(index)
         if not self.ragged:
-            return FusedBatch(img[:k], par[:k], lab[:k], self.resized_hw, self._state[slot])
+            return FusedBatch(img[:k], par[:k], lab[:k], self.resized_hw, self._state[slot], mix)
         geom = self._geom[slot][:k]
         used = int(geom[k - 1, 0] + geom[k - 1, 1] * geom[k - 1, 2] * 3)
-        return RaggedBatch(img[:used], geom, par[:k], lab[:k], self._state[slot])
+        return RaggedBatch(img[:used], geom, par[:k], lab[:k], self._state[slot], mix)
 
     def __iter__(self) -> Iterator[FusedBatch]:
         if self._pf is not None:
@@ -255,6 +268,7 @@ class _FusedLoader:
     def _iter_native(self) -> Iterator[FusedBatch]:
         self._pf.start(self._indices(), self._epoch_seed())
         prev = None
+        index = 0
         try:
             while True:
                 item = self._pf.next()           # blocks with the GIL released
@@ -267,7 +281,8 @@ class _FusedLoader:
                     break
                 slot, k = item
                 prev = slot
-                yield self._batch(slot, k)
+                yield self._batch(slot, k, index)
+                index += 1
         finally:
             self._pf.stop()
 
@@ -309,6 +324,7 @@ class _FusedLoader:
         th = threading.Thread(target=produce, daemon=True)
         th.start()
         prev = None
+        index = 0
         while True:
             item = q.get()
             if prev is not None:
@@ -317,7 +333,8 @@ class _FusedLoader:
                 break
             slot, k = item
             prev = slot
-            yield self._batch(slot, k)
+            yield self._batch(slot, k, index)
+            index += 1
         th.join()
 
 
@@ -325,9 +342,10 @@ class _ReferenceLoader:
     """Synchronous PIL + torchvision loader with the reference's exact semantics."""
 
     def __init__(self, samples, mb: int, train: bool, sampler: Optional[ShardedSampler],
-                 shuffle: bool, seed: int) -> None:
+                 shuffle: bool, seed: int, mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0) -> None:
         self.samples, self.mb, self.sampler = samples, mb, sampler
         self.shuffle, self.seed, self.epoch = shuffle, seed, 0
+        self.mixup_alpha, self.cutmix_alpha = (mixup_alpha, cutmix_alpha) if train else (0.0, 0.0)
         self.tf = T.reference_transforms(train)
 
     def __len__(self) -> int:
@@ -355,7 +373,13 @@ class _ReferenceLoader:
                 with open(path, "rb") as f:
                     xs.append(self.tf(Image.open(f).convert("RGB")))
                 ys.append(label)
-            yield torch.stack(xs), torch.tensor(ys, dtype=torch.int64)
+            x, y = torch.stack(xs), torch.tensor(ys, dtype=torch.int64)
+            mix = T.draw_mix(self.mixup_alpha, self.cutmix_alpha, self.seed, self.epoch,
+                             self.sampler.rank if self.sampler else 0, b0 // self.mb)
+            if mix is None:
+                yield x, y
+            else:       # mixed on the host by torchvision, the draw travels with the batch
+                yield T.apply_mix(x, y, mix), y, mix
 
 
 class DataManager:
@@ -363,7 +387,8 @@ class DataManager:
 
     def __init__(self, root_folder: str, mini_batch: int, train: bool = True, *,
                  world_size: int = 1, rank: int = 0, pipeline: str = "fused", seed: int = 0,
-                 reference_order: bool = False, decode_threads: int = 8, shard_eval: bool = False) -> None:
+                 reference_order: bool = False, decode_threads: int = 8, shard_eval: bool = False,
+                 mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0) -> None:
         if root_folder is None:
             raise ValueError("-rd/--root_dir is required")
         self.root_folder, self.mb_size, self.train = root_folder, mini_batch, train
@@ -390,9 +415,11 @@ class DataManager:
                 pipeline = "reference"
         self.pipeline = pipeline = "fused" if pipeline == "auto" else pipeline
         if pipeline == "fused":
-            self.loader = _FusedLoader(self.cache, mini_batch, train, sampler, True, seed)
+            self.loader = _FusedLoader(self.cache, mini_batch, train, sampler, True, seed,
+                                       mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha)
         elif pipeline == "reference":
-            self.loader = _ReferenceLoader(self.samples, mini_batch, train, sampler, True, seed)
+            self.loader = _ReferenceLoader(self.samples, mini_batch, train, sampler, True, seed,
+                                           mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha)
         else:
             raise ValueError("pipeline must be 'fused', 'reference' or 'auto'")
 

@@ -16,7 +16,7 @@ reads uint8 HWC and writes normalised bf16 NHWC / the layer-0 im2col matrix dire
 from __future__ import annotations
 
 import math
-from typing import Optional, Tuple
+from typing import NamedTuple, Optional, Tuple
 
 import torch
 
@@ -235,6 +235,73 @@ def ragged_reference(data_u8: torch.Tensor, geom: torch.Tensor, params: torch.Te
         v = torch.where(inside.unsqueeze(0), v, torch.zeros_like(v))
         out[i] = (v / 255.0 - m) / sd
     return out
+
+
+# ------------------------------------------------------------------------ MixUp / CutMix (per batch)
+class MixDraw(NamedTuple):
+    """One training batch's MixUp or CutMix draw.  Sample i is mixed with sample (i-1) mod b, where b
+    is the batch's actual size (torchvision's ``roll(1, 0)``)."""
+    kind: str                           # "mixup" | "cutmix"
+    lam: float                          # weight of sample i: MixUp's lam, CutMix's lam_adjusted
+    box: Tuple[int, int, int, int]      # CutMix: (x1, y1, x2, y2) in network-input pixels; MixUp: zeros
+
+
+def mix_seed(seed: int, epoch: int, rank: int, index: int) -> int:
+    """Seed of the draw of training batch ``index`` of ``epoch`` on ``rank``."""
+    return ((((seed * 1_000_003 + epoch) * 1_000_003 + rank) * 1_000_003 + index) * 2_654_435_761) % (1 << 63)
+
+
+def draw_mix(mixup_alpha: float, cutmix_alpha: float, seed: int, epoch: int, rank: int, index: int,
+             hw: int = DATA.crop) -> Optional[MixDraw]:
+    """The batch's draw with torchvision's own parameter code, as its classification reference script
+    builds it: ``RandomChoice([MixUp, CutMix])`` when both alphas are > 0 (its multinomial picks one),
+    else the one enabled.  Drawn under ``torch.random.fork_rng`` with ``mix_seed``: reproducible, and
+    no other random stream moves.  None when both alphas are 0 (no draw is made)."""
+    if mixup_alpha <= 0 and cutmix_alpha <= 0:
+        return None
+    from torchvision.transforms import v2
+
+    choices = []
+    if mixup_alpha > 0:
+        choices.append(v2.MixUp(alpha=mixup_alpha, num_classes=1))
+    if cutmix_alpha > 0:
+        choices.append(v2.CutMix(alpha=cutmix_alpha, num_classes=1))
+    with torch.random.fork_rng(devices=[]):
+        torch.manual_seed(mix_seed(seed, epoch, rank, index))
+        t = choices[0]
+        if len(choices) > 1:
+            rc = v2.RandomChoice(choices)
+            t = rc.transforms[int(torch.multinomial(torch.tensor(rc.p), 1))]
+        # make_params reads only the image size; a stride-0 view gives it one without a buffer
+        params = t.make_params([torch.zeros(()).expand(1, 3, hw, hw)])
+    if isinstance(t, v2.CutMix):
+        return MixDraw("cutmix", float(params["lam_adjusted"]), tuple(int(v) for v in params["box"]))
+    return MixDraw("mixup", float(params["lam"]), (0, 0, 0, 0))
+
+
+def _mix_transform(mix: MixDraw, labels: torch.Tensor):
+    from torchvision.transforms import v2
+
+    if mix.kind == "mixup":
+        return v2.MixUp(alpha=1.0, num_classes=1), dict(lam=mix.lam, labels=labels, batch_size=labels.shape[0])
+    return v2.CutMix(alpha=1.0, num_classes=1), dict(box=mix.box, lam_adjusted=mix.lam, labels=labels,
+                                                     batch_size=labels.shape[0])
+
+
+def apply_mix(x: torch.Tensor, labels: torch.Tensor, mix: Optional[MixDraw]) -> torch.Tensor:
+    """Mix a float batch [b, 3, H, W] as torchvision's ``MixUp.transform`` / ``CutMix.transform`` do
+    with the drawn params (the PIL pipeline and the oracle engine)."""
+    if mix is None:
+        return x
+    t, params = _mix_transform(mix, labels)
+    return t.transform(x, params)
+
+
+def mixed_targets(labels: torch.Tensor, num_classes: int, mix: Optional[MixDraw]) -> torch.Tensor:
+    """The probability targets torchvision hands to the loss for this draw: float32 [b, C]."""
+    t, params = _mix_transform(mix, labels)
+    t.num_classes = num_classes
+    return t.transform(labels, params)
 
 
 def reference_transforms(train: bool):

@@ -88,7 +88,8 @@ class NativeEngine:
                  profile: Optional[str] = None, input_hw: int = DATA.crop, comm_ctas: int = 48,
                  init_state: Optional[Dict[str, torch.Tensor]] = None, unpack_fp32: bool = False,
                  distributed: bool = True, zero1="auto", conv_bucket_mb: float = 9.5,
-                 tail_bucket_kb: float = 2400.0, same_dropout_all_ranks: bool = False) -> None:
+                 tail_bucket_kb: float = 2400.0, same_dropout_all_ranks: bool = False,
+                 label_smoothing: float = 0.0) -> None:
         ops.require()
         if compute_dtype != "bf16":
             raise NotImplementedError("the native engine computes in bf16 with fp32 master weights; "
@@ -102,6 +103,11 @@ class NativeEngine:
         self.lr, self.opt_name, self.momentum, self.weight_decay = lr, optimizer, momentum, weight_decay
         self.beta1, self.beta2, self.eps = TRAIN.adam_beta1, TRAIN.adam_beta2, TRAIN.adam_eps
         self.seed, self.HW = int(seed), int(input_hw)
+        if not 0.0 <= label_smoothing < 1.0:
+            raise ValueError("label_smoothing must lie in [0, 1) (got %r)" % label_smoothing)
+        # training loss only: F.cross_entropy(label_smoothing=); the evaluation loss stays plain
+        self.label_smoothing = float(label_smoothing)
+        self._mix = None                 # MixUp / CutMix draw of the staged batch (data.transforms.MixDraw)
         self.same_dropout_all_ranks = bool(same_dropout_all_ranks)
         self.step_count = 0              # optimizer updates (Adam / SGD step, LR schedule, checkpoint "step")
         self.micro_count = 0             # training micro-batches: the Philox dropout offset
@@ -354,6 +360,7 @@ class NativeEngine:
         j = self._in_slot
         self._in_slot ^= 1
         self.labels_dev = self._labels_dev[j]
+        self._mix = None
         cur = torch.cuda.current_stream(self.device)
         if isinstance(batch, FusedBatch):
             b = int(batch.labels.shape[0])
@@ -374,8 +381,10 @@ class NativeEngine:
             cur.wait_event(h2d)
             # two passes: transform once per pixel into 8-byte NHWC4 pixels (25 MB at B=64, L2
             # resident), then expand to the first conv's im2col rows with coalesced 16-byte stores
+            # MixUp / CutMix in the same pass (sample i with i-1 mod b); without a draw, the plain kernel
+            self._mix = batch.mix
             ops.augment(self._src_u8[j][:b], self._params_dev[j][:b], self.x_nhwc[:b], batch.resized_hw,
-                        out_hw=HW, mode="nhwc", pad=4)
+                        out_hw=HW, mode="nhwc", pad=4, mix=self._mix)
             if not self.fused_conv0:
                 C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
             return b
@@ -400,12 +409,16 @@ class NativeEngine:
             if batch.state is not None:
                 batch.state["event"] = h2d
             cur.wait_event(h2d)
+            self._mix = batch.mix
             ops.augment_ragged(self._src_u8[j][:nbytes], self._geom_dev[j][:b], self._params_dev[j][:b],
-                               self._inter_u8, self.x_nhwc[:b], batch.geom, batch.params, out_hw=HW)
+                               self._inter_u8, self.x_nhwc[:b], batch.geom, batch.params, out_hw=HW,
+                               mix=self._mix)
             if not self.fused_conv0:
                 C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
             return b
-        x, y = batch
+        x, y = batch[0], batch[1]
+        if len(batch) > 2:               # (mixed float batch, labels, draw) of the reference pipeline
+            self._mix = batch[2]
         b = int(y.shape[0])
         x = x.to(self.device, F32, non_blocking=True).contiguous()
         assert x.shape[2] == HW and x.shape[3] == HW, "input size differs from the engine's input_hw"
@@ -489,11 +502,14 @@ class NativeEngine:
     def _loss(self, b: int, train: bool) -> None:
         """Loss + metrics (+ dlogits when training) from the forward state."""
         meter = self.meter.buf if self.meter is not None else self.scratch_meter
+        # soft targets (label smoothing, MixUp / CutMix) shape the training loss only
+        eps, mix = (self.label_smoothing, self._mix) if train else (0.0, None)
         if not self.fused_head:
             ld = self.fc_dz[-1].shape[1]
             ops.cross_entropy(self.logits[:b], self.labels_dev[:b], self.fc_dz[-1][:b] if train else None,
                               ld if train else 0, meter, self.loss_buf,
-                              class_weights=self.class_weights if train else None)   # like the reference's loops
+                              class_weights=self.class_weights if train else None,   # like the reference's loops
+                              label_smoothing=eps, mix=mix)
             return
         f, prev = self.spec.fcs[-1], self.spec.fcs[-2]
         C = ops.require()
@@ -503,7 +519,10 @@ class NativeEngine:
                     self.fc_dz[-1][:b], self.fc_dz[-1].shape[1], self._grad(f.name + ".weight"),
                     self._grad(f.name + ".bias"), self.fc_dz[-2][:b], 1.0 / (1.0 - p), bool(prev.relu), meter,
                     self.loss_buf, self.class_weights)
-            if self._accum:                  # a later micro-batch of the group: dW += (db always accumulates)
+            soft = ops.soft_targets(eps, mix)
+            if soft is not None:
+                C.head_ce(*args, bool(self._accum), soft)
+            elif self._accum:                # a later micro-batch of the group: dW += (db always accumulates)
                 C.head_ce(*args, True)
             else:
                 C.head_ce(*args)

@@ -146,11 +146,27 @@ def fc_grad_act(acc, act, dz, *, B: int, N: int, relu: bool, drop_p: float = 0.0
 
 
 def cross_entropy(logits, target, dlogits=None, ldd: int = 0, meter=None, loss_out=None,
-                  grad_scale: Optional[float] = None, class_weights=None):
+                  grad_scale: Optional[float] = None, class_weights=None, label_smoothing: float = 0.0,
+                  mix=None):
+    """Fused cross-entropy.  ``label_smoothing`` and ``mix`` (a ``data.transforms.MixDraw``: row r's
+    target is lam e_{target[r]} + (1 - lam) e_{target[r-1 mod B]}) give F.cross_entropy's soft-target
+    loss; without them the integer-label kernel runs."""
     if grad_scale is None:
         grad_scale = 1.0 / logits.shape[0]
-    require().cross_entropy(logits, target, dlogits, ldd or logits.shape[1], meter, loss_out,
-                            grad_scale, class_weights)
+    if label_smoothing == 0.0 and mix is None:
+        require().cross_entropy(logits, target, dlogits, ldd or logits.shape[1], meter, loss_out,
+                                grad_scale, class_weights)
+        return
+    require().cross_entropy_soft(logits, target, dlogits, ldd or logits.shape[1], meter, loss_out, grad_scale,
+                                 class_weights, float(label_smoothing), mix.lam if mix is not None else 1.0,
+                                 mix is not None)
+
+
+def soft_targets(label_smoothing: float = 0.0, mix=None):
+    """``head_ce``'s ``soft`` argument: None for integer labels without smoothing."""
+    if label_smoothing == 0.0 and mix is None:
+        return None
+    return [float(label_smoothing), mix.lam if mix is not None else 1.0, 1.0 if mix is not None else 0.0]
 
 
 def adam_step(p, m, v, *, g32=None, g16=None, shadow=None, lr, beta1=0.9, beta2=0.999, eps=1e-8,
@@ -163,20 +179,37 @@ def sgd_step(p, mom, *, g32=None, g16=None, shadow=None, lr, momentum=0.9, weigh
     require().sgd(p, mom, g32, g16, shadow, lr, momentum, weight_decay, first, grad_scale, zero)
 
 
+_MIX_KIND = {"mixup": 1, "cutmix": 2}
+
+
 def augment(src_u8, params, out, resized_hw: Tuple[int, int], out_hw: int = DATA.crop,
-            mode: str = "im2col", pad: int = 64):
-    """uint8 [N,H,W,3] + params [N,8] -> normalised bf16 (NHWC padded, or layer-0 im2col rows)."""
-    require().augment(src_u8, params, out, resized_hw[0], resized_hw[1], out_hw, out_hw,
-                      1 if mode == "im2col" else 0, pad, list(DATA.mean), list(DATA.std))
+            mode: str = "im2col", pad: int = 64, mix=None):
+    """uint8 [N,H,W,3] + params [N,8] -> normalised bf16 (NHWC padded, or layer-0 im2col rows).
+    ``mix`` (a ``data.transforms.MixDraw``, NHWC only): MixUp / CutMix the batch in the same pass,
+    sample i with sample i-1 mod N."""
+    if mix is None:
+        require().augment(src_u8, params, out, resized_hw[0], resized_hw[1], out_hw, out_hw,
+                          1 if mode == "im2col" else 0, pad, list(DATA.mean), list(DATA.std))
+        return out
+    if mode != "nhwc":
+        raise ValueError("augment: MixUp / CutMix are fused into the NHWC mode only")
+    require().augment_mixed(src_u8, params, out, resized_hw[0], resized_hw[1], out_hw, out_hw, pad,
+                            list(DATA.mean), list(DATA.std), _MIX_KIND[mix.kind], mix.lam, list(mix.box))
     return out
 
 
-def augment_ragged(data_u8, geom, params, inter, out, geom_host, params_host, out_hw: int = DATA.crop):
+def augment_ragged(data_u8, geom, params, inter, out, geom_host, params_host, out_hw: int = DATA.crop,
+                   mix=None):
     """Images of any sizes (data/loader.py::RaggedBatch on the device) -> normalised bf16 NHWC4
     ``out``, resampled as Pillow does.  ``geom_host`` / ``params_host``: the CPU tensors the device
-    ``geom`` / ``params`` were copied from; ``inter`` holds ``ragged_inter_bytes(geom_host)``."""
-    require().augment_ragged(data_u8, geom, params, inter, out, geom_host, params_host, out_hw, out_hw,
-                             list(DATA.mean), list(DATA.std))
+    ``geom`` / ``params`` were copied from; ``inter`` holds ``ragged_inter_bytes(geom_host)``.
+    ``mix``: as for ``augment``."""
+    if mix is None:
+        require().augment_ragged(data_u8, geom, params, inter, out, geom_host, params_host, out_hw, out_hw,
+                                 list(DATA.mean), list(DATA.std))
+        return out
+    require().augment_ragged_mixed(data_u8, geom, params, inter, out, geom_host, params_host, out_hw, out_hw,
+                                   list(DATA.mean), list(DATA.std), _MIX_KIND[mix.kind], mix.lam, list(mix.box))
     return out
 
 

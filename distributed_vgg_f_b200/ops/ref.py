@@ -32,11 +32,15 @@ def pool_relu_bwd(y: torch.Tensor, dp: torch.Tensor) -> torch.Tensor:
 @torch.no_grad()
 def emulated_step(spec: VGGSpec, state: Dict[str, torch.Tensor], x: torch.Tensor, target: torch.Tensor,
                   dropout_masks: bool = False, return_intermediates: bool = False,
-                  override: dict = None):
+                  override: dict = None, soft_target: torch.Tensor = None, label_smoothing: float = 0.0):
     """Forward + backward of the network on fp32 torch ops with the engine's rounding points.
 
     state: torch-layout fp32 tensors (weights are rounded to bf16 here, biases stay fp32).
     Returns (logits, mean loss, grads in torch layout).  Dropout is treated as identity.
+
+    ``soft_target`` (probability targets [B][C], e.g. MixUp / CutMix) and ``label_smoothing``: the loss
+    is F.cross_entropy(logits, soft_target or target, label_smoothing=) and its gradient
+    (softmax - t) / B with t the smoothed target.
 
     ``override`` (optional) pins the forward state to tensors observed elsewhere -- keys ``acts``
     (post-ReLU conv outputs, NCHW), ``feat`` (pooled feature map), ``fc_y`` (hidden FC outputs),
@@ -81,8 +85,14 @@ def emulated_step(spec: VGGSpec, state: Dict[str, torch.Tensor], x: torch.Tensor
                 h = override["fc_y"][i].float()
     B = x.shape[0]
     logp = torch.log_softmax(logits, dim=1)
-    loss = -logp.gather(1, target.view(-1, 1)).mean()
-    dz = rb((torch.softmax(logits, 1) - F.one_hot(target, logits.shape[1]).float()) / B)
+    if soft_target is None and not label_smoothing:
+        loss = -logp.gather(1, target.view(-1, 1)).mean()
+        dz = rb((torch.softmax(logits, 1) - F.one_hot(target, logits.shape[1]).float()) / B)
+    else:
+        t = soft_target.float() if soft_target is not None else F.one_hot(target, logits.shape[1]).float()
+        t = t * (1.0 - label_smoothing) + label_smoothing / logits.shape[1]
+        loss = -(t * logp).sum(1).mean()
+        dz = rb((torch.softmax(logits, 1) - t) / B)
 
     grads: Dict[str, torch.Tensor] = {}
     inter = {"fc_dz": {}, "fc_y": {i: fc_in[i + 1] for i in range(last)}, "conv_dz": {}}

@@ -77,7 +77,9 @@ def manage_training(args) -> Trainer:
 
     dm_kw = dict(world_size=args.world_size, rank=args.rank, pipeline=args.pipeline,
                  seed=args.seed, reference_order=args.reference_order)
-    train_data_mngr = DataManager(args.root_dir, args.mini_batch, train=True, **dm_kw)
+    train_data_mngr = DataManager(args.root_dir, args.mini_batch, train=True,
+                                  mixup_alpha=getattr(args, "mixup_alpha", 0.0),
+                                  cutmix_alpha=getattr(args, "cutmix_alpha", 0.0), **dm_kw)
     valid_data_mngr = DataManager(args.root_dir, args.mini_batch, train=False,
                                   shard_eval=getattr(args, "shard_eval", False), **dm_kw)
     train_loader, valid_loader = train_data_mngr.get_loader(), valid_data_mngr.get_loader()
@@ -101,7 +103,8 @@ def manage_training(args) -> Trainer:
                              compute_dtype=args.dtype, allreduce=args.allreduce,
                              wire_dtype=args.wire_dtype, bucket_mb=args.bucket_mb, seed=args.seed,
                              pretrained_state=pretrained, profile=args.profile,
-                             zero1={"auto": "auto", "on": True, "off": False}[getattr(args, "zero1", "auto")])
+                             zero1={"auto": "auto", "on": True, "off": False}[getattr(args, "zero1", "auto")],
+                             label_smoothing=getattr(args, "label_smoothing", 0.0))
         optimizer = None            # fused into the engine
         if model.world > 1:
             model.comm_timing(True)   # [Perf] line: all-reduce GB/s and fraction of the NVLink rate per epoch
@@ -158,7 +161,8 @@ def manage_training(args) -> Trainer:
             raise ValueError("--class-weights needs %d comma-separated values" % num_classes)
     trainer = Trainer(model, optimizer, train_loader, valid_loader, device, class_weights=cw,
                       on_epoch_end=on_epoch_end, shard_eval=getattr(args, "shard_eval", False),
-                      accum_steps=getattr(args, "accum_steps", 1))
+                      accum_steps=getattr(args, "accum_steps", 1),
+                      label_smoothing=getattr(args, "label_smoothing", 0.0))
     trainer.profile_timeline = getattr(args, "profile", None) == "timeline"
     if getattr(args, "eval_only", False):        # score a checkpoint: one validation pass, no training
         test_loss, test_acc = trainer._evaluate()

@@ -13,6 +13,11 @@ Differences kept on purpose: metrics accumulate on the device and are read once 
 (``DeviceMeter``), ``set_epoch`` is called so shuffling changes between epochs, and throughput is
 reported on an extra line.
 
+``label_smoothing`` and batches that carry a MixUp / CutMix draw (``data.transforms.MixDraw``): on the
+torch path the images are mixed by torchvision and the loss is ``F.cross_entropy(outputs, targets,
+weight=, label_smoothing=)`` with torchvision's probability targets, as its classification reference
+script does; the native engine does the same in its kernels.  The test loss stays plain cross-entropy.
+
 ``accum_steps=K`` (gradient accumulation): one optimizer update per group of K consecutive training
 mini-batches, and after the epoch's last one, so the last group of an epoch may be shorter (k' < K) and
 no group crosses an epoch boundary.  Each mini-batch's loss is its own mean; the update uses the sum of
@@ -26,6 +31,7 @@ from typing import Optional
 import torch
 import torch.nn.functional as F
 
+from .data import transforms as T
 from .data.loader import FusedBatch, RaggedBatch
 from .utils.metrics import DeviceMeter
 
@@ -59,13 +65,15 @@ def _is_native(model) -> bool:
 class Trainer:
     def __init__(self, model, optimizer, train_loader, test_loader, device,
                  class_weights: Optional[torch.Tensor] = None, verbose_throughput: bool = True,
-                 on_epoch_end=None, shard_eval: bool = False, accum_steps: int = 1) -> None:
+                 on_epoch_end=None, shard_eval: bool = False, accum_steps: int = 1,
+                 label_smoothing: float = 0.0) -> None:
         if accum_steps < 1:
             raise ValueError("accum_steps must be >= 1 (got %d)" % accum_steps)
         if accum_steps > 1 and not hasattr(train_loader, "__len__"):
             raise ValueError("accum_steps > 1 needs a training loader with __len__: the last group of an epoch "
                              "ends at its last batch")
         self.accum_steps = int(accum_steps)
+        self.label_smoothing = float(label_smoothing)      # torch path; the native engine has its own
         self.model = model
         self.optimizer = optimizer
         self.train_loader = train_loader
@@ -155,8 +163,19 @@ class Trainer:
     def _to_device(self, batch):
         if isinstance(batch, (FusedBatch, RaggedBatch)):
             return batch.to_float(self.device)
-        inputs, targets = batch
+        inputs, targets = batch[0], batch[1]
         return inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
+
+    def _mixed_to_device(self, batch):
+        """(inputs, integer targets, probability targets or None) of a training batch: the batch's
+        MixUp / CutMix draw applied by torchvision (the reference pipeline has applied it already)."""
+        mix = batch.mix if isinstance(batch, (FusedBatch, RaggedBatch)) else (batch[2] if len(batch) > 2 else None)
+        inputs, targets = self._to_device(batch)
+        if mix is None:
+            return inputs, targets, None
+        if isinstance(batch, (FusedBatch, RaggedBatch)):
+            inputs = T.apply_mix(inputs, targets, mix)
+        return inputs, targets, mix
 
     def _updates_after(self, k: int, n_steps: int) -> bool:
         """Does the (k+1)-th training batch of an epoch of ``n_steps`` end its accumulation group?"""
@@ -195,9 +214,11 @@ class Trainer:
         pending = 0                                      # mini-batches accumulated since the last update
         for k, batch in enumerate(self.train_loader):
             update = self.accum_steps == 1 or self._updates_after(k, n_steps)
-            inputs, targets = self._to_device(batch)
+            inputs, targets, mix = self._mixed_to_device(batch)
             outputs = self.model(inputs)
-            loss = F.cross_entropy(outputs, targets, weight=self.class_weights)
+            soft = None if mix is None else T.mixed_targets(targets, outputs.shape[1], mix)
+            loss = F.cross_entropy(outputs, targets if soft is None else soft, weight=self.class_weights,
+                                   label_smoothing=self.label_smoothing)
             if pending == 0:                             # zeroed once per group, before its first backward
                 if wrapper is not None:
                     wrapper.zero_grad()
@@ -217,7 +238,8 @@ class Trainer:
                                 p.grad.mul_(1.0 / pending)
                 self.optimizer.step()
                 pending = 0
-            meter.add_reference(outputs.detach(), targets, self.class_weights)
+            meter.add_reference(outputs.detach(), targets, self.class_weights, soft_target=soft,
+                                label_smoothing=self.label_smoothing)
         return meter.snapshot()
 
     def _reduce_eval(self, meter: DeviceMeter):

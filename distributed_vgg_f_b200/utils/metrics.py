@@ -68,10 +68,25 @@ class DeviceMeter:
     def reset(self) -> None:
         self.buf.zero_()
 
-    def add_reference(self, logits: torch.Tensor, target: torch.Tensor, weight=None) -> None:
+    def add_reference(self, logits: torch.Tensor, target: torch.Tensor, weight=None,
+                      soft_target: torch.Tensor = None, label_smoothing: float = 0.0) -> None:
         """Torch-op fallback used by the oracle path (same arithmetic as the kernel): accumulates
         ``loss * batch`` exactly like ``Average.update(loss.item(), batch)`` in the reference's loop,
-        where ``loss`` is the (optionally class-weighted) mean torch reports."""
+        where ``loss`` is the (optionally class-weighted) mean torch reports.
+
+        ``soft_target`` (probability targets [B][C], MixUp / CutMix) and ``label_smoothing``: the loss is
+        F.cross_entropy's with them, and a sample is correct when argmax(logits) == argmax(soft_target)
+        (torchvision's classification reference, ``utils.accuracy`` on 2-D targets)."""
+        if soft_target is not None or label_smoothing:
+            with torch.no_grad():
+                tgt = soft_target if soft_target is not None else target
+                loss = torch.nn.functional.cross_entropy(logits.float(), tgt, weight=weight,
+                                                         label_smoothing=label_smoothing)
+                self.buf[0] += loss * logits.shape[0]
+                cls = soft_target.argmax(dim=1) if soft_target is not None else target
+                self.buf[1] += logits.argmax(dim=1).eq(cls).sum()
+                self.buf[2] += logits.shape[0]
+            return
         with torch.no_grad():
             logp = torch.log_softmax(logits.float(), dim=1)
             nll = -logp.gather(1, target.view(-1, 1)).view(-1)
