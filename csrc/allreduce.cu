@@ -368,8 +368,12 @@ struct Zero1Args {
   int slot;
   uint32_t epoch;
   float lr, b1, b2, eps, wd, bc1_inv, bc2_inv_sqrt;
+  float* ema;              // moving average of the weights (zero1_kernel<true>), as adam_kernel<true>
+  float ema_d, ema_a;
+  int ema_first;
 };
 
+template <bool EMA>
 __device__ __forceinline__ uint4 zero1_adam8(const Zero1Args& a, long long elem, const uint4& gred) {
   const uint32_t gw[4] = {gred.x, gred.y, gred.z, gred.w};
   float g[8];
@@ -396,6 +400,14 @@ __device__ __forceinline__ uint4 zero1_adam8(const Zero1Args& a, long long elem,
     __stcs(reinterpret_cast<float4*>(a.p + elem + 4 * h), make_float4(pp[4 * h], pp[4 * h + 1], pp[4 * h + 2], pp[4 * h + 3]));
     __stcs(reinterpret_cast<float4*>(a.m + elem + 4 * h), make_float4(mm[4 * h], mm[4 * h + 1], mm[4 * h + 2], mm[4 * h + 3]));
     __stcs(reinterpret_cast<float4*>(a.v + elem + 4 * h), make_float4(vv[4 * h], vv[4 * h + 1], vv[4 * h + 2], vv[4 * h + 3]));
+    if constexpr (EMA) {                 // one half at a time: 4 more live floats next to the Adam state
+      float4 e4 = __ldcs(reinterpret_cast<const float4*>(a.ema + elem + 4 * h));
+      e4.x = ema_update(e4.x, pp[4 * h], a.ema_d, a.ema_a, a.ema_first);
+      e4.y = ema_update(e4.y, pp[4 * h + 1], a.ema_d, a.ema_a, a.ema_first);
+      e4.z = ema_update(e4.z, pp[4 * h + 2], a.ema_d, a.ema_a, a.ema_first);
+      e4.w = ema_update(e4.w, pp[4 * h + 3], a.ema_d, a.ema_a, a.ema_first);
+      __stcs(reinterpret_cast<float4*>(a.ema + elem + 4 * h), e4);
+    }
   }
   return make_uint4(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3]), pack_bf16x2(pp[4], pp[5]),
                     pack_bf16x2(pp[6], pp[7]));
@@ -403,10 +415,11 @@ __device__ __forceinline__ uint4 zero1_adam8(const Zero1Args& a, long long elem,
 
 // 128 threads x <= 80 registers (the Adam state of 8 parameters lives in registers between the
 // reduce and the broadcast) = 10 240 registers: the same footprint as allreduce_kernel, so these CTAs
-// also co-reside with every conv kernel of backward.
+// also co-reside with every conv kernel of backward.  EMA: the owner also updates the moving average of
+// its cells (non-owned cells of `ema` are not touched; prepare_ema gathers them like prepare_export).
 constexpr int Z1_THREADS = 128;
 constexpr int Z1_MIN_BLOCKS = 6;
-template <int ALGO>
+template <int ALGO, bool EMA>
 __global__ void __launch_bounds__(Z1_THREADS, Z1_MIN_BLOCKS) zero1_kernel(const Zero1Args a) {
   static_assert(ALGO == AR_TWOSHOT || ALGO == AR_NVLS, "the owner-computes step needs a reduce-scatter");
   const CommCtx& c = a.c;
@@ -443,7 +456,7 @@ __global__ void __launch_bounds__(Z1_THREADS, Z1_MIN_BLOCKS) zero1_kernel(const 
     for (; v < cell1; v += Z1_THREADS) {
       const uint4 gred = gnext;
       if (v + Z1_THREADS < cell1) gnext = multimem_ld_reduce_bf16x8(mc + (v + Z1_THREADS) * 16);
-      multimem_st_v4(mc + v * 16, zero1_adam8(a, a.start + v * 8, gred));
+      multimem_st_v4(mc + v * 16, zero1_adam8<EMA>(a, a.start + v * 8, gred));
     }
   } else {
     for (long long v = cell0 + threadIdx.x; v < cell1; v += Z1_THREADS) {
@@ -455,7 +468,7 @@ __global__ void __launch_bounds__(Z1_THREADS, Z1_MIN_BLOCKS) zero1_kernel(const 
       }
       const uint4 gred = make_uint4(pack_bf16x2(acc[0], acc[1]), pack_bf16x2(acc[2], acc[3]),
                                     pack_bf16x2(acc[4], acc[5]), pack_bf16x2(acc[6], acc[7]));
-      const uint4 w8 = zero1_adam8(a, a.start + v * 8, gred);
+      const uint4 w8 = zero1_adam8<EMA>(a, a.start + v * 8, gred);
       for (int p = 0; p < world; ++p) {
         const int peer = (rank + p) % world;
         st_v4(reinterpret_cast<uint8_t*>(c.wire_ptrs[peer]) + boff, w8);
@@ -471,7 +484,8 @@ __global__ void __launch_bounds__(Z1_THREADS, Z1_MIN_BLOCKS) zero1_kernel(const 
 
 void zero1_step(const CommCtx& ctx, float* grad_f32, float* p, float* m, float* v, bf16* shadow,
                 long long start, long long n, float inv_world, int algo, int slot, uint32_t epoch, int max_ctas,
-                float lr, float beta1, float beta2, float eps, float weight_decay, int step, cudaStream_t s) {
+                float lr, float beta1, float beta2, float eps, float weight_decay, int step, cudaStream_t s,
+                float* ema, double ema_decay, bool ema_first) {
   if (ctx.world > AR_MAX_WORLD) throw std::runtime_error("[b200] zero1_step: world too large");
   if (n % 8 || start % 8) throw std::runtime_error("[b200] zero1_step: range must be 8-element aligned");
   if (algo == AR_NVLS && !ctx.wire_mc) throw std::runtime_error("[b200] zero1_step: NVLS needs a multicast mapping");
@@ -482,15 +496,25 @@ void zero1_step(const CommCtx& ctx, float* grad_f32, float* p, float* m, float* 
   a.lr = lr; a.b1 = beta1; a.b2 = beta2; a.eps = eps; a.wd = weight_decay;
   a.bc1_inv = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(beta1), step)));
   a.bc2_inv_sqrt = static_cast<float>(1.0 / sqrt(1.0 - pow(static_cast<double>(beta2), step)));
+  a.ema = ema; a.ema_first = ema_first ? 1 : 0;
+  a.ema_d = ema ? static_cast<float>(ema_decay) : 0.f;
+  a.ema_a = ema ? static_cast<float>(1.0 - ema_decay) : 0.f;
   const int G = allreduce_grid(n, ctx.world, max_ctas, false);
   static const bool carve = [] {
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, true>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, true>));
     return true;
   }();
   (void)carve;
-  if (algo == AR_NVLS) zero1_kernel<AR_NVLS><<<G, Z1_THREADS, 0, s>>>(a);
-  else zero1_kernel<AR_TWOSHOT><<<G, Z1_THREADS, 0, s>>>(a);
+  if (algo == AR_NVLS) {
+    if (ema) zero1_kernel<AR_NVLS, true><<<G, Z1_THREADS, 0, s>>>(a);
+    else zero1_kernel<AR_NVLS, false><<<G, Z1_THREADS, 0, s>>>(a);
+  } else {
+    if (ema) zero1_kernel<AR_TWOSHOT, true><<<G, Z1_THREADS, 0, s>>>(a);
+    else zero1_kernel<AR_TWOSHOT, false><<<G, Z1_THREADS, 0, s>>>(a);
+  }
   count_launch();
   check_last("zero1_step");
 }

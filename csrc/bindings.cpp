@@ -278,12 +278,21 @@ static void cross_entropy_soft(const at::Tensor& logits, const at::Tensor& targe
                            f32p_opt(class_weights), st, cur_stream());
 }
 
+// The optimizers' optional moving average of the weights: fp32, 16-byte aligned, p's size, decay in [0, 1].
+static void check_ema(const c10::optional<at::Tensor>& ema, int64_t n, double decay, const char* op) {
+  if (!ema.has_value()) return;
+  check_vec(*ema, at::kFloat, 16, op, "ema");
+  TORCH_CHECK(ema->numel() == n, op, ": ema must have p's size");
+  TORCH_CHECK(decay >= 0.0 && decay <= 1.0, op, ": ema_decay must lie in [0, 1], got ", decay);
+}
 static void adam(at::Tensor p, at::Tensor m, at::Tensor v, c10::optional<at::Tensor> g32,
                  c10::optional<at::Tensor> g16, c10::optional<at::Tensor> shadow, double lr, double b1, double b2,
-                 double eps, double wd, int64_t step, double grad_scale, c10::optional<at::Tensor> gzero) {
+                 double eps, double wd, int64_t step, double grad_scale, c10::optional<at::Tensor> gzero,
+                 c10::optional<at::Tensor> ema, double ema_decay, bool ema_first) {
   c10::cuda::CUDAGuard g(p.device());
   const int64_t n = p.numel();
   for (auto* t : {&p, &m, &v}) check_vec(*t, at::kFloat, 16, "adam", "p, m and v");
+  check_ema(ema, n, ema_decay, "adam");
   if (g32.has_value()) check_vec(*g32, at::kFloat, 16, "adam", "g32");
   if (gzero.has_value()) check_vec(*gzero, at::kFloat, 16, "adam", "gzero");
   if (g16.has_value()) check_vec(*g16, at::kBFloat16, 8, "adam", "g16");
@@ -294,14 +303,17 @@ static void adam(at::Tensor p, at::Tensor m, at::Tensor v, c10::optional<at::Ten
   TORCH_CHECK(m.numel() == n && v.numel() == n, "adam: every tensor has p's size");
   b200::adam_fused(f32p(p), f32p(m), f32p(v), f32p_opt(g32), bfp_opt(g16),
                    shadow.has_value() ? bfp_mut(*shadow) : nullptr, p.numel(), (float)lr, (float)b1, (float)b2,
-                   (float)eps, (float)wd, (int)step, (float)grad_scale, false, f32p_opt(gzero), cur_stream());
+                   (float)eps, (float)wd, (int)step, (float)grad_scale, false, f32p_opt(gzero), cur_stream(),
+                   f32p_opt(ema), ema_decay, ema_first);
 }
 static void sgd(at::Tensor p, at::Tensor mom, c10::optional<at::Tensor> g32, c10::optional<at::Tensor> g16,
                 c10::optional<at::Tensor> shadow, double lr, double momentum, double wd, bool first,
-                double grad_scale, c10::optional<at::Tensor> gzero) {
+                double grad_scale, c10::optional<at::Tensor> gzero, c10::optional<at::Tensor> ema, double ema_decay,
+                bool ema_first) {
   c10::cuda::CUDAGuard g(p.device());
   const int64_t n = p.numel();
   for (auto* t : {&p, &mom}) check_vec(*t, at::kFloat, 16, "sgd", "p and mom");
+  check_ema(ema, n, ema_decay, "sgd");
   if (g32.has_value()) check_vec(*g32, at::kFloat, 16, "sgd", "g32");
   if (gzero.has_value()) check_vec(*gzero, at::kFloat, 16, "sgd", "gzero");
   if (g16.has_value()) check_vec(*g16, at::kBFloat16, 8, "sgd", "g16");
@@ -312,7 +324,7 @@ static void sgd(at::Tensor p, at::Tensor mom, c10::optional<at::Tensor> g32, c10
   TORCH_CHECK(mom.numel() == n, "sgd: every tensor has p's size");
   b200::sgd_fused(f32p(p), f32p(mom), f32p_opt(g32), bfp_opt(g16), shadow.has_value() ? bfp_mut(*shadow) : nullptr,
                   p.numel(), (float)lr, (float)momentum, (float)wd, first, (float)grad_scale, f32p_opt(gzero),
-                  cur_stream());
+                  cur_stream(), f32p_opt(ema), ema_decay, ema_first);
 }
 
 static void check_augment(const at::Tensor& src, const at::Tensor& params, const at::Tensor& out, int64_t OH,
@@ -679,7 +691,8 @@ static void allreduce(const PyComm& comm, c10::optional<at::Tensor> grad, c10::o
 static void zero1_step(const PyComm& comm, c10::optional<at::Tensor> grad, at::Tensor p, at::Tensor m, at::Tensor v,
                        at::Tensor shadow, int64_t start, int64_t n, double inv_world, int64_t algo, int64_t slot,
                        int64_t epoch, int64_t max_ctas, double lr, double beta1, double beta2, double eps,
-                       double weight_decay, int64_t step) {
+                       double weight_decay, int64_t step, c10::optional<at::Tensor> ema, double ema_decay,
+                       bool ema_first) {
   TORCH_CHECK(p.scalar_type() == at::kFloat && m.scalar_type() == at::kFloat && v.scalar_type() == at::kFloat &&
                   shadow.scalar_type() == at::kBFloat16 && p.numel() == m.numel() && p.numel() == v.numel() &&
                   p.numel() == shadow.numel() && start + n <= p.numel(),
@@ -688,10 +701,15 @@ static void zero1_step(const PyComm& comm, c10::optional<at::Tensor> grad, at::T
   if (grad.has_value()) check_arena(*grad, at::kFloat, start, n, "zero1_step", "grad");
   for (auto* t : {&p, &m, &v}) check_arena(*t, at::kFloat, start, n, "zero1_step", "p, m and v");
   check_arena(shadow, at::kBFloat16, start, n, "zero1_step", "shadow");
+  if (ema.has_value()) {
+    check_arena(*ema, at::kFloat, start, n, "zero1_step", "ema");
+    TORCH_CHECK(ema->numel() == p.numel(), "zero1_step: ema must have p's size");
+    TORCH_CHECK(ema_decay >= 0.0 && ema_decay <= 1.0, "zero1_step: ema_decay must lie in [0, 1], got ", ema_decay);
+  }
   b200::zero1_step(comm.c, grad.has_value() ? grad->data_ptr<float>() : nullptr, p.data_ptr<float>(),
                    m.data_ptr<float>(), v.data_ptr<float>(), bfp_mut(shadow), start, n, (float)inv_world, (int)algo,
                    (int)slot, (uint32_t)epoch, (int)max_ctas, (float)lr, (float)beta1, (float)beta2, (float)eps,
-                   (float)weight_decay, (int)step, cur_stream());
+                   (float)weight_decay, (int)step, cur_stream(), f32p_opt(ema), ema_decay, ema_first);
 }
 static int64_t allreduce_grid(int64_t n, int64_t world, int64_t max_ctas, bool wire_fp32) {
   return b200::allreduce_grid(n, (int)world, (int)max_ctas, wire_fp32);
@@ -774,8 +792,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   py::arg("loss_out"), py::arg("class_weights"), py::arg("accumulate") = false,
   // soft = (eps, lam, mix): label smoothing and MixUp / CutMix targets (cross_entropy_soft); None: integer labels
   py::arg("soft") = py::none());
-  m.def("adam", &adam);
-  m.def("sgd", &sgd);
+  m.def("adam", &adam, py::arg("p"), py::arg("m"), py::arg("v"), py::arg("g32"), py::arg("g16"), py::arg("shadow"),
+        py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("step"),
+        py::arg("grad_scale"), py::arg("gzero"), py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0,
+        py::arg("ema_first") = false);
+  m.def("sgd", &sgd, py::arg("p"), py::arg("mom"), py::arg("g32"), py::arg("g16"), py::arg("shadow"), py::arg("lr"),
+        py::arg("momentum"), py::arg("wd"), py::arg("first"), py::arg("grad_scale"), py::arg("gzero"),
+        py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0, py::arg("ema_first") = false);
   m.def("augment", &augment);
   m.def("augment_mixed", &augment_mixed);
   m.def("augment_ragged", &augment_ragged);
@@ -800,7 +823,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   });
   m.def("make_comm", &make_comm);
   m.def("allreduce", &allreduce);
-  m.def("zero1_step", &zero1_step);
+  m.def("zero1_step", &zero1_step, py::arg("comm"), py::arg("grad"), py::arg("p"), py::arg("m"), py::arg("v"),
+        py::arg("shadow"), py::arg("start"), py::arg("n"), py::arg("inv_world"), py::arg("algo"), py::arg("slot"),
+        py::arg("epoch"), py::arg("max_ctas"), py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"),
+        py::arg("weight_decay"), py::arg("step"), py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0,
+        py::arg("ema_first") = false);
   m.def("allreduce_grid", &allreduce_grid);
   m.def("broadcast", &broadcast);
   m.def("barrier", &barrier);

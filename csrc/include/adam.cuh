@@ -1,4 +1,5 @@
-// One Adam step of one parameter (torch.optim.Adam with L2 weight decay, bias-corrected), shared by
+// One Adam step of one parameter (torch.optim.Adam with L2 weight decay, bias-corrected), and one
+// update of the weights' moving average, shared by
 // adam_kernel (loss_optim.cu) and zero1_kernel (allreduce.cu) so that the fused ZeRO-1 step and the
 // replicated optimizer give the same update bit for bit.  Every rounding is spelled out: left to
 // itself, nvcc contracted `g * gscale + wd * p` to fma(g, gscale, wd * p) in one kernel and
@@ -17,6 +18,14 @@ __device__ __forceinline__ void adam_update(float g, float gscale, float& p, flo
   v = __fmaf_rn(b2, v, __fmul_rn(__fmul_rn(1.f - b2, gk), gk));
   const float denom = __fmaf_rn(__fsqrt_rn(v), bc2_inv_sqrt, eps);
   p = __fsub_rn(p, __fdiv_rn(__fmul_rn(lr_bc1, m), denom));
+}
+
+// One update of the exponential moving average of a weight (torch.optim.swa_utils.AveragedModel with
+// torchvision's ema_avg): e' = d * e + a * p, d = fp32(decay), a = fp32(1 - decay) with 1 - decay
+// taken in double on the host.  Two multiplies and one add, each rounded, no FMA: what torch's eager
+// `decay * e + (1 - decay) * p` computes in fp32.  `first`: AveragedModel's first update copies p.
+__device__ __forceinline__ float ema_update(float e, float p, float d, float a, bool first) {
+  return first ? p : __fadd_rn(__fmul_rn(d, e), __fmul_rn(a, p));
 }
 
 }  // namespace b200

@@ -117,12 +117,17 @@ void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long l
                    cudaStream_t s, const SoftTargets* soft = nullptr);
 
 // Fused optimizers over flat arenas.  grad is fp32 (local) or bf16 (the reduced wire buffer).
+// With `ema`, the same pass also updates the weights' exponential moving average from the new p:
+// ema = decay * ema + (1 - decay) * p (fp32 rounding of each product and of the sum), or ema = p when
+// `ema_first` (AveragedModel's first update).
 void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16, bf16* shadow,
                 long long n, float lr, float beta1, float beta2, float eps, float weight_decay,
-                int step, float grad_scale, bool zero_grad, float* g32_to_zero, cudaStream_t s);
+                int step, float grad_scale, bool zero_grad, float* g32_to_zero, cudaStream_t s,
+                float* ema = nullptr, double ema_decay = 0.0, bool ema_first = false);
 void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* shadow, long long n,
                float lr, float momentum, float weight_decay, bool first_step, float grad_scale,
-               float* g32_to_zero, cudaStream_t s);
+               float* g32_to_zero, cudaStream_t s, float* ema = nullptr, double ema_decay = 0.0,
+               bool ema_first = false);
 
 // Fused input transform: uint8 HWC source -> normalised bf16.  mode 0: NHWC with C padded to
 // `cpad`; mode 1: layer-0 im2col matrix [N*OH*OW][kpad] (k = (kh*3+kw)*3 + c, zero padded).
@@ -181,9 +186,11 @@ void allreduce_fused(const CommCtx& ctx, const float* grad_f32, float* grad_out_
 int allreduce_grid(long long n, int world, int max_ctas, bool wire_fp32);
 // EXPERIMENTAL: ZeRO-1 step of arena range [start, start+n) in one kernel -- reduce-scatter, Adam on
 // the cells this rank owns, all-gather of the new bf16 weights into every rank's shadow (allreduce.cu).
+// With `ema`, the owner also updates the moving average of its cells as adam_fused does.
 void zero1_step(const CommCtx& ctx, float* grad_f32, float* p, float* m, float* v, bf16* shadow,
                 long long start, long long n, float inv_world, int algo, int slot, uint32_t epoch, int max_ctas,
-                float lr, float beta1, float beta2, float eps, float weight_decay, int step, cudaStream_t s);
+                float lr, float beta1, float beta2, float eps, float weight_decay, int step, cudaStream_t s,
+                float* ema = nullptr, double ema_decay = 0.0, bool ema_first = false);
 // Parameter broadcast rank `root` -> all through the wire buffer (K-BCAST).
 void broadcast_fused(const CommCtx& ctx, float* data_f32, long long n, int root, int slot,
                      uint32_t epoch, cudaStream_t s);

@@ -344,6 +344,17 @@ void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long l
 }
 
 // ---------------------------------------------------------------------------------------- Adam
+// The moving average of 4 new weights, streamed like every other optimizer operand.
+__device__ __forceinline__ void ema_store4(float* __restrict__ ema, long long i, const float (&pp)[4], float d, float a,
+                                           int first) {
+  float4 ev = __ldcs(reinterpret_cast<const float4*>(ema) + i);
+  ev.x = ema_update(ev.x, pp[0], d, a, first);
+  ev.y = ema_update(ev.y, pp[1], d, a, first);
+  ev.z = ema_update(ev.z, pp[2], d, a, first);
+  ev.w = ema_update(ev.w, pp[3], d, a, first);
+  __stcs(reinterpret_cast<float4*>(ema) + i, ev);
+}
+
 // One pass over the flat arena: read grad (fp32 local or bf16 reduced wire), update fp32 master
 // weight and both moments, emit the bf16 shadow used by the GEMMs, and zero the fp32 gradient so
 // the red.add wgrad epilogues of the next step start from zero.
@@ -352,11 +363,16 @@ void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long l
 // them, and the grid is one CTA per SM -- a background stream of HBM traffic.  (Round 1 launched 8
 // CTAs per SM: at every conv-kernel boundary the high-priority stream filled the SMs with optimizer
 // CTAs and the next conv kernel's persistent CTAs started late; bench/step_timeline.py.)
+// EMA: also update the weights' moving average `ema` from the new p while it is in registers (one
+// more fp32 stream, 8 B per parameter); the EMA = false instantiation is the plain optimizer.  The
+// EMA arguments come last so that the plain instantiation's parameter offsets stay where they were.
+template <bool EMA>
 __global__ void __launch_bounds__(256, 6) adam_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
                             const float* __restrict__ g32, const bf16* __restrict__ g16,
                             bf16* __restrict__ shadow, long long n4, float lr, float b1, float b2,
                             float eps, float wd, float bc1_inv, float bc2_inv_sqrt, float gscale,
-                            float* __restrict__ gzero) {
+                            float* __restrict__ gzero, float* __restrict__ ema, float ema_d, float ema_a,
+                            int ema_first) {
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     // Every stream here is touched exactly once per step: cache-streaming (evict-first) loads and
@@ -382,6 +398,7 @@ __global__ void __launch_bounds__(256, 6) adam_kernel(float* __restrict__ p, flo
     __stcs(reinterpret_cast<float4*>(p) + i, make_float4(pp[0], pp[1], pp[2], pp[3]));
     __stcs(reinterpret_cast<float4*>(m) + i, make_float4(mm[0], mm[1], mm[2], mm[3]));
     __stcs(reinterpret_cast<float4*>(v) + i, make_float4(vs[0], vs[1], vs[2], vs[3]));
+    if constexpr (EMA) ema_store4(ema, i, pp, ema_d, ema_a, ema_first);
     if (shadow)
       __stcs(reinterpret_cast<uint2*>(shadow + i * 4), make_uint2(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3])));
     if (gzero) __stcs(reinterpret_cast<float4*>(gzero) + i, make_float4(0.f, 0.f, 0.f, 0.f));
@@ -390,7 +407,8 @@ __global__ void __launch_bounds__(256, 6) adam_kernel(float* __restrict__ p, flo
 
 void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16, bf16* shadow,
                 long long n, float lr, float beta1, float beta2, float eps, float weight_decay,
-                int step, float grad_scale, bool, float* g32_to_zero, cudaStream_t s) {
+                int step, float grad_scale, bool, float* g32_to_zero, cudaStream_t s, float* ema,
+                double ema_decay, bool ema_first) {
   if (n % 4) throw std::runtime_error("[b200] adam_fused: n must be a multiple of 4");
   const double bc1 = 1.0 - pow(static_cast<double>(beta1), step);
   const double bc2 = 1.0 - pow(static_cast<double>(beta2), step);
@@ -401,22 +419,35 @@ void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16,
     const int v = e ? atoi(e) : 4;
     return v >= 1 && v <= 16 ? v : 4;
   }();
-  static const bool carve = (prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel)), true);
+  static const bool carve = [] {
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<true>));
+    return true;
+  }();
   (void)carve;
   const long long cap = static_cast<long long>(sm_count()) * per_sm;
   const int blocks = static_cast<int>(n4 / 256 + 1 < cap ? n4 / 256 + 1 : cap);
-  adam_kernel<<<blocks, 256, 0, s>>>(p, m, v, g32, g16, shadow, n4, lr, beta1, beta2, eps, weight_decay,
-                                     static_cast<float>(1.0 / bc1), static_cast<float>(1.0 / sqrt(bc2)),
-                                     grad_scale, g32_to_zero);
+  if (ema)
+    adam_kernel<true><<<blocks, 256, 0, s>>>(p, m, v, g32, g16, shadow, n4, lr, beta1, beta2, eps, weight_decay,
+                                             static_cast<float>(1.0 / bc1), static_cast<float>(1.0 / sqrt(bc2)),
+                                             grad_scale, g32_to_zero, ema, static_cast<float>(ema_decay),
+                                             static_cast<float>(1.0 - ema_decay), ema_first ? 1 : 0);
+  else
+    adam_kernel<false><<<blocks, 256, 0, s>>>(p, m, v, g32, g16, shadow, n4, lr, beta1, beta2, eps, weight_decay,
+                                              static_cast<float>(1.0 / bc1), static_cast<float>(1.0 / sqrt(bc2)),
+                                              grad_scale, g32_to_zero, nullptr, 0.f, 0.f, 0);
   count_launch();
   check_last("adam_fused");
 }
 
 // --------------------------------------------------------------------------------------- SGD
 // torch.optim.SGD(momentum) semantics: buf = g (first step) | momentum*buf + g ; p -= lr*buf.
+// EMA: as adam_kernel.
+template <bool EMA>
 __global__ void __launch_bounds__(256, 6) sgd_kernel(float* __restrict__ p, float* __restrict__ mom, const float* __restrict__ g32,
                            const bf16* __restrict__ g16, bf16* __restrict__ shadow, long long n4, float lr,
-                           float momentum, float wd, int first, float gscale, float* __restrict__ gzero) {
+                           float momentum, float wd, int first, float gscale, float* __restrict__ gzero,
+                           float* __restrict__ ema, float ema_d, float ema_a, int ema_first) {
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i);       // streaming, see adam_kernel
@@ -440,6 +471,7 @@ __global__ void __launch_bounds__(256, 6) sgd_kernel(float* __restrict__ p, floa
     }
     __stcs(reinterpret_cast<float4*>(p) + i, make_float4(pp[0], pp[1], pp[2], pp[3]));
     __stcs(reinterpret_cast<float4*>(mom) + i, make_float4(bb[0], bb[1], bb[2], bb[3]));
+    if constexpr (EMA) ema_store4(ema, i, pp, ema_d, ema_a, ema_first);
     if (shadow)
       __stcs(reinterpret_cast<uint2*>(shadow + i * 4), make_uint2(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3])));
     if (gzero) __stcs(reinterpret_cast<float4*>(gzero) + i, make_float4(0.f, 0.f, 0.f, 0.f));
@@ -448,15 +480,25 @@ __global__ void __launch_bounds__(256, 6) sgd_kernel(float* __restrict__ p, floa
 
 void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* shadow, long long n,
                float lr, float momentum, float weight_decay, bool first_step, float grad_scale,
-               float* g32_to_zero, cudaStream_t s) {
+               float* g32_to_zero, cudaStream_t s, float* ema, double ema_decay, bool ema_first) {
   if (n % 4) throw std::runtime_error("[b200] sgd_fused: n must be a multiple of 4");
   const long long n4 = n / 4;
-  static const bool carve = (prefer_max_shared_carveout(reinterpret_cast<const void*>(sgd_kernel)), true);
+  static const bool carve = [] {
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(sgd_kernel<false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(sgd_kernel<true>));
+    return true;
+  }();
   (void)carve;
   const long long cap = static_cast<long long>(sm_count()) * 4;
   const int blocks = static_cast<int>(n4 / 256 + 1 < cap ? n4 / 256 + 1 : cap);
-  sgd_kernel<<<blocks, 256, 0, s>>>(p, mom, g32, g16, shadow, n4, lr, momentum, weight_decay,
-                                    first_step ? 1 : 0, grad_scale, g32_to_zero);
+  if (ema)
+    sgd_kernel<true><<<blocks, 256, 0, s>>>(p, mom, g32, g16, shadow, n4, lr, momentum, weight_decay,
+                                            first_step ? 1 : 0, grad_scale, g32_to_zero, ema,
+                                            static_cast<float>(ema_decay), static_cast<float>(1.0 - ema_decay),
+                                            ema_first ? 1 : 0);
+  else
+    sgd_kernel<false><<<blocks, 256, 0, s>>>(p, mom, g32, g16, shadow, n4, lr, momentum, weight_decay,
+                                             first_step ? 1 : 0, grad_scale, g32_to_zero, nullptr, 0.f, 0.f, 0);
   count_launch();
   check_last("sgd_fused");
 }

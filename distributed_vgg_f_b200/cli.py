@@ -128,6 +128,14 @@ def build_parser() -> argparse.ArgumentParser:
     ext.add_argument("--accum-steps", type=int, default=1,
                      help="gradient accumulation: one optimizer update (and one gradient all-reduce) per K "
                           "mini-batches and after the last one of an epoch, with the mean of their gradients")
+    ext.add_argument("--model-ema", action="store_true",
+                     help="keep an exponential moving average of the weights (torchvision's --model-ema), evaluate it "
+                          "every epoch after the raw weights and save it in the checkpoint")
+    ext.add_argument("--model-ema-steps", type=int, default=32,
+                     help="update the EMA after every N-th optimizer update of an epoch, from its first (default 32)")
+    ext.add_argument("--model-ema-decay", type=float, default=0.99998,
+                     help="EMA decay per image seen, 0 <= d < 1; the decay of one update is adjusted as torchvision "
+                          "does: 1 - min(1, (1 - d) * world * mini_batch * accum_steps * model_ema_steps / epochs)")
     return parser
 
 
@@ -142,6 +150,10 @@ def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
         build_parser().error("--label-smoothing must lie in [0, 1)")
     if args.mixup_alpha < 0.0 or args.cutmix_alpha < 0.0:
         build_parser().error("--mixup-alpha and --cutmix-alpha must be >= 0")
+    if args.model_ema_steps < 1:
+        build_parser().error("--model-ema-steps must be >= 1")
+    if not 0.0 <= args.model_ema_decay < 1.0:
+        build_parser().error("--model-ema-decay must lie in [0, 1)")
     print(args)
     if args.socket_ifname:
         os.environ["GLOO_SOCKET_IFNAME"] = args.socket_ifname

@@ -89,7 +89,7 @@ class NativeEngine:
                  init_state: Optional[Dict[str, torch.Tensor]] = None, unpack_fp32: bool = False,
                  distributed: bool = True, zero1="auto", conv_bucket_mb: float = 9.5,
                  tail_bucket_kb: float = 2400.0, same_dropout_all_ranks: bool = False,
-                 label_smoothing: float = 0.0) -> None:
+                 label_smoothing: float = 0.0, ema_decay: Optional[float] = None) -> None:
         ops.require()
         if compute_dtype != "bf16":
             raise NotImplementedError("the native engine computes in bf16 with fp32 master weights; "
@@ -108,6 +108,13 @@ class NativeEngine:
         # training loss only: F.cross_entropy(label_smoothing=); the evaluation loss stays plain
         self.label_smoothing = float(label_smoothing)
         self._mix = None                 # MixUp / CutMix draw of the staged batch (data.transforms.MixDraw)
+        if ema_decay is not None and not 0.0 <= ema_decay <= 1.0:
+            raise ValueError("ema_decay must lie in [0, 1] (got %r)" % ema_decay)
+        # moving average of the weights (torchvision's --model-ema): ema = d * ema + (1 - d) * p, updated by
+        # the optimizer kernels of the steps that ask for it (train_step(ema=True)); None: no EMA at all
+        self.ema_decay = None if ema_decay is None else float(ema_decay)
+        self.ema_updates = 0             # AveragedModel's n_averaged
+        self._ema_step = False           # per train_step: this step's optimizer launches update the EMA
         self.same_dropout_all_ranks = bool(same_dropout_all_ranks)
         self.step_count = 0              # optimizer updates (Adam / SGD step, LR schedule, checkpoint "step")
         self.micro_count = 0             # training micro-batches: the Philox dropout offset
@@ -214,6 +221,15 @@ class NativeEngine:
         # 96 bytes of optimizer state each): more, equally thin, CTAs
         self.zero1_ctas = int(os.environ.get("B200_ZERO1_CTAS", "128"))
 
+        # EMA arenas: fp32 at p32's offsets (kept by the optimizer kernels) and its bf16 cast, made by
+        # prepare_ema() for an evaluation pass (w16 cannot hold it: under ZeRO-1 w16 is rebuilt only by
+        # the all-gather of the training step).  The average starts as the weights, like AveragedModel.
+        self.ema32 = self.p32.clone() if self.ema_decay is not None else None
+        self.ema16 = torch.zeros(n, dtype=BF16, device=dev) if self.ema_decay is not None else None
+        self._ema16_current = False
+        # arenas the forward pass reads weights (bf16) and biases (fp32) from; eval passes over the EMA swap them
+        self._wsrc, self._bsrc = self.w16, self.p32
+
         self._build_buffers()
 
     # ============================================================================ parameters
@@ -232,13 +248,16 @@ class NativeEngine:
             self._broadcast_params()
 
     def prepare_export(self) -> None:
-        """Collective.  Under --zero1 every rank holds the current fp32 master / moments only for the
-        cells it owns: sum the owned pieces over ranks so that every rank has the full state again."""
+        """Collective.  Under --zero1 every rank holds the current fp32 master / moments (and EMA) only
+        for the cells it owns: sum the owned pieces over ranks so that every rank has the full state again."""
         self._refuse_pending("prepare_export")
+        self._gather_owned((self.p32, self.m32, self.v32) + ((self.ema32,) if self.ema32 is not None else ()))
+
+    def _gather_owned(self, arenas) -> None:
         if not self._zero1_buckets:
             return
         self.sync()
-        for arena in (self.p32, self.m32, self.v32):
+        for arena in arenas:
             for bi in sorted(self._zero1_buckets):
                 bk = self.plan.buckets[bi]
                 tmp = torch.zeros(bk.end - bk.start, dtype=F32, device=self.device)
@@ -247,6 +266,36 @@ class NativeEngine:
                 dist.all_reduce(tmp)
                 arena[bk.start:bk.end] = tmp
         torch.cuda.synchronize(self.device)
+
+    def prepare_ema(self) -> None:
+        """Collective under --zero1.  Make the EMA readable by an evaluation pass: gather the owned EMA
+        cells of the sharded buckets (as prepare_export does), then cast ema32 -> ema16."""
+        self._require_ema("prepare_ema")
+        self._refuse_pending("prepare_ema")
+        self._gather_owned((self.ema32,))
+        ops.require().cast_to_bf16(self.ema32, self.ema16)
+        self._ema16_current = True
+
+    def export_ema_state(self) -> Dict[str, torch.Tensor]:
+        """The EMA in torch layout ({name: fp32 tensor}); under --zero1 call prepare_export first."""
+        self._require_ema("export_ema_state")
+        self._refuse_pending("export_ema_state")
+        return {name: L.to_torch(self.spec, name, self._view(self.ema32, name)).detach().cpu()
+                for name in self.spec.param_names}
+
+    def import_ema_state(self, state: Dict[str, torch.Tensor], n_averaged: int) -> None:
+        """Load a torch-layout EMA and its update count (AveragedModel's n_averaged)."""
+        self._require_ema("import_ema_state")
+        with torch.no_grad():
+            for name in self.spec.param_names:
+                t = state[name].detach().to(self.device, F32)
+                self._view(self.ema32, name).copy_(L.to_native(self.spec, name, t))
+        self.ema_updates = int(n_averaged)
+        self._ema16_current = False
+
+    def _require_ema(self, what: str) -> None:
+        if self.ema32 is None:
+            raise RuntimeError("%s: this engine keeps no EMA (construct it with ema_decay=)" % what)
 
     def _refuse_pending(self, what: str) -> None:
         if self._accum:
@@ -436,10 +485,10 @@ class NativeEngine:
 
     # =============================================================================== forward
     def _w(self, name: str) -> torch.Tensor:
-        return self._view(self.w16, name + ".weight")
+        return self._view(self._wsrc, name + ".weight")
 
     def _b(self, name: str) -> torch.Tensor:
-        return self._view(self.p32, name + ".bias")
+        return self._view(self._bsrc, name + ".bias")
 
     def _drop_key(self, layer: int) -> int:
         """Philox key of a dropout layer.  Every replica draws its OWN mask, like the reference's
@@ -647,6 +696,12 @@ class NativeEngine:
             if self._missing[bi] == 0 and self._update:
                 self._reduce_and_update(bi)
 
+    def _ema_kw(self, s: int, e: int) -> dict:
+        """The EMA arguments of an optimizer launch over [s, e): none unless this step updates the EMA."""
+        if not self._ema_step:
+            return {}
+        return dict(ema=self.ema32[s:e], ema_decay=self.ema_decay, ema_first=self.ema_updates == 0)
+
     def _apply_update(self, s: int, e: int, g16: Optional[torch.Tensor], zero: bool = True,
                       grad_scale: float = 1.0) -> None:
         g32 = None if g16 is not None else self.g32[s:e]
@@ -654,11 +709,12 @@ class NativeEngine:
         if self.opt_name == "adam":
             ops.adam_step(self.p32[s:e], self.m32[s:e], self.v32[s:e], g32=g32, g16=g16, shadow=self.w16[s:e],
                           lr=self.lr, beta1=self.beta1, beta2=self.beta2, eps=self.eps,
-                          weight_decay=self.weight_decay, step=self.step_count, grad_scale=grad_scale, zero=z)
+                          weight_decay=self.weight_decay, step=self.step_count, grad_scale=grad_scale, zero=z,
+                          **self._ema_kw(s, e))
         else:
             ops.sgd_step(self.p32[s:e], self.m32[s:e], g32=g32, g16=g16, shadow=self.w16[s:e], lr=self.lr,
                          momentum=self.momentum, weight_decay=self.weight_decay,
-                         first=(self.step_count == 1), grad_scale=grad_scale, zero=z)
+                         first=(self.step_count == 1), grad_scale=grad_scale, zero=z, **self._ema_kw(s, e))
 
     def _reduce_and_update(self, bi: int) -> None:
         bk = self.plan.buckets[bi]
@@ -707,7 +763,7 @@ class NativeEngine:
                                       s, e - s, algo=algo, slot=bi % self.arena.slots, max_ctas=self.zero1_ctas,
                                       inv_world=1.0 / (self.world * k), lr=self.lr, beta1=self.beta1,
                                       beta2=self.beta2, eps=self.eps, weight_decay=self.weight_decay,
-                                      step=self.step_count)
+                                      step=self.step_count, **self._ema_kw(s, e))
                 self._zero1_buckets.add(bi)
                 if zev0 is not None:             # reduce-scatter + optimizer + all-gather: same wire bytes
                     zev1 = torch.cuda.Event(enable_timing=True)
@@ -756,10 +812,15 @@ class NativeEngine:
         """Per-class loss weights (the reference's optional weighted cross-entropy)."""
         self.class_weights = None if weights is None else weights.to(self.device, F32).contiguous()
 
-    def train_step(self, batch, update: bool = True) -> torch.Tensor:
+    def train_step(self, batch, update: bool = True, ema: bool = False) -> torch.Tensor:
         """One micro-batch: forward, loss and backward into the gradient arena, and with ``update`` the
         reduction and optimizer step over the group of micro-batches accumulated since the last update
-        (mean of their gradients).  Returns the device scalar holding this batch's mean loss."""
+        (mean of their gradients).  With ``ema`` (and ``update``) the optimizer launches also update the
+        moving average of the weights from the new weights.  Returns the device scalar holding this
+        batch's mean loss."""
+        if ema:
+            self._require_ema("train_step(ema=True)")
+        self._ema_step = bool(ema and update and self.apply_updates)
         self.micro_count += 1
         if update:
             self.step_count += 1
@@ -785,29 +846,53 @@ class NativeEngine:
         self._backward(b)
         self._end_step()
         self._accum = 0 if update else self._accum + 1
+        if self._ema_step:
+            self.ema_updates += 1
+            self._ema16_current = False
+            self._ema_step = False
         self._mark("step end (joined comm)")
         t.stop("backward+reduce+update")
         if self.nvtx:
             torch.cuda.nvtx.range_pop()
         return self.loss_buf
 
-    def eval_step(self, batch) -> torch.Tensor:
-        b = self._stage_input(batch)
-        self._forward(b, train=False)
-        self._loss(b, train=False)
-        self._release_input()
+    def eval_step(self, batch, ema: bool = False) -> torch.Tensor:
+        """Evaluation forward, loss and metrics; ``ema``: with the moving average of the weights
+        (after prepare_ema())."""
+        self._use_weights(ema)
+        try:
+            b = self._stage_input(batch)
+            self._forward(b, train=False)
+            self._loss(b, train=False)
+            self._release_input()
+        finally:
+            self._use_weights(False)
         return self.loss_buf
 
-    def forward_logits(self, batch) -> torch.Tensor:
-        b = self._stage_input(batch)
-        self._forward(b, train=False)
-        if self.fused_head:          # the logits come out of the fused head kernel
-            keep = self.meter
-            self.meter = None
-            self._loss(b, train=False)
-            self.meter = keep
-        self._release_input()
+    def forward_logits(self, batch, ema: bool = False) -> torch.Tensor:
+        self._use_weights(ema)
+        try:
+            b = self._stage_input(batch)
+            self._forward(b, train=False)
+            if self.fused_head:          # the logits come out of the fused head kernel
+                keep = self.meter
+                self.meter = None
+                self._loss(b, train=False)
+                self.meter = keep
+            self._release_input()
+        finally:
+            self._use_weights(False)
         return self.logits[:b].clone()
+
+    def _use_weights(self, ema: bool) -> None:
+        """Point the forward pass at the EMA arenas (ema16 weights, ema32 biases) or back at w16 / p32."""
+        if ema:
+            self._require_ema("an EMA evaluation pass")
+            if not self._ema16_current:
+                raise RuntimeError("the EMA changed since its last cast: call prepare_ema() before an EMA pass")
+            self._wsrc, self._bsrc = self.ema16, self.ema32
+        else:
+            self._wsrc, self._bsrc = self.w16, self.p32
 
     def sync(self) -> None:
         torch.cuda.synchronize(self.device)

@@ -169,14 +169,26 @@ def soft_targets(label_smoothing: float = 0.0, mix=None):
     return [float(label_smoothing), mix.lam if mix is not None else 1.0, 1.0 if mix is not None else 0.0]
 
 
+def _ema_args(ema, ema_decay: float, ema_first: bool) -> tuple:
+    """Trailing arguments of the optimizer entries: none at all without a moving average."""
+    return () if ema is None else (ema, float(ema_decay), bool(ema_first))
+
+
 def adam_step(p, m, v, *, g32=None, g16=None, shadow=None, lr, beta1=0.9, beta2=0.999, eps=1e-8,
-              weight_decay=0.0, step: int, grad_scale: float = 1.0, zero=None):
-    require().adam(p, m, v, g32, g16, shadow, lr, beta1, beta2, eps, weight_decay, step, grad_scale, zero)
+              weight_decay=0.0, step: int, grad_scale: float = 1.0, zero=None, ema=None, ema_decay: float = 0.0,
+              ema_first: bool = False):
+    """Fused Adam over a flat range.  ``ema`` (fp32, p's size): the same pass also updates the weights'
+    moving average, ema = decay * ema + (1 - decay) * p_new, or ema = p_new with ``ema_first``."""
+    require().adam(p, m, v, g32, g16, shadow, lr, beta1, beta2, eps, weight_decay, step, grad_scale, zero,
+                   *_ema_args(ema, ema_decay, ema_first))
 
 
 def sgd_step(p, mom, *, g32=None, g16=None, shadow=None, lr, momentum=0.9, weight_decay=0.0,
-             first: bool, grad_scale: float = 1.0, zero=None):
-    require().sgd(p, mom, g32, g16, shadow, lr, momentum, weight_decay, first, grad_scale, zero)
+             first: bool, grad_scale: float = 1.0, zero=None, ema=None, ema_decay: float = 0.0,
+             ema_first: bool = False):
+    """Fused SGD (momentum) over a flat range; ``ema`` as for ``adam_step``."""
+    require().sgd(p, mom, g32, g16, shadow, lr, momentum, weight_decay, first, grad_scale, zero,
+                  *_ema_args(ema, ema_decay, ema_first))
 
 
 _MIX_KIND = {"mixup": 1, "cutmix": 2}

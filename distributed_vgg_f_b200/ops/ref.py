@@ -557,6 +557,20 @@ def sgd_step64(p, buf, g, *, lr: float, momentum: float, weight_decay: float, fi
     return {"p": (p1, e_p), "buf": (b1, e_b)}
 
 
+def ema_step64(ema, p, *, decay: float, first: bool):
+    """One update of the weights' moving average as the optimizer kernels apply it from the new weights
+    p: ema * d + p * a with d = fp32(decay), a = fp32(1 - decay) (1 - decay taken in double), or a copy
+    of p on the first update.  Returns (ref, err) like adam_step64: two rounded products and one
+    rounded sum."""
+    u = _U
+    e64, p64 = _f64(ema), _f64(p)
+    if first:
+        return p64, torch.zeros_like(p64)
+    de, ap = _f32(decay) * e64, _f32(1.0 - decay) * p64
+    r = de + ap
+    return r, u * (de.abs() + ap.abs() + r.abs())
+
+
 def nchw_to_nhwc64(x: torch.Tensor, cpad: int):
     """nchw_to_nhwc: fp32 NCHW -> NHWC with channels zero-padded to cpad (the kernel rounds to bf16)."""
     N, C, H, W = x.shape

@@ -7,6 +7,7 @@ print one line per image::
 
     python -m distributed_vgg_f_b200.tools.predict ck.pt --classes edible,other,toy img1.png img2.png
     python -m distributed_vgg_f_b200.tools.predict ck.pt --data-root /data/coil3 /data/coil3/ValidationData/toy
+    python -m distributed_vgg_f_b200.tools.predict ck.pt --ema img1.png      # the weights' moving average
 
 ``--classes`` (or ``--data-root``, whose TrainData sub-folders define them) only names the outputs;
 directories are expanded to the image files inside.  Runs on the GPU through the native engine when
@@ -38,9 +39,15 @@ def expand(paths: Sequence[str]) -> List[str]:
     return out
 
 
-def load_model(checkpoint: str, model: Optional[str] = None, num_classes: Optional[int] = None):
+def load_model(checkpoint: str, model: Optional[str] = None, num_classes: Optional[int] = None, ema: bool = False):
+    """(spec, torch-layout state) of a checkpoint; ``ema``: its moving average of the weights (--model-ema)."""
     payload = torch.load(checkpoint, map_location="cpu", weights_only=True)
-    state = strip_module_prefix(payload["model"] if "model" in payload else payload)
+    if ema:
+        if not isinstance(payload, dict) or "model_ema" not in payload:
+            raise ValueError("%s holds no model EMA (it was not saved with --model-ema)" % checkpoint)
+        state = strip_module_prefix({k: v for k, v in payload["model_ema"].items() if k != "n_averaged"})
+    else:
+        state = strip_module_prefix(payload["model"] if "model" in payload else payload)
     saved = payload.get("args", {}) if isinstance(payload, dict) else {}
     last = [k for k in state if k.endswith(".weight")][-1]
     classes = num_classes or int(state[last].shape[0])
@@ -50,11 +57,11 @@ def load_model(checkpoint: str, model: Optional[str] = None, num_classes: Option
 
 @torch.no_grad()
 def predict(checkpoint: str, images: Sequence[str], model: Optional[str] = None, engine: str = "auto",
-            batch: int = 32):
+            batch: int = 32, ema: bool = False):
     """Returns (logits [n, C] fp32 on the CPU, files)."""
     from PIL import Image
 
-    spec, state = load_model(checkpoint, model)
+    spec, state = load_model(checkpoint, model, ema=ema)
     files = expand(images)
     tf = reference_transforms(train=False)
     use_native = engine == "native" or (engine == "auto" and torch.cuda.is_available()
@@ -84,8 +91,9 @@ def main(argv=None) -> int:
     ap.add_argument("--model", default=None, help="architecture (default: the one recorded in the checkpoint)")
     ap.add_argument("--engine", default="auto", choices=["auto", "native", "oracle"])
     ap.add_argument("--batch", type=int, default=32)
+    ap.add_argument("--ema", action="store_true", help="classify with the checkpoint's EMA weights (--model-ema)")
     a = ap.parse_args(argv)
-    logits, files = predict(a.checkpoint, a.images, a.model, a.engine, a.batch)
+    logits, files = predict(a.checkpoint, a.images, a.model, a.engine, a.batch, ema=a.ema)
     names = a.classes.split(",") if a.classes else None
     if names is None and a.data_root:
         names = find_classes(os.path.join(a.data_root, DATA.train_dir))[0]

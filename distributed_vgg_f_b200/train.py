@@ -44,6 +44,25 @@ def _want_native(args, device: torch.device) -> bool:
     return native_ok
 
 
+def model_ema_decay(decay: float, world_size: int, mini_batch: int, accum_steps: int, ema_steps: int,
+                    epochs: int) -> float:
+    """The decay of one EMA update, as torchvision's classification reference adjusts --model-ema-decay
+    (a decay per image) to the images seen between two updates; K = accum_steps = 1 is its formula."""
+    adjust = world_size * mini_batch * accum_steps * ema_steps / epochs
+    alpha = min(1.0, (1.0 - decay) * adjust)
+    return 1.0 - alpha
+
+
+def build_model_ema(module: torch.nn.Module, decay: float):
+    """torchvision's ExponentialMovingAverage: AveragedModel with ema_avg, buffers averaged too."""
+    from torch.optim.swa_utils import AveragedModel
+
+    def ema_avg(avg_model_param, model_param, num_averaged):
+        return decay * avg_model_param + (1 - decay) * model_param
+
+    return AveragedModel(module, avg_fn=ema_avg, use_buffers=True)
+
+
 def build_optimizer(params, args):
     if args.optimizer == "sgd":
         return torch.optim.SGD(params, lr=args.learning_rate, momentum=args.momentum)
@@ -95,6 +114,11 @@ def manage_training(args) -> Trainer:
     if distributed_is_initialized():
         print("[Info] distributed training has been initialized")
 
+    ema_decay = None
+    if getattr(args, "model_ema", False):
+        ema_decay = model_ema_decay(args.model_ema_decay, args.world_size, args.mini_batch,
+                                    getattr(args, "accum_steps", 1), args.model_ema_steps, args.epochs)
+
     if _want_native(args, device):
         from .engine.native_engine import NativeEngine
 
@@ -104,8 +128,9 @@ def manage_training(args) -> Trainer:
                              wire_dtype=args.wire_dtype, bucket_mb=args.bucket_mb, seed=args.seed,
                              pretrained_state=pretrained, profile=args.profile,
                              zero1={"auto": "auto", "on": True, "off": False}[getattr(args, "zero1", "auto")],
-                             label_smoothing=getattr(args, "label_smoothing", 0.0))
+                             label_smoothing=getattr(args, "label_smoothing", 0.0), ema_decay=ema_decay)
         optimizer = None            # fused into the engine
+        model_ema = True if ema_decay is not None else None       # kept by the engine's optimizer kernels
         if model.world > 1:
             model.comm_timing(True)   # [Perf] line: all-reduce GB/s and fraction of the NVLink rate per epoch
     else:
@@ -113,10 +138,16 @@ def manage_training(args) -> Trainer:
         if distributed_is_initialized():
             model = FlatDDP(model, bucket_cap_mb=args.bucket_mb)
         optimizer = build_optimizer(model.parameters(), args)
+        model_ema = None
+        if ema_decay is not None:
+            model_ema = build_model_ema(model.module if isinstance(model, FlatDDP) else model, ema_decay)
 
+    if getattr(args, "eval_only", False) and model_ema is not None and not args.resume:
+        raise ValueError("--eval-only --model-ema scores a checkpoint's EMA: pass --resume <checkpoint>")
     start_epoch = 1
     if args.resume:
-        start_epoch = ckpt.load_checkpoint(args.resume, model, optimizer) + 1
+        kw = {} if model_ema is None else dict(model_ema=model_ema, ema_required=getattr(args, "eval_only", False))
+        start_epoch = ckpt.load_checkpoint(args.resume, model, optimizer, **kw) + 1
         print("[Info] resumed from {} at epoch {}".format(args.resume, start_epoch))
 
     base_lr = args.learning_rate
@@ -138,8 +169,9 @@ def manage_training(args) -> Trainer:
             else:
                 model.set_lr(new_lr)
         if args.save:
+            kw = {} if model_ema is None else dict(model_ema=model_ema)
             ckpt.save_checkpoint(args.save, model, optimizer, epoch, vars(args),
-                                 is_rank0=(args.rank == 0))
+                                 is_rank0=(args.rank == 0), **kw)
             # rank 0 is busy with a ~1.6 GB D2H copy + torch.save: hold the other ranks HERE, on the
             # host, instead of letting them spin inside the next epoch's first all-reduce kernel
             if distributed_is_initialized():
@@ -162,12 +194,18 @@ def manage_training(args) -> Trainer:
     trainer = Trainer(model, optimizer, train_loader, valid_loader, device, class_weights=cw,
                       on_epoch_end=on_epoch_end, shard_eval=getattr(args, "shard_eval", False),
                       accum_steps=getattr(args, "accum_steps", 1),
-                      label_smoothing=getattr(args, "label_smoothing", 0.0))
+                      label_smoothing=getattr(args, "label_smoothing", 0.0), model_ema=model_ema,
+                      model_ema_steps=getattr(args, "model_ema_steps", 32))
     trainer.profile_timeline = getattr(args, "profile", None) == "timeline"
     if getattr(args, "eval_only", False):        # score a checkpoint: one validation pass, no training
         test_loss, test_acc = trainer._evaluate()
         print("[Info] Evaluation: test loss: {}, test acc: {}.".format(test_loss, test_acc), flush=True)
-        trainer.history.append(dict(epoch=start_epoch - 1, test_loss=test_loss.average, test_acc=test_acc.accuracy))
+        rec = dict(epoch=start_epoch - 1, test_loss=test_loss.average, test_acc=test_acc.accuracy)
+        if model_ema is not None:
+            ema_loss, ema_acc = trainer._evaluate(ema=True)
+            print("[Info] Evaluation: EMA test loss: {}, EMA test acc: {}.".format(ema_loss, ema_acc), flush=True)
+            rec.update(ema_test_loss=ema_loss.average, ema_test_acc=ema_acc.accuracy)
+        trainer.history.append(rec)
         return trainer
     trainer.fit(args.epochs, start_epoch=start_epoch)
     return trainer

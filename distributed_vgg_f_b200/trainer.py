@@ -22,6 +22,12 @@ script does; the native engine does the same in its kernels.  The test loss stay
 mini-batches, and after the epoch's last one, so the last group of an epoch may be shorter (k' < K) and
 no group crosses an epoch boundary.  Each mini-batch's loss is its own mean; the update uses the sum of
 the group's gradients divided by k'.  Metrics count every mini-batch.
+
+``model_ema`` (torchvision's --model-ema): after the optimizer update whose 0-based index u within the
+epoch has u % model_ema_steps == 0, the moving average of the weights is updated -- by the native engine's
+optimizer kernels (``model_ema=True``, ``train_step(ema=True)``), or on the torch path by
+``model_ema.update_parameters`` (an ``AveragedModel``) after ``optimizer.step()``.  Every epoch the
+average is evaluated after the raw weights: ``[Info] Epoch: e/E, EMA test loss: .., EMA test acc: ..%.``
 """
 from __future__ import annotations
 
@@ -66,7 +72,7 @@ class Trainer:
     def __init__(self, model, optimizer, train_loader, test_loader, device,
                  class_weights: Optional[torch.Tensor] = None, verbose_throughput: bool = True,
                  on_epoch_end=None, shard_eval: bool = False, accum_steps: int = 1,
-                 label_smoothing: float = 0.0) -> None:
+                 label_smoothing: float = 0.0, model_ema=None, model_ema_steps: int = 32) -> None:
         if accum_steps < 1:
             raise ValueError("accum_steps must be >= 1 (got %d)" % accum_steps)
         if accum_steps > 1 and not hasattr(train_loader, "__len__"):
@@ -74,6 +80,12 @@ class Trainer:
                              "ends at its last batch")
         self.accum_steps = int(accum_steps)
         self.label_smoothing = float(label_smoothing)      # torch path; the native engine has its own
+        if model_ema_steps < 1:
+            raise ValueError("model_ema_steps must be >= 1 (got %d)" % model_ema_steps)
+        if model_ema is not None and _is_native(model) and getattr(model, "ema32", None) is None:
+            raise ValueError("model_ema on the native engine needs NativeEngine(ema_decay=...)")
+        self.model_ema = model_ema          # AveragedModel (torch path), True (native engine) or None
+        self.model_ema_steps = int(model_ema_steps)
         self.model = model
         self.optimizer = optimizer
         self.train_loader = train_loader
@@ -104,6 +116,13 @@ class Trainer:
                 "test loss: {}, test acc: {}.".format(test_loss, test_acc),
                 flush=True,
             )
+            ema_s = 0.0
+            if self.model_ema is not None:
+                te = time.perf_counter()
+                ema_loss, ema_acc = self._evaluate(ema=True)
+                print("[Info] Epoch: {}/{}, EMA test loss: {}, EMA test acc: {}.".format(epoch, epochs, ema_loss,
+                                                                                      ema_acc), flush=True)
+                ema_s = time.perf_counter() - te
             if self.verbose_throughput and train_loss.count:
                 print("[Perf] Epoch: {}/{}, train images/sec (this rank): {:.1f}{}{}".format(
                     epoch, epochs, train_loss.count / max(t1 - t0, 1e-9),
@@ -113,10 +132,12 @@ class Trainer:
                     print("[Perf] Epoch: {}/{}, host: first batch after {:.1f} ms, steps enqueued in {:.1f} ms, "
                           "GPU drained {:.1f} ms later; validation pass {:.1f} ms".format(
                               epoch, epochs, ht["first_batch_ms"], ht["enqueue_ms"], ht["drain_ms"],
-                              1e3 * (time.perf_counter() - t1)), flush=True)
+                              1e3 * (time.perf_counter() - t1 - ema_s)), flush=True)
             self.history.append(dict(epoch=epoch, train_loss=train_loss.average,
                                      train_acc=train_acc.accuracy, test_loss=test_loss.average,
                                      test_acc=test_acc.accuracy))
+            if self.model_ema is not None:
+                self.history[-1].update(ema_test_loss=ema_loss.average, ema_test_acc=ema_acc.accuracy)
             if self.on_epoch_end is not None:
                 self.on_epoch_end(epoch, self)
 
@@ -181,6 +202,10 @@ class Trainer:
         """Does the (k+1)-th training batch of an epoch of ``n_steps`` end its accumulation group?"""
         return (k + 1) % self.accum_steps == 0 or k + 1 == n_steps
 
+    def _ema_after(self, u: int) -> bool:
+        """Does the epoch's optimizer update of 0-based index ``u`` update the EMA?"""
+        return self.model_ema is not None and u % self.model_ema_steps == 0
+
     def _train(self):
         meter = DeviceMeter(self.device)
         if _is_native(self.model):
@@ -189,6 +214,7 @@ class Trainer:
             first = None
             want_tl = getattr(self, "profile_timeline", False) and hasattr(self.model, "timeline")
             n_steps = len(self.train_loader) if hasattr(self.train_loader, "__len__") else 0
+            u = 0                                          # optimizer updates so far in this epoch
             for k, batch in enumerate(self.train_loader):
                 if first is None:
                     first = time.perf_counter() - t0       # loader start-up: time to the first batch
@@ -196,7 +222,11 @@ class Trainer:
                     self.model.sync()
                     self.model.timeline(True)
                 if self.accum_steps == 1 or self._updates_after(k, n_steps):
-                    self.model.train_step(batch)
+                    if self._ema_after(u):
+                        self.model.train_step(batch, ema=True)
+                    else:
+                        self.model.train_step(batch)
+                    u += 1
                 else:
                     self.model.train_step(batch, update=False)
             t1 = time.perf_counter()
@@ -212,6 +242,8 @@ class Trainer:
         wrapper = self.model if hasattr(self.model, "finish_backward") else None
         n_steps = len(self.train_loader) if self.accum_steps > 1 else 0
         pending = 0                                      # mini-batches accumulated since the last update
+        u = 0                                            # optimizer updates so far in this epoch
+        module = self.model.module if wrapper is not None else self.model
         for k, batch in enumerate(self.train_loader):
             update = self.accum_steps == 1 or self._updates_after(k, n_steps)
             inputs, targets, mix = self._mixed_to_device(batch)
@@ -237,6 +269,9 @@ class Trainer:
                             if p.grad is not None:
                                 p.grad.mul_(1.0 / pending)
                 self.optimizer.step()
+                if self._ema_after(u):
+                    self.model_ema.update_parameters(module)
+                u += 1
                 pending = 0
             meter.add_reference(outputs.detach(), targets, self.class_weights, soft_target=soft,
                                 label_smoothing=self.label_smoothing)
@@ -250,19 +285,26 @@ class Trainer:
             dist.all_reduce(meter.buf)
         return meter.snapshot()
 
-    def _evaluate(self):
+    def _evaluate(self, ema: bool = False):
+        """One validation pass over the weights, or with ``ema`` over their moving average."""
         meter = DeviceMeter(self.device)
         if _is_native(self.model):
             self.model.set_meter(meter)
+            if ema:
+                self.model.prepare_ema()             # collective under ZeRO-1: gathers the owned EMA cells
             for batch in self.test_loader:
-                self.model.eval_step(batch)
+                if ema:
+                    self.model.eval_step(batch, ema=True)
+                else:
+                    self.model.eval_step(batch)
             self.model.sync()
             return self._reduce_eval(meter)
 
-        self.model.eval()
+        net = self.model_ema if ema else self.model
+        net.eval()
         with torch.no_grad():
             for batch in self.test_loader:
                 inputs, targets = self._to_device(batch)
-                outputs = self.model(inputs)
+                outputs = net(inputs)
                 meter.add_reference(outputs, targets)
         return self._reduce_eval(meter)

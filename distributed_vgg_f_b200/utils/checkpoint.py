@@ -15,6 +15,10 @@ with ``torch.save`` on rank 0 only.  ``strip_module_prefix(ckpt["model"])`` load
 reference's *unwrapped* model object (``vgg_funnel_model(C).load_state_dict``).  The native engine
 stores conv weights as OHWI and FC-1 columns in NHWC-flatten order; conversion to / from the torch
 layout happens here (``engine.export_state`` / ``import_state``).
+
+With ``--model-ema`` the payload also holds ``"model_ema"``: ``{"n_averaged": int64 tensor,
+module.<torchvision name>: fp32 tensor, ...}``, the keys of torchvision's
+``AveragedModel(vgg_funnel_model(C)).state_dict()``, so that it loads into one directly.
 """
 from __future__ import annotations
 
@@ -48,8 +52,19 @@ def optimizer_state(model, optimizer) -> Dict[str, Any]:
     return optimizer.state_dict() if optimizer is not None else {}
 
 
+def ema_state(model, model_ema) -> Dict[str, torch.Tensor]:
+    """The ``"model_ema"`` entry: an AveragedModel's state dict (torch path), or the native engine's EMA
+    (``model_ema`` is then True) under the same keys."""
+    if isinstance(model_ema, torch.nn.Module):
+        return {k: (v.detach().cpu() if k == "n_averaged" else v.detach().to("cpu", torch.float32))
+                for k, v in model_ema.state_dict().items()}
+    state = {"n_averaged": torch.tensor(model.ema_updates, dtype=torch.int64)}
+    state.update(add_module_prefix(model.export_ema_state()))
+    return state
+
+
 def save_checkpoint(path: str, model, optimizer, epoch: int, args: Optional[dict] = None,
-                    is_rank0: bool = True) -> None:
+                    is_rank0: bool = True, model_ema=None) -> None:
     if hasattr(model, "prepare_export"):     # collective: engines with sharded optimizer state gather it
         model.prepare_export()
     if not is_rank0:
@@ -57,16 +72,30 @@ def save_checkpoint(path: str, model, optimizer, epoch: int, args: Optional[dict
     payload = {"format": FORMAT, "model": model_state(model),
                "optimizer": optimizer_state(model, optimizer), "epoch": int(epoch),
                "args": dict(args or {})}
+    if model_ema is not None:
+        payload["model_ema"] = ema_state(model, model_ema)
     tmp = path + ".tmp"
     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
     torch.save(payload, tmp)
     os.replace(tmp, path)
 
 
-def load_checkpoint(path: str, model, optimizer=None) -> int:
-    """Restore model (+ optimizer) and return the epoch to resume *after*."""
+def load_checkpoint(path: str, model, optimizer=None, model_ema=None, ema_required: bool = False) -> int:
+    """Restore model (+ optimizer, + the EMA when ``model_ema`` is given) and return the epoch to resume
+    *after*.  A checkpoint without an EMA leaves the EMA fresh, or fails with ``ema_required``."""
     # our files hold tensors and plain containers only: no need to unpickle arbitrary objects
     payload = torch.load(path, map_location="cpu", weights_only=True)
+    if model_ema is not None:
+        ema = payload.get("model_ema") if isinstance(payload, dict) else None
+        if ema is None:
+            if ema_required:
+                raise ValueError("%s holds no model EMA (it was not saved with --model-ema)" % path)
+            print("[Info] %s holds no model EMA: the EMA starts fresh" % path, flush=True)
+        elif isinstance(model_ema, torch.nn.Module):
+            model_ema.load_state_dict(ema)
+        else:
+            model.import_ema_state(strip_module_prefix({k: v for k, v in ema.items() if k != "n_averaged"}),
+                                   int(ema["n_averaged"]))
     state = payload["model"] if "model" in payload else payload
     if hasattr(model, "import_state"):
         model.import_state(strip_module_prefix(state))
