@@ -368,12 +368,13 @@ struct Zero1Args {
   int slot;
   uint32_t epoch;
   float lr, b1, b2, eps, wd, bc1_inv, bc2_inv_sqrt;
+  float keep;              // AdamW (zero1_kernel<..., true>): fp32(1 - lr * wd), as adam_kernel's segment value
   float* ema;              // moving average of the weights (zero1_kernel<true>), as adam_kernel<true>
   float ema_d, ema_a;
   int ema_first;
 };
 
-template <bool EMA>
+template <bool EMA, bool DECOUPLED>
 __device__ __forceinline__ uint4 zero1_adam8(const Zero1Args& a, long long elem, const uint4& gred) {
   const uint32_t gw[4] = {gred.x, gred.y, gred.z, gred.w};
   float g[8];
@@ -393,8 +394,12 @@ __device__ __forceinline__ uint4 zero1_adam8(const Zero1Args& a, long long elem,
     vv[4 * h] = v4.x; vv[4 * h + 1] = v4.y; vv[4 * h + 2] = v4.z; vv[4 * h + 3] = v4.w;
   }
 #pragma unroll
-  for (int k = 0; k < 8; ++k)            // the update of adam_kernel at grad_scale 1, bit for bit
-    adam_update(g[k], 1.f, pp[k], mm[k], vv[k], a.lr * a.bc1_inv, a.b1, a.b2, a.eps, a.wd, a.bc2_inv_sqrt);
+  for (int k = 0; k < 8; ++k) {          // the update of adam_kernel at grad_scale 1, bit for bit
+    if constexpr (DECOUPLED)
+      adamw_update(g[k], 1.f, pp[k], mm[k], vv[k], a.lr * a.bc1_inv, a.b1, a.b2, a.eps, a.keep, a.bc2_inv_sqrt);
+    else
+      adam_update(g[k], 1.f, pp[k], mm[k], vv[k], a.lr * a.bc1_inv, a.b1, a.b2, a.eps, a.wd, a.bc2_inv_sqrt);
+  }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     __stcs(reinterpret_cast<float4*>(a.p + elem + 4 * h), make_float4(pp[4 * h], pp[4 * h + 1], pp[4 * h + 2], pp[4 * h + 3]));
@@ -417,9 +422,10 @@ __device__ __forceinline__ uint4 zero1_adam8(const Zero1Args& a, long long elem,
 // reduce and the broadcast) = 10 240 registers: the same footprint as allreduce_kernel, so these CTAs
 // also co-reside with every conv kernel of backward.  EMA: the owner also updates the moving average of
 // its cells (non-owned cells of `ema` are not touched; prepare_ema gathers them like prepare_export).
+// DECOUPLED: AdamW.  ZeRO-1 buckets hold one FC weight each, so one decay covers the whole range.
 constexpr int Z1_THREADS = 128;
 constexpr int Z1_MIN_BLOCKS = 6;
-template <int ALGO, bool EMA>
+template <int ALGO, bool EMA, bool DECOUPLED>
 __global__ void __launch_bounds__(Z1_THREADS, Z1_MIN_BLOCKS) zero1_kernel(const Zero1Args a) {
   static_assert(ALGO == AR_TWOSHOT || ALGO == AR_NVLS, "the owner-computes step needs a reduce-scatter");
   const CommCtx& c = a.c;
@@ -456,7 +462,7 @@ __global__ void __launch_bounds__(Z1_THREADS, Z1_MIN_BLOCKS) zero1_kernel(const 
     for (; v < cell1; v += Z1_THREADS) {
       const uint4 gred = gnext;
       if (v + Z1_THREADS < cell1) gnext = multimem_ld_reduce_bf16x8(mc + (v + Z1_THREADS) * 16);
-      multimem_st_v4(mc + v * 16, zero1_adam8<EMA>(a, a.start + v * 8, gred));
+      multimem_st_v4(mc + v * 16, zero1_adam8<EMA, DECOUPLED>(a, a.start + v * 8, gred));
     }
   } else {
     for (long long v = cell0 + threadIdx.x; v < cell1; v += Z1_THREADS) {
@@ -468,7 +474,7 @@ __global__ void __launch_bounds__(Z1_THREADS, Z1_MIN_BLOCKS) zero1_kernel(const 
       }
       const uint4 gred = make_uint4(pack_bf16x2(acc[0], acc[1]), pack_bf16x2(acc[2], acc[3]),
                                     pack_bf16x2(acc[4], acc[5]), pack_bf16x2(acc[6], acc[7]));
-      const uint4 w8 = zero1_adam8<EMA>(a, a.start + v * 8, gred);
+      const uint4 w8 = zero1_adam8<EMA, DECOUPLED>(a, a.start + v * 8, gred);
       for (int p = 0; p < world; ++p) {
         const int peer = (rank + p) % world;
         st_v4(reinterpret_cast<uint8_t*>(c.wire_ptrs[peer]) + boff, w8);
@@ -485,7 +491,7 @@ __global__ void __launch_bounds__(Z1_THREADS, Z1_MIN_BLOCKS) zero1_kernel(const 
 void zero1_step(const CommCtx& ctx, float* grad_f32, float* p, float* m, float* v, bf16* shadow,
                 long long start, long long n, float inv_world, int algo, int slot, uint32_t epoch, int max_ctas,
                 float lr, float beta1, float beta2, float eps, float weight_decay, int step, cudaStream_t s,
-                float* ema, double ema_decay, bool ema_first) {
+                float* ema, double ema_decay, bool ema_first, bool decoupled, float keep) {
   if (ctx.world > AR_MAX_WORLD) throw std::runtime_error("[b200] zero1_step: world too large");
   if (n % 8 || start % 8) throw std::runtime_error("[b200] zero1_step: range must be 8-element aligned");
   if (algo == AR_NVLS && !ctx.wire_mc) throw std::runtime_error("[b200] zero1_step: NVLS needs a multicast mapping");
@@ -493,7 +499,7 @@ void zero1_step(const CommCtx& ctx, float* grad_f32, float* p, float* m, float* 
   Zero1Args a;
   a.c = ctx; a.grad = grad_f32; a.p = p; a.m = m; a.v = v; a.shadow = shadow; a.start = start; a.n = n;
   a.inv_world = inv_world; a.slot = slot; a.epoch = epoch;
-  a.lr = lr; a.b1 = beta1; a.b2 = beta2; a.eps = eps; a.wd = weight_decay;
+  a.lr = lr; a.b1 = beta1; a.b2 = beta2; a.eps = eps; a.wd = weight_decay; a.keep = keep;
   a.bc1_inv = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(beta1), step)));
   a.bc2_inv_sqrt = static_cast<float>(1.0 / sqrt(1.0 - pow(static_cast<double>(beta2), step)));
   a.ema = ema; a.ema_first = ema_first ? 1 : 0;
@@ -501,20 +507,24 @@ void zero1_step(const CommCtx& ctx, float* grad_f32, float* p, float* m, float* 
   a.ema_a = ema ? static_cast<float>(1.0 - ema_decay) : 0.f;
   const int G = allreduce_grid(n, ctx.world, max_ctas, false);
   static const bool carve = [] {
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, true>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, true>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, false, false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, false, false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, true, false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, true, false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, false, true>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, false, true>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, true, true>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, true, true>));
     return true;
   }();
   (void)carve;
-  if (algo == AR_NVLS) {
-    if (ema) zero1_kernel<AR_NVLS, true><<<G, Z1_THREADS, 0, s>>>(a);
-    else zero1_kernel<AR_NVLS, false><<<G, Z1_THREADS, 0, s>>>(a);
-  } else {
-    if (ema) zero1_kernel<AR_TWOSHOT, true><<<G, Z1_THREADS, 0, s>>>(a);
-    else zero1_kernel<AR_TWOSHOT, false><<<G, Z1_THREADS, 0, s>>>(a);
-  }
+  using Kernel = void (*)(const Zero1Args);
+  static const Kernel kernels[2][2][2] = {
+      {{zero1_kernel<AR_TWOSHOT, false, false>, zero1_kernel<AR_TWOSHOT, false, true>},
+       {zero1_kernel<AR_TWOSHOT, true, false>, zero1_kernel<AR_TWOSHOT, true, true>}},
+      {{zero1_kernel<AR_NVLS, false, false>, zero1_kernel<AR_NVLS, false, true>},
+       {zero1_kernel<AR_NVLS, true, false>, zero1_kernel<AR_NVLS, true, true>}}};
+  kernels[algo == AR_NVLS][ema != nullptr][decoupled]<<<G, Z1_THREADS, 0, s>>>(a);
   count_launch();
   check_last("zero1_step");
 }

@@ -1,6 +1,7 @@
 // pybind11 surface of the native library: adapts torch tensors to the raw-pointer API of api.h.
 // Every op runs on torch's current CUDA stream of the tensor's device.
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -285,10 +286,40 @@ static void check_ema(const c10::optional<at::Tensor>& ema, int64_t n, double de
   TORCH_CHECK(ema->numel() == n, op, ": ema must have p's size");
   TORCH_CHECK(decay >= 0.0 && decay <= 1.0, op, ": ema_decay must lie in [0, 1], got ", decay);
 }
+// The weight-decay segments of one optimizer launch over n elements (WdSegments, api.h).  Without
+// `starts` the decay is `wd` everywhere; otherwise segment k covers [starts[k], starts[k + 1]) with decay
+// wds[k] (and `wd` is not used).  Starts must begin at 0, increase, be whole float4s and lie inside the
+// range; decays must be finite and >= 0.  decoupled (AdamW): the kernel takes keep = fp32(1 - lr * wd),
+// computed here in double as torch computes the Python scalar.
+static b200::WdSegments wd_segments(const char* op, int64_t n, double wd, const std::vector<int64_t>& starts,
+                                    const std::vector<double>& wds, bool decoupled, double lr) {
+  auto value = [&](double d) { return decoupled ? (float)(1.0 - lr * d) : (float)d; };
+  if (starts.empty()) {
+    TORCH_CHECK(wds.empty(), op, ": wd_starts and wd_values go together");
+    return b200::uniform_wd(value(wd));
+  }
+  TORCH_CHECK(starts.size() == wds.size(), op, ": wd_starts and wd_values must have the same length");
+  TORCH_CHECK((int)starts.size() <= b200::WD_MAX_SEGMENTS, op, ": at most ", b200::WD_MAX_SEGMENTS,
+              " weight-decay segments per launch, got ", starts.size());
+  TORCH_CHECK(starts[0] == 0, op, ": the first weight-decay segment must start at 0");
+  b200::WdSegments s{};
+  s.n = (int)starts.size();
+  for (size_t k = 0; k < starts.size(); ++k) {
+    TORCH_CHECK(k == 0 || starts[k] > starts[k - 1], op, ": weight-decay segment starts must increase");
+    TORCH_CHECK(starts[k] % 4 == 0, op, ": weight-decay segment starts must be multiples of 4, got ", starts[k]);
+    TORCH_CHECK(starts[k] < n, op, ": weight-decay segment start ", starts[k], " lies outside the range of ", n);
+    TORCH_CHECK(std::isfinite(wds[k]) && wds[k] >= 0.0, op, ": weight decays must be finite and >= 0, got ", wds[k]);
+    s.start4[k] = starts[k] / 4;
+    s.value[k] = value(wds[k]);
+  }
+  return s;
+}
+
 static void adam(at::Tensor p, at::Tensor m, at::Tensor v, c10::optional<at::Tensor> g32,
                  c10::optional<at::Tensor> g16, c10::optional<at::Tensor> shadow, double lr, double b1, double b2,
                  double eps, double wd, int64_t step, double grad_scale, c10::optional<at::Tensor> gzero,
-                 c10::optional<at::Tensor> ema, double ema_decay, bool ema_first) {
+                 c10::optional<at::Tensor> ema, double ema_decay, bool ema_first, bool decoupled,
+                 const std::vector<int64_t>& wd_starts, const std::vector<double>& wd_values) {
   c10::cuda::CUDAGuard g(p.device());
   const int64_t n = p.numel();
   for (auto* t : {&p, &m, &v}) check_vec(*t, at::kFloat, 16, "adam", "p, m and v");
@@ -301,15 +332,16 @@ static void adam(at::Tensor p, at::Tensor m, at::Tensor v, c10::optional<at::Ten
   for (const auto* t : {&g32, &g16, &shadow, &gzero})
     TORCH_CHECK(!t->has_value() || (*t)->numel() == n, "adam: every tensor has p's size");
   TORCH_CHECK(m.numel() == n && v.numel() == n, "adam: every tensor has p's size");
+  const b200::WdSegments segs = wd_segments("adam", n, wd, wd_starts, wd_values, decoupled, lr);
   b200::adam_fused(f32p(p), f32p(m), f32p(v), f32p_opt(g32), bfp_opt(g16),
                    shadow.has_value() ? bfp_mut(*shadow) : nullptr, p.numel(), (float)lr, (float)b1, (float)b2,
-                   (float)eps, (float)wd, (int)step, (float)grad_scale, false, f32p_opt(gzero), cur_stream(),
-                   f32p_opt(ema), ema_decay, ema_first);
+                   (float)eps, segs, (int)step, (float)grad_scale, false, f32p_opt(gzero), cur_stream(),
+                   f32p_opt(ema), ema_decay, ema_first, decoupled);
 }
 static void sgd(at::Tensor p, at::Tensor mom, c10::optional<at::Tensor> g32, c10::optional<at::Tensor> g16,
                 c10::optional<at::Tensor> shadow, double lr, double momentum, double wd, bool first,
                 double grad_scale, c10::optional<at::Tensor> gzero, c10::optional<at::Tensor> ema, double ema_decay,
-                bool ema_first) {
+                bool ema_first, const std::vector<int64_t>& wd_starts, const std::vector<double>& wd_values) {
   c10::cuda::CUDAGuard g(p.device());
   const int64_t n = p.numel();
   for (auto* t : {&p, &mom}) check_vec(*t, at::kFloat, 16, "sgd", "p and mom");
@@ -322,8 +354,9 @@ static void sgd(at::Tensor p, at::Tensor mom, c10::optional<at::Tensor> g32, c10
   for (const auto* t : {&g32, &g16, &shadow, &gzero})
     TORCH_CHECK(!t->has_value() || (*t)->numel() == n, "sgd: every tensor has p's size");
   TORCH_CHECK(mom.numel() == n, "sgd: every tensor has p's size");
+  const b200::WdSegments segs = wd_segments("sgd", n, wd, wd_starts, wd_values, false, lr);
   b200::sgd_fused(f32p(p), f32p(mom), f32p_opt(g32), bfp_opt(g16), shadow.has_value() ? bfp_mut(*shadow) : nullptr,
-                  p.numel(), (float)lr, (float)momentum, (float)wd, first, (float)grad_scale, f32p_opt(gzero),
+                  p.numel(), (float)lr, (float)momentum, segs, first, (float)grad_scale, f32p_opt(gzero),
                   cur_stream(), f32p_opt(ema), ema_decay, ema_first);
 }
 
@@ -692,7 +725,7 @@ static void zero1_step(const PyComm& comm, c10::optional<at::Tensor> grad, at::T
                        at::Tensor shadow, int64_t start, int64_t n, double inv_world, int64_t algo, int64_t slot,
                        int64_t epoch, int64_t max_ctas, double lr, double beta1, double beta2, double eps,
                        double weight_decay, int64_t step, c10::optional<at::Tensor> ema, double ema_decay,
-                       bool ema_first) {
+                       bool ema_first, bool decoupled) {
   TORCH_CHECK(p.scalar_type() == at::kFloat && m.scalar_type() == at::kFloat && v.scalar_type() == at::kFloat &&
                   shadow.scalar_type() == at::kBFloat16 && p.numel() == m.numel() && p.numel() == v.numel() &&
                   p.numel() == shadow.numel() && start + n <= p.numel(),
@@ -706,10 +739,13 @@ static void zero1_step(const PyComm& comm, c10::optional<at::Tensor> grad, at::T
     TORCH_CHECK(ema->numel() == p.numel(), "zero1_step: ema must have p's size");
     TORCH_CHECK(ema_decay >= 0.0 && ema_decay <= 1.0, "zero1_step: ema_decay must lie in [0, 1], got ", ema_decay);
   }
+  TORCH_CHECK(!decoupled || (std::isfinite(weight_decay) && weight_decay >= 0.0),
+              "zero1_step: the AdamW weight decay must be finite and >= 0, got ", weight_decay);
   b200::zero1_step(comm.c, grad.has_value() ? grad->data_ptr<float>() : nullptr, p.data_ptr<float>(),
                    m.data_ptr<float>(), v.data_ptr<float>(), bfp_mut(shadow), start, n, (float)inv_world, (int)algo,
                    (int)slot, (uint32_t)epoch, (int)max_ctas, (float)lr, (float)beta1, (float)beta2, (float)eps,
-                   (float)weight_decay, (int)step, cur_stream(), f32p_opt(ema), ema_decay, ema_first);
+                   (float)weight_decay, (int)step, cur_stream(), f32p_opt(ema), ema_decay, ema_first, decoupled,
+                   (float)(1.0 - lr * weight_decay));
 }
 static int64_t allreduce_grid(int64_t n, int64_t world, int64_t max_ctas, bool wire_fp32) {
   return b200::allreduce_grid(n, (int)world, (int)max_ctas, wire_fp32);
@@ -795,10 +831,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("adam", &adam, py::arg("p"), py::arg("m"), py::arg("v"), py::arg("g32"), py::arg("g16"), py::arg("shadow"),
         py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("step"),
         py::arg("grad_scale"), py::arg("gzero"), py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0,
-        py::arg("ema_first") = false);
+        py::arg("ema_first") = false, py::arg("decoupled") = false, py::arg("wd_starts") = std::vector<int64_t>(),
+        py::arg("wd_values") = std::vector<double>());
   m.def("sgd", &sgd, py::arg("p"), py::arg("mom"), py::arg("g32"), py::arg("g16"), py::arg("shadow"), py::arg("lr"),
         py::arg("momentum"), py::arg("wd"), py::arg("first"), py::arg("grad_scale"), py::arg("gzero"),
-        py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0, py::arg("ema_first") = false);
+        py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0, py::arg("ema_first") = false,
+        py::arg("wd_starts") = std::vector<int64_t>(), py::arg("wd_values") = std::vector<double>());
   m.def("augment", &augment);
   m.def("augment_mixed", &augment_mixed);
   m.def("augment_ragged", &augment_ragged);
@@ -827,7 +865,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("shadow"), py::arg("start"), py::arg("n"), py::arg("inv_world"), py::arg("algo"), py::arg("slot"),
         py::arg("epoch"), py::arg("max_ctas"), py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"),
         py::arg("weight_decay"), py::arg("step"), py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0,
-        py::arg("ema_first") = false);
+        py::arg("ema_first") = false, py::arg("decoupled") = false);
+  m.def("wd_max_segments", [] { return b200::WD_MAX_SEGMENTS; });
   m.def("allreduce_grid", &allreduce_grid);
   m.def("broadcast", &broadcast);
   m.def("barrier", &barrier);

@@ -10,14 +10,28 @@
 
 namespace b200 {
 
-// lr_bc1 = lr / (1 - beta1^step), bc2_inv_sqrt = 1 / sqrt(1 - beta2^step), both rounded to fp32 once
-__device__ __forceinline__ void adam_update(float g, float gscale, float& p, float& m, float& v, float lr_bc1,
-                                            float b1, float b2, float eps, float wd, float bc2_inv_sqrt) {
-  const float gk = __fmaf_rn(g, gscale, __fmul_rn(wd, p));
+// The moments and the step of one Adam update from the (already decayed, scaled) gradient gk.
+__device__ __forceinline__ void adam_moments_step(float gk, float& p, float& m, float& v, float lr_bc1, float b1,
+                                                  float b2, float eps, float bc2_inv_sqrt) {
   m = __fmaf_rn(b1, m, __fmul_rn(1.f - b1, gk));
   v = __fmaf_rn(b2, v, __fmul_rn(__fmul_rn(1.f - b2, gk), gk));
   const float denom = __fmaf_rn(__fsqrt_rn(v), bc2_inv_sqrt, eps);
   p = __fsub_rn(p, __fdiv_rn(__fmul_rn(lr_bc1, m), denom));
+}
+
+// lr_bc1 = lr / (1 - beta1^step), bc2_inv_sqrt = 1 / sqrt(1 - beta2^step), both rounded to fp32 once
+__device__ __forceinline__ void adam_update(float g, float gscale, float& p, float& m, float& v, float lr_bc1,
+                                            float b1, float b2, float eps, float wd, float bc2_inv_sqrt) {
+  adam_moments_step(__fmaf_rn(g, gscale, __fmul_rn(wd, p)), p, m, v, lr_bc1, b1, b2, eps, bc2_inv_sqrt);
+}
+
+// One AdamW step (torch.optim.AdamW: decoupled weight decay).  keep = fp32(1 - lr * wd), taken in double
+// on the host as torch takes the Python scalar of `p.mul_(1 - lr * weight_decay)`; then Adam on the
+// scaled gradient alone, with no L2 term.
+__device__ __forceinline__ void adamw_update(float g, float gscale, float& p, float& m, float& v, float lr_bc1,
+                                             float b1, float b2, float eps, float keep, float bc2_inv_sqrt) {
+  p = __fmul_rn(p, keep);
+  adam_moments_step(__fmul_rn(g, gscale), p, m, v, lr_bc1, b1, b2, eps, bc2_inv_sqrt);
 }
 
 // One update of the exponential moving average of a weight (torch.optim.swa_utils.AveragedModel with

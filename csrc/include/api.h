@@ -116,16 +116,35 @@ void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long l
                    float* loss_out, int B, int C, int K, const float* class_weights, bool accumulate,
                    cudaStream_t s, const SoftTargets* soft = nullptr);
 
+// Weight decay of one optimizer launch, per segment of its range: segment k covers the float4s
+// [start4[k], start4[k + 1]) (the last one runs to the end of the range) and takes value[k].  start4[0]
+// = 0 and the starts increase; a uniform decay is one segment.  value is the L2 decay wd (Adam, SGD) or,
+// for AdamW, keep = fp32(1 - lr * wd) with the product taken in double.  Passed by value
+// (__grid_constant__), so a bucket whose tensors decay differently (biases) still takes one launch.
+constexpr int WD_MAX_SEGMENTS = 16;
+struct WdSegments {
+  int n;
+  long long start4[WD_MAX_SEGMENTS];
+  float value[WD_MAX_SEGMENTS];
+};
+inline WdSegments uniform_wd(float value) {
+  WdSegments s{};
+  s.n = 1;
+  s.value[0] = value;
+  return s;
+}
+
 // Fused optimizers over flat arenas.  grad is fp32 (local) or bf16 (the reduced wire buffer).
 // With `ema`, the same pass also updates the weights' exponential moving average from the new p:
 // ema = decay * ema + (1 - decay) * p (fp32 rounding of each product and of the sum), or ema = p when
-// `ema_first` (AveragedModel's first update).
+// `ema_first` (AveragedModel's first update).  `decoupled`: AdamW (adamw_update in adam.cuh), `wd`
+// then holds keep factors.
 void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16, bf16* shadow,
-                long long n, float lr, float beta1, float beta2, float eps, float weight_decay,
+                long long n, float lr, float beta1, float beta2, float eps, const WdSegments& wd,
                 int step, float grad_scale, bool zero_grad, float* g32_to_zero, cudaStream_t s,
-                float* ema = nullptr, double ema_decay = 0.0, bool ema_first = false);
+                float* ema = nullptr, double ema_decay = 0.0, bool ema_first = false, bool decoupled = false);
 void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* shadow, long long n,
-               float lr, float momentum, float weight_decay, bool first_step, float grad_scale,
+               float lr, float momentum, const WdSegments& wd, bool first_step, float grad_scale,
                float* g32_to_zero, cudaStream_t s, float* ema = nullptr, double ema_decay = 0.0,
                bool ema_first = false);
 
@@ -186,11 +205,13 @@ void allreduce_fused(const CommCtx& ctx, const float* grad_f32, float* grad_out_
 int allreduce_grid(long long n, int world, int max_ctas, bool wire_fp32);
 // EXPERIMENTAL: ZeRO-1 step of arena range [start, start+n) in one kernel -- reduce-scatter, Adam on
 // the cells this rank owns, all-gather of the new bf16 weights into every rank's shadow (allreduce.cu).
-// With `ema`, the owner also updates the moving average of its cells as adam_fused does.
+// With `ema`, the owner also updates the moving average of its cells as adam_fused does.  `decoupled`:
+// AdamW with keep = fp32(1 - lr * wd) (weight_decay is then not used).
 void zero1_step(const CommCtx& ctx, float* grad_f32, float* p, float* m, float* v, bf16* shadow,
                 long long start, long long n, float inv_world, int algo, int slot, uint32_t epoch, int max_ctas,
                 float lr, float beta1, float beta2, float eps, float weight_decay, int step, cudaStream_t s,
-                float* ema = nullptr, double ema_decay = 0.0, bool ema_first = false);
+                float* ema = nullptr, double ema_decay = 0.0, bool ema_first = false, bool decoupled = false,
+                float keep = 1.f);
 // Parameter broadcast rank `root` -> all through the wire buffer (K-BCAST).
 void broadcast_fused(const CommCtx& ctx, float* data_f32, long long n, int root, int slot,
                      uint32_t epoch, cudaStream_t s);

@@ -364,17 +364,22 @@ __device__ __forceinline__ void ema_store4(float* __restrict__ ema, long long i,
 // CTAs per SM: at every conv-kernel boundary the high-priority stream filled the SMs with optimizer
 // CTAs and the next conv kernel's persistent CTAs started late; bench/step_timeline.py.)
 // EMA: also update the weights' moving average `ema` from the new p while it is in registers (one
-// more fp32 stream, 8 B per parameter); the EMA = false instantiation is the plain optimizer.  The
-// EMA arguments come last so that the plain instantiation's parameter offsets stay where they were.
-template <bool EMA>
+// more fp32 stream, 8 B per parameter); the EMA = false instantiation is the plain optimizer.
+// DECOUPLED: AdamW (adamw_update), the segment values being keep factors instead of L2 decays.
+// `wd` (WdSegments, api.h) sits in the parameter bank: the thread walks it forward as its grid-stride
+// loop moves through the range, one compare per iteration for a uniform decay.
+template <bool EMA, bool DECOUPLED>
 __global__ void __launch_bounds__(256, 6) adam_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
                             const float* __restrict__ g32, const bf16* __restrict__ g16,
                             bf16* __restrict__ shadow, long long n4, float lr, float b1, float b2,
-                            float eps, float wd, float bc1_inv, float bc2_inv_sqrt, float gscale,
+                            float eps, float bc1_inv, float bc2_inv_sqrt, float gscale,
                             float* __restrict__ gzero, float* __restrict__ ema, float ema_d, float ema_a,
-                            int ema_first) {
+                            int ema_first, const __grid_constant__ WdSegments wd) {
+  int seg = 0;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    while (seg + 1 < wd.n && i >= wd.start4[seg + 1]) ++seg;
+    const float w = wd.value[seg];
     // Every stream here is touched exactly once per step: cache-streaming (evict-first) loads and
     // stores, so that ~4 GB of optimizer traffic does not flush the conv kernels' L2-resident operand
     // tiles while it runs under backward (bench/step_timeline.py: +30 % on the 512-channel layers).
@@ -394,7 +399,12 @@ __global__ void __launch_bounds__(256, 6) adam_kernel(float* __restrict__ p, flo
     float mm[4] = {mv.x, mv.y, mv.z, mv.w};
     float vs[4] = {vv.x, vv.y, vv.z, vv.w};
 #pragma unroll
-    for (int k = 0; k < 4; ++k) adam_update(g[k], gscale, pp[k], mm[k], vs[k], lr * bc1_inv, b1, b2, eps, wd, bc2_inv_sqrt);
+    for (int k = 0; k < 4; ++k) {
+      if constexpr (DECOUPLED)
+        adamw_update(g[k], gscale, pp[k], mm[k], vs[k], lr * bc1_inv, b1, b2, eps, w, bc2_inv_sqrt);
+      else
+        adam_update(g[k], gscale, pp[k], mm[k], vs[k], lr * bc1_inv, b1, b2, eps, w, bc2_inv_sqrt);
+    }
     __stcs(reinterpret_cast<float4*>(p) + i, make_float4(pp[0], pp[1], pp[2], pp[3]));
     __stcs(reinterpret_cast<float4*>(m) + i, make_float4(mm[0], mm[1], mm[2], mm[3]));
     __stcs(reinterpret_cast<float4*>(v) + i, make_float4(vs[0], vs[1], vs[2], vs[3]));
@@ -405,11 +415,22 @@ __global__ void __launch_bounds__(256, 6) adam_kernel(float* __restrict__ p, flo
   }
 }
 
+template <bool EMA, bool DECOUPLED>
+static void launch_adam(int blocks, cudaStream_t s, float* p, float* m, float* v, const float* g32, const bf16* g16,
+                        bf16* shadow, long long n4, float lr, float beta1, float beta2, float eps, float bc1_inv,
+                        float bc2_inv_sqrt, float grad_scale, float* gzero, float* ema, float ema_d, float ema_a,
+                        int ema_first, const WdSegments& wd) {
+  adam_kernel<EMA, DECOUPLED><<<blocks, 256, 0, s>>>(p, m, v, g32, g16, shadow, n4, lr, beta1, beta2, eps, bc1_inv,
+                                                     bc2_inv_sqrt, grad_scale, gzero, ema, ema_d, ema_a, ema_first, wd);
+}
+
 void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16, bf16* shadow,
-                long long n, float lr, float beta1, float beta2, float eps, float weight_decay,
+                long long n, float lr, float beta1, float beta2, float eps, const WdSegments& wd,
                 int step, float grad_scale, bool, float* g32_to_zero, cudaStream_t s, float* ema,
-                double ema_decay, bool ema_first) {
+                double ema_decay, bool ema_first, bool decoupled) {
   if (n % 4) throw std::runtime_error("[b200] adam_fused: n must be a multiple of 4");
+  if (wd.n < 1 || wd.n > WD_MAX_SEGMENTS || wd.start4[0] != 0)
+    throw std::runtime_error("[b200] adam_fused: bad weight-decay segment table");
   const double bc1 = 1.0 - pow(static_cast<double>(beta1), step);
   const double bc2 = 1.0 - pow(static_cast<double>(beta2), step);
   const long long n4 = n / 4;
@@ -420,36 +441,41 @@ void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16,
     return v >= 1 && v <= 16 ? v : 4;
   }();
   static const bool carve = [] {
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<true>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<false, false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<true, false>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<false, true>));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<true, true>));
     return true;
   }();
   (void)carve;
   const long long cap = static_cast<long long>(sm_count()) * per_sm;
   const int blocks = static_cast<int>(n4 / 256 + 1 < cap ? n4 / 256 + 1 : cap);
-  if (ema)
-    adam_kernel<true><<<blocks, 256, 0, s>>>(p, m, v, g32, g16, shadow, n4, lr, beta1, beta2, eps, weight_decay,
-                                             static_cast<float>(1.0 / bc1), static_cast<float>(1.0 / sqrt(bc2)),
-                                             grad_scale, g32_to_zero, ema, static_cast<float>(ema_decay),
-                                             static_cast<float>(1.0 - ema_decay), ema_first ? 1 : 0);
-  else
-    adam_kernel<false><<<blocks, 256, 0, s>>>(p, m, v, g32, g16, shadow, n4, lr, beta1, beta2, eps, weight_decay,
-                                              static_cast<float>(1.0 / bc1), static_cast<float>(1.0 / sqrt(bc2)),
-                                              grad_scale, g32_to_zero, nullptr, 0.f, 0.f, 0);
+  const float bc1_inv = static_cast<float>(1.0 / bc1), bc2_inv_sqrt = static_cast<float>(1.0 / sqrt(bc2));
+  const float ema_d = ema ? static_cast<float>(ema_decay) : 0.f;
+  const float ema_a = ema ? static_cast<float>(1.0 - ema_decay) : 0.f;
+  const int first = ema && ema_first ? 1 : 0;
+  auto* launch = ema ? (decoupled ? launch_adam<true, true> : launch_adam<true, false>)
+                     : (decoupled ? launch_adam<false, true> : launch_adam<false, false>);
+  launch(blocks, s, p, m, v, g32, g16, shadow, n4, lr, beta1, beta2, eps, bc1_inv, bc2_inv_sqrt, grad_scale,
+         g32_to_zero, ema, ema_d, ema_a, first, wd);
   count_launch();
   check_last("adam_fused");
 }
 
 // --------------------------------------------------------------------------------------- SGD
 // torch.optim.SGD(momentum) semantics: buf = g (first step) | momentum*buf + g ; p -= lr*buf.
-// EMA: as adam_kernel.
+// EMA and the weight-decay segments `wd`: as adam_kernel.  SGD has no decoupled form in torch: wd is L2.
 template <bool EMA>
 __global__ void __launch_bounds__(256, 6) sgd_kernel(float* __restrict__ p, float* __restrict__ mom, const float* __restrict__ g32,
                            const bf16* __restrict__ g16, bf16* __restrict__ shadow, long long n4, float lr,
-                           float momentum, float wd, int first, float gscale, float* __restrict__ gzero,
-                           float* __restrict__ ema, float ema_d, float ema_a, int ema_first) {
+                           float momentum, int first, float gscale, float* __restrict__ gzero,
+                           float* __restrict__ ema, float ema_d, float ema_a, int ema_first,
+                           const __grid_constant__ WdSegments wd) {
+  int seg = 0;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    while (seg + 1 < wd.n && i >= wd.start4[seg + 1]) ++seg;
+    const float w = wd.value[seg];
     float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i);       // streaming, see adam_kernel
     float4 bv = __ldcs(reinterpret_cast<const float4*>(mom) + i);
     float g[4];
@@ -465,7 +491,7 @@ __global__ void __launch_bounds__(256, 6) sgd_kernel(float* __restrict__ p, floa
     float bb[4] = {bv.x, bv.y, bv.z, bv.w};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float gk = g[k] * gscale + wd * pp[k];
+      const float gk = g[k] * gscale + w * pp[k];
       bb[k] = first ? gk : momentum * bb[k] + gk;
       pp[k] -= lr * bb[k];
     }
@@ -479,9 +505,11 @@ __global__ void __launch_bounds__(256, 6) sgd_kernel(float* __restrict__ p, floa
 }
 
 void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* shadow, long long n,
-               float lr, float momentum, float weight_decay, bool first_step, float grad_scale,
+               float lr, float momentum, const WdSegments& wd, bool first_step, float grad_scale,
                float* g32_to_zero, cudaStream_t s, float* ema, double ema_decay, bool ema_first) {
   if (n % 4) throw std::runtime_error("[b200] sgd_fused: n must be a multiple of 4");
+  if (wd.n < 1 || wd.n > WD_MAX_SEGMENTS || wd.start4[0] != 0)
+    throw std::runtime_error("[b200] sgd_fused: bad weight-decay segment table");
   const long long n4 = n / 4;
   static const bool carve = [] {
     prefer_max_shared_carveout(reinterpret_cast<const void*>(sgd_kernel<false>));
@@ -492,13 +520,12 @@ void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* sh
   const long long cap = static_cast<long long>(sm_count()) * 4;
   const int blocks = static_cast<int>(n4 / 256 + 1 < cap ? n4 / 256 + 1 : cap);
   if (ema)
-    sgd_kernel<true><<<blocks, 256, 0, s>>>(p, mom, g32, g16, shadow, n4, lr, momentum, weight_decay,
-                                            first_step ? 1 : 0, grad_scale, g32_to_zero, ema,
-                                            static_cast<float>(ema_decay), static_cast<float>(1.0 - ema_decay),
-                                            ema_first ? 1 : 0);
+    sgd_kernel<true><<<blocks, 256, 0, s>>>(p, mom, g32, g16, shadow, n4, lr, momentum, first_step ? 1 : 0,
+                                            grad_scale, g32_to_zero, ema, static_cast<float>(ema_decay),
+                                            static_cast<float>(1.0 - ema_decay), ema_first ? 1 : 0, wd);
   else
-    sgd_kernel<false><<<blocks, 256, 0, s>>>(p, mom, g32, g16, shadow, n4, lr, momentum, weight_decay,
-                                             first_step ? 1 : 0, grad_scale, g32_to_zero, nullptr, 0.f, 0.f, 0);
+    sgd_kernel<false><<<blocks, 256, 0, s>>>(p, mom, g32, g16, shadow, n4, lr, momentum, first_step ? 1 : 0,
+                                             grad_scale, g32_to_zero, nullptr, 0.f, 0.f, 0, wd);
   count_launch();
   check_last("sgd_fused");
 }

@@ -72,11 +72,29 @@ def build_parser() -> argparse.ArgumentParser:
                      help="bf16: the sm_90a engine (bf16 activations / weights / wire, fp32 master weights, moments and "
                           "accumulators).  fp32: the reference's arithmetic on the torch-op engine (the native kernels "
                           "have no tf32 path yet)")
-    ext.add_argument("--optimizer", default="adam", choices=["adam", "sgd"])
+    ext.add_argument("--optimizer", default="adam", choices=["adam", "adamw", "sgd"],
+                     help="adam / sgd: L2 weight decay (torch.optim.Adam / SGD); adamw: decoupled weight decay "
+                          "(torch.optim.AdamW)")
     ext.add_argument("--momentum", type=float, default=TRAIN.momentum)
+    ext.add_argument("--weight-decay", type=float, default=0.0,
+                     help="weight decay of every parameter, >= 0 (default 0 = none, as the reference)")
+    ext.add_argument("--bias-weight-decay", type=float, default=None,
+                     help="weight decay of the biases, >= 0 (torchvision's --bias-weight-decay; default: "
+                          "--weight-decay)")
+    ext.add_argument("--lr-scheduler", default="step", choices=["step", "cosine"],
+                     help="step: StepLR(--lr-step, --lr-gamma); cosine: CosineAnnealingLR over the epochs after "
+                          "the warmup, down to --lr-min.  Stepped once per epoch")
     ext.add_argument("--lr-step", type=int, default=0,
                      help="StepLR period in epochs (0 = constant lr, as the reference)")
     ext.add_argument("--lr-gamma", type=float, default=TRAIN.decay_gamma)
+    ext.add_argument("--lr-min", type=float, default=0.0, help="the cosine schedule's final rate (eta_min)")
+    ext.add_argument("--lr-warmup-epochs", type=int, default=0,
+                     help="epochs of warmup before the main schedule (torchvision's SequentialLR; 0 = none)")
+    ext.add_argument("--lr-warmup-method", default="constant", choices=["linear", "constant"],
+                     help="linear: LinearLR from --lr-warmup-decay x lr up to lr; constant: ConstantLR at "
+                          "--lr-warmup-decay x lr")
+    ext.add_argument("--lr-warmup-decay", type=float, default=0.01,
+                     help="the warmup's (starting) factor of the rate, in (0, 1]")
     ext.add_argument("--backend", default=None, choices=[None, "gloo", "nccl"],
                      help="rendezvous backend (default: nccl on GPU, gloo on CPU)")
     ext.add_argument("--allreduce", default="auto",
@@ -154,6 +172,16 @@ def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
         build_parser().error("--model-ema-steps must be >= 1")
     if not 0.0 <= args.model_ema_decay < 1.0:
         build_parser().error("--model-ema-decay must lie in [0, 1)")
+    if not args.weight_decay >= 0.0 or (args.bias_weight_decay is not None and not args.bias_weight_decay >= 0.0):
+        build_parser().error("--weight-decay and --bias-weight-decay must be >= 0")
+    if args.lr_warmup_epochs < 0:
+        build_parser().error("--lr-warmup-epochs must be >= 0")
+    if args.lr_scheduler == "cosine" and args.lr_warmup_epochs >= args.epochs:
+        build_parser().error("--lr-scheduler cosine needs --lr-warmup-epochs < --epochs")
+    if not 0.0 < args.lr_warmup_decay <= 1.0:
+        build_parser().error("--lr-warmup-decay must lie in (0, 1]")
+    if not args.lr_min >= 0.0:
+        build_parser().error("--lr-min must be >= 0")
     print(args)
     if args.socket_ifname:
         os.environ["GLOO_SOCKET_IFNAME"] = args.socket_ifname

@@ -89,7 +89,8 @@ class NativeEngine:
                  init_state: Optional[Dict[str, torch.Tensor]] = None, unpack_fp32: bool = False,
                  distributed: bool = True, zero1="auto", conv_bucket_mb: float = 9.5,
                  tail_bucket_kb: float = 2400.0, same_dropout_all_ranks: bool = False,
-                 label_smoothing: float = 0.0, ema_decay: Optional[float] = None) -> None:
+                 label_smoothing: float = 0.0, ema_decay: Optional[float] = None,
+                 bias_weight_decay: Optional[float] = None) -> None:
         ops.require()
         if compute_dtype != "bf16":
             raise NotImplementedError("the native engine computes in bf16 with fp32 master weights; "
@@ -100,7 +101,14 @@ class NativeEngine:
         if spec.convs[0].cout % 64 or spec.convs[0].cin != 3:
             raise ValueError("first conv must be 3 -> multiple of 64 channels")
         self.spec, self.device, self.B = spec, torch.device(device), int(batch)
+        if optimizer not in ("adam", "adamw", "sgd"):
+            raise ValueError("optimizer must be adam, adamw or sgd (got %r)" % optimizer)
+        for what, wd in (("weight_decay", weight_decay), ("bias_weight_decay", bias_weight_decay)):
+            if wd is not None and not wd >= 0.0:
+                raise ValueError("%s must be >= 0 (got %r)" % (what, wd))
         self.lr, self.opt_name, self.momentum, self.weight_decay = lr, optimizer, momentum, weight_decay
+        # torchvision's --bias-weight-decay: the biases' own decay (None: the biases take weight_decay)
+        self.bias_weight_decay = bias_weight_decay
         self.beta1, self.beta2, self.eps = TRAIN.adam_beta1, TRAIN.adam_beta2, TRAIN.adam_eps
         self.seed, self.HW = int(seed), int(input_hw)
         if not 0.0 <= label_smoothing < 1.0:
@@ -143,7 +151,10 @@ class NativeEngine:
         self.p32 = torch.zeros(n, dtype=F32, device=dev)
         self.g32 = torch.zeros(n, dtype=F32, device=dev)
         self.m32 = torch.zeros(n, dtype=F32, device=dev)
-        self.v32 = torch.zeros(n, dtype=F32, device=dev) if optimizer == "adam" else None
+        self.v32 = torch.zeros(n, dtype=F32, device=dev) if optimizer in ("adam", "adamw") else None
+        # each bucket's weight-decay segments [(start within the bucket, decay), ...], one entry when the
+        # decay is uniform: biases and weights share buckets, and one launch per bucket stays one launch
+        self._wd_segments = {bk.start: self.decay_segments(bk) for bk in self.plan.buckets}
         self.w16 = torch.zeros(n, dtype=BF16, device=dev)
 
         if init_state is None:
@@ -210,12 +221,12 @@ class NativeEngine:
         # GPU this was first tuned on; at 2 ranks every rank still owns half of the optimizer
         # state and the fused kernel's thin CTAs are slower than all-reduce + replicated Adam).
         z1_ok = self.arena is not None and self.arena.wire_dtype == BF16 and self.cross_group is None \
-            and optimizer == "adam"
+            and optimizer in ("adam", "adamw")
         if zero1 == "auto":
             zero1 = z1_ok and self.world >= 4
         self.zero1 = bool(zero1) and z1_ok
         if zero1 and not self.zero1 and self.world > 1:
-            raise ValueError("--zero1 needs Adam, the bf16 wire and all ranks in one NVLink domain")
+            raise ValueError("--zero1 needs Adam or AdamW, the bf16 wire and all ranks in one NVLink domain")
         self._zero1_buckets: set = set()
         # the fused ZeRO-1 kernel keeps less in flight per CTA (128 threads, one switch reduction +
         # 96 bytes of optimizer state each): more, equally thin, CTAs
@@ -309,7 +320,7 @@ class NativeEngine:
 
     def export_optimizer_state(self) -> dict:
         st = {"name": self.opt_name, "step": self.step_count, "micro_step": self.micro_count, "lr": self.lr}
-        if self.opt_name == "adam":
+        if self.opt_name in ("adam", "adamw"):
             st["exp_avg"] = {n: L.to_torch(self.spec, n, self._view(self.m32, n)).cpu() for n in self.spec.param_names}
             st["exp_avg_sq"] = {n: L.to_torch(self.spec, n, self._view(self.v32, n)).cpu() for n in self.spec.param_names}
         else:
@@ -330,6 +341,37 @@ class NativeEngine:
 
     def set_lr(self, lr: float) -> None:
         self.lr = lr
+
+    def decay_of(self, name: str) -> float:
+        """The weight decay of parameter ``name``: bias_weight_decay for ``*.bias`` when it is set."""
+        if name.endswith(".bias") and self.bias_weight_decay is not None:
+            return float(self.bias_weight_decay)
+        return float(self.weight_decay)
+
+    def decay_segments(self, bk) -> list:
+        """[(start within bucket ``bk``, weight decay), ...] with neighbours of equal decay merged.  Every
+        tensor starts on an ``align``-element boundary of the arena, so the starts are whole float4s; the
+        padding behind a tensor takes its decay (its weights and gradients stay zero)."""
+        segs = []
+        for name in sorted(bk.tensors, key=lambda t: self.plan.offsets[t]):
+            start, wd = max(self.plan.offsets[name] - bk.start, 0), self.decay_of(name)
+            if not segs or segs[-1][1] != wd:
+                segs.append((start, wd))
+        segs[0] = (0, segs[0][1])
+        return segs
+
+    def _update_ranges(self, s: int, e: int) -> list:
+        """The optimizer launches of bucket [s, e): [(start, end, segment table relative to start)].  One
+        launch unless the bucket has more decay segments than a launch takes (the test-sized models pack
+        all their layers into a few buckets); VGG-F's buckets have at most ten."""
+        segs, cap = self._wd_segments[s], ops.wd_max_segments()
+        out = []
+        for k in range(0, len(segs), cap):
+            part = segs[k:k + cap]
+            lo = part[0][0]
+            hi = segs[k + cap][0] if k + cap < len(segs) else e - s
+            out.append((s + lo, s + hi, [(a - lo, w) for a, w in part]))
+        return out
 
     def _broadcast_params(self) -> None:
         """DDP's constructor sync (distributedVggf.py:225): everybody adopts rank 0's weights."""
@@ -704,17 +746,29 @@ class NativeEngine:
 
     def _apply_update(self, s: int, e: int, g16: Optional[torch.Tensor], zero: bool = True,
                       grad_scale: float = 1.0) -> None:
+        ranges = self._update_ranges(s, e)
+        if len(ranges) == 1:
+            self._launch_update(s, e, g16, zero, grad_scale, ranges[0][2])
+            return
+        for a, b, segs in ranges:
+            self._launch_update(a, b, None if g16 is None else g16[a - s:b - s], zero, grad_scale, segs)
+
+    def _launch_update(self, s: int, e: int, g16: Optional[torch.Tensor], zero: bool, grad_scale: float,
+                       segs: list) -> None:
         g32 = None if g16 is not None else self.g32[s:e]
         z = self.g32[s:e] if zero else None      # ranges written with plain stores need no re-zeroing
-        if self.opt_name == "adam":
+        # a uniform decay goes as the scalar: the launch is the one made before segment tables existed
+        wd_kw = dict(weight_decay=segs[0][1]) if len(segs) == 1 else dict(weight_decay=segs[0][1], wd_segments=segs)
+        if self.opt_name in ("adam", "adamw"):
+            if self.opt_name == "adamw":
+                wd_kw["decoupled"] = True
             ops.adam_step(self.p32[s:e], self.m32[s:e], self.v32[s:e], g32=g32, g16=g16, shadow=self.w16[s:e],
                           lr=self.lr, beta1=self.beta1, beta2=self.beta2, eps=self.eps,
-                          weight_decay=self.weight_decay, step=self.step_count, grad_scale=grad_scale, zero=z,
-                          **self._ema_kw(s, e))
+                          step=self.step_count, grad_scale=grad_scale, zero=z, **wd_kw, **self._ema_kw(s, e))
         else:
             ops.sgd_step(self.p32[s:e], self.m32[s:e], g32=g32, g16=g16, shadow=self.w16[s:e], lr=self.lr,
-                         momentum=self.momentum, weight_decay=self.weight_decay,
-                         first=(self.step_count == 1), grad_scale=grad_scale, zero=z, **self._ema_kw(s, e))
+                         momentum=self.momentum, first=(self.step_count == 1), grad_scale=grad_scale, zero=z,
+                         **wd_kw, **self._ema_kw(s, e))
 
     def _reduce_and_update(self, bi: int) -> None:
         bk = self.plan.buckets[bi]
@@ -762,8 +816,9 @@ class NativeEngine:
                 self.arena.zero1_step(None if prepacked else self.g32, self.p32, self.m32, self.v32, self.w16,
                                       s, e - s, algo=algo, slot=bi % self.arena.slots, max_ctas=self.zero1_ctas,
                                       inv_world=1.0 / (self.world * k), lr=self.lr, beta1=self.beta1,
-                                      beta2=self.beta2, eps=self.eps, weight_decay=self.weight_decay,
-                                      step=self.step_count, **self._ema_kw(s, e))
+                                      beta2=self.beta2, eps=self.eps, weight_decay=self._wd_segments[s][0][1],
+                                      step=self.step_count, decoupled=self.opt_name == "adamw",
+                                      **self._ema_kw(s, e))
                 self._zero1_buckets.add(bi)
                 if zev0 is not None:             # reduce-scatter + optimizer + all-gather: same wire bytes
                     zev1 = torch.cuda.Event(enable_timing=True)

@@ -174,21 +174,42 @@ def _ema_args(ema, ema_decay: float, ema_first: bool) -> tuple:
     return () if ema is None else (ema, float(ema_decay), bool(ema_first))
 
 
+def wd_max_segments() -> int:
+    """Weight-decay segments one optimizer launch can take (``wd_segments``)."""
+    return int(require().wd_max_segments())
+
+
+def _wd_args(wd_segments) -> tuple:
+    """(starts, decays) of a segment table [(start, weight decay), ...], ordered as given."""
+    return [int(s) for s, _ in wd_segments], [float(w) for _, w in wd_segments]
+
+
 def adam_step(p, m, v, *, g32=None, g16=None, shadow=None, lr, beta1=0.9, beta2=0.999, eps=1e-8,
               weight_decay=0.0, step: int, grad_scale: float = 1.0, zero=None, ema=None, ema_decay: float = 0.0,
-              ema_first: bool = False):
+              ema_first: bool = False, decoupled: bool = False, wd_segments=None):
     """Fused Adam over a flat range.  ``ema`` (fp32, p's size): the same pass also updates the weights'
-    moving average, ema = decay * ema + (1 - decay) * p_new, or ema = p_new with ``ema_first``."""
-    require().adam(p, m, v, g32, g16, shadow, lr, beta1, beta2, eps, weight_decay, step, grad_scale, zero,
-                   *_ema_args(ema, ema_decay, ema_first))
+    moving average, ema = decay * ema + (1 - decay) * p_new, or ema = p_new with ``ema_first``.
+    ``decoupled``: AdamW (torch.optim.AdamW: p *= 1 - lr * wd, then Adam without the L2 term).
+    ``wd_segments`` [(start, wd), ...] (starts in elements of the range, the first 0, increasing,
+    multiples of 4): a per-segment weight decay in the same launch, in place of ``weight_decay``."""
+    args = (p, m, v, g32, g16, shadow, lr, beta1, beta2, eps, weight_decay, step, grad_scale, zero)
+    if not decoupled and wd_segments is None:
+        require().adam(*args, *_ema_args(ema, ema_decay, ema_first))
+        return
+    require().adam(*args, ema, float(ema_decay), bool(ema_first), bool(decoupled),
+                   *_wd_args(wd_segments or ()))
 
 
 def sgd_step(p, mom, *, g32=None, g16=None, shadow=None, lr, momentum=0.9, weight_decay=0.0,
              first: bool, grad_scale: float = 1.0, zero=None, ema=None, ema_decay: float = 0.0,
-             ema_first: bool = False):
-    """Fused SGD (momentum) over a flat range; ``ema`` as for ``adam_step``."""
-    require().sgd(p, mom, g32, g16, shadow, lr, momentum, weight_decay, first, grad_scale, zero,
-                  *_ema_args(ema, ema_decay, ema_first))
+             ema_first: bool = False, wd_segments=None):
+    """Fused SGD (momentum, L2 weight decay) over a flat range; ``ema`` and ``wd_segments`` as for
+    ``adam_step``."""
+    args = (p, mom, g32, g16, shadow, lr, momentum, weight_decay, first, grad_scale, zero)
+    if wd_segments is None:
+        require().sgd(*args, *_ema_args(ema, ema_decay, ema_first))
+        return
+    require().sgd(*args, ema, float(ema_decay), bool(ema_first), *_wd_args(wd_segments))
 
 
 _MIX_KIND = {"mixup": 1, "cutmix": 2}

@@ -508,11 +508,19 @@ def adam_step64(p, m, v, g, *, lr: float, beta1: float, beta2: float, eps: float
     corrections included)."""
     u = _U
     p, m, v, g = _f64(p), _f64(m), _f64(v), _f64(g)
-    b1, b2 = beta1, beta2
-    bc1i, bc2i = 1.0 / (1.0 - b1 ** step), 1.0 / (1.0 - b2 ** step) ** 0.5
     gs, wdp = g * grad_scale, weight_decay * p
     gk = gs + wdp
     e_gk = u * (gs.abs() + wdp.abs() + gk.abs())
+    return _adam_moments_step64(p, torch.zeros_like(p), m, v, gk, e_gk, lr=lr, beta1=beta1, beta2=beta2, eps=eps,
+                                step=step)
+
+
+def _adam_moments_step64(p, e_p0, m, v, gk, e_gk, *, lr, beta1, beta2, eps, step):
+    """The moments and step of adam_update (adam.cuh) from the gradient gk (error e_gk) and the weight p
+    (error e_p0 that p carries in already)."""
+    u = _U
+    b1, b2 = beta1, beta2
+    bc1i, bc2i = 1.0 / (1.0 - b1 ** step), 1.0 / (1.0 - b2 ** step) ** 0.5
     m1 = b1 * m + (1 - b1) * gk
     e_m = u * (b1 * m.abs() + m1.abs()) + (1 - b1) * (e_gk + u * gk.abs())
     t = (1 - b2) * gk
@@ -531,8 +539,33 @@ def adam_step64(p, m, v, g, *, lr: float, beta1: float, beta2: float, eps: float
     q = num / d
     e_q = e_num / d + num.abs() * e_d / d ** 2 + u * q.abs()
     p1 = p - q
-    e_p = e_q + u * p1.abs()
+    e_p = e_p0 + e_q + u * p1.abs()
     return {"p": (p1, e_p), "m": (m1, e_m), "v": (v1, e_v)}
+
+
+def adamw_keep(lr: float, weight_decay):
+    """AdamW's weight factor as the kernels take it: fp32(1 - lr * wd), the product in double (torch's
+    Python scalar).  ``weight_decay`` may be a float64 tensor (one decay per element)."""
+    if isinstance(weight_decay, torch.Tensor):
+        return (1.0 - lr * weight_decay.to(torch.float64)).to(torch.float32).to(torch.float64)
+    return _f32(1.0 - lr * weight_decay)
+
+
+def adamw_step64(p, m, v, g, *, lr: float, beta1: float, beta2: float, eps: float, weight_decay,
+                 step: int, grad_scale: float = 1.0, keep_lr: float = None):
+    """One step of adam_kernel's decoupled form (torch.optim.AdamW): p' = p * keep with keep =
+    adamw_keep(keep_lr or lr, weight_decay), then Adam on g * grad_scale with no L2 term.  ``lr`` is
+    taken as given, like adam_step64's (pass the fp32 value the kernel receives); ``keep_lr`` is the
+    double-precision rate the host forms keep from (default ``lr``).  ``weight_decay``: a float or a
+    tensor of per-element decays.  Returns {"p", "m", "v": (ref, err)} as adam_step64; the error of
+    keep itself is not counted: the kernel receives the same fp32 factor."""
+    u = _U
+    p, m, v, g = _f64(p), _f64(m), _f64(v), _f64(g)
+    keep = adamw_keep(lr if keep_lr is None else keep_lr, weight_decay)
+    p0 = p * keep
+    gk = g * grad_scale
+    return _adam_moments_step64(p0, u * p0.abs(), m, v, gk, u * gk.abs(), lr=lr, beta1=beta1, beta2=beta2,
+                                eps=eps, step=step)
 
 
 def sgd_step64(p, buf, g, *, lr: float, momentum: float, weight_decay: float, first: bool,

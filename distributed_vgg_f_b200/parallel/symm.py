@@ -104,15 +104,18 @@ class SymmetricArena:
                    v32: torch.Tensor, w16: torch.Tensor, start: int, n: int, *, algo: str, slot: int,
                    max_ctas: int, inv_world: float, lr: float, beta1: float, beta2: float, eps: float,
                    weight_decay: float, step: int, ema: Optional[torch.Tensor] = None, ema_decay: float = 0.0,
-                   ema_first: bool = False) -> None:
+                   ema_first: bool = False, decoupled: bool = False) -> None:
         """EXPERIMENTAL: reduce-scatter + Adam on the cells this rank owns + all-gather of the new
         bf16 weights, one kernel (csrc/allreduce.cu::zero1_kernel).  bf16 wire, two-shot or NVLS.
-        ``ema``: the owner also updates the weights' moving average of its cells (ops.adam_step)."""
+        ``ema``: the owner also updates the weights' moving average of its cells (ops.adam_step).
+        ``decoupled``: AdamW, as ops.adam_step."""
         if self.wire_dtype != torch.bfloat16 or algo not in ("twoshot", "nvls"):
             raise ValueError("zero1_step needs the bf16 wire and a reduce-scatter algorithm")
+        tail = ops._ema_args(ema, ema_decay, ema_first) if not decoupled else \
+            (ema, float(ema_decay), bool(ema_first), True)
         ops.require().zero1_step(self.comm, grad_f32, p32, m32, v32, w16, start, n, inv_world,
                                  self._algo[algo], slot, self.next_epoch(slot), max_ctas, lr, beta1, beta2,
-                                 eps, weight_decay, step, *ops._ema_args(ema, ema_decay, ema_first))
+                                 eps, weight_decay, step, *tail)
 
     def owned_ranges(self, start: int, n: int, max_ctas: int):
         """Element ranges of [start, start+n) whose fp32 master this rank owns under zero1_step

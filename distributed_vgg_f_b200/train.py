@@ -25,6 +25,7 @@ from .parallel.process_group import (device_name, distributed_is_initialized, in
                                      pick_device)
 from .trainer import Trainer
 from .utils import checkpoint as ckpt
+from .utils.lr_schedule import LRSchedule
 
 
 def _want_native(args, device: torch.device) -> bool:
@@ -63,10 +64,29 @@ def build_model_ema(module: torch.nn.Module, decay: float):
     return AveragedModel(module, avg_fn=ema_avg, use_buffers=True)
 
 
-def build_optimizer(params, args):
+def parameter_groups(model: torch.nn.Module, weight_decay: float, bias_weight_decay=None):
+    """torchvision's set_weight_decay(custom_keys_weight_decay=[("bias", bias_weight_decay)]): the
+    ``*.bias`` tensors in a group of their own at ``bias_weight_decay``, everything else at
+    ``weight_decay``.  Without a bias decay, one group (the parent's layout of the optimizer state)."""
+    if bias_weight_decay is None:
+        return [{"params": list(model.parameters()), "weight_decay": weight_decay}]
+    named = list(model.named_parameters())
+    return [{"params": [p for n, p in named if not n.endswith(".bias")], "weight_decay": weight_decay},
+            {"params": [p for n, p in named if n.endswith(".bias")], "weight_decay": bias_weight_decay}]
+
+
+def build_optimizer(model_or_params, args):
+    """The torch-op engine's optimizer.  The decay is always passed: AdamW's own default is 0.01."""
+    wd = getattr(args, "weight_decay", 0.0)
+    if isinstance(model_or_params, torch.nn.Module):
+        params = parameter_groups(model_or_params, wd, getattr(args, "bias_weight_decay", None))
+    else:
+        params = [{"params": list(model_or_params), "weight_decay": wd}]
     if args.optimizer == "sgd":
-        return torch.optim.SGD(params, lr=args.learning_rate, momentum=args.momentum)
-    return torch.optim.Adam(params, lr=args.learning_rate)     # distributedVggf.py:230
+        return torch.optim.SGD(params, lr=args.learning_rate, momentum=args.momentum, weight_decay=wd)
+    if args.optimizer == "adamw":
+        return torch.optim.AdamW(params, lr=args.learning_rate, weight_decay=wd)
+    return torch.optim.Adam(params, lr=args.learning_rate, weight_decay=wd)     # distributedVggf.py:230
 
 
 def manage_training(args) -> Trainer:
@@ -128,7 +148,9 @@ def manage_training(args) -> Trainer:
                              wire_dtype=args.wire_dtype, bucket_mb=args.bucket_mb, seed=args.seed,
                              pretrained_state=pretrained, profile=args.profile,
                              zero1={"auto": "auto", "on": True, "off": False}[getattr(args, "zero1", "auto")],
-                             label_smoothing=getattr(args, "label_smoothing", 0.0), ema_decay=ema_decay)
+                             label_smoothing=getattr(args, "label_smoothing", 0.0), ema_decay=ema_decay,
+                             weight_decay=getattr(args, "weight_decay", 0.0),
+                             bias_weight_decay=getattr(args, "bias_weight_decay", None))
         optimizer = None            # fused into the engine
         model_ema = True if ema_decay is not None else None       # kept by the engine's optimizer kernels
         if model.world > 1:
@@ -137,7 +159,7 @@ def manage_training(args) -> Trainer:
         model = build_oracle(spec, seed=args.seed, pretrained_state=pretrained).to(device)
         if distributed_is_initialized():
             model = FlatDDP(model, bucket_cap_mb=args.bucket_mb)
-        optimizer = build_optimizer(model.parameters(), args)
+        optimizer = build_optimizer(model.module if isinstance(model, FlatDDP) else model, args)
         model_ema = None
         if ema_decay is not None:
             model_ema = build_model_ema(model.module if isinstance(model, FlatDDP) else model, ema_decay)
@@ -150,24 +172,27 @@ def manage_training(args) -> Trainer:
         start_epoch = ckpt.load_checkpoint(args.resume, model, optimizer, **kw) + 1
         print("[Info] resumed from {} at epoch {}".format(args.resume, start_epoch))
 
-    base_lr = args.learning_rate
-    if args.resume and args.lr_step and start_epoch > 1:
-        # a run resumed behind an LR-step boundary continues at the decayed rate on BOTH back ends
-        resumed_lr = base_lr * (args.lr_gamma ** ((start_epoch - 1) // args.lr_step))
+    schedule = LRSchedule.from_args(args)
+
+    def set_lr(lr: float) -> None:
         if optimizer is not None:
             for g in optimizer.param_groups:
-                g["lr"] = resumed_lr
+                g["lr"] = lr
         else:
-            model.set_lr(resumed_lr)
+            model.set_lr(lr)
+
+    def current_lr() -> float:
+        return optimizer.param_groups[0]["lr"] if optimizer is not None else model.lr
+
+    if not schedule.constant:
+        # the rate of the first epoch to run, on BOTH back ends: a warmup's first rate, or a resumed
+        # run's rate behind the schedule's steps
+        set_lr(schedule.lr_at(start_epoch - 1))
 
     def on_epoch_end(epoch: int, trainer: Trainer) -> None:
-        if args.lr_step and epoch % args.lr_step == 0:
-            new_lr = base_lr * (args.lr_gamma ** (epoch // args.lr_step))
-            if optimizer is not None:
-                for g in optimizer.param_groups:
-                    g["lr"] = new_lr
-            else:
-                model.set_lr(new_lr)
+        epoch_lr = current_lr()
+        if not schedule.constant:
+            set_lr(schedule.lr_at(epoch))
         if args.save:
             kw = {} if model_ema is None else dict(model_ema=model_ema)
             ckpt.save_checkpoint(args.save, model, optimizer, epoch, vars(args),
@@ -178,6 +203,8 @@ def manage_training(args) -> Trainer:
                 torch.distributed.barrier()
         if args.log_jsonl and args.rank == 0:
             rec = dict(trainer.history[-1], time=time.time(), world_size=args.world_size)
+            if not schedule.constant:
+                rec["lr"] = epoch_lr
             if hasattr(model, "phase_times"):
                 rec["phase_ms"] = model.phase_times()
             for key in ("epoch_host_times", "epoch_allreduce"):       # set by Trainer for native engines
