@@ -145,6 +145,58 @@ static void conv0_wgrad(const at::Tensor& dz, const at::Tensor& x4, at::Tensor d
   b200::conv0_wgrad(bfp(dz), bfp(x4), f32p(dw0), x4.size(0), x4.size(1), x4.size(2), cur_stream());
 }
 
+// ------------------------------------------------------------- split-K without atomics (api.h)
+static void check_workspace_tensor(const at::Tensor& ws, const char* op) {
+  check_vec(ws, at::kFloat, 16, op, "the workspace");
+}
+static int64_t gemm_partial(const at::Tensor& A, bool a_mn, const at::Tensor& B, bool b_mn, int64_t M, int64_t N,
+                            int64_t K, at::Tensor ws, int64_t ldo, bool transposed, double alpha, int64_t ksplit,
+                            int64_t bn) {
+  c10::cuda::CUDAGuard g(A.device());
+  TORCH_CHECK(A.dim() == 2 && B.dim() == 2 && A.stride(1) == 1 && B.stride(1) == 1, "gemm_partial: 2-D row-major operands");
+  TORCH_CHECK(M > 0 && N > 0 && K > 0, "gemm_partial: M, N and K must be positive");
+  TORCH_CHECK(A.size(0) >= (a_mn ? K : M) && A.size(1) >= (a_mn ? M : K), "gemm_partial: A must be at least ",
+              a_mn ? "[K, M]" : "[M, K]", ", got ", A.sizes());
+  TORCH_CHECK(B.size(0) >= (b_mn ? K : N) && B.size(1) >= (b_mn ? N : K), "gemm_partial: B must be at least ",
+              b_mn ? "[K, N]" : "[N, K]", ", got ", B.sizes());
+  // every element of a slice must be written: the reduction reads whole slices
+  TORCH_CHECK(ldo == (transposed ? M : N), "gemm_partial: slices are dense, ldo must be ", transposed ? M : N);
+  check_workspace_tensor(ws, "gemm_partial");
+  return b200::gemm_bf16_partial(bfp(A), A.stride(0), a_mn, bfp(B), B.stride(0), b_mn, (int)M, (int)N, (int)K, f32p(ws),
+                                 ws.numel(), ldo, transposed, (float)alpha, (int)ksplit, (int)bn, cur_stream());
+}
+static int64_t conv_wgrad_partial(const at::Tensor& dz, const at::Tensor& x, at::Tensor ws, double scale) {
+  c10::cuda::CUDAGuard g(dz.device());
+  TORCH_CHECK(dz.dim() == 4 && dz.is_contiguous() && x.is_contiguous(), "conv_wgrad_partial: contiguous NHWC");
+  const int N = dz.size(0), H = dz.size(1), W = dz.size(2), Cout = dz.size(3), Cin = x.size(3);
+  check_nhwc(x, N, H, W, Cin, "conv_wgrad_partial", "x");
+  check_workspace_tensor(ws, "conv_wgrad_partial");
+  return b200::conv3x3_wgrad_partial(bfp(dz), bfp(x), f32p(ws), ws.numel(), N, H, W, Cin, Cout, (float)scale, cur_stream());
+}
+static int64_t conv0_wgrad_partial(const at::Tensor& dz, const at::Tensor& x4, at::Tensor ws) {
+  c10::cuda::CUDAGuard g(x4.device());
+  TORCH_CHECK(x4.dim() == 4 && x4.size(3) == 4 && x4.is_contiguous() && dz.is_contiguous(),
+              "conv0_wgrad_partial: x4 [N,H,W,4]");
+  check_nhwc(dz, x4.size(0), x4.size(1), x4.size(2), 64, "conv0_wgrad_partial", "dz");
+  check_workspace_tensor(ws, "conv0_wgrad_partial");
+  return b200::conv0_wgrad_partial(bfp(dz), bfp(x4), f32p(ws), ws.numel(), x4.size(0), x4.size(1), x4.size(2), cur_stream());
+}
+static int64_t colsum_partial(const at::Tensor& dz, at::Tensor ws, int64_t rows, int64_t C, double scale) {
+  c10::cuda::CUDAGuard g(dz.device());
+  TORCH_CHECK(C > 0 && C % 8 == 0 && rows > 0 && dz.numel() >= rows * C, "colsum_partial: dz must hold rows x C, C % 8 == 0");
+  check_vec(dz, at::kBFloat16, 16, "colsum_partial", "dz");
+  check_workspace_tensor(ws, "colsum_partial");
+  return b200::colsum_partial(bfp(dz), f32p(ws), ws.numel(), rows, (int)C, (float)scale, cur_stream());
+}
+static void splitk_reduce(const at::Tensor& ws, at::Tensor dst, int64_t n, int64_t slice, int64_t splits, double alpha,
+                          bool accumulate) {
+  c10::cuda::CUDAGuard g(ws.device());
+  check_workspace_tensor(ws, "splitk_reduce");
+  check_vec(dst, at::kFloat, 16, "splitk_reduce", "dst");
+  TORCH_CHECK(dst.numel() >= n, "splitk_reduce: dst must hold n = ", n, " elements, got ", dst.numel());
+  b200::splitk_reduce(f32p(ws), ws.numel(), f32p(dst), n, slice, (int)splits, (float)alpha, accumulate, cur_stream());
+}
+
 // ------------------------------------------------------------------------------------ element-wise
 static void maxpool_fwd(const at::Tensor& x, at::Tensor y) {
   c10::cuda::CUDAGuard g(x.device());
@@ -775,6 +827,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("unpool2x2", &unpool);
   m.def("conv_dgrad", &conv_dgrad);
   m.def("conv_wgrad", &conv_wgrad);
+  m.def("gemm_partial", &gemm_partial);
+  m.def("conv_wgrad_partial", &conv_wgrad_partial);
+  m.def("conv0_wgrad_partial", &conv0_wgrad_partial);
+  m.def("colsum_partial", &colsum_partial);
+  m.def("splitk_reduce", &splitk_reduce);
+  m.def("conv_wgrad_splits", [](int64_t N, int64_t H, int64_t W, int64_t Cin, int64_t Cout, int64_t sms) {
+    return b200::conv_wgrad_splits((int)N, (int)H, (int)W, (int)Cin, (int)Cout, (int)sms); });
+  m.def("conv0_wgrad_splits", [](int64_t N, int64_t H, int64_t W, int64_t sms) {
+    return b200::conv0_wgrad_splits((int)N, (int)H, (int)W, (int)sms); });
+  m.def("gemm_splits", [](int64_t K, int64_t ksplit) { return b200::gemm_splits((int)K, (int)ksplit); });
+  m.def("colsum_partial_blocks", [](int64_t rows, int64_t C, int64_t sms) {
+    return b200::colsum_partial_blocks(rows, (int)C, (int)sms); });
+  m.def("workspace_slice", [](int64_t elems) { return (int64_t)b200::workspace_slice(elems); });
+  m.def("sm_count", [] { return b200::sm_count(); });
   m.def("maxpool_fwd", &maxpool_fwd);
   m.def("maxpool_relu_bwd", &maxpool_relu_bwd);
   m.def("avgpool_fwd", &avgpool_fwd);

@@ -2,6 +2,7 @@
 // average pool, bias gradients, FC epilogues (bias + ReLU + Philox dropout), casts.
 // All activations are NHWC bf16; every thread moves 16-byte vectors (8 channels).
 #include <stdexcept>
+#include <string>
 
 #include "api.h"
 #include "ptx.cuh"
@@ -287,6 +288,9 @@ void adaptive_avgpool_bwd(const bf16* dy, bf16* dx, int N, int H, int W, int C, 
 
 // ---------------------------------------------------------------------------------- bias grad
 // db[c] += scale * sum_r dz[r][c].  Block = CG column groups (8 channels each) x RL row lanes.
+// PARTIAL: block x stores its row of sums to db[x][C] instead (the sum inside a block has a fixed order;
+// only the order in which the blocks' atomics arrive does not), for splitk_reduce to add up in block order.
+template <bool PARTIAL>
 __global__ void bias_grad_kernel(const bf16* __restrict__ dz, float* __restrict__ db, long long rows,
                                  int C, float scale, int CG, int RL, long long rows_per_block) {
   extern __shared__ float red[];      // [RL][CG*8]
@@ -327,7 +331,10 @@ __global__ void bias_grad_kernel(const bf16* __restrict__ dz, float* __restrict_
 #pragma unroll
       for (int k = 0; k < 8; ++k) acc[k] += red[(j * CG + cg) * 8 + k];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) atomicAdd(db + col8 * 8 + k, acc[k] * scale);
+    for (int k = 0; k < 8; ++k) {
+      if constexpr (PARTIAL) db[static_cast<long long>(blockIdx.x) * C + col8 * 8 + k] = acc[k] * scale;
+      else atomicAdd(db + col8 * 8 + k, acc[k] * scale);
+    }
   }
 }
 // Generic fallback (C not a multiple of 8, e.g. the 3-class logits): one thread per channel.
@@ -340,22 +347,118 @@ __global__ void bias_grad_small_kernel(const bf16* __restrict__ dz, float* __res
   atomicAdd(db + c, acc * scale);
 }
 
-void bias_grad(const bf16* dz, float* db, long long rows, int C, float scale, cudaStream_t s) {
-  if (C % 8 != 0) throw std::runtime_error("[b200] bias_grad: C%8 != 0 (use bias_grad_ld)");
+// Block shape and row blocks of bias_grad for `rows` x C on `sms` SMs; returns the row blocks (grid.x).
+static int bias_grad_shape(long long rows, int C, int sms, int* CG, int* RL, long long* rpb) {
   const int c8 = C / 8;
-  const int CG = c8 < 256 ? c8 : 256;
-  int RL = 256 / CG;
-  if (RL < 1) RL = 1;
-  const int threads = CG * RL;
-  long long nblk = (rows + RL * 16 - 1) / (RL * 16);
-  const long long cap = static_cast<long long>(sm_count()) * 8 / ((c8 + CG - 1) / CG);
+  *CG = c8 < 256 ? c8 : 256;
+  *RL = 256 / *CG;
+  if (*RL < 1) *RL = 1;
+  long long nblk = (rows + *RL * 16 - 1) / (*RL * 16);
+  const long long cap = static_cast<long long>(sms) * 8 / ((c8 + *CG - 1) / *CG);
   if (nblk > cap) nblk = cap;
   if (nblk < 1) nblk = 1;
-  const long long rpb = (rows + nblk - 1) / nblk;
-  dim3 grid(static_cast<unsigned>((rows + rpb - 1) / rpb), (c8 + CG - 1) / CG);
-  bias_grad_kernel<<<grid, threads, threads * 8 * sizeof(float), s>>>(dz, db, rows, C, scale, CG, RL, rpb);
+  *rpb = (rows + nblk - 1) / nblk;
+  return static_cast<int>((rows + *rpb - 1) / *rpb);
+}
+int colsum_partial_blocks(long long rows, int C, int sms) {
+  int CG, RL;
+  long long rpb;
+  return bias_grad_shape(rows, C, sms, &CG, &RL, &rpb);
+}
+
+template <bool PARTIAL>
+static int bias_grad_launch(const bf16* dz, float* db, long long ws_elems, long long rows, int C, float scale,
+                            cudaStream_t s) {
+  if (C % 8 != 0) throw std::runtime_error("[b200] bias_grad: C%8 != 0 (use bias_grad_ld)");
+  int CG, RL;
+  long long rpb;
+  const int blocks = bias_grad_shape(rows, C, sm_count(), &CG, &RL, &rpb);
+  if (PARTIAL && (!db || ws_elems < static_cast<long long>(blocks) * C))
+    throw std::runtime_error("[b200] colsum_partial: the workspace must hold " + std::to_string(blocks) +
+                             " rows of " + std::to_string(C) + " floats");
+  const int threads = CG * RL;
+  dim3 grid(blocks, (C / 8 + CG - 1) / CG);
+  bias_grad_kernel<PARTIAL><<<grid, threads, threads * 8 * sizeof(float), s>>>(dz, db, rows, C, scale, CG, RL, rpb);
   count_launch();
-  check_last("bias_grad");
+  check_last(PARTIAL ? "colsum_partial" : "bias_grad");
+  return blocks;
+}
+void bias_grad(const bf16* dz, float* db, long long rows, int C, float scale, cudaStream_t s) {
+  bias_grad_launch<false>(dz, db, 0, rows, C, scale, s);
+}
+int colsum_partial(const bf16* dz, float* ws, long long ws_elems, long long rows, int C, float scale, cudaStream_t s) {
+  return bias_grad_launch<true>(dz, ws, ws_elems, rows, C, scale, s);
+}
+
+// ------------------------------------------------------------------------- split-K reduction
+// dst[i] = (accumulate ? dst[i] : 0) + alpha * (((ws[0][i] + ws[1][i]) + ws[2][i]) + ...): the slices a
+// PARTIAL epilogue stored, added in split order.  Every add and the product round to fp32 on their own
+// (no contraction into an FMA), so the result is a function of the slices alone.  Bandwidth-bound: one
+// float4 per thread and pass, four slices' loads in flight, the workspace read once and not kept in L2.
+__device__ __forceinline__ uint64_t l2_evict_first_policy() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ float4 ld_evict_first_v4(const float* p, uint64_t pol) {
+  float4 v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ void add4(float4& a, const float4& b) {
+  a.x = __fadd_rn(a.x, b.x); a.y = __fadd_rn(a.y, b.y); a.z = __fadd_rn(a.z, b.z); a.w = __fadd_rn(a.w, b.w);
+}
+__global__ void __launch_bounds__(256)
+splitk_reduce_kernel(const float* __restrict__ ws, float* __restrict__ dst, long long n, long long slice,
+                     int splits, float alpha, int accumulate) {
+  const long long n4 = n / 4;
+  const uint64_t pol = l2_evict_first_policy();
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float* src = ws + i * 4;
+    float4 acc = ld_evict_first_v4(src, pol);
+    int k = 1;
+    for (; k + 4 <= splits; k += 4) {
+      float4 v[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) v[u] = ld_evict_first_v4(src + (k + u) * slice, pol);
+#pragma unroll
+      for (int u = 0; u < 4; ++u) add4(acc, v[u]);
+    }
+    for (; k < splits; ++k) add4(acc, ld_evict_first_v4(src + k * slice, pol));
+    acc = make_float4(__fmul_rn(alpha, acc.x), __fmul_rn(alpha, acc.y), __fmul_rn(alpha, acc.z), __fmul_rn(alpha, acc.w));
+    float4* o = reinterpret_cast<float4*>(dst) + i;
+    if (accumulate) {
+      float4 d = *o;
+      add4(d, acc);
+      acc = d;
+    }
+    *o = acc;
+  }
+  if (blockIdx.x == 0) {                // scalar tail
+    for (long long i = n4 * 4 + threadIdx.x; i < n; i += blockDim.x) {
+      float acc = ws[i];
+      for (int k = 1; k < splits; ++k) acc = __fadd_rn(acc, ws[i + k * slice]);
+      acc = __fmul_rn(alpha, acc);
+      dst[i] = accumulate ? __fadd_rn(dst[i], acc) : acc;
+    }
+  }
+}
+
+void splitk_reduce(const float* ws, long long ws_elems, float* dst, long long n, long long slice, int splits,
+                   float alpha, bool accumulate, cudaStream_t s) {
+  if (n <= 0 || splits < 1 || slice < n || slice % 4 != 0)
+    throw std::runtime_error("[b200] splitk_reduce: needs n > 0, splits >= 1 and a slice stride >= n in whole float4s");
+  if (!ws || !dst || (reinterpret_cast<uintptr_t>(ws) & 15) || (reinterpret_cast<uintptr_t>(dst) & 15))
+    throw std::runtime_error("[b200] splitk_reduce: the workspace and the destination must be 16-byte aligned");
+  if (ws_elems < (splits - 1) * slice + n)
+    throw std::runtime_error("[b200] splitk_reduce: the workspace holds " + std::to_string(ws_elems) + " floats, " +
+                             std::to_string(splits) + " slices need " + std::to_string((splits - 1) * slice + n));
+  splitk_reduce_kernel<<<min(ceil_div_ll(n / 4 + 1, 256), sm_count() * 8), 256, 0, s>>>(ws, dst, n, slice, splits, alpha,
+                                                                                      accumulate ? 1 : 0);
+  count_launch();
+  check_last("splitk_reduce");
 }
 void bias_grad_ld(const bf16* dz, float* db, long long rows, int C, int ld, float scale,
                   cudaStream_t s) {

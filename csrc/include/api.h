@@ -54,6 +54,36 @@ void conv3x3_dgrad(const bf16* dz, const bf16* w, const bf16* mask_src, bf16* dx
 void conv3x3_wgrad(const bf16* dz, const bf16* x, float* dw, int N, int H, int W, int Cin,
                    int Cout, float scale, int ksplit, int bn, cudaStream_t stream);
 
+// ---- split-K without atomics (bit-reproducible training) --------------------------------------
+// Each split-K kernel has a `_partial` form that stores every split's tile into its own slice of a
+// workspace, ws[split][output elements] (plain stores, one writer per element), and returns the number
+// of slices it wrote; splitk_reduce then adds the slices in split order.  The `_splits` queries are the
+// launchers' own split arithmetic as pure host functions of the shape and an SM count, for sizing the
+// workspace (also where no GPU is present).  A launch refuses a workspace that is null, misaligned or
+// too small before anything is enqueued.
+inline long long workspace_slice(long long elems) { return (elems + 3) / 4 * 4; }   // slices start on float4s
+int conv_wgrad_splits(int N, int H, int W, int Cin, int Cout, int sms);
+int conv0_wgrad_splits(int N, int H, int W, int sms);      // 2 per CTA: one per consumer warpgroup
+int gemm_splits(int K, int ksplit);
+int colsum_partial_blocks(long long rows, int C, int sms);
+// ws[splits][Cout][9][Cin].  The split count differs from conv3x3_wgrad's: see wgrad_partial_ksplit.
+int conv3x3_wgrad_partial(const bf16* dz, const bf16* x, float* ws, long long ws_elems, int N, int H, int W,
+                          int Cin, int Cout, float scale, cudaStream_t stream);
+// ws[splits][64][64]; a consumer warpgroup that had no k-block stores zeros.
+int conv0_wgrad_partial(const bf16* dz, const bf16* x4, float* ws, long long ws_elems, int N, int H, int W,
+                        cudaStream_t stream);
+// gemm_bf16 with split-K into ws[splits][workspace_slice(M * ldo)] ([N * ldo] when `transposed`), each
+// slice addressed as EPI_F32_ATOMIC (_T) addresses the output.
+int gemm_bf16_partial(const bf16* A, long long lda, bool a_mn, const bf16* B, long long ldb, bool b_mn, int M,
+                      int N, int K, float* ws, long long ws_elems, long long ldo, bool transposed, float alpha,
+                      int ksplit, int bn, cudaStream_t stream);
+// bias_grad's per-block sums as rows ws[blocks][C] (C % 8 == 0); returns blocks.
+int colsum_partial(const bf16* dz, float* ws, long long ws_elems, long long rows, int C, float scale, cudaStream_t s);
+// dst[i] = (accumulate ? dst[i] : 0) + alpha * (((ws[0][i] + ws[1][i]) + ws[2][i]) + ...) for i < n, slices
+// `slice` floats apart, every operation rounded to fp32 on its own.
+void splitk_reduce(const float* ws, long long ws_elems, float* dst, long long n, long long slice, int splits,
+                   float alpha, bool accumulate, cudaStream_t s);
+
 // ---- element-wise / reduction kernels (elementwise.cu) ----------------------------------------
 void maxpool2x2_fwd(const bf16* x, bf16* y, int N, int H, int W, int C, cudaStream_t s);
 // dz[N,H,W,C] = (y == pooled(y) first match && y > 0) ? dp[N,H/2,W/2,C] : 0

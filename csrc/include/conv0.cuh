@@ -11,7 +11,9 @@
 //           B = the 64x64 weight (resident), epilogue bias + ReLU -> bf16 NHWC;
 //   wgrad : the same bytes are the MN-major B operand (rows = K = pixels); A = dZ via TMA (MN-major,
 //           M = 64 output channels).  The two consumer warpgroups take alternate k-blocks, keep
-//           their accumulators in registers over the CTA's pixel range and add them into dW.
+//           their accumulators in registers over the CTA's pixel range and add them into dW
+//           (PARTIAL: each stores its own slice ws[2 * CTA + consumer][64][64], zeros when it had
+//           no k-block, for splitk_reduce to add up in slice order).
 #pragma once
 #include "umma_core.cuh"
 
@@ -29,7 +31,7 @@ struct Conv0Params {
   const __nv_bfloat16* x4;     // [N][H][W][4] bf16 (3 channels + pad)
   __nv_bfloat16* out;          // fprop: [pixels][64] bf16
   const float* bias;
-  float* dW;                   // wgrad: [64][64] fp32
+  float* dW;                   // wgrad: [64][64] fp32; PARTIAL: [2 * grid][64][64]
   int N, H, W;
   long long pixels;            // N*H*W
   int num_tiles;               // fprop: ceil(pixels/128); wgrad: k-blocks of 64 pixels
@@ -68,7 +70,7 @@ __device__ __forceinline__ void c0_build_row(const Conv0Params& p, int pix, uint
   }
 }
 
-template <bool WGRAD>
+template <bool WGRAD, bool PARTIAL = false>
 __global__ void __launch_bounds__(C0_THREADS, 1) conv0_kernel(const __grid_constant__ Conv0Params prm) {
   constexpr int ROWS = WGRAD ? 64 : 128;                       // pixels per stage
   constexpr int A_BYTES = WGRAD ? UMMA_SLAB_BYTES : 0;         // wgrad: the dZ slab
@@ -176,7 +178,16 @@ __global__ void __launch_bounds__(C0_THREADS, 1) conv0_kernel(const __grid_const
         ++mine;
       }
       wgmma_fence_acc(d);
-      if (mine > 0) {
+      if constexpr (PARTIAL) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float* o = prm.dW + (2 * blockIdx.x + cw) * (64 * 64) + (r0 + 8 * h) * 64 + cq;
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<float2*>(o + 8 * j) =
+                mine > 0 ? make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]) : make_float2(0.f, 0.f);
+        }
+      } else if (mine > 0) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           float* o = prm.dW + (r0 + 8 * h) * 64 + cq;

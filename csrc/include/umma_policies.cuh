@@ -8,6 +8,9 @@
 //   WgradPolicy  dW[cout][tap][cin] = sum_pixels dZ[p][cout] * X[p+tap][cin]: both operands are
 //                MN-major 4-D boxes (K = 64 pixels per k-block), split-K over pixel tiles,
 //                fp32 red.add epilogue straight into the gradient arena.
+// The split-K epilogues (GemmPolicy's ATOMIC kinds, WgradPolicy) each have a PARTIAL form for
+// bit-reproducible training: plain stores into slice `split` of a workspace, which splitk_reduce
+// (elementwise.cu) then adds up in split order.
 #pragma once
 #include "umma_core.cuh"
 
@@ -46,6 +49,8 @@ enum GemmEpi : int {
   EPI_BF16_BIAS_RELU = 3, // out[row*ldo + col] = bf16(relu(acc + bias[col]))
   EPI_F32_STORE_T = 4,    // out[col*ldo + row] = acc
   EPI_BF16_STORE = 5,     // out[row*ldo + col] = bf16(alpha * acc)   (FC wgrad straight into the bf16 wire)
+  EPI_F32_PARTIAL = 6,    // out[split*slice + row*ldo + col] = acc        (fp32, split-K without atomics)
+  EPI_F32_PARTIAL_T = 7,  // out[split*slice + col*ldo + row] = acc
 };
 
 struct GemmParams {
@@ -60,6 +65,7 @@ struct GemmParams {
   long long ldo;
   const float* bias;
   float alpha;
+  long long slice;        // PARTIAL epilogues: elements between the workspace slices of two splits
 };
 
 template <int BN_, int STAGES_, bool A_MN_, bool B_MN_, int EPI>
@@ -73,8 +79,10 @@ struct GemmPolicy {
   static constexpr int EPI_SMEM = 0;
   __device__ static void epi_begin(const Params&, float*, int) {}
   __device__ static void epi_end(const Params&, float*, int) {}
+  static constexpr bool PARTIAL = EPI == EPI_F32_PARTIAL || EPI == EPI_F32_PARTIAL_T;
   struct Ctx {
     int m0, n0, k_begin, nk;
+    int split;            // set for the PARTIAL epilogues only
   };
   struct RowCtx {};
   __device__ static RowCtx row_ctx(const Params&, const Ctx&, int) { return RowCtx{}; }
@@ -89,6 +97,7 @@ struct GemmPolicy {
     const int rest = tile / p.tiles_m;
     const int tn = rest % p.tiles_n;
     const int tz = rest / p.tiles_n;
+    if constexpr (PARTIAL) c.split = tz;
     c.m0 = tm * UMMA_BM;
     c.n0 = tn * BN;
     c.k_begin = tz * p.k_iters_per_split;
@@ -123,10 +132,13 @@ struct GemmPolicy {
     const int cb = c.n0 + col0;
     if (r >= p.M || cb >= p.N) return;
     const float alpha = p.alpha;
-    if constexpr (EPI == EPI_F32_STORE || EPI == EPI_F32_ATOMIC) {
-      float* o = reinterpret_cast<float*>(p.out) + static_cast<long long>(r) * p.ldo + cb;
+    float* out32 = reinterpret_cast<float*>(p.out);
+    if constexpr (PARTIAL) out32 += c.split * p.slice;
+    constexpr bool STORE = EPI == EPI_F32_STORE || EPI == EPI_F32_PARTIAL;
+    if constexpr (STORE || EPI == EPI_F32_ATOMIC) {
+      float* o = out32 + static_cast<long long>(r) * p.ldo + cb;
       const bool vec = (cb + 32 <= p.N) && ((reinterpret_cast<uintptr_t>(o) & 15) == 0);
-      if (EPI == EPI_F32_STORE && vec && (reinterpret_cast<uintptr_t>(o) & 31) == 0) {
+      if (STORE && vec && (reinterpret_cast<uintptr_t>(o) & 31) == 0) {
         // a thread owns one 128-byte line of the output: four full-sector 32-byte stores
 #pragma unroll
         for (int j = 0; j < 32; j += 8) {
@@ -140,7 +152,7 @@ struct GemmPolicy {
         for (int j = 0; j < 32; j += 4) {
           float4 v = make_float4(__uint_as_float(acc[j]) * alpha, __uint_as_float(acc[j + 1]) * alpha,
                                  __uint_as_float(acc[j + 2]) * alpha, __uint_as_float(acc[j + 3]) * alpha);
-          if constexpr (EPI == EPI_F32_STORE) {
+          if constexpr (STORE) {
             *reinterpret_cast<float4*>(o + j) = v;
           } else {
             asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(o + j), "f"(v.x),
@@ -150,12 +162,12 @@ struct GemmPolicy {
         }
       } else {
         for (int j = 0; j < 32 && cb + j < p.N; ++j) {
-          if constexpr (EPI == EPI_F32_STORE) o[j] = __uint_as_float(acc[j]) * alpha;
+          if constexpr (STORE) o[j] = __uint_as_float(acc[j]) * alpha;
           else atomicAdd(o + j, __uint_as_float(acc[j]) * alpha);
         }
       }
-    } else if constexpr (EPI == EPI_F32_ATOMIC_T || EPI == EPI_F32_STORE_T) {
-      float* o = reinterpret_cast<float*>(p.out) + static_cast<long long>(cb) * p.ldo + r;
+    } else if constexpr (EPI == EPI_F32_ATOMIC_T || EPI == EPI_F32_STORE_T || EPI == EPI_F32_PARTIAL_T) {
+      float* o = out32 + static_cast<long long>(cb) * p.ldo + r;
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         if (cb + j < p.N) {
@@ -515,11 +527,11 @@ struct WgradParams {
   int total_tiles;        // pixel tiles = tiles_w * tiles_h * tiles_n
   int tiles_per_split;
   int ksplit;
-  float* dW;              // [Cout][9][Cin] fp32, accumulated with red.add
+  float* dW;              // [Cout][9][Cin] fp32, accumulated with red.add; PARTIAL: [ksplit][Cout][9][Cin], stored
   float scale;
 };
 
-template <int BN_, int STAGES_>
+template <int BN_, int STAGES_, bool PARTIAL = false>
 struct WgradPolicy {
   static constexpr int BN = BN_;
   static constexpr int STAGES = STAGES_;
@@ -532,6 +544,7 @@ struct WgradPolicy {
   __device__ static void epi_end(const Params&, float*, int) {}
   struct Ctx {
     int m0, c0, tap, tile_begin, nk;
+    int split;            // set for PARTIAL only
   };
   struct RowCtx {};
   __device__ static RowCtx row_ctx(const Params&, const Ctx&, int) { return RowCtx{}; }
@@ -551,6 +564,7 @@ struct WgradPolicy {
     rest /= p.tiles_m;
     c.c0 = (rest % p.tiles_n) * BN;
     const int split = rest / p.tiles_n;
+    if constexpr (PARTIAL) c.split = split;
     c.tile_begin = split * p.tiles_per_split;
     int rem = p.total_tiles - c.tile_begin;
     c.nk = rem < 0 ? 0 : (rem < p.tiles_per_split ? rem : p.tiles_per_split);
@@ -578,6 +592,14 @@ struct WgradPolicy {
     if (co >= p.Cout || ci >= p.Cin) return;
     float* o = p.dW + (static_cast<long long>(co) * 9 + c.tap) * p.Cin + ci;
     const float s = p.scale;
+    if constexpr (PARTIAL) {     // this split's own slice: every element has one writer
+      o += static_cast<long long>(c.split) * p.Cout * 9 * p.Cin;
+#pragma unroll
+      for (int j = 0; j < 32; j += 4)
+        *reinterpret_cast<float4*>(o + j) = make_float4(__uint_as_float(acc[j]) * s, __uint_as_float(acc[j + 1]) * s,
+                                                        __uint_as_float(acc[j + 2]) * s, __uint_as_float(acc[j + 3]) * s);
+      return;
+    }
 #pragma unroll
     for (int j = 0; j < 32; j += 4) {
       asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(o + j),

@@ -16,7 +16,8 @@
 //   * three consumer warpgroups own three taps each (kh = warpgroup); the nine 64 x 64 fp32
 //     accumulators stay in registers for the CTA's whole pixel range (split-K over pixel tiles,
 //     one work item per CTA);
-//   * epilogue: fp32 red.add straight into dW[co][tap][ci].
+//   * epilogue: fp32 red.add straight into dW[co][tap][ci]; PARTIAL: plain stores into the work
+//     item's own slice ws[split][co][tap][ci], added up in split order by splitk_reduce.
 // Operand traffic per k-block drops from 9 x 24 KB to 21 KB.
 #pragma once
 #include "umma_core.cuh"
@@ -48,10 +49,11 @@ struct WgradHaloParams {
   int total_tiles;         // N * tiles_h * tiles_w
   int tiles_per_split;
   int Cout;
-  float* dW;               // [Cout][9][64] fp32
+  float* dW;               // [Cout][9][64] fp32; PARTIAL: [splits][Cout][9][64]
   float scale;
 };
 
+template <bool PARTIAL = false>
 __global__ void __launch_bounds__(WH_THREADS, 1)
 wgrad_halo64_kernel(const __grid_constant__ WgradHaloParams prm) {
   extern __shared__ uint8_t smem_raw[];
@@ -149,6 +151,8 @@ wgrad_halo64_kernel(const __grid_constant__ WgradHaloParams prm) {
         // fragment rows = ci (16 w + lane / 4, + 8), columns = co (8 j + 2 (lane & 3), + 1)
         const int ci0 = 16 * w + (lane >> 2);
         const int co0 = n_tile * 64 + 2 * (lane & 3);
+        float* dW = prm.dW;
+        if constexpr (PARTIAL) dW += static_cast<long long>(item / prm.tiles_n) * prm.Cout * (9 * 64);
 #pragma unroll
         for (int kw = 0; kw < 3; ++kw) {
           const int tap = kh * 3 + kw;
@@ -158,8 +162,11 @@ wgrad_halo64_kernel(const __grid_constant__ WgradHaloParams prm) {
             for (int e = 0; e < 4; ++e) {
               const int ci = ci0 + 8 * (e >> 1);
               const int co = co0 + 8 * j + (e & 1);
-              if (co < prm.Cout)
-                atomicAdd(prm.dW + (static_cast<long long>(co) * 9 + tap) * 64 + ci, d[kw][4 * j + e] * prm.scale);
+              if (co < prm.Cout) {
+                float* o = dW + (static_cast<long long>(co) * 9 + tap) * 64 + ci;
+                if constexpr (PARTIAL) *o = d[kw][4 * j + e] * prm.scale;
+                else atomicAdd(o, d[kw][4 * j + e] * prm.scale);
+              }
             }
           }
         }

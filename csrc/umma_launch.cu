@@ -207,18 +207,18 @@ static void conv_halo_launch(ConvParams& prm, const bf16* act, cudaStream_t stre
 }
 
 // ------------------------------------------------------------------------- first conv (no im2col)
-template <bool WGRAD>
+template <bool WGRAD, bool PARTIAL = false>
 static void conv0_launch(Conv0Params& prm, int grid, cudaStream_t stream) {
   constexpr int stage = C0_TILE_BYTES + (WGRAD ? UMMA_SLAB_BYTES : 0);
   constexpr int smem = C0_STAGES * stage + 8192 + 512 + 1024;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv0_kernel<WGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(conv0_kernel<WGRAD, PARTIAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess)
       throw std::runtime_error(std::string("[b200] cudaFuncSetAttribute(conv0): ") + cudaGetErrorString(e));
     configured = true;
   }
-  conv0_kernel<WGRAD><<<grid, C0_THREADS, smem, stream>>>(prm);
+  conv0_kernel<WGRAD, PARTIAL><<<grid, C0_THREADS, smem, stream>>>(prm);
   count_launch();
   check_last("conv0_kernel launch");
 }
@@ -235,17 +235,48 @@ void conv0_fprop(const bf16* x4, const bf16* w0, const float* bias, bf16* y, int
   conv0_launch<false>(prm, prm.num_tiles < num_sms() ? prm.num_tiles : num_sms(), stream);
 }
 
-void conv0_wgrad(const bf16* dz, const bf16* x4, float* dw0, int N, int H, int W, cudaStream_t stream) {
+// CTAs of the layer-0 wgrad and the 64-pixel k-blocks each takes.
+static int conv0_wgrad_grid(int N, int H, int W, int sms, int* num_tiles, int* blocks_per_cta) {
+  const long long pixels = static_cast<long long>(N) * H * W;
+  *num_tiles = static_cast<int>((pixels + 63) / 64);
+  int grid = *num_tiles < sms ? *num_tiles : sms;
+  *blocks_per_cta = (*num_tiles + grid - 1) / grid;
+  return (*num_tiles + *blocks_per_cta - 1) / *blocks_per_cta;
+}
+int conv0_wgrad_splits(int N, int H, int W, int sms) {
+  int tiles, per_cta;
+  return 2 * conv0_wgrad_grid(N, H, W, sms, &tiles, &per_cta);   // one slice per (CTA, consumer warpgroup)
+}
+
+// A split-K workspace must hold `splits` slices of `elems` floats (each padded to whole float4s).
+static void check_workspace(const char* what, const float* ws, long long ws_elems, int splits, long long elems) {
+  if (!ws || (reinterpret_cast<uintptr_t>(ws) & 15) != 0)
+    throw std::runtime_error(std::string("[b200] ") + what + ": the split-K workspace must be a 16-byte aligned buffer");
+  if (ws_elems < splits * workspace_slice(elems))
+    throw std::runtime_error(std::string("[b200] ") + what + ": the split-K workspace holds " + std::to_string(ws_elems) +
+                             " floats, this launch writes " + std::to_string(splits) + " slices of " +
+                             std::to_string(workspace_slice(elems)));
+}
+
+static void conv0_wgrad_impl(const bf16* dz, const bf16* x4, float* dw0, long long ws_elems, bool partial, int N,
+                             int H, int W, cudaStream_t stream) {
   Conv0Params prm;
   prm.x4 = x4; prm.out = nullptr; prm.bias = nullptr; prm.dW = dw0;
   prm.N = N; prm.H = H; prm.W = W; prm.pixels = static_cast<long long>(N) * H * W;
-  prm.num_tiles = static_cast<int>((prm.pixels + 63) / 64);
-  int grid = prm.num_tiles < num_sms() ? prm.num_tiles : num_sms();
-  prm.blocks_per_cta = (prm.num_tiles + grid - 1) / grid;
-  grid = (prm.num_tiles + prm.blocks_per_cta - 1) / prm.blocks_per_cta;
+  const int grid = conv0_wgrad_grid(N, H, W, num_sms(), &prm.num_tiles, &prm.blocks_per_cta);
+  if (partial) check_workspace("conv0_wgrad_partial", dw0, ws_elems, 2 * grid, 64 * 64);
   map_2d(&prm.mapZ, dz, prm.pixels, 64, 64, 64, 64);
   prm.mapW = prm.mapZ;
-  conv0_launch<true>(prm, grid, stream);
+  if (partial) conv0_launch<true, true>(prm, grid, stream);
+  else conv0_launch<true>(prm, grid, stream);
+}
+void conv0_wgrad(const bf16* dz, const bf16* x4, float* dw0, int N, int H, int W, cudaStream_t stream) {
+  conv0_wgrad_impl(dz, x4, dw0, 0, false, N, H, W, stream);
+}
+int conv0_wgrad_partial(const bf16* dz, const bf16* x4, float* ws, long long ws_elems, int N, int H, int W,
+                        cudaStream_t stream) {
+  conv0_wgrad_impl(dz, x4, ws, ws_elems, true, N, H, W, stream);
+  return conv0_wgrad_splits(N, H, W, num_sms());
 }
 
 // ---------------------------------------------------------------------------------------- GEMM
@@ -271,9 +302,18 @@ static void gemm_launch(GemmParams& prm, const bf16* A, long long lda, const bf1
   if (bn == 32) { gemm_launch<32, AMN, BMN, EPI>(prm, A, lda, B, ldb, M, N, K, ksplit, stream); return; } \
   GEMM_BN_SWITCH(AMN, BMN, EPI)
 
-void gemm_bf16(const bf16* A, long long lda, bool a_mn, const bf16* B, long long ldb, bool b_mn,
-               int M, int N, int K, void* out, long long ldo, int epi, const float* bias,
-               float alpha, int ksplit, int bn, cudaStream_t stream) {
+// Splits a GEMM over K really makes when asked for `ksplit`: whole 64-wide k-blocks, none empty.
+int gemm_splits(int K, int ksplit) {
+  const int total = (K + UMMA_BK - 1) / UMMA_BK;
+  if (ksplit < 1) ksplit = 1;
+  const int per_split = (total + ksplit - 1) / ksplit;
+  return (total + per_split - 1) / per_split;
+}
+
+// `ws_elems` > 0: `out` is a split-K workspace of that many floats (the PARTIAL epilogues).
+static void gemm_impl(const bf16* A, long long lda, bool a_mn, const bf16* B, long long ldb, bool b_mn,
+                      int M, int N, int K, void* out, long long ldo, int epi, const float* bias,
+                      float alpha, int ksplit, int bn, long long ws_elems, cudaStream_t stream) {
   // Tiles are at most 128 wide here: the FC forward and dgrad have the batch as N (swap-AB), and
   // the FC wgrad has it as K -- one k-block per tile, bound by storing its output, which a wider
   // tile does not shorten.  256-wide tiles are built for the convolutions only (conv_bn).
@@ -285,22 +325,46 @@ void gemm_bf16(const bf16* A, long long lda, bool a_mn, const bf16* B, long long
   prm.k_iters_per_split = (prm.k_iters_total + ksplit - 1) / ksplit;
   ksplit = (prm.k_iters_total + prm.k_iters_per_split - 1) / prm.k_iters_per_split;
   prm.out = out; prm.ldo = ldo; prm.bias = bias; prm.alpha = alpha;
-  if (ksplit > 1 && !(epi == EPI_F32_ATOMIC || epi == EPI_F32_ATOMIC_T))
-    throw std::runtime_error("[b200] gemm_bf16: split-K needs an atomic epilogue");
+  const bool partial = epi == EPI_F32_PARTIAL || epi == EPI_F32_PARTIAL_T;
+  // a slice is the output as the matching ATOMIC epilogue addresses it: [M][ldo], transposed [N][ldo]
+  const long long slice_elems = static_cast<long long>(epi == EPI_F32_PARTIAL_T ? N : M) * ldo;
+  prm.slice = partial ? workspace_slice(slice_elems) : 0;
+  if (partial) check_workspace("gemm_bf16_partial", static_cast<const float*>(out), ws_elems, ksplit, slice_elems);
+  if (ksplit > 1 && !(epi == EPI_F32_ATOMIC || epi == EPI_F32_ATOMIC_T || partial))
+    throw std::runtime_error("[b200] gemm_bf16: split-K needs an atomic or a partial epilogue");
   if (!a_mn && !b_mn) {
+    if (epi == EPI_F32_PARTIAL_T) { GEMM_BN_SWITCH_32(false, false, EPI_F32_PARTIAL_T) }
     if (epi == EPI_F32_ATOMIC_T) { GEMM_BN_SWITCH_32(false, false, EPI_F32_ATOMIC_T) }
     if (epi == EPI_F32_STORE_T) { GEMM_BN_SWITCH_32(false, false, EPI_F32_STORE_T) }
     if (epi == EPI_BF16_BIAS_RELU) { GEMM_BN_SWITCH(false, false, EPI_BF16_BIAS_RELU) }
     if (epi == EPI_F32_STORE) { GEMM_BN_SWITCH(false, false, EPI_F32_STORE) }
   } else if (a_mn && !b_mn) {
+    if (epi == EPI_F32_PARTIAL_T) { GEMM_BN_SWITCH_32(true, false, EPI_F32_PARTIAL_T) }
     if (epi == EPI_F32_ATOMIC_T) { GEMM_BN_SWITCH_32(true, false, EPI_F32_ATOMIC_T) }
     if (epi == EPI_F32_STORE_T) { GEMM_BN_SWITCH_32(true, false, EPI_F32_STORE_T) }
   } else if (a_mn && b_mn) {
     if (epi == EPI_F32_STORE) { GEMM_BN_SWITCH(true, true, EPI_F32_STORE) }
     if (epi == EPI_F32_ATOMIC) { GEMM_BN_SWITCH(true, true, EPI_F32_ATOMIC) }
+    if (epi == EPI_F32_PARTIAL) { GEMM_BN_SWITCH(true, true, EPI_F32_PARTIAL) }
     if (epi == EPI_BF16_STORE) { GEMM_BN_SWITCH(true, true, EPI_BF16_STORE) }
   }
   throw std::runtime_error("[b200] gemm_bf16: unsupported (layout, epilogue, bn) combination");
+}
+
+void gemm_bf16(const bf16* A, long long lda, bool a_mn, const bf16* B, long long ldb, bool b_mn,
+               int M, int N, int K, void* out, long long ldo, int epi, const float* bias,
+               float alpha, int ksplit, int bn, cudaStream_t stream) {
+  if (epi == EPI_F32_PARTIAL || epi == EPI_F32_PARTIAL_T)
+    throw std::runtime_error("[b200] gemm_bf16: the partial epilogues take a workspace (gemm_bf16_partial)");
+  gemm_impl(A, lda, a_mn, B, ldb, b_mn, M, N, K, out, ldo, epi, bias, alpha, ksplit, bn, 0, stream);
+}
+int gemm_bf16_partial(const bf16* A, long long lda, bool a_mn, const bf16* B, long long ldb, bool b_mn, int M,
+                      int N, int K, float* ws, long long ws_elems, long long ldo, bool transposed, float alpha,
+                      int ksplit, int bn, cudaStream_t stream) {
+  const int splits = gemm_splits(K, ksplit);
+  gemm_impl(A, lda, a_mn, B, ldb, b_mn, M, N, K, ws, ldo, transposed ? EPI_F32_PARTIAL_T : EPI_F32_PARTIAL, nullptr,
+            alpha, splits, bn, ws_elems, stream);
+  return splits;
 }
 
 // ---------------------------------------------------------------------------------------- conv
@@ -424,53 +488,80 @@ void conv3x3_dgrad(const bf16* dz, const bf16* w, const bf16* mask_src, bf16* dx
   }
 }
 
-template <int BN>
+template <int BN, bool PARTIAL = false>
 static void wgrad_launch(WgradParams& prm, cudaStream_t stream) {
-  using P = WgradPolicy<BN, umma_stages<BN, 0>()>;
+  using P = WgradPolicy<BN, umma_stages<BN, 0>(), PARTIAL>;
   prm.tiles_m = (prm.Cout + UMMA_BM - 1) / UMMA_BM;
   prm.tiles_n = (prm.Cin + BN - 1) / BN;
   prm.num_tiles = prm.tiles_m * prm.tiles_n * 9 * prm.ksplit;
   launch<P>(prm, stream);
 }
 
+// Pixel-tile splits of the halo wgrad: one work item per SM, none empty.
+static int wgrad_halo64_splits(int total_tiles, int tiles_n, int sms, int* tiles_per_split) {
+  int ksplit = sms / tiles_n;
+  if (ksplit < 1) ksplit = 1;
+  if (ksplit > total_tiles) ksplit = total_tiles;
+  *tiles_per_split = (total_tiles + ksplit - 1) / ksplit;
+  return (total_tiles + *tiles_per_split - 1) / *tiles_per_split;
+}
+static bool wgrad_halo64_applicable(int H, int W, int Cin) {
+  return Cin == 64 && H % WH_T == 0 && W % WH_T == 0 && W >= 16 && halo_enabled();
+}
+
 // 64-input-channel layers on 8-divisible maps: nine tap views of one X halo per pixel tile.
-static void wgrad_halo64_launch(const bf16* dz, const bf16* x, float* dw, int N, int H, int W, int Cout,
-                                float scale, cudaStream_t stream) {
+template <bool PARTIAL = false>
+static int wgrad_halo64_launch(const bf16* dz, const bf16* x, float* dw, long long ws_elems, int N, int H, int W,
+                               int Cout, float scale, cudaStream_t stream) {
   WgradHaloParams prm;
   prm.tiles_n = (Cout + 63) / 64;
   prm.tiles_w = W / WH_T; prm.tiles_h = H / WH_T;
   prm.total_tiles = N * prm.tiles_w * prm.tiles_h;
-  int ksplit = num_sms() / prm.tiles_n;
-  if (ksplit < 1) ksplit = 1;
-  if (ksplit > prm.total_tiles) ksplit = prm.total_tiles;
-  prm.tiles_per_split = (prm.total_tiles + ksplit - 1) / ksplit;
-  ksplit = (prm.total_tiles + prm.tiles_per_split - 1) / prm.tiles_per_split;
+  const int ksplit = wgrad_halo64_splits(prm.total_tiles, prm.tiles_n, num_sms(), &prm.tiles_per_split);
+  if (PARTIAL) check_workspace("conv3x3_wgrad_partial", dw, ws_elems, ksplit, static_cast<long long>(Cout) * 9 * 64);
   prm.num_items = prm.tiles_n * ksplit;
   prm.Cout = Cout; prm.dW = dw; prm.scale = scale;
   map_nhwc(&prm.mapX, x, N, H, W, 64, WH_PITCH, WH_PITCH, 1);
   map_nhwc(&prm.mapZ, dz, N, H, W, Cout, WH_T, WH_T, 1);
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_halo64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WH_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_halo64_kernel<PARTIAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, WH_SMEM);
     if (e != cudaSuccess)
       throw std::runtime_error(std::string("[b200] cudaFuncSetAttribute(wgrad halo): ") + cudaGetErrorString(e));
     configured = true;
   }
   dim3 grid(prm.num_items < num_sms() ? prm.num_items : num_sms());
-  wgrad_halo64_kernel<<<grid, WH_THREADS, WH_SMEM, stream>>>(prm);
+  wgrad_halo64_kernel<PARTIAL><<<grid, WH_THREADS, WH_SMEM, stream>>>(prm);
   count_launch();
   check_last("wgrad_halo64_kernel launch");
+  return ksplit;
 }
 
-void conv3x3_wgrad(const bf16* dz, const bf16* x, float* dw, int N, int H, int W, int Cin,
-                   int Cout, float scale, int ksplit, int bn, cudaStream_t stream) {
-  check_channels(Cin, "conv3x3_wgrad Cin");
-  check_channels(Cout, "conv3x3_wgrad Cout");
-  if (Cin == 64 && H % WH_T == 0 && W % WH_T == 0 && W >= 16 && halo_enabled() && bn == 0 && ksplit <= 0) {
-    wgrad_halo64_launch(dz, x, dw, N, H, W, Cout, scale, stream);
-    return;
+// Pixel-tile splits of the generic wgrad when every split stores a slice of partials that a second
+// kernel adds up.  A slice costs a write and a read of Cout*9*Cin floats, so the 4096-pixel work
+// items of the atomic path (196 splits, 115 MB of partials at 128 -> 128 channels, 112^2, batch 64)
+// are too fine.  Of the counts that give at most ~4 work items per SM, take the one with the least
+// modelled time: waves over the SMs x k-blocks per item, plus the slices' traffic in the same unit
+// (WS_ELEMS_PER_KBLOCK floats written and read back in the time one SM takes for a k-block:
+// ~0.5 us against ~2.5 TB/s; a model, see DESIGN 2.9 for what was measured).  Ties: fewer splits.
+constexpr long long WS_ELEMS_PER_KBLOCK = 160000;
+static int wgrad_partial_ksplit(int total_tiles, int base, long long slice_elems, int sms) {
+  int kmax = (4 * sms + base - 1) / base;
+  if (kmax > total_tiles) kmax = total_tiles;
+  int best = 1;
+  long long best_cost = -1;
+  for (int k = 1; k <= kmax; ++k) {
+    const long long waves = (static_cast<long long>(base) * k + sms - 1) / sms;
+    const long long depth = (total_tiles + k - 1) / k;
+    const long long cost = waves * depth * WS_ELEMS_PER_KBLOCK + k * slice_elems;
+    if (best_cost < 0 || cost < best_cost) { best = k; best_cost = cost; }
   }
-  WgradParams prm;
+  return best;
+}
+
+// Pixel tiles and split of the generic wgrad.  ksplit <= 0: chosen here.
+static void wgrad_split(WgradParams& prm, int N, int H, int W, int Cin, int Cout, int ksplit, int bn, int sms,
+                        bool partial) {
   prm.t = make_tile(N, H, W, 64);
   const int tiles_n = (N + prm.t.Nb - 1) / prm.t.Nb;
   prm.Cout = Cout; prm.Cin = Cin;
@@ -480,13 +571,40 @@ void conv3x3_wgrad(const bf16* dz, const bf16* x, float* dw, int N, int H, int W
   const int split_bn = bn ? bn : (Cin <= 64 ? 64 : 128);
   if (ksplit <= 0) {     // work items of <= ~64 k-blocks (4096 pixels), and at least ~4 per SM
     const int base = ((Cout + UMMA_BM - 1) / UMMA_BM) * ((Cin + split_bn - 1) / split_bn) * 9;
-    ksplit = (prm.total_tiles + 63) / 64;
-    const int min_split = (4 * num_sms() + base - 1) / base;
-    if (ksplit < min_split) ksplit = min_split;
+    if (partial) {
+      ksplit = wgrad_partial_ksplit(prm.total_tiles, base, static_cast<long long>(Cout) * 9 * Cin, sms);
+    } else {
+      ksplit = (prm.total_tiles + 63) / 64;
+      const int min_split = (4 * sms + base - 1) / base;
+      if (ksplit < min_split) ksplit = min_split;
+    }
   }
   if (ksplit > prm.total_tiles) ksplit = prm.total_tiles;
   prm.tiles_per_split = (prm.total_tiles + ksplit - 1) / ksplit;
   prm.ksplit = (prm.total_tiles + prm.tiles_per_split - 1) / prm.tiles_per_split;
+}
+
+int conv_wgrad_splits(int N, int H, int W, int Cin, int Cout, int sms) {
+  if (wgrad_halo64_applicable(H, W, Cin)) {
+    int per_split;
+    return wgrad_halo64_splits(N * (W / WH_T) * (H / WH_T), (Cout + 63) / 64, sms, &per_split);
+  }
+  WgradParams prm;
+  wgrad_split(prm, N, H, W, Cin, Cout, 0, 0, sms, true);
+  return prm.ksplit;
+}
+
+static int wgrad_impl(const bf16* dz, const bf16* x, float* dw, long long ws_elems, bool partial, int N, int H,
+                      int W, int Cin, int Cout, float scale, int ksplit, int bn, cudaStream_t stream) {
+  check_channels(Cin, "conv3x3_wgrad Cin");
+  check_channels(Cout, "conv3x3_wgrad Cout");
+  if (wgrad_halo64_applicable(H, W, Cin) && bn == 0 && ksplit <= 0) {
+    if (partial) return wgrad_halo64_launch<true>(dz, x, dw, ws_elems, N, H, W, Cout, scale, stream);
+    return wgrad_halo64_launch(dz, x, dw, 0, N, H, W, Cout, scale, stream);
+  }
+  WgradParams prm;
+  wgrad_split(prm, N, H, W, Cin, Cout, ksplit, bn, num_sms(), partial);
+  if (partial) check_workspace("conv3x3_wgrad_partial", dw, ws_elems, prm.ksplit, static_cast<long long>(Cout) * 9 * Cin);
   if (bn == 0) {
     const long long items = static_cast<long long>((Cout + UMMA_BM - 1) / UMMA_BM) * 9 * prm.ksplit;
     bn = conv_bn(Cin, items * ((Cin + 127) / 128), items * ((Cin + 255) / 256));
@@ -495,11 +613,21 @@ void conv3x3_wgrad(const bf16* dz, const bf16* x, float* dw, int N, int H, int W
   map_nhwc(&prm.mapA, dz, N, H, W, Cout, prm.t.Wb, prm.t.Hb, prm.t.Nb);
   map_nhwc(&prm.mapB, x, N, H, W, Cin, prm.t.Wb, prm.t.Hb, prm.t.Nb);
   switch (bn) {
-    case 64: wgrad_launch<64>(prm, stream); break;
-    case 128: wgrad_launch<128>(prm, stream); break;
-    case 256: wgrad_launch<256>(prm, stream); break;
+    case 64: partial ? wgrad_launch<64, true>(prm, stream) : wgrad_launch<64>(prm, stream); break;
+    case 128: partial ? wgrad_launch<128, true>(prm, stream) : wgrad_launch<128>(prm, stream); break;
+    case 256: partial ? wgrad_launch<256, true>(prm, stream) : wgrad_launch<256>(prm, stream); break;
     default: throw std::runtime_error("[b200] conv3x3_wgrad: bn must be 64, 128 or 256");
   }
+  return prm.ksplit;
+}
+
+void conv3x3_wgrad(const bf16* dz, const bf16* x, float* dw, int N, int H, int W, int Cin,
+                   int Cout, float scale, int ksplit, int bn, cudaStream_t stream) {
+  wgrad_impl(dz, x, dw, 0, false, N, H, W, Cin, Cout, scale, ksplit, bn, stream);
+}
+int conv3x3_wgrad_partial(const bf16* dz, const bf16* x, float* ws, long long ws_elems, int N, int H, int W,
+                          int Cin, int Cout, float scale, cudaStream_t stream) {
+  return wgrad_impl(dz, x, ws, ws_elems, true, N, H, W, Cin, Cout, scale, 0, 0, stream);
 }
 
 }  // namespace b200

@@ -111,6 +111,11 @@ def build_parser() -> argparse.ArgumentParser:
     ext.add_argument("--save", default=None, help="checkpoint path written by rank 0 every epoch")
     ext.add_argument("--resume", default=None, help="checkpoint path to resume from")
     ext.add_argument("--seed", type=int, default=0)
+    ext.add_argument("--deterministic", action="store_true",
+                     help="bit-reproducible training: two runs of the same command on the same GPU model, world size "
+                          "and build give identical weights, optimizer state and losses.  Native engine: split-K and "
+                          "column sums are reduced in a fixed order instead of with fp32 atomics (slightly slower; "
+                          "refuses --allreduce nvls).  Torch-op engine: torch.use_deterministic_algorithms(True)")
     ext.add_argument("--synthetic", type=int, default=0,
                      help="generate a synthetic ImageFolder with this many train images per class "
                           "under --root_dir if it does not exist")

@@ -44,6 +44,49 @@ def _round_up(x: int, m: int) -> int:
     return (x + m - 1) // m * m
 
 
+def fc_ksplit(m_tiles: int, k_iters: int, target: int = 256) -> int:
+    """Split-K factor the engine asks of a swap-AB FC GEMM (forward and dgrad)."""
+    return max(1, min(k_iters, target // max(m_tiles, 1)))
+
+
+def deterministic_plan(spec: VGGSpec, batch: int, input_hw: int, sms: int, fused_head: bool = True) -> list:
+    """The split-K launches of one deterministic training step, as [(layer, what, splits, elements per
+    slice)]: what the workspace has to hold (``deterministic_workspace_elems``) and what ``tools.plan
+    --deterministic`` prints.  The split counts are the launchers' own arithmetic (the extension's
+    ``*_splits`` queries: pure host code), for ``sms`` SMs."""
+    C = ops.require()
+    rows, fcs, convs = [], spec.fcs, spec.convs
+    last = len(fcs) - 1
+    for i, f in enumerate(fcs):
+        if i == last and fused_head:
+            continue
+        ks = fc_ksplit((f.fout + 127) // 128, (f.fin + 63) // 64)
+        rows.append((f.name, "fprop", C.gemm_splits(f.fin, ks), C.workspace_slice(batch * f.fout)))
+        if f.fout % 8 == 0:
+            rows.append((f.name, "bias", C.colsum_partial_blocks(batch, f.fout, sms), f.fout))
+        ks = fc_ksplit((f.fin + 127) // 128, (f.fout + 63) // 64)
+        if ks > 1:
+            rows.append((f.name, "dgrad", C.gemm_splits(f.fout, ks), C.workspace_slice(batch * f.fin)))
+    h = input_hw
+    for i, c in enumerate(convs):
+        rows.append((c.name, "bias", C.colsum_partial_blocks(batch * h * h, c.cout, sms), c.cout))
+        if i == 0 and c.cout == 64:
+            rows.append((c.name, "wgrad", C.conv0_wgrad_splits(batch, h, h, sms), 64 * 64))
+        elif i == 0:
+            M = batch * h * h
+            rows.append((c.name, "wgrad", C.gemm_splits(M, max(1, min(M // 64, 296))),
+                         C.workspace_slice(c.cout * L.CONV0_K)))
+        else:
+            rows.append((c.name, "wgrad", C.conv_wgrad_splits(batch, h, h, c.cin, c.cout, sms), c.cout * 9 * c.cin))
+        if c.pool_after:
+            h //= 2
+    return rows
+
+
+def deterministic_workspace_elems(plan: list) -> int:
+    return max(splits * elems for _, _, splits, elems in plan)
+
+
 class PhaseTimer:
     """CUDA-event timers around the phases of a step (``--profile events``)."""
 
@@ -90,7 +133,7 @@ class NativeEngine:
                  distributed: bool = True, zero1="auto", conv_bucket_mb: float = 9.5,
                  tail_bucket_kb: float = 2400.0, same_dropout_all_ranks: bool = False,
                  label_smoothing: float = 0.0, ema_decay: Optional[float] = None,
-                 bias_weight_decay: Optional[float] = None) -> None:
+                 bias_weight_decay: Optional[float] = None, deterministic: bool = False) -> None:
         ops.require()
         if compute_dtype != "bf16":
             raise NotImplementedError("the native engine computes in bf16 with fp32 master weights; "
@@ -138,6 +181,13 @@ class NativeEngine:
         self.nvtx = profile == "nvtx"
         self.world = dist.get_world_size() if (distributed and distributed_is_initialized()) else 1
         self.rank = dist.get_rank() if (distributed and distributed_is_initialized()) else 0
+        # Same inputs, same bits: every split-K and column sum stores per-split partials into one workspace
+        # and adds them in split order (DESIGN 2.9) instead of letting fp32 atomics arrive in any order.
+        self.deterministic = bool(deterministic)
+        self._ws: Optional[torch.Tensor] = None      # the split-K workspace, allocated by _build_buffers
+        if self.deterministic and allreduce == "nvls":
+            raise ValueError("--deterministic: --allreduce nvls leaves the summation order to the NVLink switch; "
+                             "use auto, oneshot or twoshot (they add the ranks in a fixed order)")
         self.ar_algo, self.comm_ctas, self.unpack_fp32 = allreduce, comm_ctas, unpack_fp32
         self.use_nccl = allreduce == "nccl"
         dev = self.device
@@ -320,6 +370,8 @@ class NativeEngine:
 
     def export_optimizer_state(self) -> dict:
         st = {"name": self.opt_name, "step": self.step_count, "micro_step": self.micro_count, "lr": self.lr}
+        if getattr(self, "deterministic", False):     # key absent without the flag: the parent's checkpoint
+            st["deterministic"] = True
         if self.opt_name in ("adam", "adamw"):
             st["exp_avg"] = {n: L.to_torch(self.spec, n, self._view(self.m32, n)).cpu() for n in self.spec.param_names}
             st["exp_avg_sq"] = {n: L.to_torch(self.spec, n, self._view(self.v32, n)).cpu() for n in self.spec.param_names}
@@ -330,6 +382,10 @@ class NativeEngine:
 
     def import_optimizer_state(self, st: dict) -> None:
         self.step_count = int(st.get("step", 0))
+        if "name" in st and bool(st.get("deterministic", False)) != getattr(self, "deterministic", False):
+            print("[Warn] the checkpoint was written %s --deterministic, this run is %s it: the run continues, "
+                  "but not bit for bit as the one that wrote it would have" %
+                  (("with", "without") if st.get("deterministic") else ("without", "with")), flush=True)
         self.micro_count = int(st.get("micro_step", self.step_count))    # one micro-batch per update before
         if "lr" in st:                       # a run resumed behind an LR-step boundary keeps the decayed rate
             self.lr = float(st["lr"])
@@ -442,6 +498,10 @@ class NativeEngine:
         biggest = max(a.numel() for a in self.acts)
         self.dbuf = [torch.empty(biggest, dtype=BF16, device=dev) for _ in range(2)]
         self.dfeat = torch.empty(B, ph, ph, cl, dtype=BF16, device=dev)
+        if self.deterministic:
+            # one workspace for every split-K launch of the step: they all run on the compute stream
+            plan = deterministic_plan(spec, B, HW, ops.require().sm_count(), self.fused_head)
+            self._ws = torch.empty(deterministic_workspace_elems(plan), dtype=F32, device=dev)
 
     # ================================================================================ inputs
     def _stage_input(self, batch) -> int:
@@ -539,9 +599,7 @@ class NativeEngine:
         r = 0 if self.same_dropout_all_ranks else self.rank
         return self.seed * 1000003 + layer + 7919 * r
 
-    @staticmethod
-    def _ksplit(m_tiles: int, k_iters: int, target: int = 256) -> int:
-        return max(1, min(k_iters, target // max(m_tiles, 1)))
+    _ksplit = staticmethod(fc_ksplit)
 
     def _forward(self, b: int, train: bool) -> None:
         C = ops.require()
@@ -581,7 +639,10 @@ class NativeEngine:
             m_tiles = (f.fout + 127) // 128
             ks = self._ksplit(m_tiles, (f.fin + 63) // 64)
             acc = self.fc_acc[i][:b]
-            ops.gemm(self._w(f.name), h, acc, M=f.fout, N=b, K=f.fin, epi="f32_atomic_t", ksplit=ks, ldo=f.fout)
+            if self.deterministic:
+                ops.gemm_det(self._w(f.name), h, acc, self._ws, M=f.fout, N=b, K=f.fin, transposed=True, ksplit=ks)
+            else:
+                ops.gemm(self._w(f.name), h, acc, M=f.fout, N=b, K=f.fin, epi="f32_atomic_t", ksplit=ks, ldo=f.fout)
             if i == last:
                 ops.fc_bias_act(acc, self._b(f.name), None, self.logits[:b], B=b, N=f.fout, relu=False)
             else:
@@ -625,8 +686,19 @@ class NativeEngine:
     def _grad(self, name: str) -> torch.Tensor:
         return self._view(self.g32, name)
 
+    def _bias_grad(self, dz2d: torch.Tensor, name: str, rows: int, C: int, ld: Optional[int] = None) -> None:
+        """Bias gradient of layer ``name`` from its dz.  Deterministic: per-block column sums added in block
+        order; a width the vector kernel does not take goes to the one-thread-per-channel kernel, which
+        adds each element once per launch in row order (reproducible as it is)."""
+        db = self._grad(name + ".bias")
+        if self.deterministic and C % 8 == 0 and ld in (None, C):
+            ops.colsum_det(dz2d, db, self._ws, rows, C, accumulate=True)     # db: zeroed by the optimizer
+        else:
+            ops.bias_grad(dz2d, db, rows, C, ld=ld)
+
     def _backward(self, b: int) -> None:
         C = ops.require()
+        det, acc_g = self.deterministic, bool(self._accum)
         spec = self.spec
         fcs, convs = spec.fcs, spec.convs
         last = len(fcs) - 1
@@ -641,7 +713,7 @@ class NativeEngine:
             ld = self.fc_dz[i].shape[1]
             dz = self.fc_dz[i][:b]                                   # [b][ld] bf16, cols >= fout are 0
             x_in = self.fc_y[i - 1][:b] if i > 0 else self.feat.reshape(b, -1)
-            ops.bias_grad(dz, self._grad(f.name + ".bias"), b, f.fout, ld=ld)
+            self._bias_grad(dz, f.name, b, f.fout, ld=ld)
             self._bucket_done(f.name + ".bias")
             # wgrad: dW[fout][fin] = dz^T x_in   (both operands MN-major: stored [K=b][*])
             if self._wire_direct and (f.name + ".weight") in self._prepacked:
@@ -653,15 +725,20 @@ class NativeEngine:
                          ldo=f.fin, alpha=1.0 / self.world)
             else:
                 # the first micro-batch of a group stores, later ones add (ksplit 1: each tile owns its
-                # elements, so the red.add epilogue adds every element exactly once)
+                # elements, so the red.add epilogue adds every element exactly once -- which is why the FC
+                # wgrads, this one and the bf16 one above, are the same launches under `deterministic`)
                 ops.gemm(dz, x_in, self._grad(f.name + ".weight"), M=f.fout, N=f.fin, K=b, a_mn=True,
                          b_mn=True, epi="f32_atomic" if self._accum else "f32_store", ldo=f.fin)
             # dgrad: dX[b][fin] = dz W ; swap-AB with W read MN-major (stored [K=fout][M=fin])
             m_tiles = (f.fin + 127) // 128
             ks = self._ksplit(m_tiles, (f.fout + 63) // 64)
             dacc = self.fc_dacc[i][:b]
-            ops.gemm(self._w(f.name), dz, dacc, M=f.fin, N=b, K=f.fout, a_mn=True,
-                     epi="f32_atomic_t" if ks > 1 else "f32_store_t", ksplit=ks, ldo=f.fin)
+            if det and ks > 1:
+                ops.gemm_det(self._w(f.name), dz, dacc, self._ws, M=f.fin, N=b, K=f.fout, a_mn=True, transposed=True,
+                             ksplit=ks)
+            else:
+                ops.gemm(self._w(f.name), dz, dacc, M=f.fin, N=b, K=f.fout, a_mn=True,
+                         epi="f32_atomic_t" if ks > 1 else "f32_store_t", ksplit=ks, ldo=f.fin)
             # only now may the optimizer touch W_i: the dgrad above still reads the old weights
             self._bucket_done(f.name + ".weight")
             if i > 0:
@@ -688,21 +765,29 @@ class NativeEngine:
             if c.pool_after:
                 dz = self.dbuf[pp][:y.numel()].view_as(y)
                 # ReLU + pool backward, bias gradient (column sum of dz) fused
+                # (deterministic: no fused column sum, its atomics arrive in any order; _bias_grad below)
+                colsum = None if det else self._grad(c.name + ".bias")
                 if self.pool_masks[i] is not None:
-                    ops.unpool2x2(g, self.pool_masks[i][:b], out=dz, colsum=self._grad(c.name + ".bias"))
+                    ops.unpool2x2(g, self.pool_masks[i][:b], out=dz, colsum=colsum)
                 else:
-                    ops.maxpool2x2_relu_bwd(y, g, out=dz, colsum=self._grad(c.name + ".bias"))
+                    ops.maxpool2x2_relu_bwd(y, g, out=dz, colsum=colsum)
                 pp ^= 1
-                bias_fused = True
+                bias_fused = not det
             else:
                 dz = g
             M = y.numel() // c.cout
             if not bias_fused:
-                ops.bias_grad(dz.view(M, c.cout), self._grad(c.name + ".bias"), M, c.cout)
+                self._bias_grad(dz.view(M, c.cout), c.name, M, c.cout)
             self._bucket_done(c.name + ".bias")
             if i == 0:
-                if self.fused_conv0:
+                if self.fused_conv0 and det:
+                    ops.conv0_wgrad_det(dz, self.x_nhwc[:b], self._grad(c.name + ".weight"), self._ws, accumulate=acc_g)
+                elif self.fused_conv0:
                     C.conv0_wgrad(dz, self.x_nhwc[:b], self._grad(c.name + ".weight"))
+                elif det:
+                    ops.gemm_det(dz.view(M, c.cout), self.col0[:M], self._grad(c.name + ".weight"), self._ws, M=c.cout,
+                                 N=L.CONV0_K, K=M, a_mn=True, b_mn=True, ksplit=max(1, min(M // 64, 296)),
+                                 accumulate=acc_g)
                 else:
                     ks = max(1, min(M // 64, 296))
                     ops.gemm(dz.view(M, c.cout), self.col0[:M], self._grad(c.name + ".weight"), M=c.cout,
@@ -712,14 +797,17 @@ class NativeEngine:
                 break
             prev = convs[i - 1]
             x_in = self.pools[i - 1][:b] if prev.pool_after else self.acts[i - 1][:b]
-            C.conv_wgrad(dz, x_in, self._grad(c.name + ".weight"), 1.0, 0, 0)
+            if det:
+                ops.conv3x3_wgrad_det(dz, x_in, self._grad(c.name + ".weight"), self._ws, accumulate=acc_g)
+            else:
+                C.conv_wgrad(dz, x_in, self._grad(c.name + ".weight"), 1.0, 0, 0)
             dx = self.dbuf[pp][:x_in.numel()].view_as(x_in)
             # ReLU backward of layer i-1 is fused here unless a pool sits in between; when it is,
             # dx IS dZ_{i-1} and its column sum (layer i-1's bias gradient) comes for free
             fuse = not prev.pool_after
             C.conv_dgrad(dz, self._w(c.name), x_in if fuse else None, dx,
-                         self._grad(prev.name + ".bias") if fuse else None, 0)
-            bias_fused = fuse
+                         self._grad(prev.name + ".bias") if fuse and not det else None, 0)
+            bias_fused = fuse and not det
             self._bucket_done(c.name + ".weight")      # after dgrad: it reads the pre-update weights
             self._mark("bwd " + c.name)
             pp ^= 1
@@ -800,6 +888,8 @@ class NativeEngine:
                     self._apply_update(s, e, None)
                 return
             algo = self.arena.pick_algo(e - s, self.ar_algo)
+            if self.deterministic and algo == "nvls":        # auto may pick it: the two-shot adds in rank order
+                algo = "twoshot"
             prepacked = self._wire_direct and self._bucket_prepacked[bi]
             if self._bucket_prepacked[bi] and algo == "oneshot":
                 algo = "twoshot"                 # one-shot cannot leave its result on the wire

@@ -103,6 +103,53 @@ def conv3x3_wgrad(dz, x, dw, scale: float = 1.0, ksplit: int = 0, bn: int = 0):
     return dw
 
 
+# --------------------------------------------------------- split-K without atomics (--deterministic)
+# Each function runs the PARTIAL form of a split-K kernel (every split stores its own slice of the
+# workspace ``ws``, a flat fp32 tensor) and then ``splitk_reduce``, which adds the slices in split
+# order: the result is a function of the operands alone, not of the order the CTAs finish in.
+def splitk_reduce(ws, dst, n: int, splits: int, *, slice_elems: Optional[int] = None, alpha: float = 1.0,
+                  accumulate: bool = False):
+    """dst[:n] = (dst[:n] if accumulate else 0) + alpha * (((ws[0] + ws[1]) + ws[2]) + ...), slices
+    ``slice_elems`` apart (default: n rounded up to whole float4s), each operation rounded to fp32."""
+    C = require()
+    C.splitk_reduce(ws, dst, n, C.workspace_slice(n) if slice_elems is None else slice_elems, splits, alpha,
+                    accumulate)
+
+
+def gemm_det(a, b, out, ws, *, M: int, N: int, K: int, a_mn: bool = False, b_mn: bool = False,
+             transposed: bool = False, alpha: float = 1.0, ksplit: int = 1, bn: int = 0,
+             accumulate: bool = False) -> int:
+    """``gemm`` with epi f32_atomic (f32_atomic_t when ``transposed``) and split-K, reproducibly: ``out``
+    is dense ([M][N], transposed [N][M]) and is overwritten unless ``accumulate``.  Returns the splits."""
+    n = M * N
+    splits = int(require().gemm_partial(a, a_mn, b, b_mn, M, N, K, ws, M if transposed else N, transposed, alpha,
+                                        ksplit, bn))
+    splitk_reduce(ws, out, n, splits, accumulate=accumulate)
+    return splits
+
+
+def conv3x3_wgrad_det(dz, x, dw, ws, scale: float = 1.0, accumulate: bool = False) -> int:
+    """dw (fp32 [Cout][3][3][Cin]) = (dw if accumulate else 0) + scale * dz^T (*) x, reproducibly."""
+    splits = int(require().conv_wgrad_partial(dz, x, ws, scale))
+    splitk_reduce(ws, dw, dw.numel(), splits, accumulate=accumulate)
+    return splits
+
+
+def conv0_wgrad_det(dz, x4, dw0, ws, accumulate: bool = False) -> int:
+    """Layer-0 weight gradient (``conv0_wgrad``), reproducibly."""
+    splits = int(require().conv0_wgrad_partial(dz, x4, ws))
+    splitk_reduce(ws, dw0, 64 * 64, splits, accumulate=accumulate)
+    return splits
+
+
+def colsum_det(dz2d, db, ws, rows: int, C: int, scale: float = 1.0, accumulate: bool = False) -> int:
+    """db[:C] = (db if accumulate else 0) + scale * dz2d[:rows].sum(0) with C % 8 == 0: ``bias_grad``'s
+    per-block sums stored as rows of ``ws`` and added in block order."""
+    blocks = int(require().colsum_partial(dz2d, ws, rows, C, scale))
+    splitk_reduce(ws, db, C, blocks, slice_elems=C, accumulate=accumulate)
+    return blocks
+
+
 # ---------------------------------------------------------------------------------- element-wise
 def maxpool2x2(x, out=None):
     N, H, W, Cc = x.shape

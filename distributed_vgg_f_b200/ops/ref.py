@@ -610,3 +610,30 @@ def nchw_to_nhwc64(x: torch.Tensor, cpad: int):
     y = torch.zeros(N, H, W, cpad, dtype=torch.float64, device=x.device)
     y[..., :C] = _f64(x).permute(0, 2, 3, 1)
     return y, y.abs()
+
+
+# ------------------------------------------------------------------ split-K without atomics
+def splitk_reduce64(slices: torch.Tensor, dst=None, alpha: float = 1.0):
+    """splitk_reduce in float64: (dst or 0) + alpha * sum over slices [splits, n].  Returns (ref, err)
+    with err the fp32 rounding of the kernel's splits - 1 ordered adds, its product and its final add."""
+    s64 = _f64(slices)
+    tot = s64.sum(0)
+    mag = s64.abs().sum(0)
+    r = _f32(alpha) * tot
+    err = _U * abs(_f32(alpha)) * mag * slices.shape[0]
+    if dst is not None:
+        r = r + _f64(dst)
+        err = err + _U * r.abs()
+    return r, err
+
+
+def splitk_reduce_ordered(slices: torch.Tensor, dst=None, alpha: float = 1.0) -> torch.Tensor:
+    """splitk_reduce bit for bit: fp32 adds in slice order, one rounded product by fp32(alpha), one
+    rounded add onto dst.  (fp32 tensor arithmetic on the CPU rounds every operation: no FMA.)"""
+    acc = slices[0].to("cpu", torch.float32).clone()
+    for k in range(1, slices.shape[0]):
+        acc = acc + slices[k].to("cpu", torch.float32)
+    acc = acc * torch.tensor(alpha, dtype=torch.float32)
+    if dst is not None:
+        acc = dst.to("cpu", torch.float32) + acc
+    return acc

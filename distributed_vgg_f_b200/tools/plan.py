@@ -44,6 +44,28 @@ def describe(model: str = "vggf", num_classes: int = 3, world: int = 8, multicas
     return plan, rows
 
 
+def deterministic(model: str, num_classes: int, batch: int, input_hw: int, sms: int) -> int:
+    """Split count and partial-sum bytes of every split-K launch of a --deterministic step, from the
+    launchers' own host arithmetic: needs the built extension, not a GPU."""
+    from .. import ops
+    if not ops.available():
+        print("tools.plan --deterministic asks the native extension for its split counts: build it first "
+              "(python build_native.py)")
+        return 1
+    from ..engine.native_engine import deterministic_plan, deterministic_workspace_elems
+    spec = get_spec(model, num_classes)
+    last = spec.fcs[-1]
+    fused_head = len(spec.fcs) >= 2 and bool(ops.require().head_ce_supported(batch, last.fout, last.fin))
+    rows = deterministic_plan(spec, batch, input_hw, sms, fused_head)
+    print("%s, %d classes, batch %d, %d x %d, %d SMs: workspace %.1f MB, %.1f MB of partial sums written and read per step"
+          % (model, num_classes, batch, input_hw, input_hw, sms, deterministic_workspace_elems(rows) * 4 / 1e6,
+             sum(s * e for _, _, s, e in rows) * 4 / 1e6))
+    print("%-16s %-6s %7s %12s %10s" % ("layer", "what", "splits", "slice elems", "MB"))
+    for name, what, splits, elems in rows:
+        print("%-16s %-6s %7d %12d %10.2f" % (name, what, splits, elems, splits * elems * 4 / 1e6))
+    return 0
+
+
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--model", default="vggf")
@@ -52,7 +74,14 @@ def main(argv=None) -> int:
     ap.add_argument("--no-multicast", action="store_true", help="plan for a fabric without NVLS")
     ap.add_argument("--zero1", default="auto", choices=["auto", "on", "off"])
     ap.add_argument("--bucket-mb", type=float, default=32.0)
+    ap.add_argument("--deterministic", action="store_true",
+                    help="print the split-K launches of a --deterministic step and the workspace they need, instead")
+    ap.add_argument("--batch", type=int, default=64, help="--deterministic: mini-batch per GPU")
+    ap.add_argument("--input-hw", type=int, default=224, help="--deterministic: input side")
+    ap.add_argument("--sms", type=int, default=132, help="--deterministic: SMs of the GPU planned for (H100 SXM: 132)")
     a = ap.parse_args(argv)
+    if a.deterministic:
+        return deterministic(a.model, a.num_classes, a.batch, a.input_hw, a.sms)
     plan, rows = describe(a.model, a.num_classes, a.world, not a.no_multicast, a.zero1, a.bucket_mb)
     total = sum(r[2] for r in rows)
     print("%s, %d classes: %d elements (native layouts) in %d tensors, arena %d elements (tensors aligned to %d), %d buckets, %.1f MB of bf16 wire per step"

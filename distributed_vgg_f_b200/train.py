@@ -150,12 +150,17 @@ def manage_training(args) -> Trainer:
                              zero1={"auto": "auto", "on": True, "off": False}[getattr(args, "zero1", "auto")],
                              label_smoothing=getattr(args, "label_smoothing", 0.0), ema_decay=ema_decay,
                              weight_decay=getattr(args, "weight_decay", 0.0),
-                             bias_weight_decay=getattr(args, "bias_weight_decay", None))
+                             bias_weight_decay=getattr(args, "bias_weight_decay", None),
+                             deterministic=getattr(args, "deterministic", False))
         optimizer = None            # fused into the engine
         model_ema = True if ema_decay is not None else None       # kept by the engine's optimizer kernels
         if model.world > 1:
             model.comm_timing(True)   # [Perf] line: all-reduce GB/s and fraction of the NVLink rate per epoch
     else:
+        if getattr(args, "deterministic", False):
+            torch.use_deterministic_algorithms(True)
+            # dropout draws from the global generator, which nothing else seeds (each rank its own masks)
+            torch.manual_seed(args.seed * 1000003 + args.rank)
         model = build_oracle(spec, seed=args.seed, pretrained_state=pretrained).to(device)
         if distributed_is_initialized():
             model = FlatDDP(model, bucket_cap_mb=args.bucket_mb)
