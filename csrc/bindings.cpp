@@ -411,6 +411,12 @@ static void sgd(at::Tensor p, at::Tensor mom, c10::optional<at::Tensor> g32, c10
                   p.numel(), (float)lr, (float)momentum, segs, first, (float)grad_scale, f32p_opt(gzero),
                   cur_stream(), f32p_opt(ema), ema_decay, ema_first);
 }
+static void ema_update(const at::Tensor& p, at::Tensor ema, double decay, bool first) {
+  c10::cuda::CUDAGuard g(p.device());
+  check_vec(p, at::kFloat, 16, "ema_update", "p");
+  check_ema(ema, p.numel(), decay, "ema_update");
+  b200::ema_fused(f32p(p), f32p(ema), p.numel(), decay, first, cur_stream());
+}
 
 static void check_augment(const at::Tensor& src, const at::Tensor& params, const at::Tensor& out, int64_t OH,
                           int64_t OW, int64_t mode, int64_t pad, const std::vector<double>& mean,
@@ -903,6 +909,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("momentum"), py::arg("wd"), py::arg("first"), py::arg("grad_scale"), py::arg("gzero"),
         py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0, py::arg("ema_first") = false,
         py::arg("wd_starts") = std::vector<int64_t>(), py::arg("wd_values") = std::vector<double>());
+  m.def("ema_update", &ema_update, py::arg("p"), py::arg("ema"), py::arg("decay"), py::arg("first"));
   m.def("augment", &augment);
   m.def("augment_mixed", &augment_mixed);
   m.def("augment_ragged", &augment_ragged);

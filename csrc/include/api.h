@@ -177,6 +177,10 @@ void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* sh
                float lr, float momentum, const WdSegments& wd, bool first_step, float grad_scale,
                float* g32_to_zero, cudaStream_t s, float* ema = nullptr, double ema_decay = 0.0,
                bool ema_first = false);
+// The EMA update of the optimizers alone, for weights no optimizer launch covers (frozen layers):
+// ema[i] = decay * ema[i] + (1 - decay) * p[i] with each operation rounded to fp32, or p[i] when `first`.
+// n elements, any n >= 0; p and ema 16-byte aligned.
+void ema_fused(const float* p, float* ema, long long n, double decay, bool first, cudaStream_t s);
 
 // Fused input transform: uint8 HWC source -> normalised bf16.  mode 0: NHWC with C padded to
 // `cpad`; mode 1: layer-0 im2col matrix [N*OH*OW][kpad] (k = (kh*3+kw)*3 + c, zero padded).

@@ -530,4 +530,41 @@ void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* sh
   check_last("sgd_fused");
 }
 
+// ------------------------------------------------------------------------- EMA without an update
+// The moving average of weights that no optimizer launch covers (--freeze-layers: the frozen suffix of
+// the arena, which AveragedModel still averages): ema_update of every element, the update and the
+// `first` rule of the optimizer kernels' EMA.  Same footprint as adam_kernel (256 threads, no shared
+// memory, evict-first streams, one grid-stride pass).  n need not be a multiple of 4: the last n % 4
+// elements go through thread 0 one by one.
+__global__ void __launch_bounds__(256, 6) ema_kernel(const float* __restrict__ p, float* __restrict__ ema, long long n,
+                                                      float d, float a, int first) {
+  const long long n4 = n / 4;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i);
+    const float pp[4] = {pv.x, pv.y, pv.z, pv.w};
+    ema_store4(ema, i, pp, d, a, first);
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0)
+    for (long long i = n4 * 4; i < n; ++i) ema[i] = ema_update(ema[i], p[i], d, a, first);
+}
+
+void ema_fused(const float* p, float* ema, long long n, double decay, bool first, cudaStream_t s) {
+  if (n <= 0) return;
+  static const bool carve = [] {
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(ema_kernel));
+    return true;
+  }();
+  (void)carve;
+  // The grid cap of the optimizer launches it shares the side stream with (adam_fused's default of 4 CTAs per
+  // SM, B200_ADAM_CTAS_PER_SM, and sgd_fused's fixed 4), so that it competes with the conv kernels no more
+  // than they do.  It runs once per EMA step; its cost in the step is measured by bench/freeze_bench.py.
+  const long long cap = static_cast<long long>(sm_count()) * 4;
+  const int blocks = static_cast<int>(n / 1024 + 1 < cap ? n / 1024 + 1 : cap);
+  ema_kernel<<<blocks, 256, 0, s>>>(p, ema, n, static_cast<float>(decay), static_cast<float>(1.0 - decay),
+                                    first ? 1 : 0);
+  count_launch();
+  check_last("ema_fused");
+}
+
 }  // namespace b200

@@ -156,6 +156,12 @@ def build_parser() -> argparse.ArgumentParser:
                           "every epoch after the raw weights and save it in the checkpoint")
     ext.add_argument("--model-ema-steps", type=int, default=32,
                      help="update the EMA after every N-th optimizer update of an epoch, from its first (default 32)")
+    ext.add_argument("--freeze-layers", type=int, default=0,
+                     help="fine-tune with the first N layers of the model frozen (convolutions, then Linears; VGG-F: "
+                          "13 = all of features, 16 = only the last Linear trains), 0 <= N < number of layers.  "
+                          "Frozen layers run forward in train mode and get no gradient, no exchange, no optimizer "
+                          "state and no weight decay (torch's requires_grad_(False)); the EMA still averages them "
+                          "(default 0 = everything trains)")
     ext.add_argument("--model-ema-decay", type=float, default=0.99998,
                      help="EMA decay per image seen, 0 <= d < 1; the decay of one update is adjusted as torchvision "
                           "does: 1 - min(1, (1 - d) * world * mini_batch * accum_steps * model_ema_steps / epochs)")
@@ -187,6 +193,12 @@ def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
         build_parser().error("--lr-warmup-decay must lie in (0, 1]")
     if not args.lr_min >= 0.0:
         build_parser().error("--lr-min must be >= 0")
+    if args.freeze_layers:
+        from .models.vggf import get_spec
+        try:
+            get_spec(args.model, args.num_classes or 3).check_freeze_layers(args.freeze_layers)
+        except ValueError as e:
+            build_parser().error("%s (%s)" % (e, args.model))
     print(args)
     if args.socket_ifname:
         os.environ["GLOO_SOCKET_IFNAME"] = args.socket_ifname

@@ -49,26 +49,33 @@ def fc_ksplit(m_tiles: int, k_iters: int, target: int = 256) -> int:
     return max(1, min(k_iters, target // max(m_tiles, 1)))
 
 
-def deterministic_plan(spec: VGGSpec, batch: int, input_hw: int, sms: int, fused_head: bool = True) -> list:
+def deterministic_plan(spec: VGGSpec, batch: int, input_hw: int, sms: int, fused_head: bool = True,
+                       freeze_layers: int = 0) -> list:
     """The split-K launches of one deterministic training step, as [(layer, what, splits, elements per
     slice)]: what the workspace has to hold (``deterministic_workspace_elems``) and what ``tools.plan
     --deterministic`` prints.  The split counts are the launchers' own arithmetic (the extension's
-    ``*_splits`` queries: pure host code), for ``sms`` SMs."""
+    ``*_splits`` queries: pure host code), for ``sms`` SMs.  ``freeze_layers``: the frozen layers keep their
+    forward launches only, and the first trainable layer has no dgrad."""
     C = ops.require()
     rows, fcs, convs = [], spec.fcs, spec.convs
     last = len(fcs) - 1
+    k = spec.check_freeze_layers(freeze_layers)
     for i, f in enumerate(fcs):
         if i == last and fused_head:
             continue
         ks = fc_ksplit((f.fout + 127) // 128, (f.fin + 63) // 64)
         rows.append((f.name, "fprop", C.gemm_splits(f.fin, ks), C.workspace_slice(batch * f.fout)))
-        if f.fout % 8 == 0:
+        if f.fout % 8 == 0 and len(convs) + i >= k:
             rows.append((f.name, "bias", C.colsum_partial_blocks(batch, f.fout, sms), f.fout))
         ks = fc_ksplit((f.fin + 127) // 128, (f.fout + 63) // 64)
-        if ks > 1:
+        if ks > 1 and len(convs) + i > k:
             rows.append((f.name, "dgrad", C.gemm_splits(f.fout, ks), C.workspace_slice(batch * f.fin)))
     h = input_hw
     for i, c in enumerate(convs):
+        if i < k:
+            if c.pool_after:
+                h //= 2
+            continue
         rows.append((c.name, "bias", C.colsum_partial_blocks(batch * h * h, c.cout, sms), c.cout))
         if i == 0 and c.cout == 64:
             rows.append((c.name, "wgrad", C.conv0_wgrad_splits(batch, h, h, sms), 64 * 64))
@@ -133,7 +140,8 @@ class NativeEngine:
                  distributed: bool = True, zero1="auto", conv_bucket_mb: float = 9.5,
                  tail_bucket_kb: float = 2400.0, same_dropout_all_ranks: bool = False,
                  label_smoothing: float = 0.0, ema_decay: Optional[float] = None,
-                 bias_weight_decay: Optional[float] = None, deterministic: bool = False) -> None:
+                 bias_weight_decay: Optional[float] = None, deterministic: bool = False,
+                 freeze_layers: int = 0) -> None:
         ops.require()
         if compute_dtype != "bf16":
             raise NotImplementedError("the native engine computes in bf16 with fp32 master weights; "
@@ -192,16 +200,27 @@ class NativeEngine:
         self.use_nccl = allreduce == "nccl"
         dev = self.device
 
+        # --freeze-layers: the first ``freeze_layers`` entries of the layer table (convs, then fcs) keep
+        # their weights, as torch with requires_grad_(False): forward as usual, no gradient, no exchange,
+        # no optimizer state; the EMA still averages them (_frozen_ema)
+        self.freeze_layers = spec.check_freeze_layers(freeze_layers)
+        self._frozen = set(spec.frozen_param_names(self.freeze_layers))
+
         # ---- flat arenas (gradient-ready order) --------------------------------------------------
         # FC weights (ready first, 88 % of the bytes): ``bucket_mb`` messages.  Convolution gradients
         # (ready one layer at a time over the rest of backward): one bucket per big layer, and a small
         # final bucket -- its reduction and update are the only exposed part of the exchange.
-        self.plan: BucketPlan = engine_bucket_plan(L.ready_order(spec), bucket_mb, conv_bucket_mb, tail_bucket_kb)
-        n = self.plan.total
+        # Frozen layers come last in ready order: the buckets, g32, the moments and the wire cover the
+        # trainable prefix [0, n_grad) alone; p32, w16 and the EMA span every tensor.
+        ready = L.ready_order(spec)
+        self.plan: BucketPlan = engine_bucket_plan(ready, bucket_mb, conv_bucket_mb, tail_bucket_kb,
+                                                   trainable=len(ready) - len(self._frozen))
+        n, ng = self.plan.total, self.plan.grad_total
+        self.n_grad = ng
         self.p32 = torch.zeros(n, dtype=F32, device=dev)
-        self.g32 = torch.zeros(n, dtype=F32, device=dev)
-        self.m32 = torch.zeros(n, dtype=F32, device=dev)
-        self.v32 = torch.zeros(n, dtype=F32, device=dev) if optimizer in ("adam", "adamw") else None
+        self.g32 = torch.zeros(ng, dtype=F32, device=dev)
+        self.m32 = torch.zeros(ng, dtype=F32, device=dev)
+        self.v32 = torch.zeros(ng, dtype=F32, device=dev) if optimizer in ("adam", "adamw") else None
         # each bucket's weight-decay segments [(start within the bucket, decay), ...], one entry when the
         # decay is uniform: biases and weights share buckets, and one launch per bucket stays one launch
         self._wd_segments = {bk.start: self.decay_segments(bk) for bk in self.plan.buckets}
@@ -243,7 +262,7 @@ class NativeEngine:
                           f"falls back to NCCL (--allreduce {allreduce} needs an NVLink domain)", flush=True)
             else:
                 wdt = BF16 if wire_dtype == "bf16" else F32
-                self.arena = SymmetricArena(n, dev, wire_dtype=wdt, group=node_group)
+                self.arena = SymmetricArena(ng, dev, wire_dtype=wdt, group=node_group)
         if self.world > 1:
             self._broadcast_params()
         # buckets holding only FC weight gradients are written with plain stores by the wgrad GEMM:
@@ -372,15 +391,30 @@ class NativeEngine:
         st = {"name": self.opt_name, "step": self.step_count, "micro_step": self.micro_count, "lr": self.lr}
         if getattr(self, "deterministic", False):     # key absent without the flag: the parent's checkpoint
             st["deterministic"] = True
+        frozen = getattr(self, "freeze_layers", 0)
+        if frozen:
+            st["frozen_layers"] = frozen
+        # state for the trainable tensors only: torch keeps none for parameters without a gradient
+        names = self.trainable_names()
         if self.opt_name in ("adam", "adamw"):
-            st["exp_avg"] = {n: L.to_torch(self.spec, n, self._view(self.m32, n)).cpu() for n in self.spec.param_names}
-            st["exp_avg_sq"] = {n: L.to_torch(self.spec, n, self._view(self.v32, n)).cpu() for n in self.spec.param_names}
+            st["exp_avg"] = {n: L.to_torch(self.spec, n, self._view(self.m32, n)).cpu() for n in names}
+            st["exp_avg_sq"] = {n: L.to_torch(self.spec, n, self._view(self.v32, n)).cpu() for n in names}
         else:
-            st["momentum_buffer"] = {n: L.to_torch(self.spec, n, self._view(self.m32, n)).cpu()
-                                     for n in self.spec.param_names}
+            st["momentum_buffer"] = {n: L.to_torch(self.spec, n, self._view(self.m32, n)).cpu() for n in names}
         return st
 
+    def trainable_names(self) -> List[str]:
+        """The parameters that train, in layer-table order (all of them without --freeze-layers)."""
+        frozen = getattr(self, "_frozen", ())
+        return [n for n in self.spec.param_names if n not in frozen]
+
     def import_optimizer_state(self, st: dict) -> None:
+        # Per-parameter Adam step counts make "unfreeze and continue" a different optimizer: refuse it
+        mine, theirs = getattr(self, "freeze_layers", 0), int(st.get("frozen_layers", 0))
+        if "name" in st and theirs != mine:
+            raise ValueError("the checkpoint's optimizer state was written with --freeze-layers %d, this run has "
+                             "--freeze-layers %d: resume with %d (or evaluate it with --eval-only)"
+                             % (theirs, mine, theirs))
         self.step_count = int(st.get("step", 0))
         if "name" in st and bool(st.get("deterministic", False)) != getattr(self, "deterministic", False):
             print("[Warn] the checkpoint was written %s --deterministic, this run is %s it: the run continues, "
@@ -432,7 +466,11 @@ class NativeEngine:
     def _broadcast_params(self) -> None:
         """DDP's constructor sync (distributedVggf.py:225): everybody adopts rank 0's weights."""
         if self.arena is not None and self.cross_group is None:
-            self.arena.broadcast_(self.p32, root=0)
+            # the wire spans the trainable prefix only: the frozen range (up to all of VGG-F's 136 M weights for
+            # a linear probe) goes as one collective instead of thousands of wire-sized chunks
+            self.arena.broadcast_(self.p32[:self.n_grad], root=0)
+            if self.n_grad < self.plan.total:
+                dist.broadcast(self.p32[self.n_grad:], src=0)
         else:
             dist.broadcast(self.p32, src=0)
         ops.require().cast_to_bf16(self.p32, self.w16)
@@ -500,7 +538,7 @@ class NativeEngine:
         self.dfeat = torch.empty(B, ph, ph, cl, dtype=BF16, device=dev)
         if self.deterministic:
             # one workspace for every split-K launch of the step: they all run on the compute stream
-            plan = deterministic_plan(spec, B, HW, ops.require().sm_count(), self.fused_head)
+            plan = deterministic_plan(spec, B, HW, ops.require().sm_count(), self.fused_head, self.freeze_layers)
             self._ws = torch.empty(deterministic_workspace_elems(plan), dtype=F32, device=dev)
 
     # ================================================================================ inputs
@@ -667,9 +705,11 @@ class NativeEngine:
         C = ops.require()
         if train:
             p = prev.dropout if self.train_dropout else 0.0
+            # linear probe (every layer before the head frozen): no gradient for the head's input
+            dh = None if self.freeze_layers == self.spec.num_layers - 1 else self.fc_dz[-2][:b]
             args = (self._head_in, self._w(f.name), self._b(f.name), self.labels_dev[:b], self.logits[:b],
                     self.fc_dz[-1][:b], self.fc_dz[-1].shape[1], self._grad(f.name + ".weight"),
-                    self._grad(f.name + ".bias"), self.fc_dz[-2][:b], 1.0 / (1.0 - p), bool(prev.relu), meter,
+                    self._grad(f.name + ".bias"), dh, 1.0 / (1.0 - p), bool(prev.relu), meter,
                     self.loss_buf, self.class_weights)
             soft = ops.soft_targets(eps, mix)
             if soft is not None:
@@ -702,6 +742,9 @@ class NativeEngine:
         spec = self.spec
         fcs, convs = spec.fcs, spec.convs
         last = len(fcs) - 1
+        # backward stops at the first trainable layer k (layer-table index): its bias gradient and wgrad
+        # run, its dgrad does not, and nothing below it is launched
+        k = self.freeze_layers
         # ---- FC stack ----------------------------------------------------------------------
         for i in range(last, -1, -1):
             f = fcs[i]
@@ -709,6 +752,8 @@ class NativeEngine:
                 self._bucket_done(f.name + ".bias")
                 self._bucket_done(f.name + ".weight")
                 self._mark("bwd " + f.name)
+                if k == len(convs) + i:
+                    return
                 continue
             ld = self.fc_dz[i].shape[1]
             dz = self.fc_dz[i][:b]                                   # [b][ld] bf16, cols >= fout are 0
@@ -729,6 +774,10 @@ class NativeEngine:
                 # wgrads, this one and the bf16 one above, are the same launches under `deterministic`)
                 ops.gemm(dz, x_in, self._grad(f.name + ".weight"), M=f.fout, N=f.fin, K=b, a_mn=True,
                          b_mn=True, epi="f32_atomic" if self._accum else "f32_store", ldo=f.fin)
+            if k == len(convs) + i:              # the first trainable layer: its input needs no gradient
+                self._bucket_done(f.name + ".weight")
+                self._mark("bwd " + f.name)
+                return
             # dgrad: dX[b][fin] = dz W ; swap-AB with W read MN-major (stored [K=fout][M=fin])
             m_tiles = (f.fin + 127) // 128
             ks = self._ksplit(m_tiles, (f.fout + 63) // 64)
@@ -801,6 +850,10 @@ class NativeEngine:
                 ops.conv3x3_wgrad_det(dz, x_in, self._grad(c.name + ".weight"), self._ws, accumulate=acc_g)
             else:
                 C.conv_wgrad(dz, x_in, self._grad(c.name + ".weight"), 1.0, 0, 0)
+            if i == k:                            # the first trainable layer: no dgrad, layer i-1 is frozen
+                self._bucket_done(c.name + ".weight")
+                self._mark("bwd " + c.name)
+                break
             dx = self.dbuf[pp][:x_in.numel()].view_as(x_in)
             # ReLU backward of layer i-1 is fused here unless a pool sits in between; when it is,
             # dx IS dZ_{i-1} and its column sum (layer i-1's bias gradient) comes for free
@@ -825,6 +878,19 @@ class NativeEngine:
             self._missing[bi] -= 1
             if self._missing[bi] == 0 and self._update:
                 self._reduce_and_update(bi)
+
+    def _frozen_ema(self) -> None:
+        """On an EMA step, the moving average of the frozen range [n_grad, total), which no optimizer launch
+        covers (AveragedModel averages every parameter): one launch on the optimizer's side stream, under
+        backward.  The frozen weights never change, so it may run anywhere in the step."""
+        if not self._ema_step or self.n_grad == self.plan.total:
+            return
+        ev = torch.cuda.Event()
+        ev.record()                      # an evaluation pass may still read the EMA biases
+        self.opt_stream.wait_event(ev)
+        with torch.cuda.stream(self.opt_stream):
+            ops.ema_update(self.p32[self.n_grad:], self.ema32[self.n_grad:], decay=self.ema_decay,
+                           first=self.ema_updates == 0)
 
     def _ema_kw(self, s: int, e: int) -> dict:
         """The EMA arguments of an optimizer launch over [s, e): none unless this step updates the EMA."""
@@ -988,6 +1054,7 @@ class NativeEngine:
         t.stop("forward")
         t.start("backward+reduce+update")
         self._begin_step()
+        self._frozen_ema()
         self._backward(b)
         self._end_step()
         self._accum = 0 if update else self._accum + 1

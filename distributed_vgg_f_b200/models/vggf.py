@@ -62,6 +62,21 @@ class VGGSpec:
             out += [l.name + ".weight", l.name + ".bias"]
         return out
 
+    @property
+    def num_layers(self) -> int:
+        """Entries of the layer table, convs then fcs: what --freeze-layers counts."""
+        return len(self.convs) + len(self.fcs)
+
+    def check_freeze_layers(self, n: int) -> int:
+        """``n`` leading layers frozen: 0 <= n < num_layers (the last Linear always trains)."""
+        if not 0 <= int(n) < self.num_layers:
+            raise ValueError("--freeze-layers must lie in [0, %d) for this model (got %d)" % (self.num_layers, n))
+        return int(n)
+
+    def frozen_param_names(self, n: int) -> List[str]:
+        """The weights and biases of the first ``n`` layers."""
+        return self.param_names[:2 * self.check_freeze_layers(n)]
+
     def param_shape(self, name: str):
         """Shape in the torch/torchvision layout (what a checkpoint stores)."""
         base, kind = name.rsplit(".", 1)
@@ -273,12 +288,37 @@ def build_oracle(spec: VGGSpec, seed: Optional[int] = None,
     return model
 
 
+def freeze_leading_layers_(model: nn.Module, n: int) -> List[str]:
+    """``requires_grad_(False)`` on both tensors of the first ``n`` layers of ``model.spec`` (--freeze-layers).
+    Returns their names."""
+    names = model.spec.frozen_param_names(n)
+    params = dict(model.named_parameters())
+    for name in names:
+        params[name].requires_grad_(False)
+    return names
+
+
+def count_frozen_layers(model: nn.Module) -> int:
+    """How many leading layers of ``model.spec`` have both tensors frozen."""
+    params = dict(model.named_parameters())
+    n = 0
+    for layer in list(model.spec.convs) + list(model.spec.fcs):
+        if params[layer.name + ".weight"].requires_grad or params[layer.name + ".bias"].requires_grad:
+            break
+        n += 1
+    return n
+
+
 def load_pretrained_vgg16_(model: nn.Module, state: dict) -> List[str]:
     """Copy every tensor of a torchvision ``vgg16`` state dict whose name and shape match.
 
     This is the offline counterpart of ``models.vgg16(pretrained=True)`` (distributedVggf.py:46):
-    features.* and classifier.0/.3 are taken, the funnel keeps its fresh init.
+    features.* and classifier.0/.3 are taken, the funnel keeps its fresh init.  A checkpoint of this
+    project (``{"model": {"module.<name>": ...}, ...}``, e.g. the first stage of a fine-tune run with
+    --freeze-layers) loads the same way, funnel included.
     """
+    if isinstance(state.get("model"), dict):
+        state = {(k[len("module."):] if k.startswith("module.") else k): v for k, v in state["model"].items()}
     own = model.state_dict()
     loaded = []
     for k, v in state.items():

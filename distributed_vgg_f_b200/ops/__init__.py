@@ -259,6 +259,12 @@ def sgd_step(p, mom, *, g32=None, g16=None, shadow=None, lr, momentum=0.9, weigh
     require().sgd(*args, ema, float(ema_decay), bool(ema_first), *_wd_args(wd_segments))
 
 
+def ema_update(p, ema, *, decay: float, first: bool = False):
+    """ema = decay * ema + (1 - decay) * p (fp32, each operation rounded, no FMA), or ema = p with ``first``:
+    the EMA update of ``adam_step`` / ``sgd_step`` for weights no optimizer launch covers (frozen layers)."""
+    require().ema_update(p, ema, float(decay), bool(first))
+
+
 _MIX_KIND = {"mixup": 1, "cutmix": 2}
 
 

@@ -18,7 +18,7 @@ simply a half-open element range ``[start, end)`` of that arena:
 from __future__ import annotations
 
 import dataclasses
-from typing import Dict, List, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 
 @dataclasses.dataclass(frozen=True)
@@ -48,6 +48,12 @@ class BucketPlan:
     def last_tensor_of_bucket(self, b: Bucket) -> str:
         """The tensor whose gradient completes the bucket (latest in ready order)."""
         return max(b.tensors, key=self.order.index)
+
+    @property
+    def grad_total(self) -> int:
+        """Length of the arena prefix the buckets cover: the tensors that have gradients.  ``total``
+        unless the plan was made for frozen layers (engine_bucket_plan(trainable=))."""
+        return self.buckets[-1].end if self.buckets else 0
 
 
 def _round_up(x: int, m: int) -> int:
@@ -119,11 +125,24 @@ def make_bucket_plan(ready_order: Sequence[Tuple[str, int]], cap_elems: int = 16
 
 
 def engine_bucket_plan(ready_order: Sequence[Tuple[str, int]], bucket_mb: float = 32.0, conv_bucket_mb: float = 9.5,
-                       tail_bucket_kb: float = 2400.0) -> BucketPlan:
+                       tail_bucket_kb: float = 2400.0, trainable: Optional[int] = None) -> BucketPlan:
     """The plan NativeEngine uses (sizes in MB / KB of fp32 gradient): ``bucket_mb`` messages for the FC weights
     that are ready first, ``conv_bucket_mb`` (one big conv layer) from the first ``features.*`` tensor on, and a
-    final bucket of at most ``tail_bucket_kb``.  Also what ``python -m distributed_vgg_f_b200.tools.plan`` prints."""
+    final bucket of at most ``tail_bucket_kb``.  Also what ``python -m distributed_vgg_f_b200.tools.plan`` prints.
+
+    ``trainable``: only the first ``trainable`` tensors of the ready order have gradients (frozen leading layers
+    are a suffix of it).  Every tensor keeps the offset of the full plan; the buckets, and the tail rule, cover
+    the trainable prefix ``[0, grad_total)`` alone.  None: every tensor trains."""
+    trainable = len(ready_order) if trainable is None else int(trainable)
+    if not 0 < trainable <= len(ready_order):
+        raise ValueError("trainable must lie in [1, %d] (got %d)" % (len(ready_order), trainable))
     cap = int(bucket_mb * 1024 * 1024 / 4)
-    first_conv = next((n for n, _ in ready_order if n.startswith("features.")), "")
-    return make_bucket_plan(ready_order, cap_elems=cap, late_cap_elems=min(cap, int(conv_bucket_mb * 1024 * 1024 / 4)),
+    head = list(ready_order[:trainable])
+    first_conv = next((n for n, _ in head if n.startswith("features.")), "")
+    plan = make_bucket_plan(head, cap_elems=cap, late_cap_elems=min(cap, int(conv_bucket_mb * 1024 * 1024 / 4)),
                             late_from=first_conv, tail_elems=int(tail_bucket_kb * 1024 / 4))
+    for name, n in ready_order[trainable:]:          # frozen: offsets and sizes only, in no bucket
+        plan.offsets[name], plan.numels[name] = plan.total, n
+        plan.order.append(name)
+        plan.total += _round_up(n, plan.align)
+    return plan

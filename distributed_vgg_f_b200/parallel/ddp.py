@@ -75,11 +75,13 @@ class FlatDDP(nn.Module):
 
     # -- construction-time sync (DDP's _sync_module_states) -------------------------------------
     def _sync_parameters(self) -> None:
+        # every parameter, frozen ones (requires_grad off) included, as DDP's _sync_module_states does
+        params = list(self.module.parameters())
         with torch.no_grad():
-            flat = torch.cat([p.detach().reshape(-1) for p in self._params.values()])
+            flat = torch.cat([p.detach().reshape(-1) for p in params])
             self.collective.broadcast_(flat, 0)
             pos = 0
-            for p in self._params.values():
+            for p in params:
                 p.copy_(flat[pos:pos + p.numel()].view_as(p))
                 pos += p.numel()
 

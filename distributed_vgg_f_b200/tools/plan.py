@@ -17,9 +17,12 @@ from ..parallel.symm import ONESHOT_MAX_BYTES, ONESHOT_MAX_BYTES_NVLS
 
 
 def describe(model: str = "vggf", num_classes: int = 3, world: int = 8, multicast: bool = True, zero1: str = "auto",
-             bucket_mb: float = 32.0, conv_bucket_mb: float = 9.5, tail_bucket_kb: float = 2400.0):
+             bucket_mb: float = 32.0, conv_bucket_mb: float = 9.5, tail_bucket_kb: float = 2400.0,
+             freeze_layers: int = 0):
     spec = get_spec(model, num_classes)
-    plan = engine_bucket_plan(L.ready_order(spec), bucket_mb, conv_bucket_mb, tail_bucket_kb)
+    ready = L.ready_order(spec)
+    plan = engine_bucket_plan(ready, bucket_mb, conv_bucket_mb, tail_bucket_kb,
+                              trainable=len(ready) - len(spec.frozen_param_names(freeze_layers)))
     fc_w = {f.name + ".weight" for f in spec.fcs}
     prepacked = set()
     for name in fc_w:
@@ -44,7 +47,21 @@ def describe(model: str = "vggf", num_classes: int = 3, world: int = 8, multicas
     return plan, rows
 
 
-def deterministic(model: str, num_classes: int, batch: int, input_hw: int, sms: int) -> int:
+def frozen_lines(model: str, num_classes: int, plan, freeze_layers: int) -> list:
+    """What --freeze-layers leaves out of the exchange: the frozen layers and where the gradient arena ends."""
+    spec = get_spec(model, num_classes)
+    names = spec.frozen_param_names(freeze_layers)
+    if not names:
+        return []
+    layers = [l.name for l in list(spec.convs) + list(spec.fcs)][:freeze_layers]
+    n = sum(plan.numels[t] for t in names)
+    return ["frozen: %d layers, %s .. %s, %d parameters (native layouts); gradient arena, moments and wire end at "
+            "T = %d of %d elements (%.1f MB of fp32 gradient instead of %.1f)"
+            % (freeze_layers, layers[0], layers[-1], n, plan.grad_total, plan.total, plan.grad_total * 4 / 1e6,
+               plan.total * 4 / 1e6)]
+
+
+def deterministic(model: str, num_classes: int, batch: int, input_hw: int, sms: int, freeze_layers: int = 0) -> int:
     """Split count and partial-sum bytes of every split-K launch of a --deterministic step, from the
     launchers' own host arithmetic: needs the built extension, not a GPU."""
     from .. import ops
@@ -56,10 +73,11 @@ def deterministic(model: str, num_classes: int, batch: int, input_hw: int, sms: 
     spec = get_spec(model, num_classes)
     last = spec.fcs[-1]
     fused_head = len(spec.fcs) >= 2 and bool(ops.require().head_ce_supported(batch, last.fout, last.fin))
-    rows = deterministic_plan(spec, batch, input_hw, sms, fused_head)
-    print("%s, %d classes, batch %d, %d x %d, %d SMs: workspace %.1f MB, %.1f MB of partial sums written and read per step"
-          % (model, num_classes, batch, input_hw, input_hw, sms, deterministic_workspace_elems(rows) * 4 / 1e6,
-             sum(s * e for _, _, s, e in rows) * 4 / 1e6))
+    rows = deterministic_plan(spec, batch, input_hw, sms, fused_head, freeze_layers)
+    print("%s, %d classes, batch %d, %d x %d, %d SMs%s: workspace %.1f MB, %.1f MB of partial sums written and read "
+          "per step" % (model, num_classes, batch, input_hw, input_hw, sms,
+                        ", %d layers frozen" % freeze_layers if freeze_layers else "",
+                        deterministic_workspace_elems(rows) * 4 / 1e6, sum(s * e for _, _, s, e in rows) * 4 / 1e6))
     print("%-16s %-6s %7s %12s %10s" % ("layer", "what", "splits", "slice elems", "MB"))
     for name, what, splits, elems in rows:
         print("%-16s %-6s %7d %12d %10.2f" % (name, what, splits, elems, splits * elems * 4 / 1e6))
@@ -79,13 +97,22 @@ def main(argv=None) -> int:
     ap.add_argument("--batch", type=int, default=64, help="--deterministic: mini-batch per GPU")
     ap.add_argument("--input-hw", type=int, default=224, help="--deterministic: input side")
     ap.add_argument("--sms", type=int, default=132, help="--deterministic: SMs of the GPU planned for (H100 SXM: 132)")
+    ap.add_argument("--freeze-layers", type=int, default=0,
+                    help="plan for the first N layers frozen (the training option of the same name)")
     a = ap.parse_args(argv)
+    try:
+        get_spec(a.model, a.num_classes).check_freeze_layers(a.freeze_layers)
+    except ValueError as e:
+        ap.error(str(e))
     if a.deterministic:
-        return deterministic(a.model, a.num_classes, a.batch, a.input_hw, a.sms)
-    plan, rows = describe(a.model, a.num_classes, a.world, not a.no_multicast, a.zero1, a.bucket_mb)
+        return deterministic(a.model, a.num_classes, a.batch, a.input_hw, a.sms, a.freeze_layers)
+    plan, rows = describe(a.model, a.num_classes, a.world, not a.no_multicast, a.zero1, a.bucket_mb,
+                          freeze_layers=a.freeze_layers)
     total = sum(r[2] for r in rows)
     print("%s, %d classes: %d elements (native layouts) in %d tensors, arena %d elements (tensors aligned to %d), %d buckets, %.1f MB of bf16 wire per step"
           % (a.model, a.num_classes, sum(plan.numels.values()), len(plan.order), plan.total, plan.align, len(rows), total / 1e6))
+    for line in frozen_lines(a.model, a.num_classes, plan, a.freeze_layers):
+        print(line)
     print("%3s %11s %9s %3s  %-24s %-24s %s" % ("#", "elements", "wire MB", "n", "first tensor", "last tensor (completes it)", "path at world=%d" % a.world))
     for i, n, wire, cnt, first, last, path in rows:
         print("%3d %11d %9.2f %3d  %-24s %-24s %s" % (i, n, wire / 1e6, cnt, first, last, path))

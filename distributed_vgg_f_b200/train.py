@@ -13,13 +13,14 @@ JSONL logging are available as additive options.
 from __future__ import annotations
 
 import json
+import math
 import os
 import time
 
 import torch
 
 from .data.loader import DataManager
-from .models.vggf import build_oracle, get_spec
+from .models.vggf import build_oracle, freeze_leading_layers_, get_spec
 from .parallel.ddp import FlatDDP
 from .parallel.process_group import (device_name, distributed_is_initialized, init_distributed,
                                      pick_device)
@@ -67,10 +68,12 @@ def build_model_ema(module: torch.nn.Module, decay: float):
 def parameter_groups(model: torch.nn.Module, weight_decay: float, bias_weight_decay=None):
     """torchvision's set_weight_decay(custom_keys_weight_decay=[("bias", bias_weight_decay)]): the
     ``*.bias`` tensors in a group of their own at ``bias_weight_decay``, everything else at
-    ``weight_decay``.  Without a bias decay, one group (the parent's layout of the optimizer state)."""
+    ``weight_decay``.  Without a bias decay, one group (the parent's layout of the optimizer state).
+    Frozen parameters (``requires_grad`` off: --freeze-layers) are in no group, as a torch fine-tuning
+    script leaves them out."""
     if bias_weight_decay is None:
-        return [{"params": list(model.parameters()), "weight_decay": weight_decay}]
-    named = list(model.named_parameters())
+        return [{"params": [p for p in model.parameters() if p.requires_grad], "weight_decay": weight_decay}]
+    named = [(n, p) for n, p in model.named_parameters() if p.requires_grad]
     return [{"params": [p for n, p in named if not n.endswith(".bias")], "weight_decay": weight_decay},
             {"params": [p for n, p in named if n.endswith(".bias")], "weight_decay": bias_weight_decay}]
 
@@ -81,7 +84,7 @@ def build_optimizer(model_or_params, args):
     if isinstance(model_or_params, torch.nn.Module):
         params = parameter_groups(model_or_params, wd, getattr(args, "bias_weight_decay", None))
     else:
-        params = [{"params": list(model_or_params), "weight_decay": wd}]
+        params = [{"params": [p for p in model_or_params if p.requires_grad], "weight_decay": wd}]
     if args.optimizer == "sgd":
         return torch.optim.SGD(params, lr=args.learning_rate, momentum=args.momentum, weight_decay=wd)
     if args.optimizer == "adamw":
@@ -130,6 +133,12 @@ def manage_training(args) -> Trainer:
 
     spec = get_spec(args.model, num_classes)
     pretrained = torch.load(args.pretrained, map_location="cpu") if args.pretrained else None
+    freeze = spec.check_freeze_layers(getattr(args, "freeze_layers", 0))
+    if freeze:
+        frozen = spec.frozen_param_names(freeze)
+        print("[Info] frozen layers: {} .. {} ({} layers, {} parameters)".format(
+            frozen[0].rsplit(".", 1)[0], frozen[-1].rsplit(".", 1)[0], freeze,
+            sum(math.prod(spec.param_shape(n)) for n in frozen)))
 
     if distributed_is_initialized():
         print("[Info] distributed training has been initialized")
@@ -151,7 +160,7 @@ def manage_training(args) -> Trainer:
                              label_smoothing=getattr(args, "label_smoothing", 0.0), ema_decay=ema_decay,
                              weight_decay=getattr(args, "weight_decay", 0.0),
                              bias_weight_decay=getattr(args, "bias_weight_decay", None),
-                             deterministic=getattr(args, "deterministic", False))
+                             deterministic=getattr(args, "deterministic", False), freeze_layers=freeze)
         optimizer = None            # fused into the engine
         model_ema = True if ema_decay is not None else None       # kept by the engine's optimizer kernels
         if model.world > 1:
@@ -162,6 +171,7 @@ def manage_training(args) -> Trainer:
             # dropout draws from the global generator, which nothing else seeds (each rank its own masks)
             torch.manual_seed(args.seed * 1000003 + args.rank)
         model = build_oracle(spec, seed=args.seed, pretrained_state=pretrained).to(device)
+        freeze_leading_layers_(model, freeze)            # before FlatDDP: it buckets trainable tensors only
         if distributed_is_initialized():
             model = FlatDDP(model, bucket_cap_mb=args.bucket_mb)
         optimizer = build_optimizer(model.module if isinstance(model, FlatDDP) else model, args)
@@ -174,6 +184,8 @@ def manage_training(args) -> Trainer:
     start_epoch = 1
     if args.resume:
         kw = {} if model_ema is None else dict(model_ema=model_ema, ema_required=getattr(args, "eval_only", False))
+        if getattr(args, "eval_only", False):   # scoring needs no optimizer state: any frozen count will do
+            kw["skip_frozen_mismatch"] = True
         start_epoch = ckpt.load_checkpoint(args.resume, model, optimizer, **kw) + 1
         print("[Info] resumed from {} at epoch {}".format(args.resume, start_epoch))
 

@@ -46,10 +46,36 @@ def model_state(model) -> Dict[str, torch.Tensor]:
     return add_module_prefix({k: v.detach().to("cpu", torch.float32) for k, v in state.items()})
 
 
+def frozen_layers_of(model) -> int:
+    """The --freeze-layers count of a native engine or of a torch model (leading layers without gradients)."""
+    if hasattr(model, "freeze_layers"):
+        return int(model.freeze_layers)
+    module = model.module if hasattr(model, "module") and not hasattr(model, "features") else model
+    if not hasattr(module, "spec"):
+        return 0
+    from ..models.vggf import count_frozen_layers
+    return count_frozen_layers(module)
+
+
 def optimizer_state(model, optimizer) -> Dict[str, Any]:
     if hasattr(model, "export_optimizer_state"):
         return model.export_optimizer_state()
-    return optimizer.state_dict() if optimizer is not None else {}
+    if optimizer is None:
+        return {}
+    st = optimizer.state_dict()
+    frozen = frozen_layers_of(model)
+    if frozen:                 # as the native engine records it; absent without frozen layers
+        st["frozen_layers"] = frozen
+    return st
+
+
+def _check_frozen(path: str, st: dict, model) -> bool:
+    """Does the optimizer state ``st`` belong to this run's frozen layers?  Raises when it does not."""
+    theirs, mine = int(st.get("frozen_layers", 0)), frozen_layers_of(model)
+    if theirs != mine:
+        raise ValueError("%s: its optimizer state was written with --freeze-layers %d, this run has --freeze-layers "
+                         "%d: resume with %d (or evaluate it with --eval-only)" % (path, theirs, mine, theirs))
+    return True
 
 
 def ema_state(model, model_ema) -> Dict[str, torch.Tensor]:
@@ -80,9 +106,12 @@ def save_checkpoint(path: str, model, optimizer, epoch: int, args: Optional[dict
     os.replace(tmp, path)
 
 
-def load_checkpoint(path: str, model, optimizer=None, model_ema=None, ema_required: bool = False) -> int:
+def load_checkpoint(path: str, model, optimizer=None, model_ema=None, ema_required: bool = False,
+                    skip_frozen_mismatch: bool = False) -> int:
     """Restore model (+ optimizer, + the EMA when ``model_ema`` is given) and return the epoch to resume
-    *after*.  A checkpoint without an EMA leaves the EMA fresh, or fails with ``ema_required``."""
+    *after*.  A checkpoint without an EMA leaves the EMA fresh, or fails with ``ema_required``.  An optimizer
+    state written with a different --freeze-layers count is refused (per-parameter Adam step counts make
+    "unfreeze and continue" a different optimizer), or with ``skip_frozen_mismatch`` (evaluation) not loaded."""
     # our files hold tensors and plain containers only: no need to unpickle arbitrary objects
     payload = torch.load(path, map_location="cpu", weights_only=True)
     if model_ema is not None:
@@ -97,13 +126,16 @@ def load_checkpoint(path: str, model, optimizer=None, model_ema=None, ema_requir
             model.import_ema_state(strip_module_prefix({k: v for k, v in ema.items() if k != "n_averaged"}),
                                    int(ema["n_averaged"]))
     state = payload["model"] if "model" in payload else payload
+    opt = payload.get("optimizer") if isinstance(payload, dict) else None
+    if opt and skip_frozen_mismatch and int(opt.get("frozen_layers", 0)) != frozen_layers_of(model):
+        opt = None
     if hasattr(model, "import_state"):
         model.import_state(strip_module_prefix(state))
-        if "optimizer" in payload and payload["optimizer"]:
-            model.import_optimizer_state(payload["optimizer"])
+        if "optimizer" in payload and opt:
+            model.import_optimizer_state(opt)
     else:
         target = model.module if hasattr(model, "module") and not hasattr(model, "features") else model
         target.load_state_dict(strip_module_prefix(state))
-        if optimizer is not None and payload.get("optimizer"):
-            optimizer.load_state_dict(payload["optimizer"])
+        if optimizer is not None and opt and _check_frozen(path, opt, model):
+            optimizer.load_state_dict({k: v for k, v in opt.items() if k != "frozen_layers"})
     return int(payload.get("epoch", 0))
