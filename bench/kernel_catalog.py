@@ -37,6 +37,10 @@ ROLE = [   # (regex on the demangled name, role, what it replaces in the referen
     (r"broadcast_kernel", "K-BCAST: rank 0's parameters pulled over NVLink through the wire buffer", "DDP constructor `_sync_module_states` — `:225`"),
     (r"barrier_kernel", "device-side barrier (tests)", "—"),
     (r"cast_", "fp32 ↔ bf16 casts (start-up: master → shadow)", "—"),
+    (r"psgd_project_kernel", "PowerSGD: M = g/k′ + e over the error arena and P = M·Q, one row per CTA", "`powerSGD_hook`: error add + `torch.bmm`"),
+    (r"psgd_backproject_kernel", "PowerSGD: Q = Mᵀ·P per row split (added in order by splitk_reduce)", "`powerSGD_hook`: `torch.bmm`"),
+    (r"psgd_orthogonalize_kernel", "PowerSGD: modified Gram–Schmidt of P or Q, one CTA per matrix", "`powerSGD_hook`: `_orthogonalize`"),
+    (r"psgd_decompress_kernel", "PowerSGD: G = P·Qᵀ/W over the gradient, e = M − G", "`powerSGD_hook`: `torch.bmm` + error store"),
 ]
 
 

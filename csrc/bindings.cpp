@@ -418,6 +418,56 @@ static void ema_update(const at::Tensor& p, at::Tensor ema, double decay, bool f
   b200::ema_fused(f32p(p), f32p(ema), p.numel(), decay, first, cur_stream());
 }
 
+// ---- PowerSGD (powersgd.cu): one n x m fp32 matrix, P [n][rank], Q [m][rank]
+static void check_psgd(const char* op, int64_t n, int64_t m, int64_t rank) {
+  TORCH_CHECK(rank >= 1 && rank <= b200::PSGD_MAX_RANK, op, ": rank must lie in [1, ", b200::PSGD_MAX_RANK,
+              "] (got ", rank, "): each thread keeps rank fp32 accumulators in a 40-register budget");
+  TORCH_CHECK(n >= 1 && m >= 4 && m % 4 == 0 && n <= INT32_MAX && m <= INT32_MAX, op,
+              ": needs n >= 1 and m >= 4 a multiple of 4 (got ", n, " x ", m, ")");
+}
+static void check_psgd_operand(const at::Tensor& t, int64_t elems, const char* op, const char* name) {
+  check_vec(t, at::kFloat, 16, op, name);
+  TORCH_CHECK(t.numel() >= elems, op, ": ", name, " must hold ", elems, " elements, got ", t.numel());
+}
+static void psgd_project(const at::Tensor& g, at::Tensor e, const at::Tensor& q, at::Tensor p, int64_t n, int64_t m,
+                         int64_t rank, double scale) {
+  c10::cuda::CUDAGuard guard(g.device());
+  check_psgd("psgd_project", n, m, rank);
+  check_psgd_operand(g, n * m, "psgd_project", "g");
+  check_psgd_operand(e, n * m, "psgd_project", "e");
+  check_psgd_operand(q, m * rank, "psgd_project", "q");
+  check_psgd_operand(p, n * rank, "psgd_project", "p");
+  b200::psgd_project(f32p(g), f32p(e), f32p(q), f32p(p), (int)n, (int)m, (int)rank, (float)scale, cur_stream());
+}
+static void psgd_backproject(const at::Tensor& M, const at::Tensor& p, at::Tensor q, at::Tensor ws, int64_t n, int64_t m,
+                             int64_t rank) {
+  c10::cuda::CUDAGuard guard(M.device());
+  check_psgd("psgd_backproject", n, m, rank);
+  check_psgd_operand(M, n * m, "psgd_backproject", "M");
+  check_psgd_operand(p, n * rank, "psgd_backproject", "p");
+  check_psgd_operand(q, m * rank, "psgd_backproject", "q");
+  check_psgd_operand(ws, b200::psgd_workspace_elems((int)n, (int)m, (int)rank, b200::sm_count()), "psgd_backproject",
+                     "the workspace");
+  b200::psgd_backproject(f32p(M), f32p(p), f32p(q), f32p(ws), ws.numel(), (int)n, (int)m, (int)rank, cur_stream());
+}
+static void psgd_orthogonalize(at::Tensor x, int64_t rows, int64_t rank, int64_t count) {
+  c10::cuda::CUDAGuard guard(x.device());
+  check_psgd("psgd_orthogonalize", 1, 4, rank);
+  TORCH_CHECK(count >= 1 && rows >= rank && rows <= INT32_MAX, "psgd_orthogonalize: needs count >= 1 and rows >= rank");
+  check_psgd_operand(x, count * rows * rank, "psgd_orthogonalize", "x");
+  b200::psgd_orthogonalize(f32p(x), (int)rows, (int)count, (int)rank, cur_stream());
+}
+static void psgd_decompress(const at::Tensor& p, const at::Tensor& q, at::Tensor g, at::Tensor e, int64_t n, int64_t m,
+                            int64_t rank, double alpha) {
+  c10::cuda::CUDAGuard guard(g.device());
+  check_psgd("psgd_decompress", n, m, rank);
+  check_psgd_operand(p, n * rank, "psgd_decompress", "p");
+  check_psgd_operand(q, m * rank, "psgd_decompress", "q");
+  check_psgd_operand(g, n * m, "psgd_decompress", "g");
+  check_psgd_operand(e, n * m, "psgd_decompress", "e");
+  b200::psgd_decompress(f32p(p), f32p(q), f32p(g), f32p(e), (int)n, (int)m, (int)rank, (float)alpha, cur_stream());
+}
+
 static void check_augment(const at::Tensor& src, const at::Tensor& params, const at::Tensor& out, int64_t OH,
                           int64_t OW, int64_t mode, int64_t pad, const std::vector<double>& mean,
                           const std::vector<double>& stdv) {
@@ -910,6 +960,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0, py::arg("ema_first") = false,
         py::arg("wd_starts") = std::vector<int64_t>(), py::arg("wd_values") = std::vector<double>());
   m.def("ema_update", &ema_update, py::arg("p"), py::arg("ema"), py::arg("decay"), py::arg("first"));
+  m.def("psgd_project", &psgd_project, py::arg("g"), py::arg("e"), py::arg("q"), py::arg("p"), py::arg("n"),
+        py::arg("m"), py::arg("rank"), py::arg("scale"));
+  m.def("psgd_backproject", &psgd_backproject, py::arg("M"), py::arg("p"), py::arg("q"), py::arg("ws"), py::arg("n"),
+        py::arg("m"), py::arg("rank"));
+  m.def("psgd_orthogonalize", &psgd_orthogonalize, py::arg("x"), py::arg("rows"), py::arg("rank"),
+        py::arg("count") = 1);
+  m.def("psgd_decompress", &psgd_decompress, py::arg("p"), py::arg("q"), py::arg("g"), py::arg("e"), py::arg("n"),
+        py::arg("m"), py::arg("rank"), py::arg("alpha"));
+  // host arithmetic of the back-projection's row splits (no GPU needed): the workspace a launch needs
+  m.def("psgd_workspace_elems", [](int64_t n, int64_t m, int64_t rank, int64_t sms) {
+    return (int64_t)b200::psgd_workspace_elems((int)n, (int)m, (int)rank, (int)sms);
+  });
+  m.attr("PSGD_MAX_RANK") = b200::PSGD_MAX_RANK;
   m.def("augment", &augment);
   m.def("augment_mixed", &augment_mixed);
   m.def("augment_ragged", &augment_ragged);

@@ -182,6 +182,24 @@ void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* sh
 // n elements, any n >= 0; p and ema 16-byte aligned.
 void ema_fused(const float* p, float* ema, long long n, double decay, bool first, cudaStream_t s);
 
+// ---- PowerSGD gradient compression (powersgd.cu) ----------------------------------------------
+// A compressed tensor is an n x m row-major fp32 matrix (m % 4 == 0); P is [n][rank], Q is [m][rank],
+// 1 <= rank <= PSGD_MAX_RANK; every operand 16-byte aligned.
+constexpr int PSGD_MAX_RANK = 8;
+// e = g * scale + e (M, stored over e); p = M q.
+void psgd_project(const float* g, float* e, const float* q, float* p, int n, int m, int rank, float scale,
+                  cudaStream_t s);
+// q = M^T p, from per-row-split partial sums in ws[splits][workspace_slice(m * rank)] added in split order.
+void psgd_backproject(const float* M, const float* p, float* q, float* ws, long long ws_elems, int n, int m, int rank,
+                      cudaStream_t s);
+int psgd_backproject_splits(int n, int m, int sms);
+long long psgd_workspace_elems(int n, int m, int rank, int sms);
+// Modified Gram-Schmidt of `count` consecutive [rows][rank] matrices, one per CTA; zero columns stay zero.
+void psgd_orthogonalize(float* x, int rows, int count, int rank, cudaStream_t s);
+// g = alpha * p q^T, e = e - g (e held M).
+void psgd_decompress(const float* p, const float* q, float* g, float* e, int n, int m, int rank, float alpha,
+                     cudaStream_t s);
+
 // Fused input transform: uint8 HWC source -> normalised bf16.  mode 0: NHWC with C padded to
 // `cpad`; mode 1: layer-0 im2col matrix [N*OH*OW][kpad] (k = (kh*3+kw)*3 + c, zero padded).
 void augment_fused(const uint8_t* src, const float* params, bf16* out, int N, int SH, int SW,

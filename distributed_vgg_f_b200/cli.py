@@ -162,6 +162,13 @@ def build_parser() -> argparse.ArgumentParser:
                           "Frozen layers run forward in train mode and get no gradient, no exchange, no optimizer "
                           "state and no weight decay (torch's requires_grad_(False)); the EMA still averages them "
                           "(default 0 = everything trains)")
+    ext.add_argument("--powersgd-rank", type=int, default=0,
+                     help="compress the gradient exchange with PowerSGD at this rank, 1 <= r <= 8 (torch's "
+                          "powerSGD_hook with error feedback and warm start, one bucket per tensor): every weight matrix "
+                          "where it pays goes over the wire as rank-r fp32 factors P and Q (default 0 = off)")
+    ext.add_argument("--powersgd-start-iter", type=int, default=1000,
+                     help="optimizer updates exchanged uncompressed before PowerSGD starts, >= 2 (torch's "
+                          "start_powerSGD_iter; default 1000)")
     ext.add_argument("--model-ema-decay", type=float, default=0.99998,
                      help="EMA decay per image seen, 0 <= d < 1; the decay of one update is adjusted as torchvision "
                           "does: 1 - min(1, (1 - d) * world * mini_batch * accum_steps * model_ema_steps / epochs)")
@@ -199,6 +206,14 @@ def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
             get_spec(args.model, args.num_classes or 3).check_freeze_layers(args.freeze_layers)
         except ValueError as e:
             build_parser().error("%s (%s)" % (e, args.model))
+    if args.powersgd_rank:
+        from .parallel import powersgd
+        try:
+            powersgd.check_config(args.powersgd_rank, args.powersgd_start_iter)
+            powersgd.resolve_zero1({"auto": "auto", "on": True, "off": False}[args.zero1], args.powersgd_rank)
+            powersgd.check_deterministic(args.powersgd_rank, args.deterministic, args.world_size)
+        except ValueError as e:
+            build_parser().error(str(e))
     print(args)
     if args.socket_ifname:
         os.environ["GLOO_SOCKET_IFNAME"] = args.socket_ifname

@@ -32,7 +32,8 @@ from ..config import DATA, TRAIN
 from ..data.loader import FusedBatch, RaggedBatch
 from ..models import layout as L
 from ..models.vggf import VGGSpec, build_oracle
-from ..parallel.buckets import BucketPlan, engine_bucket_plan
+from ..parallel import powersgd as psgd
+from ..parallel.buckets import Bucket, BucketPlan, engine_bucket_plan
 from ..parallel.process_group import distributed_is_initialized
 from ..utils.metrics import DeviceMeter
 
@@ -141,7 +142,8 @@ class NativeEngine:
                  tail_bucket_kb: float = 2400.0, same_dropout_all_ranks: bool = False,
                  label_smoothing: float = 0.0, ema_decay: Optional[float] = None,
                  bias_weight_decay: Optional[float] = None, deterministic: bool = False,
-                 freeze_layers: int = 0) -> None:
+                 freeze_layers: int = 0, powersgd_rank: int = 0,
+                 powersgd_start_iter: int = psgd.DEFAULT_START_ITER) -> None:
         ops.require()
         if compute_dtype != "bf16":
             raise NotImplementedError("the native engine computes in bf16 with fp32 master weights; "
@@ -196,6 +198,12 @@ class NativeEngine:
         if self.deterministic and allreduce == "nvls":
             raise ValueError("--deterministic: --allreduce nvls leaves the summation order to the NVLink switch; "
                              "use auto, oneshot or twoshot (they add the ranks in a fixed order)")
+        # --powersgd-rank: from update powersgd_start_iter + 1 on, the tensors torch's powerSGD_hook compresses
+        # are exchanged as rank-r factors P and Q (DESIGN 3.1); 0: off, and nothing below changes
+        psgd.check_config(powersgd_rank, powersgd_start_iter)
+        self.powersgd_rank, self.powersgd_start_iter = int(powersgd_rank), int(powersgd_start_iter)
+        psgd.check_deterministic(self.powersgd_rank, self.deterministic, self.world)
+        zero1 = psgd.resolve_zero1(zero1, self.powersgd_rank)
         self.ar_algo, self.comm_ctas, self.unpack_fp32 = allreduce, comm_ctas, unpack_fp32
         self.use_nccl = allreduce == "nccl"
         dev = self.device
@@ -311,6 +319,118 @@ class NativeEngine:
         self._wsrc, self._bsrc = self.w16, self.p32
 
         self._build_buffers()
+        self._psgd_now = False           # per train_step: this update compresses (update index > start iter)
+        if self.powersgd_rank:
+            self._powersgd_setup(ready, bucket_mb, conv_bucket_mb, tail_bucket_kb, wire_dtype)
+
+    # ============================================================================== PowerSGD
+    def _plan_tables(self) -> tuple:
+        return (self.plan, self._wd_segments, self._bucket_store_only, self._bucket_prepacked, self._prepacked,
+                self._tensor_buckets)
+
+    def _set_plan_tables(self, tables: tuple) -> None:
+        (self.plan, self._wd_segments, self._bucket_store_only, self._bucket_prepacked, self._prepacked,
+         self._tensor_buckets) = tables
+
+    def _powersgd_setup(self, ready, bucket_mb: float, conv_bucket_mb: float, tail_bucket_kb: float,
+                        wire_dtype: str) -> None:
+        """The second bucket plan (the compressed tensors in no bucket, every offset kept), the error arena over
+        the compressed tensors, P and Q, and the back-projection workspace."""
+        spec, dev = self.spec, self.device
+        rows = psgd.plan(spec, self.powersgd_rank, self.freeze_layers)
+        self._psgd_rows = rows
+        comp = [t for t in rows if t.compressed]
+        self._psgd: Dict[str, tuple] = {}
+        eo = po = qo = 0
+        for t in comp:
+            n, m = psgd.native_nm(spec, t.name)
+            if m % 4:
+                raise ValueError("--powersgd-rank: %s has %d columns; the compression kernels need a multiple of 4"
+                                 % (t.name, m))
+            self._psgd[t.name] = (n, m, t.rank, eo, po, qo)
+            eo += _round_up(n * m, 4)
+            po += _round_up(n * t.rank, 4)
+            qo += _round_up(m * t.rank, 4)
+        self._psgd_e = torch.zeros(max(eo, 4), dtype=F32, device=dev)        # local error, M while compressing
+        self._psgd_p = torch.zeros(max(po, 4), dtype=F32, device=dev)
+        self._psgd_q = torch.zeros(max(qo, 4), dtype=F32, device=dev)
+        self._psgd_ws = torch.empty(psgd.workspace_elems(rows, spec, ops.require().sm_count(), ops.require()),
+                                    dtype=F32, device=dev)
+        self._psgd_started = False       # e and Q start afresh at the first compressed update of this process
+        # tables of the plain plan, then the same for the plan without the compressed tensors
+        self._tensor_buckets = {n: self.plan.bucket_of(n) for n in self.plan.order}
+        plain = self._plan_tables()
+        plan2 = engine_bucket_plan(ready, bucket_mb, conv_bucket_mb, tail_bucket_kb,
+                                   trainable=len(ready) - len(self._frozen), exclude=list(self._psgd))
+        self.plan = plan2
+        self._wd_segments = {bk.start: self.decay_segments(bk) for bk in plan2.buckets}
+        for name in self._psgd:          # one optimizer launch per compressed tensor, over its aligned range
+            s0 = plan2.offsets[name]
+            bk = Bucket(-1, s0, s0 + _round_up(plan2.numels[name], plan2.align), (name,))
+            self._wd_segments[s0] = self.decay_segments(bk)
+        fc_w = {f.name + ".weight" for f in spec.fcs}
+        self._bucket_store_only = [all(t in fc_w for t in bk.tensors) for bk in plan2.buckets]
+        self._psgd_store_only = {name: name in fc_w for name in self._psgd}
+        # the compressed FC wgrads go to g32 in fp32; the other FC weights that own whole buckets stay on the wire
+        self._bucket_prepacked = [False] * len(plan2.buckets)
+        self._prepacked = {n for n in self._prepacked if n not in self._psgd and
+                           all(plan2.buckets[i].tensors == (n,) for i in plan2.bucket_of(n))}
+        for name in self._prepacked:
+            for i in plan2.bucket_of(name):
+                self._bucket_prepacked[i] = True
+        self._tensor_buckets = {n: plan2.bucket_of(n) for n in plan2.order}
+        self._psgd_tables = (plain, self._plan_tables())
+        self._set_plan_tables(plain)
+        if self.rank == 0:
+            print(psgd.summary_line(rows, self.powersgd_rank, 2 if wire_dtype == "bf16" else 4), flush=True)
+
+    def _powersgd_begin(self, update_index: int) -> None:
+        """Pick the bucket plan of this micro-batch's update; at the first compressed update, zero the error
+        and load the hook's initial Q draws (permuted into the native column order)."""
+        if not self.powersgd_rank:
+            return
+        self._psgd_now = update_index > self.powersgd_start_iter
+        self._set_plan_tables(self._psgd_tables[1 if self._psgd_now else 0])
+        if self._psgd_now and not self._psgd_started:
+            self._psgd_e.zero_()
+            for name, q in psgd.initial_q_torch(self._psgd_rows, self.seed).items():
+                _, m, r, _, _, qo = self._psgd[name]
+                self._psgd_q[qo:qo + m * r].copy_(psgd.q_to_native(self.spec, name, q).reshape(-1))
+            self._psgd_started = True
+
+    def _powersgd_update(self, name: str) -> None:
+        """One compressed tensor, on the comm stream as soon as its gradient is final: project, all-reduce P,
+        orthogonalise, back-project, all-reduce Q, decompress; then its optimizer launch."""
+        n, m, r, eo, po, qo = self._psgd[name]
+        s0 = self.plan.offsets[name]
+        s1 = s0 + _round_up(self.plan.numels[name], self.plan.align)
+        g, e = self.g32[s0:s0 + n * m], self._psgd_e[eo:eo + n * m]
+        p, q = self._psgd_p[po:po + n * r], self._psgd_q[qo:qo + m * r]
+        ev = torch.cuda.Event()
+        ev.record()
+        self.comm_stream.wait_event(ev)
+        with torch.cuda.stream(self.comm_stream):
+            self._mark("psgd %s start" % name, "comm")
+            ops.psgd_orthogonalize(q, rows=m, rank=r)
+            # g32 holds the sum of the group's k' micro-batch means: the hook sees their mean
+            ops.psgd_project(g, e, q, p, n=n, m=m, rank=r, scale=1.0 / (self._accum + 1))
+            if self.world > 1:
+                dist.all_reduce(p)
+            ops.psgd_orthogonalize(p, rows=n, rank=r)
+            ops.psgd_backproject(e, p, q, self._psgd_ws, n=n, m=m, rank=r)
+            if self.world > 1:
+                dist.all_reduce(q)
+            # q keeps the sum over ranks; torch's Q is q / W, and the next orthogonalisation removes the scale
+            ops.psgd_decompress(p, q, g, e, n=n, m=m, rank=r, alpha=1.0 / self.world)
+            self._mark("psgd %s end" % name, "comm")
+        if not self.apply_updates:
+            return
+        if self.opt_stream is not self.comm_stream:
+            done = torch.cuda.Event()
+            done.record(self.comm_stream)
+            self.opt_stream.wait_event(done)
+        with torch.cuda.stream(self.opt_stream):
+            self._apply_update(s0, s1, None, zero=not self._psgd_store_only[name])
 
     # ============================================================================ parameters
     def _view(self, arena: torch.Tensor, name: str) -> torch.Tensor:
@@ -394,6 +514,8 @@ class NativeEngine:
         frozen = getattr(self, "freeze_layers", 0)
         if frozen:
             st["frozen_layers"] = frozen
+        if getattr(self, "powersgd_rank", 0):      # the error and Q are per rank and not saved (as DDP's hook)
+            st["powersgd"] = {"rank": self.powersgd_rank, "start_iter": self.powersgd_start_iter}
         # state for the trainable tensors only: torch keeps none for parameters without a gradient
         names = self.trainable_names()
         if self.opt_name in ("adam", "adamw"):
@@ -874,6 +996,9 @@ class NativeEngine:
 
     def _bucket_done(self, name: str) -> None:
         """Called right after the kernels producing ``name``'s gradient were enqueued."""
+        if self._psgd_now and self._update and name in self._psgd:
+            self._powersgd_update(name)
+            return
         for bi in self._tensor_buckets[name]:
             self._missing[bi] -= 1
             if self._missing[bi] == 0 and self._update:
@@ -1032,6 +1157,7 @@ class NativeEngine:
         if ema:
             self._require_ema("train_step(ema=True)")
         self._ema_step = bool(ema and update and self.apply_updates)
+        self._powersgd_begin(self.step_count + 1)
         self.micro_count += 1
         if update:
             self.step_count += 1

@@ -265,6 +265,33 @@ def ema_update(p, ema, *, decay: float, first: bool = False):
     require().ema_update(p, ema, float(decay), bool(first))
 
 
+# ---------------------------------------------------------------------------------------- PowerSGD
+# One compressed tensor is an n x m row-major fp32 matrix (m % 4 == 0); P is [n][rank], Q is [m][rank].
+def psgd_project(g, e, q, p, *, n: int, m: int, rank: int, scale: float = 1.0) -> None:
+    """M = g * scale + e written over ``e``, and P = M Q into ``p``."""
+    require().psgd_project(g, e, q, p, n, m, rank, float(scale))
+
+
+def psgd_backproject(M, p, q, ws, *, n: int, m: int, rank: int) -> None:
+    """Q = M^T P into ``q``; per-row-split partial sums go to ``ws`` and are added in split order."""
+    require().psgd_backproject(M, p, q, ws, n, m, rank)
+
+
+def psgd_workspace_elems(n: int, m: int, rank: int, sms: Optional[int] = None) -> int:
+    C = require()
+    return int(C.psgd_workspace_elems(n, m, rank, C.sm_count() if sms is None else sms))
+
+
+def psgd_orthogonalize(x, *, rows: int, rank: int, count: int = 1) -> None:
+    """Modified Gram-Schmidt of ``count`` consecutive [rows][rank] matrices in place; zero columns stay zero."""
+    require().psgd_orthogonalize(x, rows, rank, count)
+
+
+def psgd_decompress(p, q, g, e, *, n: int, m: int, rank: int, alpha: float = 1.0) -> None:
+    """G = alpha P Q^T written over ``g``; e = M - G (``e`` holds M from psgd_project)."""
+    require().psgd_decompress(p, q, g, e, n, m, rank, float(alpha))
+
+
 _MIX_KIND = {"mixup": 1, "cutmix": 2}
 
 

@@ -62,7 +62,7 @@ def _round_up(x: int, m: int) -> int:
 
 def make_bucket_plan(ready_order: Sequence[Tuple[str, int]], cap_elems: int = 16 * 1024 * 1024,
                      first_cap_elems: int = 0, align: int = 2048, late_cap_elems: int = 0,
-                     late_from: str = "", tail_elems: int = 0) -> BucketPlan:
+                     late_from: str = "", tail_elems: int = 0, exclude: Sequence[str] = ()) -> BucketPlan:
     """``ready_order``: (name, numel) in the order gradients are produced by backward.
 
     ``late_cap_elems`` / ``late_from``: from tensor ``late_from`` on, buckets are capped at the smaller
@@ -71,7 +71,11 @@ def make_bucket_plan(ready_order: Sequence[Tuple[str, int]], cap_elems: int = 16
     backward and the LAST bucket's reduction + optimizer step is the only part of the whole gradient
     exchange that nothing can hide, so the late buckets are one layer each and the final one is
     additionally held to ``tail_elems`` (the first convolutions: a few hundred KB, latency-bound).
+
+    ``exclude``: tensors that keep their offsets but belong to no bucket (exchanged some other way: PowerSGD);
+    a bucket never spans one.
     """
+    exclude = frozenset(exclude)
     if cap_elems % align:
         cap_elems = _round_up(cap_elems, align)
     if late_cap_elems and late_cap_elems % align:
@@ -106,6 +110,10 @@ def make_bucket_plan(ready_order: Sequence[Tuple[str, int]], cap_elems: int = 16
         cap = first_cap_elems if (first_cap_elems and not buckets) else cap_elems
         if late and late_cap_elems:
             cap = late_cap_elems
+        if name in exclude:
+            close(t0)
+            cur_start = t1
+            continue
         if t0 == tail_start and cur_names:
             close(t0)
         if (t1 - t0) > cap:
@@ -125,14 +133,17 @@ def make_bucket_plan(ready_order: Sequence[Tuple[str, int]], cap_elems: int = 16
 
 
 def engine_bucket_plan(ready_order: Sequence[Tuple[str, int]], bucket_mb: float = 32.0, conv_bucket_mb: float = 9.5,
-                       tail_bucket_kb: float = 2400.0, trainable: Optional[int] = None) -> BucketPlan:
+                       tail_bucket_kb: float = 2400.0, trainable: Optional[int] = None,
+                       exclude: Sequence[str] = ()) -> BucketPlan:
     """The plan NativeEngine uses (sizes in MB / KB of fp32 gradient): ``bucket_mb`` messages for the FC weights
     that are ready first, ``conv_bucket_mb`` (one big conv layer) from the first ``features.*`` tensor on, and a
     final bucket of at most ``tail_bucket_kb``.  Also what ``python -m distributed_vgg_f_b200.tools.plan`` prints.
 
     ``trainable``: only the first ``trainable`` tensors of the ready order have gradients (frozen leading layers
     are a suffix of it).  Every tensor keeps the offset of the full plan; the buckets, and the tail rule, cover
-    the trainable prefix ``[0, grad_total)`` alone.  None: every tensor trains."""
+    the trainable prefix ``[0, grad_total)`` alone.  None: every tensor trains.
+
+    ``exclude``: trainable tensors left out of every bucket, offsets unchanged (the PowerSGD-compressed ones)."""
     trainable = len(ready_order) if trainable is None else int(trainable)
     if not 0 < trainable <= len(ready_order):
         raise ValueError("trainable must lie in [1, %d] (got %d)" % (len(ready_order), trainable))
@@ -140,7 +151,7 @@ def engine_bucket_plan(ready_order: Sequence[Tuple[str, int]], bucket_mb: float 
     head = list(ready_order[:trainable])
     first_conv = next((n for n, _ in head if n.startswith("features.")), "")
     plan = make_bucket_plan(head, cap_elems=cap, late_cap_elems=min(cap, int(conv_bucket_mb * 1024 * 1024 / 4)),
-                            late_from=first_conv, tail_elems=int(tail_bucket_kb * 1024 / 4))
+                            late_from=first_conv, tail_elems=int(tail_bucket_kb * 1024 / 4), exclude=exclude)
     for name, n in ready_order[trainable:]:          # frozen: offsets and sizes only, in no bucket
         plan.offsets[name], plan.numels[name] = plan.total, n
         plan.order.append(name)

@@ -10,6 +10,11 @@ rest of backward, gradients averaged (divided by world size before the sum).
   * ``register_post_accumulate_grad_hook`` marks tensors ready; when the last tensor of a bucket
     lands the bucket is pre-scaled by 1/ws and handed to a ``Collective`` asynchronously;
   * ``finish_backward()`` drains outstanding work before the optimizer step.
+With ``powersgd=`` (a torch ``PowerSGDState``) the buckets are not all-reduced as they land: on the
+synchronising backward, ``finish_backward()`` forms the accumulation group's mean and calls torch's own
+``powerSGD_hook`` once per tensor, each tensor a bucket of its own, in the order autograd finished the
+gradients of the first backward pass (DDP's rebuilt bucket order); the oracle of the native engine's
+``--powersgd-rank``.
 The ``Collective`` is ``TorchCollective`` (gloo on CPU -- BASELINE config #1) or
 ``parallel.fused.FusedCollective`` (our sm_90a P2P/NVLS kernels on the symmetric arena).
 ``state_dict()`` emits ``module.``-prefixed keys like the reference's wrapped model would.
@@ -47,7 +52,7 @@ class TorchCollective:
 
 class FlatDDP(nn.Module):
     def __init__(self, module: nn.Module, collective=None, bucket_cap_mb: float = 64.0,
-                 broadcast_from_rank0: bool = True) -> None:
+                 broadcast_from_rank0: bool = True, powersgd=None) -> None:
         super().__init__()
         self.module = module
         if collective is None and distributed_is_initialized():
@@ -65,6 +70,11 @@ class FlatDDP(nn.Module):
         self._pending: List[int] = []
         self._works: list = []
         self._require_sync = True
+        self.powersgd = powersgd
+        # the order autograd finished the gradients in the first backward pass: DDP rebuilds its buckets in this order
+        # after the first iteration, and the hook's bucket indices (its initial Q draws) follow it
+        self._ready_order: List[str] = []
+        self._backwards = 0              # backward passes since zero_grad (the accumulation group)
         for name, p in params:
             off = self.plan.offsets[name]
             p.grad = self.grad_arena[off:off + p.numel()].view_as(p)
@@ -91,7 +101,10 @@ class FlatDDP(nn.Module):
 
         def hook(_param) -> None:
             nonlocal bucket_ids
-            if self.collective is None or not self._require_sync:
+            if self.powersgd is not None and len(self._ready_order) < len(self._params) \
+                    and name not in self._ready_order:
+                self._ready_order.append(name)
+            if self.collective is None or not self._require_sync or self.powersgd is not None:
                 return
             if bucket_ids is None:
                 bucket_ids = self.plan.bucket_of(name)
@@ -109,8 +122,32 @@ class FlatDDP(nn.Module):
     def zero_grad(self, set_to_none: bool = False) -> None:   # grads are arena views: never None
         self.grad_arena.zero_()
         self._bucket_missing = [len(b.tensors) for b in self.plan.buckets]
+        self._backwards = 0
+
+    @property
+    def averages_group(self) -> bool:
+        """True when finish_backward already leaves the mean of the accumulation group in the gradients."""
+        return self.powersgd is not None
+
+    def _powersgd_exchange(self) -> None:
+        from torch.distributed.algorithms.ddp_comm_hooks.powerSGD_hook import powerSGD_hook
+
+        from .powersgd import HookBucket
+
+        if self._backwards > 1:          # the hook sees the group's mean, as under DDP with a loss / K
+            self.grad_arena.mul_(1.0 / self._backwards)
+        names = self._ready_order
+        for j, name in enumerate(names):
+            off, p = self.plan.offsets[name], self._params[name]
+            flat = self.grad_arena[off:off + p.numel()]
+            out = powerSGD_hook(self.powersgd, HookBucket(j, flat, p.shape, j == len(names) - 1)).wait()
+            if out.data_ptr() != flat.data_ptr():
+                flat.copy_(out)
 
     def finish_backward(self) -> None:
+        self._backwards += 1
+        if self.powersgd is not None and self.collective is not None and self._require_sync:
+            self._powersgd_exchange()
         for w in self._works:
             if w is not None:
                 w.wait()

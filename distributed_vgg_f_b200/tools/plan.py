@@ -84,6 +84,26 @@ def deterministic(model: str, num_classes: int, batch: int, input_hw: int, sms: 
     return 0
 
 
+def powersgd_table(model: str, num_classes: int, rank: int, freeze_layers: int = 0) -> int:
+    """Per trainable tensor (in DDP's bucket order): torch's n x m view, r' = min(n, m, r), whether
+    PowerSGD compresses it, and the P + Q elements it exchanges; then the bytes of one update."""
+    from ..parallel import powersgd
+    spec = get_spec(model, num_classes)
+    rows = powersgd.plan(spec, rank, freeze_layers)
+    b = powersgd.exchange_bytes(rows)
+    comp = [t for t in rows if t.compressed]
+    print("%s, %d classes, PowerSGD rank %d: %d of %d tensors compressed (%d parameters), %d P + Q elements"
+          % (model, num_classes, rank, len(comp), len(rows), sum(t.n * t.m for t in comp), sum(t.pq_elems for t in rows)))
+    print("%3s %-24s %7s %8s %3s %-10s %9s" % ("#", "tensor", "n", "m", "r'", "exchange", "P + Q"))
+    for j, t in enumerate(rows):
+        print("%3d %-24s %7d %8d %3d %-10s %9d" % (j, t.name, t.n, t.m, t.rank,
+                                                  "P, Q fp32" if t.compressed else "bf16 wire", t.pq_elems))
+    print("bytes per update: %d of P + Q (fp32) + %d uncompressed (bf16) = %d (%.2f MB; %.2f MB without PowerSGD, "
+          "%.0fx fewer)" % (b["compressed"], b["uncompressed"], b["total"], b["total"] / 1e6,
+                            b["without_powersgd"] / 1e6, b["without_powersgd"] / b["total"]))
+    return 0
+
+
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--model", default="vggf")
@@ -99,11 +119,18 @@ def main(argv=None) -> int:
     ap.add_argument("--sms", type=int, default=132, help="--deterministic: SMs of the GPU planned for (H100 SXM: 132)")
     ap.add_argument("--freeze-layers", type=int, default=0,
                     help="plan for the first N layers frozen (the training option of the same name)")
+    ap.add_argument("--powersgd-rank", type=int, default=0,
+                    help="print which tensors PowerSGD at this rank compresses and the bytes per update, instead")
     a = ap.parse_args(argv)
     try:
         get_spec(a.model, a.num_classes).check_freeze_layers(a.freeze_layers)
+        if a.powersgd_rank:
+            from ..parallel.powersgd import check_config
+            check_config(a.powersgd_rank, 2)
     except ValueError as e:
         ap.error(str(e))
+    if a.powersgd_rank:
+        return powersgd_table(a.model, a.num_classes, a.powersgd_rank, a.freeze_layers)
     if a.deterministic:
         return deterministic(a.model, a.num_classes, a.batch, a.input_hw, a.sms, a.freeze_layers)
     plan, rows = describe(a.model, a.num_classes, a.world, not a.no_multicast, a.zero1, a.bucket_mb,

@@ -160,7 +160,9 @@ def manage_training(args) -> Trainer:
                              label_smoothing=getattr(args, "label_smoothing", 0.0), ema_decay=ema_decay,
                              weight_decay=getattr(args, "weight_decay", 0.0),
                              bias_weight_decay=getattr(args, "bias_weight_decay", None),
-                             deterministic=getattr(args, "deterministic", False), freeze_layers=freeze)
+                             deterministic=getattr(args, "deterministic", False), freeze_layers=freeze,
+                             powersgd_rank=getattr(args, "powersgd_rank", 0),
+                             powersgd_start_iter=getattr(args, "powersgd_start_iter", 1000))
         optimizer = None            # fused into the engine
         model_ema = True if ema_decay is not None else None       # kept by the engine's optimizer kernels
         if model.world > 1:
@@ -173,7 +175,11 @@ def manage_training(args) -> Trainer:
         model = build_oracle(spec, seed=args.seed, pretrained_state=pretrained).to(device)
         freeze_leading_layers_(model, freeze)            # before FlatDDP: it buckets trainable tensors only
         if distributed_is_initialized():
-            model = FlatDDP(model, bucket_cap_mb=args.bucket_mb)
+            state = None
+            if getattr(args, "powersgd_rank", 0):
+                from .parallel import powersgd
+                state = powersgd.make_state(args.powersgd_rank, args.powersgd_start_iter, args.seed)
+            model = FlatDDP(model, bucket_cap_mb=args.bucket_mb, powersgd=state)
         optimizer = build_optimizer(model.module if isinstance(model, FlatDDP) else model, args)
         model_ema = None
         if ema_decay is not None:

@@ -263,7 +263,7 @@ class Trainer:
             if wrapper is not None:
                 wrapper.finish_backward()
             if update:
-                if pending > 1:                          # the mean of the group's gradients
+                if pending > 1 and not getattr(wrapper, "averages_group", False):      # the group's mean
                     with torch.no_grad():
                         for p in self.model.parameters():
                             if p.grad is not None:
