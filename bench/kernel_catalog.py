@@ -23,7 +23,7 @@ ROLE = [   # (regex on the demangled name, role, what it replaces in the referen
     (r"fc_bias_act_kernel", "FC epilogue: bias + ReLU + Philox dropout → bf16 (mask never stored)", "ATen bias/relu/dropout — `:52-57`"),
     (r"fc_grad_act_kernel", "FC backward epilogue: ReLU / dropout mask regenerated from the activation", "ATen threshold_backward / dropout backward"),
     (r"bias_grad", "bias gradients that no GEMM / pool epilogue already produced", "autograd sum"),
-    (r"maxpool2x2_fwd_kernel|maxpool2x2_relu_bwd_kernel", "un-fused max-pool fwd / ReLU + pool bwd (tile shapes the epilogue cannot pool, `B200_FUSE_POOL=0`)", "cuDNN / ATen max_pool2d"),
+    (r"maxpool2x2_fwd_kernel|maxpool2x2_relu_bwd_kernel|maxpool2x2_relu_bwd_odd_kernel", "un-fused max-pool fwd / ReLU + pool bwd (tile shapes the epilogue cannot pool, odd maps in floor mode, `B200_FUSE_POOL=0`)", "cuDNN / ATen max_pool2d"),
     (r"unpool2x2_kernel", "backward of the epilogue-fused pool: pooled gradient + argmax bit masks → full-resolution dz, bias gradient fused", "max_pool2d_backward + threshold_backward"),
     (r"adaptive_avgpool", "AdaptiveAvgPool2d(7,7) fwd / bwd (elided when the map is already 7×7)", "ATen adaptive_avg_pool2d — torchvision VGG"),
     (r"augment_nhwc_kernel|augment_im2col_kernel", "the six PIL transforms as one coordinate chain per output pixel: uint8 HWC → normalised bf16 NHWC4", "PIL / torchvision transforms — `:88-95`, `:103-108`"),

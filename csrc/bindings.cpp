@@ -90,6 +90,14 @@ static void conv_fprop_pool(const at::Tensor& x, const at::Tensor& w, c10::optio
                            reinterpret_cast<uint32_t*>(mask.data_ptr<int>()), N, H, W, Cin, Cout, (int)bn, cur_stream());
 }
 static bool conv_pool_fusable(int64_t N, int64_t H, int64_t W) { return b200::conv3x3_pool_fusable((int)N, (int)H, (int)W); }
+static std::vector<int64_t> conv_pixel_box(int64_t N, int64_t H, int64_t W) {
+  int b[4];
+  b200::conv_pixel_box((int)N, (int)H, (int)W, b);
+  return {b[0], b[1], b[2], b[3]};
+}
+static int64_t conv_bn_choice(int64_t N, int64_t H, int64_t W, int64_t cn) {
+  return b200::conv_bn_choice((int)N, (int)H, (int)W, (int)cn);
+}
 static void unpool(const at::Tensor& dp, const at::Tensor& mask, at::Tensor dz, c10::optional<at::Tensor> colsum) {
   c10::cuda::CUDAGuard g(dp.device());
   TORCH_CHECK(dp.dim() == 4 && dz.dim() == 4 && dp.is_contiguous() && dz.is_contiguous() && mask.is_contiguous() &&
@@ -880,6 +888,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv_fprop", &conv_fprop);
   m.def("conv_fprop_pool", &conv_fprop_pool);
   m.def("conv_pool_fusable", &conv_pool_fusable);
+  m.def("conv_pixel_box", &conv_pixel_box);
+  m.def("conv_bn_choice", &conv_bn_choice);
   m.def("unpool2x2", &unpool);
   m.def("conv_dgrad", &conv_dgrad);
   m.def("conv_wgrad", &conv_wgrad);

@@ -42,6 +42,8 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
                     pack_bf16x2(f[6], f[7]));
 }
 
+// Floor mode: the output is floor(H/2) x floor(W/2); at odd H or W the last row / column lies in no
+// window and is never read.
 __global__ void maxpool2x2_fwd_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, int N, int H,
                                       int W, int C) {
   const int OH = H / 2, OW = W / 2, C8 = C / 8;
@@ -66,7 +68,8 @@ __global__ void maxpool2x2_fwd_kernel(const bf16* __restrict__ x, bf16* __restri
 }
 
 void maxpool2x2_fwd(const bf16* x, bf16* y, int N, int H, int W, int C, cudaStream_t s) {
-  if (C % 8 || H % 2 || W % 2) throw std::runtime_error("[b200] maxpool2x2: need C%8==0 and even H,W");
+  // floor mode (torch's MaxPool2d(2, 2)): an odd last row / column is never read
+  if (C % 8 || H < 2 || W < 2) throw std::runtime_error("[b200] maxpool2x2: need C%8==0 and H,W >= 2");
   const long long total = static_cast<long long>(N) * (H / 2) * (W / 2) * (C / 8);
   const int blocks = min(ceil_div_ll(total, 256), sm_count() * 16);
   maxpool2x2_fwd_kernel<<<blocks, 256, 0, s>>>(x, y, N, H, W, C);
@@ -79,9 +82,12 @@ void maxpool2x2_fwd(const bf16* x, bf16* y, int N, int H, int W, int C, cudaStre
 // also accumulates colsum[c] += sum of dz over pixels (the conv layer's bias gradient): the grid
 // stride is a multiple of C/8, so a thread always sees the same 8 channels and keeps them in
 // registers; one shared-memory reduction and C global atomics per block at the end.
-__global__ void maxpool2x2_relu_bwd_kernel(const bf16* __restrict__ y, const bf16* __restrict__ dp,
-                                           bf16* __restrict__ dz, float* __restrict__ colsum, int N, int H,
-                                           int W, int C) {
+// ODD (odd H or W, floor mode): the last row / column lies in no window and its dz is stored as 0,
+// by the threads of the last window row / column; the even-size kernel is the ODD = false body.
+template <bool ODD>
+__device__ __forceinline__ void maxpool2x2_relu_bwd_body(const bf16* __restrict__ y, const bf16* __restrict__ dp,
+                                                         bf16* __restrict__ dz, float* __restrict__ colsum, int N,
+                                                         int H, int W, int C) {
   extern __shared__ float s_sum[];      // [C] when colsum
   const int OH = H / 2, OW = W / 2, C8 = C / 8;
   const long long total = static_cast<long long>(N) * OH * OW * C8;
@@ -121,6 +127,19 @@ __global__ void maxpool2x2_relu_bwd_kernel(const bf16* __restrict__ y, const bf1
     *reinterpret_cast<uint4*>(dz + o00 + C) = pack8(rb);
     *reinterpret_cast<uint4*>(dz + o00 + rowstride) = pack8(rc);
     *reinterpret_cast<uint4*>(dz + o00 + rowstride + C) = pack8(rd);
+    if constexpr (ODD) {
+      const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+      const bool last_h = (H & 1) && oh == OH - 1, last_w = (W & 1) && ow == OW - 1;
+      if (last_h) {
+        *reinterpret_cast<uint4*>(dz + o00 + 2 * rowstride) = z;
+        *reinterpret_cast<uint4*>(dz + o00 + 2 * rowstride + C) = z;
+      }
+      if (last_w) {
+        *reinterpret_cast<uint4*>(dz + o00 + 2 * C) = z;
+        *reinterpret_cast<uint4*>(dz + o00 + rowstride + 2 * C) = z;
+      }
+      if (last_h && last_w) *reinterpret_cast<uint4*>(dz + o00 + 2 * rowstride + 2 * C) = z;
+    }
   }
   if (colsum) {
     const int c8 = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) % C8;
@@ -132,14 +151,29 @@ __global__ void maxpool2x2_relu_bwd_kernel(const bf16* __restrict__ y, const bf1
   }
 }
 
+__global__ void maxpool2x2_relu_bwd_kernel(const bf16* __restrict__ y, const bf16* __restrict__ dp,
+                                           bf16* __restrict__ dz, float* __restrict__ colsum, int N, int H,
+                                           int W, int C) {
+  maxpool2x2_relu_bwd_body<false>(y, dp, dz, colsum, N, H, W, C);
+}
+__global__ void maxpool2x2_relu_bwd_odd_kernel(const bf16* __restrict__ y, const bf16* __restrict__ dp,
+                                               bf16* __restrict__ dz, float* __restrict__ colsum, int N, int H,
+                                               int W, int C) {
+  maxpool2x2_relu_bwd_body<true>(y, dp, dz, colsum, N, H, W, C);
+}
+
 void maxpool2x2_relu_bwd(const bf16* y, const bf16* dp, bf16* dz, float* colsum, int N, int H, int W,
                          int C, cudaStream_t s) {
-  if (C % 8 || H % 2 || W % 2) throw std::runtime_error("[b200] maxpool2x2_bwd: need C%8==0 and even H,W");
+  if (C % 8 || H < 2 || W < 2) throw std::runtime_error("[b200] maxpool2x2_bwd: need C%8==0 and H,W >= 2");
   if (colsum && 256 % (C / 8) != 0)
     throw std::runtime_error("[b200] maxpool2x2_bwd: fused column sum needs C/8 to divide 256");
   const long long total = static_cast<long long>(N) * (H / 2) * (W / 2) * (C / 8);
   const int blocks = min(ceil_div_ll(total, 256), sm_count() * 16);
-  maxpool2x2_relu_bwd_kernel<<<blocks, 256, colsum ? C * sizeof(float) : 0, s>>>(y, dp, dz, colsum, N, H, W, C);
+  const size_t smem = colsum ? C * sizeof(float) : 0;
+  if ((H | W) & 1)
+    maxpool2x2_relu_bwd_odd_kernel<<<blocks, 256, smem, s>>>(y, dp, dz, colsum, N, H, W, C);
+  else
+    maxpool2x2_relu_bwd_kernel<<<blocks, 256, smem, s>>>(y, dp, dz, colsum, N, H, W, C);
   count_launch();
   check_last("maxpool2x2_relu_bwd");
 }

@@ -44,6 +44,11 @@ void conv3x3_fprop(const bf16* x, const bf16* w, const float* bias, bf16* y, int
 // argmax bit 1, max > 0, 0}; the un-pooled activation is never materialised.  unpool2x2 is the
 // matching backward (elementwise.cu).
 bool conv3x3_pool_fusable(int N, int H, int W);
+// The pixel box {Wb, Hb, Nb, fill} the fprop / dgrad launchers of the implicit-GEMM path choose (fill = 1:
+// a box of any sides that fills more of the 128-row tile than make_tile's power-of-two one).
+void conv_pixel_box(int N, int H, int W, int* box);
+// The channel-tile width (64, 128 or 256) fprop / dgrad pick for cn output channels at that shape.
+int conv_bn_choice(int N, int H, int W, int cn);
 void conv3x3_fprop_pool(const bf16* x, const bf16* w, const float* bias, bf16* pool_out, uint32_t* pool_mask,
                         int N, int H, int W, int Cin, int Cout, int bn, cudaStream_t stream);
 // dx[N,H,W,Cin] = conv_transpose(dz[N,H,W,Cout], w); optional mask: zero where mask_src <= 0;

@@ -42,6 +42,8 @@
 //   __device__ static void epi_begin(const Params&, float* epi_smem, int tid);  // tid in [0,128)
 //   __device__ static void epi_end(const Params&, float* epi_smem, int tid);    // after all tiles
 #pragma once
+#include <type_traits>
+
 #include "ptx.cuh"
 
 namespace b200 {
@@ -171,6 +173,14 @@ __device__ __forceinline__ void stage_take(const float* stage_base, int c0, int 
 constexpr uint32_t STAGE_FULL_ARRIVALS = UMMA_CONSUMERS * 4;
 constexpr uint32_t STAGE_EMPTY_ARRIVALS = UMMA_EPI_THREADS / 32;
 
+// A policy whose A box may hold fewer than UMMA_BM rows (ConvPolicy<..., FILL = true>) declares
+// FILL_BOX = true and carries the bytes one A box delivers in Params::a_tx; every other policy's
+// stage transaction is the constant UMMA_A_BYTES + B bytes.
+template <class P, class = void>
+struct umma_fill_box : std::false_type {};
+template <class P>
+struct umma_fill_box<P, std::enable_if_t<P::FILL_BOX>> : std::true_type {};
+
 template <class P>
 __global__ void __launch_bounds__(UMMA_THREADS, 1)
 umma_kernel(const __grid_constant__ typename P::Params prm) {
@@ -222,7 +232,10 @@ umma_kernel(const __grid_constant__ typename P::Params prm) {
         for (int i = 0; i < nk; ++i) {
           mbar_wait(&empty_bar[s], ph ^ 1, 1);
           if (elect_one()) {
-            mbar_arrive_expect_tx(&full_bar[s], STAGE_TX);
+            if constexpr (umma_fill_box<P>::value)
+              mbar_arrive_expect_tx(&full_bar[s], prm.a_tx + B_BYTES);
+            else
+              mbar_arrive_expect_tx(&full_bar[s], STAGE_TX);
             P::load(prm, ctx, i, sA + s * UMMA_A_BYTES, sB + s * B_BYTES, &full_bar[s]);
           }
           __syncwarp();

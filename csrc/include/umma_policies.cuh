@@ -261,6 +261,9 @@ struct ConvParams {
   uint32_t* pool_mask;      // CONV_POOL: [N][H/2][W/2][Cn/32][4] = {argmax bit 0, argmax bit 1, max > 0, 0}
   int flags;
   int resident;           // halo kernel: all weight tiles stay in shared memory for the CTA lifetime
+  // FILL instantiations only (a box of any Wb x Hb x Nb <= 128 pixels): row -> (w, h, n) by division
+  FastDiv div_wb, div_hb;
+  uint32_t a_tx;          // bytes one A box delivers: Wb * Hb * Nb * 64 channels * 2
 };
 
 __device__ __forceinline__ void conv_tile_origin(const ConvTile& t, int tile, int& n0, int& h0,
@@ -274,9 +277,14 @@ __device__ __forceinline__ void conv_tile_origin(const ConvTile& t, int tile, in
 }
 
 // POOL (fprop only): a separate instantiation, so the un-pooled fprop kernels carry none of its code.
-template <int BN_, int STAGES_, bool DGRAD, bool POOL = false>
+// FILL: the pixel box is any Wb x Hb x Nb <= 128 pixels (conv_fill_tile; 11 x 11 x 1 on an 11^2 map), not
+// power-of-two sides: a row is decoded with fastdiv, rows past the box are neither stored nor summed, and
+// the A box delivers a_tx bytes.  The power-of-two instantiations keep their shift decode.
+template <int BN_, int STAGES_, bool DGRAD, bool POOL = false, bool FILL = false>
 struct ConvPolicy {
   static_assert(!(DGRAD && POOL), "the fused pool is an fprop epilogue");
+  static_assert(!(POOL && FILL), "the fused pool needs the power-of-two boxes of make_tile");
+  static constexpr bool FILL_BOX = FILL;
   static constexpr int BN = BN_;
   static constexpr int STAGES = STAGES_;
   static constexpr bool A_MN = false;
@@ -314,13 +322,22 @@ struct ConvPolicy {
   };
   __device__ static RowCtx row_ctx(const Params& p, const Ctx& c, int row) {
     const ConvTile& t = p.t;
-    const int ww = row & (t.Wb - 1);
-    const int r2 = row >> t.wb_shift;
-    const int hh = r2 & (t.Hb - 1);
-    const int nn = r2 >> t.hb_shift;
+    int ww, hh, nn;
+    if constexpr (FILL) {
+      uint32_t r2, r3, rw, rh;
+      fast_divmod(p.div_wb, static_cast<uint32_t>(row), r2, rw);
+      fast_divmod(p.div_hb, r2, r3, rh);
+      ww = static_cast<int>(rw); hh = static_cast<int>(rh); nn = static_cast<int>(r3);
+    } else {
+      ww = row & (t.Wb - 1);
+      const int r2 = row >> t.wb_shift;
+      hh = r2 & (t.Hb - 1);
+      nn = r2 >> t.hb_shift;
+    }
     const int n = c.n0 + nn, h = c.h0 + hh, w = c.w0 + ww;
     RowCtx rc;
     rc.valid = n < t.N && h < t.H && w < t.W;
+    if constexpr (FILL) rc.valid = rc.valid && nn < t.Nb;      // rows past the box: stale shared memory
     rc.pix_off = ((static_cast<long long>(n) * t.H + h) * t.W + w) * p.Cn;
     return rc;
   }

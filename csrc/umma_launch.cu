@@ -3,6 +3,7 @@
 // picks the tile width and launches umma_kernel<Policy>.
 #include <cudaTypedefs.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
@@ -160,6 +161,44 @@ static ConvTile make_tile(int N, int H, int W, int pixels) {
   t.div_tw = make_fastdiv(t.tiles_w);
   t.div_th = make_fastdiv(t.tiles_h);
   return t;
+}
+
+static long long conv_tile_count(const ConvTile& t) {
+  return static_cast<long long>(t.tiles_w) * t.tiles_h * ((t.N + t.Nb - 1) / t.Nb);
+}
+// Maps without a large power-of-two factor (11^2, 25^2) leave make_tile's 1 x 1 x 128 box half empty at
+// batch 64: 121 tiles do the work of 61.  conv_fill_tile searches every box Wb x Hb x Nb <= 128 pixels for
+// the fewest tiles (ties: the most pixels per box, then the widest rows) and returns true only where that
+// beats make_tile -- never where make_tile's tiles are already full, so those shapes keep their box and
+// their kernels.  11^2 at batch 64 -> 11 x 11 x 1 (64 tiles), 25^2 -> 25 x 5 x 1 (320 tiles instead of 625).
+static bool conv_fill_tile(int N, int H, int W, ConvTile* out) {
+  const ConvTile base = make_tile(N, H, W, UMMA_BM);
+  long long best = conv_tile_count(base);
+  int bw = 0, bh = 0, bn = 0, bpix = 0;
+  for (int wb = 1; wb <= W && wb <= UMMA_BM; ++wb)
+    for (int hb = 1; hb <= H && wb * hb <= UMMA_BM; ++hb) {
+      const int nb = std::min(N, UMMA_BM / (wb * hb));
+      const long long tiles = static_cast<long long>((W + wb - 1) / wb) * ((H + hb - 1) / hb) * ((N + nb - 1) / nb);
+      const int pix = wb * hb * nb;
+      if (tiles < best || (bw && tiles == best && (pix > bpix || (pix == bpix && wb > bw)))) {
+        best = tiles; bw = wb; bh = hb; bn = nb; bpix = pix;
+      }
+    }
+  if (!bw) return false;
+  ConvTile& t = *out;
+  t = base;
+  t.Wb = bw; t.Hb = bh; t.Nb = bn;
+  t.tiles_w = (W + bw - 1) / bw;
+  t.tiles_h = (H + bh - 1) / bh;
+  t.wb_shift = t.hb_shift = -1;             // not powers of two: the FILL kernels divide
+  t.div_tw = make_fastdiv(t.tiles_w);
+  t.div_th = make_fastdiv(t.tiles_h);
+  return true;
+}
+static void set_fill(ConvParams& prm) {
+  prm.div_wb = make_fastdiv(prm.t.Wb);
+  prm.div_hb = make_fastdiv(prm.t.Hb);
+  prm.a_tx = static_cast<uint32_t>(prm.t.Wb * prm.t.Hb * prm.t.Nb * UMMA_BK * 2);
 }
 
 // NHWC activation with an explicit pixel box {64, bw, bh, bn} (the halo kernel's (8+2) x (16+2)).
@@ -372,9 +411,9 @@ static void check_channels(int c, const char* what) {
   if (c % 64 != 0) throw std::runtime_error(std::string("[b200] ") + what + " must be a multiple of 64");
 }
 
-template <int BN, bool DGRAD, bool POOL = false>
+template <int BN, bool DGRAD, bool POOL = false, bool FILL = false>
 static void conv_launch(ConvParams& prm, cudaStream_t stream) {
-  using P = ConvPolicy<BN, umma_stages<BN, ConvPolicy<BN, 1, DGRAD, POOL>::EPI_SMEM>(), DGRAD, POOL>;
+  using P = ConvPolicy<BN, umma_stages<BN, ConvPolicy<BN, 1, DGRAD, POOL>::EPI_SMEM>(), DGRAD, POOL, FILL>;
   const ConvTile& t = prm.t;
   const int tiles_n = (t.N + t.Nb - 1) / t.Nb;
   prm.tiles_m = t.tiles_w * t.tiles_h * tiles_n;
@@ -401,6 +440,19 @@ static int conv_bn_pixels(const ConvTile& t, int cn) {
   return conv_bn(cn, tiles_m * ((cn + 127) / 128), tiles_m * ((cn + 255) / 256));
 }
 
+void conv_pixel_box(int N, int H, int W, int* box) {
+  ConvTile t = make_tile(N, H, W, UMMA_BM);
+  const bool fill = !halo_applicable(H, W) && conv_fill_tile(N, H, W, &t);
+  box[0] = t.Wb; box[1] = t.Hb; box[2] = t.Nb; box[3] = fill ? 1 : 0;
+}
+
+int conv_bn_choice(int N, int H, int W, int cn) {
+  if (halo_applicable(H, W)) return cn <= 64 ? 64 : 128;
+  ConvTile t = make_tile(N, H, W, UMMA_BM);
+  conv_fill_tile(N, H, W, &t);
+  return conv_bn_pixels(t, cn);
+}
+
 static void fprop_impl(const bf16* x, const bf16* w, const float* bias, bf16* y, bf16* pool_out,
                        uint32_t* pool_mask, int N, int H, int W, int Cin, int Cout, bool relu, int bn,
                        cudaStream_t stream) {
@@ -425,9 +477,19 @@ static void fprop_impl(const bf16* x, const bf16* w, const float* bias, bf16* y,
       default: throw std::runtime_error("[b200] conv3x3_fprop: bn must be 64 or 128");
     }
   }
+  const bool fill = !pool && conv_fill_tile(N, H, W, &prm.t);
+  if (fill) set_fill(prm);
   if (bn == 0) bn = conv_bn_pixels(prm.t, Cout);
   map_2d(&prm.mapB, w, Cout, 9LL * Cin, 9LL * Cin, 64, bn);
   map_nhwc(&prm.mapA, x, N, H, W, Cin, prm.t.Wb, prm.t.Hb, prm.t.Nb);
+  if (fill) {
+    switch (bn) {
+      case 64: conv_launch<64, false, false, true>(prm, stream); return;
+      case 128: conv_launch<128, false, false, true>(prm, stream); return;
+      case 256: conv_launch<256, false, false, true>(prm, stream); return;
+      default: throw std::runtime_error("[b200] conv3x3_fprop: bn must be 64, 128 or 256");
+    }
+  }
   switch (bn) {
     case 64: pool ? conv_launch<64, false, true>(prm, stream) : conv_launch<64, false>(prm, stream); break;
     case 128: pool ? conv_launch<128, false, true>(prm, stream) : conv_launch<128, false>(prm, stream); break;
@@ -478,8 +540,18 @@ void conv3x3_dgrad(const bf16* dz, const bf16* w, const bf16* mask_src, bf16* dx
       default: throw std::runtime_error("[b200] conv3x3_dgrad: bn must be 64 or 128");
     }
   }
+  const bool fill = conv_fill_tile(N, H, W, &prm.t);
+  if (fill) set_fill(prm);
   if (bn == 0) bn = conv_bn_pixels(prm.t, Cin);
   map_nhwc(&prm.mapA, dz, N, H, W, Cout, prm.t.Wb, prm.t.Hb, prm.t.Nb);
+  if (fill) {
+    switch (bn) {
+      case 64: conv_launch<64, true, false, true>(prm, stream); return;
+      case 128: conv_launch<128, true, false, true>(prm, stream); return;
+      case 256: conv_launch<256, true, false, true>(prm, stream); return;
+      default: throw std::runtime_error("[b200] conv3x3_dgrad: bn must be 64, 128 or 256");
+    }
+  }
   switch (bn) {
     case 64: conv_launch<64, true>(prm, stream); break;
     case 128: conv_launch<128, true>(prm, stream); break;

@@ -21,7 +21,10 @@ import os
 import sys
 from typing import Optional, Sequence
 
-from .config import TRAIN
+from .config import DATA, TRAIN
+
+# Below 32 the fifth 2x2 pool of VGG leaves an empty feature map.
+MIN_CROP = 32
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -169,10 +172,42 @@ def build_parser() -> argparse.ArgumentParser:
     ext.add_argument("--powersgd-start-iter", type=int, default=1000,
                      help="optimizer updates exchanged uncompressed before PowerSGD starts, >= 2 (torch's "
                           "start_powerSGD_iter; default 1000)")
+    ext.add_argument("--train-resize-size", type=int, default=DATA.resize,
+                     help="size of the training RandomResizedCrop (default %d, the reference's)" % DATA.resize)
+    ext.add_argument("--train-crop-size", type=int, default=DATA.crop,
+                     help="CenterCrop after rotation and flip: the network's training input, <= --train-resize-size "
+                          "(torchvision's --train-crop-size; default %d).  The native engine takes multiples of 8 from "
+                          "64 to 512" % DATA.crop)
+    ext.add_argument("--val-resize-size", type=int, default=DATA.resize,
+                     help="Resize of the shorter side for validation (torchvision's --val-resize-size; default %d)"
+                          % DATA.resize)
+    ext.add_argument("--val-crop-size", type=int, default=DATA.crop,
+                     help="CenterCrop after it: the network's evaluation input, <= --val-resize-size (torchvision's "
+                          "--val-crop-size; default %d).  Training and evaluation sizes may differ (FixRes: e.g. "
+                          "--train-crop-size 176 --val-resize-size 232 --val-crop-size 224)" % DATA.crop)
     ext.add_argument("--model-ema-decay", type=float, default=0.99998,
                      help="EMA decay per image seen, 0 <= d < 1; the decay of one update is adjusted as torchvision "
                           "does: 1 - min(1, (1 - d) * world * mini_batch * accum_steps * model_ema_steps / epochs)")
     return parser
+
+
+def check_sizes(args) -> Optional[str]:
+    """What is wrong with the four input sizes, or None."""
+    for split in ("train", "val"):
+        resize, crop = getattr(args, split + "_resize_size"), getattr(args, split + "_crop_size")
+        if crop < MIN_CROP:
+            return "--%s-crop-size must be >= %d (got %d): the fifth 2x2 max-pool would leave an empty map" % (
+                split, MIN_CROP, crop)
+        if crop > resize:
+            return "--%s-crop-size %d exceeds --%s-resize-size %d: the crop must lie inside the resized image" % (
+                split, crop, split, resize)
+    return None
+
+
+def input_sizes(args) -> dict:
+    """The four input sizes of a run (an args namespace without them: the reference's)."""
+    return {k: int(getattr(args, k, DATA.resize if k.endswith("resize_size") else DATA.crop))
+            for k in ("train_resize_size", "train_crop_size", "val_resize_size", "val_crop_size")}
 
 
 def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
@@ -200,6 +235,9 @@ def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
         build_parser().error("--lr-warmup-decay must lie in (0, 1]")
     if not args.lr_min >= 0.0:
         build_parser().error("--lr-min must be >= 0")
+    err = check_sizes(args)
+    if err:
+        build_parser().error(err)
     if args.freeze_layers:
         from .models.vggf import get_spec
         try:

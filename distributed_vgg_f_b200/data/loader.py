@@ -48,9 +48,9 @@ class FusedBatch(NamedTuple):
     state: Optional[dict] = None    # consumer may set state["event"]: slot is reusable after it fires
     mix: Optional[T.MixDraw] = None     # MixUp / CutMix of this training batch
 
-    def to_float(self, device="cpu") -> Tuple[torch.Tensor, torch.Tensor]:
-        """Evaluate the fused transform with torch ops (CPU / oracle path)."""
-        x = T.augment_reference(self.images_u8.to(device), self.params, self.resized_hw)
+    def to_float(self, device="cpu", out_hw: int = DATA.crop) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Evaluate the fused transform with torch ops (CPU / oracle path), cut to ``out_hw``."""
+        x = T.augment_reference(self.images_u8.to(device), self.params, self.resized_hw, out_hw=out_hw)
         return x, self.labels.to(device)
 
 
@@ -64,9 +64,9 @@ class RaggedBatch(NamedTuple):
     state: Optional[dict] = None    # consumer may set state["event"]: slot is reusable after it fires
     mix: Optional[T.MixDraw] = None     # MixUp / CutMix of this training batch
 
-    def to_float(self, device="cpu") -> Tuple[torch.Tensor, torch.Tensor]:
-        """Evaluate the transform with Pillow's resampling on the CPU (CPU / oracle path)."""
-        x = T.ragged_reference(self.data_u8, self.geom, self.params)
+    def to_float(self, device="cpu", out_hw: int = DATA.crop) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Evaluate the transform with Pillow's resampling on the CPU (CPU / oracle path), cut to ``out_hw``."""
+        x = T.ragged_reference(self.data_u8, self.geom, self.params, out_hw=out_hw)
         return x.to(device), self.labels.to(device)
 
 
@@ -107,13 +107,13 @@ def _header_hw(path: str) -> Tuple[int, int]:
 class DecodedCache:
     """All images of a split, decoded once to uint8 HWC (PNGs by the native decoder where it can).
 
-    One image size of at most ``DATA.resize`` on both sides: ``images`` is [N,H,W,3].  Otherwise
+    One image size of at most ``resize`` (the split's resize size) on both sides: ``images`` is [N,H,W,3].  Otherwise
     (``ragged``): ``flat`` holds the images back to back, image i at ``offsets[i]`` with size
     ``hw[i]``.  ``allow_mixed=False`` refuses a split of mixed sizes.  The budget is checked from
     the file headers before anything is decoded."""
 
     def __init__(self, samples: List[Tuple[str, int]], threads: int = 8, max_bytes: Optional[int] = None,
-                 allow_mixed: bool = True) -> None:
+                 allow_mixed: bool = True, resize: int = DATA.resize) -> None:
         paths = [p for p, _ in samples]
         with ThreadPoolExecutor(max_workers=threads) as ex:
             hw = list(ex.map(_header_hw, paths))
@@ -126,7 +126,7 @@ class DecodedCache:
             raise CacheUnavailable("decoded cache needs %.1f GB for %d images, budget %.1f GB "
                                    "(B200_MAX_CACHE_GB)" % (need / 2**30, len(paths), budget / 2**30))
         self.labels = torch.tensor([l for _, l in samples], dtype=torch.int64)
-        self.ragged = bool(paths) and (len(sizes) > 1 or max(hw[0]) > DATA.resize)
+        self.ragged = bool(paths) and (len(sizes) > 1 or max(hw[0]) > resize)
         if self.ragged:
             self._decode_ragged(paths, hw, threads)
             return
@@ -180,8 +180,10 @@ class _FusedLoader:
 
     def __init__(self, cache: DecodedCache, mb: int, train: bool, sampler: Optional[ShardedSampler],
                  shuffle: bool, seed: int, prefetch: int = 3, pin: Optional[bool] = None,
-                 native: Optional[bool] = None, mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0) -> None:
+                 native: Optional[bool] = None, mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0,
+                 resize: int = DATA.resize, crop: int = DATA.crop) -> None:
         self.cache, self.mb, self.train = cache, mb, train
+        self.resize, self.crop = resize, crop          # the network input the batches are cut to
         self.mixup_alpha, self.cutmix_alpha = (mixup_alpha, cutmix_alpha) if train else (0.0, 0.0)
         self.sampler, self.shuffle, self.seed = sampler, shuffle, seed
         self.prefetch = prefetch
@@ -199,7 +201,7 @@ class _FusedLoader:
             self._geom = self._buf((slots, mb, T.GEOM_DIM), torch.int64)
         else:
             H, W = cache.src_hw
-            self.resized_hw = T.resized_dims(train, H, W)
+            self.resized_hw = T.resized_dims(train, H, W, resize)
             self._img = self._buf((slots, mb, H, W, 3), torch.uint8)
             self._geom = None
         self._ring = [(self._img[s], self._par[s], self._lab[s]) for s in range(slots)]
@@ -211,7 +213,7 @@ class _FusedLoader:
                 if ops.available() and hasattr(ops.require(), "Prefetcher"):
                     extra = {}
                     if self.ragged:
-                        extra = dict(offsets=cache.offsets, hw=cache.hw, ring_geom=self._geom, resize=DATA.resize)
+                        extra = dict(offsets=cache.offsets, hw=cache.hw, ring_geom=self._geom, resize=resize)
                     self._pf = ops.require().Prefetcher(
                         cache.flat if self.ragged else cache.images, cache.labels, self._img, self._par, self._lab,
                         train, DATA.crop_scale[0], DATA.crop_scale[1], DATA.crop_ratio[0], DATA.crop_ratio[1],
@@ -248,7 +250,7 @@ class _FusedLoader:
 
     def _draw(self, index: int) -> Optional[T.MixDraw]:
         return T.draw_mix(self.mixup_alpha, self.cutmix_alpha, self.seed, self.epoch,
-                          self.sampler.rank if self.sampler else 0, index)
+                          self.sampler.rank if self.sampler else 0, index, hw=self.crop)
 
     def _batch(self, slot: int, k: int, index: int = 0):
         img, par, lab = self._ring[slot]
@@ -309,7 +311,7 @@ class _FusedLoader:
                 if self.ragged:
                     hw = self.cache.hw[sel]
                     geom = self._geom[slot][:k]
-                    geom.copy_(T.ragged_geometry(hw.tolist(), self.train))
+                    geom.copy_(T.ragged_geometry(hw.tolist(), self.train, self.resize))
                     for i, (h, w) in enumerate(hw.tolist()):
                         off, o, n = int(self.cache.offsets[sel[i]]), int(geom[i, 0]), h * w * 3
                         img[o:o + n].copy_(self.cache.flat[off:off + n])
@@ -342,11 +344,13 @@ class _ReferenceLoader:
     """Synchronous PIL + torchvision loader with the reference's exact semantics."""
 
     def __init__(self, samples, mb: int, train: bool, sampler: Optional[ShardedSampler],
-                 shuffle: bool, seed: int, mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0) -> None:
+                 shuffle: bool, seed: int, mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0,
+                 resize: int = DATA.resize, crop: int = DATA.crop) -> None:
         self.samples, self.mb, self.sampler = samples, mb, sampler
+        self.crop = crop
         self.shuffle, self.seed, self.epoch = shuffle, seed, 0
         self.mixup_alpha, self.cutmix_alpha = (mixup_alpha, cutmix_alpha) if train else (0.0, 0.0)
-        self.tf = T.reference_transforms(train)
+        self.tf = T.reference_transforms(train, resize, crop)
 
     def __len__(self) -> int:
         n = len(self.sampler) if self.sampler is not None else len(self.samples)
@@ -375,7 +379,7 @@ class _ReferenceLoader:
                 ys.append(label)
             x, y = torch.stack(xs), torch.tensor(ys, dtype=torch.int64)
             mix = T.draw_mix(self.mixup_alpha, self.cutmix_alpha, self.seed, self.epoch,
-                             self.sampler.rank if self.sampler else 0, b0 // self.mb)
+                             self.sampler.rank if self.sampler else 0, b0 // self.mb, hw=self.crop)
             if mix is None:
                 yield x, y
             else:       # mixed on the host by torchvision, the draw travels with the batch
@@ -388,10 +392,15 @@ class DataManager:
     def __init__(self, root_folder: str, mini_batch: int, train: bool = True, *,
                  world_size: int = 1, rank: int = 0, pipeline: str = "fused", seed: int = 0,
                  reference_order: bool = False, decode_threads: int = 8, shard_eval: bool = False,
-                 mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0) -> None:
+                 mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0, resize_size: int = DATA.resize,
+                 crop_size: int = DATA.crop) -> None:
+        """``resize_size`` / ``crop_size``: the split's RandomResizedCrop (train) or Resize (val) size and
+        the CenterCrop after it, the network's input (torchvision's --train-crop-size, --val-resize-size,
+        --val-crop-size)."""
         if root_folder is None:
             raise ValueError("-rd/--root_dir is required")
         self.root_folder, self.mb_size, self.train = root_folder, mini_batch, train
+        self.resize_size, self.crop_size = int(resize_size), int(crop_size)
         self.path = os.path.join(root_folder, DATA.train_dir if train else DATA.val_dir)
         self.class_names, self.samples = scan_image_folder(self.path)
         self.number_classes = len(self.class_names)
@@ -404,7 +413,8 @@ class DataManager:
             sampler = ShardedSampler(self.data_size, world_size, rank, shuffle=False, pad=False)
         if pipeline in ("fused", "auto"):
             try:
-                self.cache = DecodedCache(self.samples, decode_threads, allow_mixed=pipeline == "fused")
+                self.cache = DecodedCache(self.samples, decode_threads, allow_mixed=pipeline == "fused",
+                                          resize=self.resize_size)
             except CacheUnavailable as e:
                 if pipeline == "fused":
                     raise
@@ -416,10 +426,12 @@ class DataManager:
         self.pipeline = pipeline = "fused" if pipeline == "auto" else pipeline
         if pipeline == "fused":
             self.loader = _FusedLoader(self.cache, mini_batch, train, sampler, True, seed,
-                                       mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha)
+                                       mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha,
+                                       resize=self.resize_size, crop=self.crop_size)
         elif pipeline == "reference":
             self.loader = _ReferenceLoader(self.samples, mini_batch, train, sampler, True, seed,
-                                           mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha)
+                                           mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha,
+                                           resize=self.resize_size, crop=self.crop_size)
         else:
             raise ValueError("pipeline must be 'fused', 'reference' or 'auto'")
 

@@ -304,21 +304,22 @@ def mixed_targets(labels: torch.Tensor, num_classes: int, mix: Optional[MixDraw]
     return t.transform(labels, params)
 
 
-def reference_transforms(train: bool):
-    """The literal torchvision pipeline of the reference (distributedVggf.py:88-95 / :103-108)."""
+def reference_transforms(train: bool, resize: int = DATA.resize, crop: int = DATA.crop):
+    """The literal torchvision pipeline of the reference (distributedVggf.py:88-95 / :103-108), with
+    its 256 / 224 made ``resize`` / ``crop`` (--train-crop-size, --val-resize-size, --val-crop-size)."""
     from torchvision import transforms as T
 
     norm = T.Normalize(list(DATA.mean), list(DATA.std))
     if train:
         return T.Compose([
-            T.RandomResizedCrop(size=DATA.resize, scale=DATA.crop_scale),
+            T.RandomResizedCrop(size=resize, scale=DATA.crop_scale),
             T.RandomRotation(degrees=DATA.rotation_deg),
             T.RandomHorizontalFlip(),
-            T.CenterCrop(size=DATA.crop),
+            T.CenterCrop(size=crop),
             T.ToTensor(),
             norm,
         ])
-    return T.Compose([T.Resize(size=DATA.resize), T.CenterCrop(size=DATA.crop), T.ToTensor(), norm])
+    return T.Compose([T.Resize(size=resize), T.CenterCrop(size=crop), T.ToTensor(), norm])
 
 
 def torchvision_chain_fixed(img_hwc_u8, params_row, resize: int = DATA.resize, crop: int = DATA.crop) -> torch.Tensor:

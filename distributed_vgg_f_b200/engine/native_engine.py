@@ -20,6 +20,7 @@ Nothing synchronises with the host inside a step; loss / accuracy accumulate in 
 """
 from __future__ import annotations
 
+import math
 import os
 
 from typing import Dict, List, Optional, Tuple
@@ -91,6 +92,21 @@ def deterministic_plan(spec: VGGSpec, batch: int, input_hw: int, sms: int, fused
     return rows
 
 
+# Network input sizes the native engine runs: multiples of 8 keep every odd feature map (a crop that is not
+# a multiple of 32, e.g. 176 -> 11 x 11 before the last pool) to the implicit-GEMM convolutions at <= 64 x 64,
+# never the halo or first-layer kernels.
+NATIVE_HW_MIN, NATIVE_HW_MAX, NATIVE_HW_STEP = 64, 512, 8
+
+
+def check_native_hw(hw: int, what: str = "input_hw") -> int:
+    """``hw`` if the native engine runs it, else ValueError naming the rule."""
+    hw = int(hw)
+    if not (NATIVE_HW_MIN <= hw <= NATIVE_HW_MAX and hw % NATIVE_HW_STEP == 0):
+        raise ValueError("%s = %d: the native engine takes crops that are multiples of %d from %d to %d"
+                         % (what, hw, NATIVE_HW_STEP, NATIVE_HW_MIN, NATIVE_HW_MAX))
+    return hw
+
+
 def deterministic_workspace_elems(plan: list) -> int:
     return max(splits * elems for _, _, splits, elems in plan)
 
@@ -136,7 +152,8 @@ class NativeEngine:
                  optimizer: str = "adam", momentum: float = TRAIN.momentum, weight_decay: float = 0.0,
                  compute_dtype: str = "bf16", allreduce: str = "auto", wire_dtype: str = "bf16",
                  bucket_mb: float = 32.0, seed: int = 0, pretrained_state: Optional[dict] = None,
-                 profile: Optional[str] = None, input_hw: int = DATA.crop, comm_ctas: int = 48,
+                 profile: Optional[str] = None, input_hw: int = DATA.crop, eval_hw: Optional[int] = None,
+                 comm_ctas: int = 48,
                  init_state: Optional[Dict[str, torch.Tensor]] = None, unpack_fp32: bool = False,
                  distributed: bool = True, zero1="auto", conv_bucket_mb: float = 9.5,
                  tail_bucket_kb: float = 2400.0, same_dropout_all_ranks: bool = False,
@@ -163,7 +180,10 @@ class NativeEngine:
         # torchvision's --bias-weight-decay: the biases' own decay (None: the biases take weight_decay)
         self.bias_weight_decay = bias_weight_decay
         self.beta1, self.beta2, self.eps = TRAIN.adam_beta1, TRAIN.adam_beta2, TRAIN.adam_eps
-        self.seed, self.HW = int(seed), int(input_hw)
+        # HW: the network input of training passes; eval_hw: of eval_step / forward_logits (FixRes: train at
+        # a smaller crop than the one evaluated).  AdaptiveAvgPool2d((7, 7)) makes every weight size-free.
+        self.seed, self.HW = int(seed), check_native_hw(input_hw, "input_hw")
+        self.eval_hw = self.HW if eval_hw is None else check_native_hw(eval_hw, "eval_hw")
         if not 0.0 <= label_smoothing < 1.0:
             raise ValueError("label_smoothing must lie in [0, 1) (got %r)" % label_smoothing)
         # training loss only: F.cross_entropy(label_smoothing=); the evaluation loss stays plain
@@ -614,31 +634,58 @@ class NativeEngine:
         # first conv: fused kernels build the im2col operand in shared memory from NHWC4 pixels
         # (csrc/include/conv0.cuh); the explicit im2col matrix only exists for other widths
         self.fused_conv0 = spec.convs[0].cout == 64
-        self.col0 = None if self.fused_conv0 else torch.empty(B * HW * HW, L.CONV0_K, dtype=BF16, device=dev)
-        self.x_nhwc = torch.empty(B, HW, HW, 4, dtype=BF16, device=dev)
-        self.acts: List[torch.Tensor] = []      # post-ReLU conv outputs
-        self.pools: List[Optional[torch.Tensor]] = []
         # On by default (B200_FUSE_POOL=0 turns it off): the pooled layers' conv epilogue pools in
         # registers and records argmax / ReLU bit masks; the un-pooled activation is never written
         # (acts[i] of such a layer then holds stale data) and backward is an "unpool" kernel.
         want_fused_pool = os.environ.get("B200_FUSE_POOL", "1") == "1"
-        self.pool_masks: List[Optional[torch.Tensor]] = []
-        h = HW
-        for i, c in enumerate(spec.convs):
-            self.acts.append(torch.empty(B, h, h, c.cout, dtype=BF16, device=dev))
-            fused = (want_fused_pool and c.pool_after and i > 0 and c.cout % 32 == 0
-                     and bool(ops.require().conv_pool_fusable(B, h, h)))
-            self.pool_masks.append(ops.pool_mask_like(B, h, h, c.cout, dev) if fused else None)
-            if c.pool_after:
-                h //= 2
-                self.pools.append(torch.empty(B, h, h, c.cout, dtype=BF16, device=dev))
-            else:
-                self.pools.append(None)
-        self.feat_hw = h
         cl = spec.convs[-1].cout
         ph = spec.pooled_hw
         assert spec.fcs[0].fin == cl * ph * ph, "classifier.0 must consume the pooled feature map"
-        self.avg = None if h == ph else torch.empty(B, ph, ph, cl, dtype=BF16, device=dev)
+        # The buffers of every size-dependent tensor hold the larger of the training and evaluation sizes;
+        # each pass takes views at its own size (_set_hw).  An evaluation pass runs between training
+        # steps, never between a step's forward and backward, so it may reuse them.
+        shapes = {}
+        for hw in sorted({self.HW, self.eval_hw}):
+            g = dict(x_nhwc=(B, hw, hw, 4), acts=[], pools=[], masks=[])
+            if not self.fused_conv0:
+                g["col0"] = (B * hw * hw, L.CONV0_K)
+            h = hw
+            for i, c in enumerate(spec.convs):
+                g["acts"].append((B, h, h, c.cout))
+                fused = (want_fused_pool and c.pool_after and i > 0 and c.cout % 32 == 0
+                         and bool(ops.require().conv_pool_fusable(B, h, h)))
+                g["masks"].append(tuple(ops.pool_mask_like(B, h, h, c.cout, "meta").shape) if fused else None)
+                if c.pool_after:
+                    h //= 2
+                g["pools"].append((B, h, h, c.cout) if c.pool_after else None)
+            g["feat_hw"] = h
+            shapes[hw] = g
+
+        def arena(key, dtype, zero=False, i=None):
+            """One buffer for slot ``key`` (layer ``i``), large enough for every size; {hw: view}."""
+            want = {hw: (g[key] if i is None else g[key][i]) for hw, g in shapes.items()}
+            n = max((math.prod(v) for v in want.values() if v is not None), default=0)
+            if not n:
+                return {hw: None for hw in want}
+            buf = (torch.zeros if zero else torch.empty)(n, dtype=dtype, device=dev)
+            return {hw: None if v is None else buf[:math.prod(v)].view(v) for hw, v in want.items()}
+
+        col0 = arena("col0", BF16) if not self.fused_conv0 else {hw: None for hw in shapes}
+        x_nhwc = arena("x_nhwc", BF16)
+        acts, pools, masks = [], [], []
+        for i in range(len(spec.convs)):
+            acts.append(arena("acts", BF16, i=i))
+            masks.append(arena("masks", torch.int32, zero=True, i=i))
+            pools.append(arena("pools", BF16, i=i))
+        avg = None
+        if any(g["feat_hw"] != ph for g in shapes.values()):
+            avg = torch.empty(B, ph, ph, cl, dtype=BF16, device=dev)
+        self._geo = {hw: dict(x_nhwc=x_nhwc[hw], col0=col0[hw], acts=[a[hw] for a in acts],
+                              pools=[p[hw] for p in pools], pool_masks=[m[hw] for m in masks],
+                              feat_hw=g["feat_hw"], avg=None if g["feat_hw"] == ph else avg)
+                     for hw, g in shapes.items()}
+        self._hw = None
+        self._set_hw(self.HW)
         # FC stack
         self.fc_acc = [torch.zeros(B, f.fout, dtype=F32, device=dev) for f in spec.fcs]
         self.fc_y = [torch.empty(B, f.fout, dtype=BF16, device=dev) if i < len(spec.fcs) - 1 else None
@@ -655,7 +702,7 @@ class NativeEngine:
                            and bool(ops.require().head_ce_supported(B, lastf.fout, lastf.fin)))
         self._head_in = None
         # backward activations-gradients: two ping-pong buffers big enough for the largest map
-        biggest = max(a.numel() for a in self.acts)
+        biggest = max(a.numel() for g in self._geo.values() for a in g["acts"])
         self.dbuf = [torch.empty(biggest, dtype=BF16, device=dev) for _ in range(2)]
         self.dfeat = torch.empty(B, ph, ph, cl, dtype=BF16, device=dev)
         if self.deterministic:
@@ -663,11 +710,21 @@ class NativeEngine:
             plan = deterministic_plan(spec, B, HW, ops.require().sm_count(), self.fused_head, self.freeze_layers)
             self._ws = torch.empty(deterministic_workspace_elems(plan), dtype=F32, device=dev)
 
+    def _set_hw(self, hw: int) -> None:
+        """Point the size-dependent buffers (input, activations, pools, pool masks, feature map) at the
+        views of a pass at network input ``hw``."""
+        if hw == self._hw:
+            return
+        g = self._geo[hw]
+        self.x_nhwc, self.col0, self.acts, self.pools = g["x_nhwc"], g["col0"], g["acts"], g["pools"]
+        self.pool_masks, self.feat_hw, self.avg = g["pool_masks"], g["feat_hw"], g["avg"]
+        self._hw = hw
+
     # ================================================================================ inputs
     def _stage_input(self, batch) -> int:
         """Copy a batch to the device and produce the first conv's im2col rows.  Returns b."""
         C = ops.require()
-        HW = self.HW
+        HW = self._hw
         j = self._in_slot
         self._in_slot ^= 1
         self.labels_dev = self._labels_dev[j]
@@ -732,7 +789,7 @@ class NativeEngine:
             self._mix = batch[2]
         b = int(y.shape[0])
         x = x.to(self.device, F32, non_blocking=True).contiguous()
-        assert x.shape[2] == HW and x.shape[3] == HW, "input size differs from the engine's input_hw"
+        assert x.shape[2] == HW and x.shape[3] == HW, "input size differs from the pass's size (input_hw / eval_hw)"
         self.labels_dev[:b].copy_(y, non_blocking=True)
         C.nchw_to_nhwc(x, self.x_nhwc[:b])
         if not self.fused_conv0:
@@ -763,7 +820,7 @@ class NativeEngine:
 
     def _forward(self, b: int, train: bool) -> None:
         C = ops.require()
-        spec, HW = self.spec, self.HW
+        spec, HW = self.spec, self._hw
         c0 = spec.convs[0]
         M0 = b * HW * HW
         # conv0 (K = 27): im2col GEMM with fused bias + ReLU -> bf16 NHWC
@@ -1169,6 +1226,7 @@ class NativeEngine:
             torch.cuda.nvtx.range_push("step")
         self._mark("step start")
         t.start("input")
+        self._set_hw(self.HW)
         b = self._stage_input(batch)
         t.stop("input")
         self._mark("input")
@@ -1198,6 +1256,7 @@ class NativeEngine:
         """Evaluation forward, loss and metrics; ``ema``: with the moving average of the weights
         (after prepare_ema())."""
         self._use_weights(ema)
+        self._set_hw(self.eval_hw)
         try:
             b = self._stage_input(batch)
             self._forward(b, train=False)
@@ -1205,10 +1264,12 @@ class NativeEngine:
             self._release_input()
         finally:
             self._use_weights(False)
+            self._set_hw(self.HW)
         return self.loss_buf
 
     def forward_logits(self, batch, ema: bool = False) -> torch.Tensor:
         self._use_weights(ema)
+        self._set_hw(self.eval_hw)
         try:
             b = self._stage_input(batch)
             self._forward(b, train=False)
@@ -1220,6 +1281,7 @@ class NativeEngine:
             self._release_input()
         finally:
             self._use_weights(False)
+            self._set_hw(self.HW)
         return self.logits[:b].clone()
 
     def _use_weights(self, ema: bool) -> None:

@@ -240,9 +240,10 @@ def conv0_wgrad64(dz: torch.Tensor, x4: torch.Tensor):
 
 
 def pool_windows(t: torch.Tensor) -> torch.Tensor:
-    """[N,H,W,C] -> [N,H/2,W/2,C,4]: the 2x2 windows in the order (0,0), (0,1), (1,0), (1,1)."""
+    """[N,H,W,C] -> [N,H/2,W/2,C,4]: the 2x2 windows in the order (0,0), (0,1), (1,0), (1,1).  Floor mode:
+    an odd last row / column lies in no window."""
     N, H, W, C = t.shape
-    v = t.reshape(N, H // 2, 2, W // 2, 2, C)
+    v = t[:, :H // 2 * 2, :W // 2 * 2].reshape(N, H // 2, 2, W // 2, 2, C)
     return v.permute(0, 1, 3, 5, 2, 4).reshape(N, H // 2, W // 2, C, 4)
 
 
@@ -319,7 +320,11 @@ def maxpool2x2_relu_bwd64(y: torch.Tensor, dp: torch.Tensor):
     """Backward of [ReLU -> maxpool2x2] from the stored post-ReLU map y: dp goes to the first maximum
     of each window whose maximum is > 0.  Returns (dz, column sum of dz, column sum of |dz|)."""
     val, idx = maxpool2x2_64(y)
-    return unpool2x2_64(dp, idx, val > 0)
+    dz, cs, mag = unpool2x2_64(dp, idx, val > 0)
+    H, W = y.shape[1], y.shape[2]
+    if (H, W) != dz.shape[1:3]:         # floor mode: the odd last row / column gets dz = 0
+        dz = F.pad(dz, (0, 0, 0, W - dz.shape[2], 0, H - dz.shape[1]))
+    return dz, cs, mag
 
 
 def _ap_windows(n_in: int, n_out: int):

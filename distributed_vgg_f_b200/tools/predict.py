@@ -1,9 +1,10 @@
 """Classify images with a checkpoint written by ``--save``.
 
 The reference stops at the per-epoch validation line; this is the missing last step for a user who
-trained a model: load the checkpoint (its ``args`` record the architecture), apply the reference's
-validation transform (Resize 256 -> CenterCrop 224 -> Normalize, distributedVggf.py:103-108) and
-print one line per image::
+trained a model: load the checkpoint (its ``args`` record the architecture and the input sizes), apply
+the reference's validation transform (Resize 256 -> CenterCrop 224 -> Normalize, distributedVggf.py:103-108,
+or the run's --val-resize-size / --val-crop-size; ``--resize`` / ``--crop`` override them) and print one
+line per image::
 
     python -m distributed_vgg_f_b200.tools.predict ck.pt --classes edible,other,toy img1.png img2.png
     python -m distributed_vgg_f_b200.tools.predict ck.pt --data-root /data/coil3 /data/coil3/ValidationData/toy
@@ -39,8 +40,16 @@ def expand(paths: Sequence[str]) -> List[str]:
     return out
 
 
-def load_model(checkpoint: str, model: Optional[str] = None, num_classes: Optional[int] = None, ema: bool = False):
-    """(spec, torch-layout state) of a checkpoint; ``ema``: its moving average of the weights (--model-ema)."""
+def eval_sizes(saved: dict):
+    """(resize, crop) of the validation transform a run used, from the checkpoint's ``"args"`` (the reference's
+    256 / 224 for a checkpoint that records none)."""
+    return int(saved.get("val_resize_size") or DATA.resize), int(saved.get("val_crop_size") or DATA.crop)
+
+
+def load_model(checkpoint: str, model: Optional[str] = None, num_classes: Optional[int] = None, ema: bool = False,
+               with_args: bool = False):
+    """(spec, torch-layout state) of a checkpoint; ``ema``: its moving average of the weights (--model-ema);
+    ``with_args``: also the ``"args"`` the checkpoint's run recorded."""
     payload = torch.load(checkpoint, map_location="cpu", weights_only=True)
     if ema:
         if not isinstance(payload, dict) or "model_ema" not in payload:
@@ -52,23 +61,40 @@ def load_model(checkpoint: str, model: Optional[str] = None, num_classes: Option
     last = [k for k in state if k.endswith(".weight")][-1]
     classes = num_classes or int(state[last].shape[0])
     spec = get_spec(model or saved.get("model") or "vggf", classes)
-    return spec, state
+    return (spec, state, saved) if with_args else (spec, state)
 
 
 @torch.no_grad()
 def predict(checkpoint: str, images: Sequence[str], model: Optional[str] = None, engine: str = "auto",
-            batch: int = 32, ema: bool = False):
-    """Returns (logits [n, C] fp32 on the CPU, files)."""
+            batch: int = 32, ema: bool = False, resize: Optional[int] = None, crop: Optional[int] = None):
+    """Returns (logits [n, C] fp32 on the CPU, files).  ``resize`` / ``crop``: the validation transform's
+    sizes (default: the ones recorded in the checkpoint)."""
     from PIL import Image
 
-    spec, state = load_model(checkpoint, model, ema=ema)
+    spec, state, saved = load_model(checkpoint, model, ema=ema, with_args=True)
     files = expand(images)
-    tf = reference_transforms(train=False)
+    saved_resize, saved_crop = eval_sizes(saved)
+    resize, crop = resize or saved_resize, crop or saved_crop
+    if crop > resize:
+        raise ValueError("crop %d exceeds resize %d: the crop must lie inside the resized image" % (crop, resize))
+    tf = reference_transforms(False, resize, crop)
+    from ..engine.native_engine import check_native_hw
+
+    def native_runs(hw):
+        try:
+            check_native_hw(hw)
+            return True
+        except ValueError:
+            return False
+
+    # auto: the native engine on an H100 at a crop it runs, else the oracle (which takes any crop >= 32);
+    # --engine native at a crop it does not run is refused by the engine
     use_native = engine == "native" or (engine == "auto" and torch.cuda.is_available()
-                                        and torch.cuda.get_device_capability() == (9, 0))
+                                        and torch.cuda.get_device_capability() == (9, 0) and native_runs(crop))
     if use_native:
         from ..engine.native_engine import NativeEngine
-        net = NativeEngine(spec, device=torch.device("cuda", 0), batch=batch, init_state=state, distributed=False)
+        net = NativeEngine(spec, device=torch.device("cuda", 0), batch=batch, init_state=state, distributed=False,
+                           input_hw=crop)
     else:
         net = build_oracle(spec, seed=0).eval()
         net.load_state_dict(state)
@@ -92,8 +118,13 @@ def main(argv=None) -> int:
     ap.add_argument("--engine", default="auto", choices=["auto", "native", "oracle"])
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--ema", action="store_true", help="classify with the checkpoint's EMA weights (--model-ema)")
+    ap.add_argument("--resize", type=int, default=None,
+                    help="Resize of the shorter side (default: the checkpoint's --val-resize-size, else %d)" % DATA.resize)
+    ap.add_argument("--crop", type=int, default=None,
+                    help="CenterCrop, the network's input (default: the checkpoint's --val-crop-size, else %d)" % DATA.crop)
     a = ap.parse_args(argv)
-    logits, files = predict(a.checkpoint, a.images, a.model, a.engine, a.batch, ema=a.ema)
+    logits, files = predict(a.checkpoint, a.images, a.model, a.engine, a.batch, ema=a.ema, resize=a.resize,
+                            crop=a.crop)
     names = a.classes.split(",") if a.classes else None
     if names is None and a.data_root:
         names = find_classes(os.path.join(a.data_root, DATA.train_dir))[0]

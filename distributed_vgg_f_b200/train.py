@@ -19,6 +19,7 @@ import time
 
 import torch
 
+from .cli import input_sizes
 from .data.loader import DataManager
 from .models.vggf import build_oracle, freeze_leading_layers_, get_spec
 from .parallel.ddp import FlatDDP
@@ -119,17 +120,23 @@ def manage_training(args) -> Trainer:
 
     dm_kw = dict(world_size=args.world_size, rank=args.rank, pipeline=args.pipeline,
                  seed=args.seed, reference_order=args.reference_order)
+    sizes = input_sizes(args)
     train_data_mngr = DataManager(args.root_dir, args.mini_batch, train=True,
                                   mixup_alpha=getattr(args, "mixup_alpha", 0.0),
-                                  cutmix_alpha=getattr(args, "cutmix_alpha", 0.0), **dm_kw)
+                                  cutmix_alpha=getattr(args, "cutmix_alpha", 0.0),
+                                  resize_size=sizes["train_resize_size"], crop_size=sizes["train_crop_size"], **dm_kw)
     valid_data_mngr = DataManager(args.root_dir, args.mini_batch, train=False,
-                                  shard_eval=getattr(args, "shard_eval", False), **dm_kw)
+                                  shard_eval=getattr(args, "shard_eval", False),
+                                  resize_size=sizes["val_resize_size"], crop_size=sizes["val_crop_size"], **dm_kw)
     train_loader, valid_loader = train_data_mngr.get_loader(), valid_data_mngr.get_loader()
 
     num_classes = args.num_classes or train_data_mngr.number_classes
     print("[Info] number of classes: {}".format(num_classes))
     print("[Info] class labels: {}".format(train_data_mngr.class_names))
     print("[Info] Running instance {} using {}".format(args.rank, device_name(device)))
+    if sizes != input_sizes(None):
+        print("[Info] input sizes: train RandomResizedCrop {} -> crop {}, eval Resize {} -> crop {}".format(
+            sizes["train_resize_size"], sizes["train_crop_size"], sizes["val_resize_size"], sizes["val_crop_size"]))
 
     spec = get_spec(args.model, num_classes)
     pretrained = torch.load(args.pretrained, map_location="cpu") if args.pretrained else None
@@ -162,7 +169,8 @@ def manage_training(args) -> Trainer:
                              bias_weight_decay=getattr(args, "bias_weight_decay", None),
                              deterministic=getattr(args, "deterministic", False), freeze_layers=freeze,
                              powersgd_rank=getattr(args, "powersgd_rank", 0),
-                             powersgd_start_iter=getattr(args, "powersgd_start_iter", 1000))
+                             powersgd_start_iter=getattr(args, "powersgd_start_iter", 1000),
+                             input_hw=sizes["train_crop_size"], eval_hw=sizes["val_crop_size"])
         optimizer = None            # fused into the engine
         model_ema = True if ema_decay is not None else None       # kept by the engine's optimizer kernels
         if model.world > 1:
@@ -226,6 +234,8 @@ def manage_training(args) -> Trainer:
                 torch.distributed.barrier()
         if args.log_jsonl and args.rank == 0:
             rec = dict(trainer.history[-1], time=time.time(), world_size=args.world_size)
+            if sizes != input_sizes(None):
+                rec["input_sizes"] = sizes
             if not schedule.constant:
                 rec["lr"] = epoch_lr
             if hasattr(model, "phase_times"):

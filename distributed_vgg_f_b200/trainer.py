@@ -37,6 +37,7 @@ from typing import Optional
 import torch
 import torch.nn.functional as F
 
+from .config import DATA
 from .data import transforms as T
 from .data.loader import FusedBatch, RaggedBatch
 from .utils.metrics import DeviceMeter
@@ -181,9 +182,9 @@ class Trainer:
         return ", {:.0f} TFLOP/s ({:.0f}% of the bf16 peak)".format(tflops, 100.0 * tflops / _bf16_peak())
 
     # ------------------------------------------------------------------------------------------
-    def _to_device(self, batch):
-        if isinstance(batch, (FusedBatch, RaggedBatch)):
-            return batch.to_float(self.device)
+    def _to_device(self, batch, loader=None):
+        if isinstance(batch, (FusedBatch, RaggedBatch)):     # cut to the network input its loader is set to
+            return batch.to_float(self.device, out_hw=getattr(loader, "crop", DATA.crop))
         inputs, targets = batch[0], batch[1]
         return inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
 
@@ -191,7 +192,7 @@ class Trainer:
         """(inputs, integer targets, probability targets or None) of a training batch: the batch's
         MixUp / CutMix draw applied by torchvision (the reference pipeline has applied it already)."""
         mix = batch.mix if isinstance(batch, (FusedBatch, RaggedBatch)) else (batch[2] if len(batch) > 2 else None)
-        inputs, targets = self._to_device(batch)
+        inputs, targets = self._to_device(batch, self.train_loader)
         if mix is None:
             return inputs, targets, None
         if isinstance(batch, (FusedBatch, RaggedBatch)):
@@ -304,7 +305,7 @@ class Trainer:
         net.eval()
         with torch.no_grad():
             for batch in self.test_loader:
-                inputs, targets = self._to_device(batch)
+                inputs, targets = self._to_device(batch, self.test_loader)
                 outputs = net(inputs)
                 meter.add_reference(outputs, targets)
         return self._reduce_eval(meter)
