@@ -363,15 +363,12 @@ struct Zero1Args {
   float* grad;             // local fp32 arena (nullptr: wire already holds the packed data)
   float* p; float* m; float* v;
   bf16* shadow;
+  float* ema;              // moving average of the weights (zero1_kernel<..., true, ...>)
   long long start, n;
   float inv_world;
   int slot;
   uint32_t epoch;
-  float lr, b1, b2, eps, wd, bc1_inv, bc2_inv_sqrt;
-  float keep;              // AdamW (zero1_kernel<..., true>): fp32(1 - lr * wd), as adam_kernel's segment value
-  float* ema;              // moving average of the weights (zero1_kernel<true>), as adam_kernel<true>
-  float ema_d, ema_a;
-  int ema_first;
+  OptStep o;               // Adam or AdamW, one decay (o.wd.value[0]) for the whole range
 };
 
 template <bool EMA, bool DECOUPLED>
@@ -394,25 +391,15 @@ __device__ __forceinline__ uint4 zero1_adam8(const Zero1Args& a, long long elem,
     vv[4 * h] = v4.x; vv[4 * h + 1] = v4.y; vv[4 * h + 2] = v4.z; vv[4 * h + 3] = v4.w;
   }
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {          // the update of adam_kernel at grad_scale 1, bit for bit
-    if constexpr (DECOUPLED)
-      adamw_update(g[k], 1.f, pp[k], mm[k], vv[k], a.lr * a.bc1_inv, a.b1, a.b2, a.eps, a.keep, a.bc2_inv_sqrt);
-    else
-      adam_update(g[k], 1.f, pp[k], mm[k], vv[k], a.lr * a.bc1_inv, a.b1, a.b2, a.eps, a.wd, a.bc2_inv_sqrt);
-  }
+  for (int k = 0; k < 8; ++k)            // the update of adam_kernel at grad_scale 1, bit for bit
+    optimizer_update<DECOUPLED ? OPT_ADAMW : OPT_ADAM>(a.o, g[k], 1.f, a.o.wd.value[0], pp[k], mm[k], vv[k]);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     __stcs(reinterpret_cast<float4*>(a.p + elem + 4 * h), make_float4(pp[4 * h], pp[4 * h + 1], pp[4 * h + 2], pp[4 * h + 3]));
     __stcs(reinterpret_cast<float4*>(a.m + elem + 4 * h), make_float4(mm[4 * h], mm[4 * h + 1], mm[4 * h + 2], mm[4 * h + 3]));
     __stcs(reinterpret_cast<float4*>(a.v + elem + 4 * h), make_float4(vv[4 * h], vv[4 * h + 1], vv[4 * h + 2], vv[4 * h + 3]));
-    if constexpr (EMA) {                 // one half at a time: 4 more live floats next to the Adam state
-      float4 e4 = __ldcs(reinterpret_cast<const float4*>(a.ema + elem + 4 * h));
-      e4.x = ema_update(e4.x, pp[4 * h], a.ema_d, a.ema_a, a.ema_first);
-      e4.y = ema_update(e4.y, pp[4 * h + 1], a.ema_d, a.ema_a, a.ema_first);
-      e4.z = ema_update(e4.z, pp[4 * h + 2], a.ema_d, a.ema_a, a.ema_first);
-      e4.w = ema_update(e4.w, pp[4 * h + 3], a.ema_d, a.ema_a, a.ema_first);
-      __stcs(reinterpret_cast<float4*>(a.ema + elem + 4 * h), e4);
-    }
+    // one half at a time: 4 more live floats next to the Adam state
+    if constexpr (EMA) ema_update4(a.ema + elem + 4 * h, pp + 4 * h, a.o.ema);
   }
   return make_uint4(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3]), pack_bf16x2(pp[4], pp[5]),
                     pack_bf16x2(pp[6], pp[7]));
@@ -488,43 +475,33 @@ __global__ void __launch_bounds__(Z1_THREADS, Z1_MIN_BLOCKS) zero1_kernel(const 
     __stcs(reinterpret_cast<uint4*>(sh + v * 8), ld_v4(my_wire + v * 16));
 }
 
-void zero1_step(const CommCtx& ctx, float* grad_f32, float* p, float* m, float* v, bf16* shadow,
-                long long start, long long n, float inv_world, int algo, int slot, uint32_t epoch, int max_ctas,
-                float lr, float beta1, float beta2, float eps, float weight_decay, int step, cudaStream_t s,
-                float* ema, double ema_decay, bool ema_first, bool decoupled, float keep) {
+void zero1_step(const CommCtx& ctx, const OptStep& o, float* grad_f32, float* p, float* m, float* v, bf16* shadow,
+                float* ema, long long start, long long n, float inv_world, int algo, int slot, uint32_t epoch,
+                int max_ctas, cudaStream_t s) {
   if (ctx.world > AR_MAX_WORLD) throw std::runtime_error("[b200] zero1_step: world too large");
   if (n % 8 || start % 8) throw std::runtime_error("[b200] zero1_step: range must be 8-element aligned");
   if (algo == AR_NVLS && !ctx.wire_mc) throw std::runtime_error("[b200] zero1_step: NVLS needs a multicast mapping");
   if (algo != AR_NVLS && algo != AR_TWOSHOT) throw std::runtime_error("[b200] zero1_step: two-shot or NVLS only");
+  if (o.kind == OPT_SGD || o.wd.n != 1 || o.grad_scale != 1.f)
+    throw std::runtime_error("[b200] zero1_step: Adam or AdamW with one weight decay and grad_scale 1 only");
   Zero1Args a;
-  a.c = ctx; a.grad = grad_f32; a.p = p; a.m = m; a.v = v; a.shadow = shadow; a.start = start; a.n = n;
-  a.inv_world = inv_world; a.slot = slot; a.epoch = epoch;
-  a.lr = lr; a.b1 = beta1; a.b2 = beta2; a.eps = eps; a.wd = weight_decay; a.keep = keep;
-  a.bc1_inv = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(beta1), step)));
-  a.bc2_inv_sqrt = static_cast<float>(1.0 / sqrt(1.0 - pow(static_cast<double>(beta2), step)));
-  a.ema = ema; a.ema_first = ema_first ? 1 : 0;
-  a.ema_d = ema ? static_cast<float>(ema_decay) : 0.f;
-  a.ema_a = ema ? static_cast<float>(1.0 - ema_decay) : 0.f;
+  a.c = ctx; a.grad = grad_f32; a.p = p; a.m = m; a.v = v; a.shadow = shadow; a.ema = ema; a.start = start; a.n = n;
+  a.inv_world = inv_world; a.slot = slot; a.epoch = epoch; a.o = o;
   const int G = allreduce_grid(n, ctx.world, max_ctas, false);
-  static const bool carve = [] {
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, false, false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, false, false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, true, false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, true, false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, false, true>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, false, true>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_NVLS, true, true>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(zero1_kernel<AR_TWOSHOT, true, true>));
-    return true;
-  }();
-  (void)carve;
   using Kernel = void (*)(const Zero1Args);
-  static const Kernel kernels[2][2][2] = {
+  static const Kernel kernels[2][2][2] = {   // [NVLS][EMA][DECOUPLED]
       {{zero1_kernel<AR_TWOSHOT, false, false>, zero1_kernel<AR_TWOSHOT, false, true>},
        {zero1_kernel<AR_TWOSHOT, true, false>, zero1_kernel<AR_TWOSHOT, true, true>}},
       {{zero1_kernel<AR_NVLS, false, false>, zero1_kernel<AR_NVLS, false, true>},
        {zero1_kernel<AR_NVLS, true, false>, zero1_kernel<AR_NVLS, true, true>}}};
-  kernels[algo == AR_NVLS][ema != nullptr][decoupled]<<<G, Z1_THREADS, 0, s>>>(a);
+  static const bool carve = [] {
+    for (const auto& by_ema : kernels)
+      for (const auto& by_kind : by_ema)
+        for (Kernel k : by_kind) prefer_max_shared_carveout(reinterpret_cast<const void*>(k));
+    return true;
+  }();
+  (void)carve;
+  kernels[algo == AR_NVLS][ema != nullptr][o.kind == OPT_ADAMW]<<<G, Z1_THREADS, 0, s>>>(a);
   count_launch();
   check_last("zero1_step");
 }

@@ -346,33 +346,23 @@ static void check_ema(const c10::optional<at::Tensor>& ema, int64_t n, double de
   TORCH_CHECK(ema->numel() == n, op, ": ema must have p's size");
   TORCH_CHECK(decay >= 0.0 && decay <= 1.0, op, ": ema_decay must lie in [0, 1], got ", decay);
 }
-// The weight-decay segments of one optimizer launch over n elements (WdSegments, api.h).  Without
-// `starts` the decay is `wd` everywhere; otherwise segment k covers [starts[k], starts[k + 1]) with decay
-// wds[k] (and `wd` is not used).  Starts must begin at 0, increase, be whole float4s and lie inside the
-// range; decays must be finite and >= 0.  decoupled (AdamW): the kernel takes keep = fp32(1 - lr * wd),
-// computed here in double as torch computes the Python scalar.
-static b200::WdSegments wd_segments(const char* op, int64_t n, double wd, const std::vector<int64_t>& starts,
-                                    const std::vector<double>& wds, bool decoupled, double lr) {
-  auto value = [&](double d) { return decoupled ? (float)(1.0 - lr * d) : (float)d; };
-  if (starts.empty()) {
-    TORCH_CHECK(wds.empty(), op, ": wd_starts and wd_values go together");
-    return b200::uniform_wd(value(wd));
-  }
-  TORCH_CHECK(starts.size() == wds.size(), op, ": wd_starts and wd_values must have the same length");
-  TORCH_CHECK((int)starts.size() <= b200::WD_MAX_SEGMENTS, op, ": at most ", b200::WD_MAX_SEGMENTS,
-              " weight-decay segments per launch, got ", starts.size());
-  TORCH_CHECK(starts[0] == 0, op, ": the first weight-decay segment must start at 0");
-  b200::WdSegments s{};
-  s.n = (int)starts.size();
-  for (size_t k = 0; k < starts.size(); ++k) {
-    TORCH_CHECK(k == 0 || starts[k] > starts[k - 1], op, ": weight-decay segment starts must increase");
-    TORCH_CHECK(starts[k] % 4 == 0, op, ": weight-decay segment starts must be multiples of 4, got ", starts[k]);
-    TORCH_CHECK(starts[k] < n, op, ": weight-decay segment start ", starts[k], " lies outside the range of ", n);
-    TORCH_CHECK(std::isfinite(wds[k]) && wds[k] >= 0.0, op, ": weight decays must be finite and >= 0, got ", wds[k]);
-    s.start4[k] = starts[k] / 4;
-    s.value[k] = value(wds[k]);
-  }
-  return s;
+// The operands of one adam / sgd launch over p's n elements: the fp32 state (p first), exactly one of the
+// fp32 and bf16 gradients, and the optional shadow, gradient range to clear and moving average.
+static void check_optimizer(const char* op, const char* state_names, std::initializer_list<const at::Tensor*> state,
+                            const c10::optional<at::Tensor>& g32, const c10::optional<at::Tensor>& g16,
+                            const c10::optional<at::Tensor>& shadow, const c10::optional<at::Tensor>& gzero,
+                            const c10::optional<at::Tensor>& ema, double ema_decay) {
+  const int64_t n = (*state.begin())->numel();
+  for (const at::Tensor* t : state) check_vec(*t, at::kFloat, 16, op, state_names);
+  check_ema(ema, n, ema_decay, op);
+  if (g32.has_value()) check_vec(*g32, at::kFloat, 16, op, "g32");
+  if (gzero.has_value()) check_vec(*gzero, at::kFloat, 16, op, "gzero");
+  if (g16.has_value()) check_vec(*g16, at::kBFloat16, 8, op, "g16");
+  if (shadow.has_value()) check_vec(*shadow, at::kBFloat16, 8, op, "shadow");
+  TORCH_CHECK(g32.has_value() != g16.has_value(), op, ": exactly one of g32 and g16");
+  for (const auto* t : {&g32, &g16, &shadow, &gzero})
+    TORCH_CHECK(!t->has_value() || (*t)->numel() == n, op, ": every tensor has p's size");
+  for (const at::Tensor* t : state) TORCH_CHECK(t->numel() == n, op, ": every tensor has p's size");
 }
 
 static void adam(at::Tensor p, at::Tensor m, at::Tensor v, c10::optional<at::Tensor> g32,
@@ -381,43 +371,25 @@ static void adam(at::Tensor p, at::Tensor m, at::Tensor v, c10::optional<at::Ten
                  c10::optional<at::Tensor> ema, double ema_decay, bool ema_first, bool decoupled,
                  const std::vector<int64_t>& wd_starts, const std::vector<double>& wd_values) {
   c10::cuda::CUDAGuard g(p.device());
-  const int64_t n = p.numel();
-  for (auto* t : {&p, &m, &v}) check_vec(*t, at::kFloat, 16, "adam", "p, m and v");
-  check_ema(ema, n, ema_decay, "adam");
-  if (g32.has_value()) check_vec(*g32, at::kFloat, 16, "adam", "g32");
-  if (gzero.has_value()) check_vec(*gzero, at::kFloat, 16, "adam", "gzero");
-  if (g16.has_value()) check_vec(*g16, at::kBFloat16, 8, "adam", "g16");
-  if (shadow.has_value()) check_vec(*shadow, at::kBFloat16, 8, "adam", "shadow");
-  TORCH_CHECK(g32.has_value() != g16.has_value(), "adam: exactly one of g32 and g16");
-  for (const auto* t : {&g32, &g16, &shadow, &gzero})
-    TORCH_CHECK(!t->has_value() || (*t)->numel() == n, "adam: every tensor has p's size");
-  TORCH_CHECK(m.numel() == n && v.numel() == n, "adam: every tensor has p's size");
-  const b200::WdSegments segs = wd_segments("adam", n, wd, wd_starts, wd_values, decoupled, lr);
-  b200::adam_fused(f32p(p), f32p(m), f32p(v), f32p_opt(g32), bfp_opt(g16),
-                   shadow.has_value() ? bfp_mut(*shadow) : nullptr, p.numel(), (float)lr, (float)b1, (float)b2,
-                   (float)eps, segs, (int)step, (float)grad_scale, false, f32p_opt(gzero), cur_stream(),
-                   f32p_opt(ema), ema_decay, ema_first, decoupled);
+  check_optimizer("adam", "p, m and v", {&p, &m, &v}, g32, g16, shadow, gzero, ema, ema_decay);
+  const b200::OptStep o =
+      b200::make_opt_step("adam", decoupled ? b200::OPT_ADAMW : b200::OPT_ADAM, p.numel(), lr, b1, b2, eps, 0.0,
+                          (int)step, false, grad_scale, wd, wd_starts, wd_values, ema_decay, ema_first);
+  b200::optimizer_fused(o, f32p(p), f32p(m), f32p(v), f32p_opt(g32), bfp_opt(g16),
+                        shadow.has_value() ? bfp_mut(*shadow) : nullptr, f32p_opt(gzero), f32p_opt(ema), p.numel(),
+                        cur_stream());
 }
 static void sgd(at::Tensor p, at::Tensor mom, c10::optional<at::Tensor> g32, c10::optional<at::Tensor> g16,
                 c10::optional<at::Tensor> shadow, double lr, double momentum, double wd, bool first,
                 double grad_scale, c10::optional<at::Tensor> gzero, c10::optional<at::Tensor> ema, double ema_decay,
                 bool ema_first, const std::vector<int64_t>& wd_starts, const std::vector<double>& wd_values) {
   c10::cuda::CUDAGuard g(p.device());
-  const int64_t n = p.numel();
-  for (auto* t : {&p, &mom}) check_vec(*t, at::kFloat, 16, "sgd", "p and mom");
-  check_ema(ema, n, ema_decay, "sgd");
-  if (g32.has_value()) check_vec(*g32, at::kFloat, 16, "sgd", "g32");
-  if (gzero.has_value()) check_vec(*gzero, at::kFloat, 16, "sgd", "gzero");
-  if (g16.has_value()) check_vec(*g16, at::kBFloat16, 8, "sgd", "g16");
-  if (shadow.has_value()) check_vec(*shadow, at::kBFloat16, 8, "sgd", "shadow");
-  TORCH_CHECK(g32.has_value() != g16.has_value(), "sgd: exactly one of g32 and g16");
-  for (const auto* t : {&g32, &g16, &shadow, &gzero})
-    TORCH_CHECK(!t->has_value() || (*t)->numel() == n, "sgd: every tensor has p's size");
-  TORCH_CHECK(mom.numel() == n, "sgd: every tensor has p's size");
-  const b200::WdSegments segs = wd_segments("sgd", n, wd, wd_starts, wd_values, false, lr);
-  b200::sgd_fused(f32p(p), f32p(mom), f32p_opt(g32), bfp_opt(g16), shadow.has_value() ? bfp_mut(*shadow) : nullptr,
-                  p.numel(), (float)lr, (float)momentum, segs, first, (float)grad_scale, f32p_opt(gzero),
-                  cur_stream(), f32p_opt(ema), ema_decay, ema_first);
+  check_optimizer("sgd", "p and mom", {&p, &mom}, g32, g16, shadow, gzero, ema, ema_decay);
+  const b200::OptStep o = b200::make_opt_step("sgd", b200::OPT_SGD, p.numel(), lr, 0.0, 0.0, 0.0, momentum, 0, first,
+                                              grad_scale, wd, wd_starts, wd_values, ema_decay, ema_first);
+  b200::optimizer_fused(o, f32p(p), f32p(mom), nullptr, f32p_opt(g32), bfp_opt(g16),
+                        shadow.has_value() ? bfp_mut(*shadow) : nullptr, f32p_opt(gzero), f32p_opt(ema), p.numel(),
+                        cur_stream());
 }
 static void ema_update(const at::Tensor& p, at::Tensor ema, double decay, bool first) {
   c10::cuda::CUDAGuard g(p.device());
@@ -857,11 +829,12 @@ static void zero1_step(const PyComm& comm, c10::optional<at::Tensor> grad, at::T
   }
   TORCH_CHECK(!decoupled || (std::isfinite(weight_decay) && weight_decay >= 0.0),
               "zero1_step: the AdamW weight decay must be finite and >= 0, got ", weight_decay);
-  b200::zero1_step(comm.c, grad.has_value() ? grad->data_ptr<float>() : nullptr, p.data_ptr<float>(),
-                   m.data_ptr<float>(), v.data_ptr<float>(), bfp_mut(shadow), start, n, (float)inv_world, (int)algo,
-                   (int)slot, (uint32_t)epoch, (int)max_ctas, (float)lr, (float)beta1, (float)beta2, (float)eps,
-                   (float)weight_decay, (int)step, cur_stream(), f32p_opt(ema), ema_decay, ema_first, decoupled,
-                   (float)(1.0 - lr * weight_decay));
+  const b200::OptStep o =
+      b200::make_opt_step("zero1_step", decoupled ? b200::OPT_ADAMW : b200::OPT_ADAM, n, lr, beta1, beta2, eps, 0.0,
+                          (int)step, false, 1.0, weight_decay, {}, {}, ema_decay, ema_first);
+  b200::zero1_step(comm.c, o, grad.has_value() ? grad->data_ptr<float>() : nullptr, p.data_ptr<float>(),
+                   m.data_ptr<float>(), v.data_ptr<float>(), bfp_mut(shadow), f32p_opt(ema), start, n,
+                   (float)inv_world, (int)algo, (int)slot, (uint32_t)epoch, (int)max_ctas, cur_stream());
 }
 static int64_t allreduce_grid(int64_t n, int64_t world, int64_t max_ctas, bool wire_fp32) {
   return b200::allreduce_grid(n, (int)world, (int)max_ctas, wire_fp32);

@@ -1,12 +1,12 @@
-// One Adam step of one parameter (torch.optim.Adam with L2 weight decay, bias-corrected), and one
-// update of the weights' moving average, shared by
-// adam_kernel (loss_optim.cu) and zero1_kernel (allreduce.cu) so that the fused ZeRO-1 step and the
-// replicated optimizer give the same update bit for bit.  Every rounding is spelled out: left to
-// itself, nvcc contracted `g * gscale + wd * p` to fma(g, gscale, wd * p) in one kernel and
+// The per-element updates of the optimizers (Adam, AdamW, SGD) and of the weights' moving average,
+// shared by the optimizer kernels (loss_optim.cu) and zero1_kernel (allreduce.cu) so that the fused
+// ZeRO-1 step and the replicated optimizer give the same update bit for bit.  Every rounding is spelled
+// out: left to itself, nvcc contracted `g * gscale + wd * p` to fma(g, gscale, wd * p) in one kernel and
 // `g + wd * p` to fma(wd, p, g) in the other, and the two differ in the last bit of the moments
 // (tests/test_collectives_gpu.py).
 #pragma once
 #include <cuda_runtime.h>
+#include "api.h"
 
 namespace b200 {
 
@@ -40,6 +40,40 @@ __device__ __forceinline__ void adamw_update(float g, float gscale, float& p, fl
 // `decay * e + (1 - decay) * p` computes in fp32.  `first`: AveragedModel's first update copies p.
 __device__ __forceinline__ float ema_update(float e, float p, float d, float a, bool first) {
   return first ? p : __fadd_rn(__fmul_rn(d, e), __fmul_rn(a, p));
+}
+
+// ema_update of 4 consecutive weights; ema is 16-byte aligned and streamed like every optimizer operand.
+__device__ __forceinline__ void ema_update4(float* __restrict__ ema, const float* pp, const EmaCoef& c) {
+  float4 e = __ldcs(reinterpret_cast<const float4*>(ema));
+  e.x = ema_update(e.x, pp[0], c.d, c.a, c.first);
+  e.y = ema_update(e.y, pp[1], c.d, c.a, c.first);
+  e.z = ema_update(e.z, pp[2], c.d, c.a, c.first);
+  e.w = ema_update(e.w, pp[3], c.d, c.a, c.first);
+  __stcs(reinterpret_cast<float4*>(ema), e);
+}
+
+// One step of torch.optim.SGD with momentum and L2 weight decay: buf = g (first step) or
+// momentum * buf + g, then p -= lr * buf.  The roundings are the ones nvcc's contraction chose when this
+// was written as plain expressions: the decay product alone, everything else fused.
+__device__ __forceinline__ void sgd_update(float g, float gscale, float& p, float& buf, float lr, float momentum,
+                                           float wd, bool first) {
+  const float gk = __fmaf_rn(g, gscale, __fmul_rn(wd, p));
+  const float acc = __fmaf_rn(momentum, buf, gk);   // unconditional: keeps sgd_kernel at 32 registers
+  buf = first ? gk : acc;
+  p = __fmaf_rn(-lr, buf, p);
+}
+
+// The update of one element for the optimizer KIND (OptKind) of the step `o`, with decay value w (an L2
+// decay, or AdamW's keep factor).  m is SGD's momentum buffer; SGD leaves v alone.
+template <int KIND>
+__device__ __forceinline__ void optimizer_update(const OptStep& o, float g, float gscale, float w, float& p, float& m,
+                                                 float& v) {
+  if constexpr (KIND == OPT_SGD)
+    sgd_update(g, gscale, p, m, o.lr, o.momentum, w, o.first);
+  else if constexpr (KIND == OPT_ADAMW)
+    adamw_update(g, gscale, p, m, v, o.lr * o.bc1_inv, o.beta1, o.beta2, o.eps, w, o.bc2_inv_sqrt);
+  else
+    adam_update(g, gscale, p, m, v, o.lr * o.bc1_inv, o.beta1, o.beta2, o.eps, w, o.bc2_inv_sqrt);
 }
 
 }  // namespace b200

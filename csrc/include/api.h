@@ -4,6 +4,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <vector>
 
 namespace b200 {
 
@@ -162,26 +163,45 @@ struct WdSegments {
   long long start4[WD_MAX_SEGMENTS];
   float value[WD_MAX_SEGMENTS];
 };
-inline WdSegments uniform_wd(float value) {
-  WdSegments s{};
-  s.n = 1;
-  s.value[0] = value;
-  return s;
-}
 
-// Fused optimizers over flat arenas.  grad is fp32 (local) or bf16 (the reduced wire buffer).
-// With `ema`, the same pass also updates the weights' exponential moving average from the new p:
-// ema = decay * ema + (1 - decay) * p (fp32 rounding of each product and of the sum), or ema = p when
-// `ema_first` (AveragedModel's first update).  `decoupled`: AdamW (adamw_update in adam.cuh), `wd`
-// then holds keep factors.
-void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16, bf16* shadow,
-                long long n, float lr, float beta1, float beta2, float eps, const WdSegments& wd,
-                int step, float grad_scale, bool zero_grad, float* g32_to_zero, cudaStream_t s,
-                float* ema = nullptr, double ema_decay = 0.0, bool ema_first = false, bool decoupled = false);
-void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* shadow, long long n,
-               float lr, float momentum, const WdSegments& wd, bool first_step, float grad_scale,
-               float* g32_to_zero, cudaStream_t s, float* ema = nullptr, double ema_decay = 0.0,
-               bool ema_first = false);
+// One update of the weights' exponential moving average (ema_update in adam.cuh): d = fp32(decay) and
+// a = fp32(1 - decay) with 1 - decay taken in double; `first`: AveragedModel's first update, ema = p.
+struct EmaCoef {
+  float d, a;
+  int first;
+};
+EmaCoef ema_coef(double decay, bool first);
+
+// The scalars of one optimizer launch, in the form the kernels consume.  Built by make_opt_step only.
+// The field order matters to the kernels' register allocation: in some orders nvcc loads neighbouring
+// fields as pairs, which costs adam_kernel spills at its 40-register cap.
+enum OptKind : int { OPT_ADAM = 0, OPT_ADAMW = 1, OPT_SGD = 2 };
+struct OptStep {
+  float lr, beta1, beta2, eps;   // beta1, beta2, eps: Adam / AdamW
+  float bc1_inv, bc2_inv_sqrt;   // 1 / (1 - beta1^step), 1 / sqrt(1 - beta2^step): double, rounded once
+  float grad_scale;
+  float momentum;                // SGD
+  OptKind kind;
+  int first;                     // SGD's first step: the momentum buffer starts as the gradient
+  EmaCoef ema;                   // used by the launches that are given an `ema` arena
+  WdSegments wd;                 // L2 decays (Adam, SGD) or AdamW keep factors
+};
+// Validates the weight-decay table and refuses a bad one naming `op`.  Without `wd_starts` the decay is
+// `wd` everywhere; otherwise segment k covers elements [wd_starts[k], wd_starts[k + 1]) of the n-element
+// range with decay wd_values[k] (and `wd` is not used).  Starts must begin at 0, increase, be multiples of
+// 4 and lie inside the range; decays must be finite and >= 0.  AdamW's keep factors 1 - lr * wd are
+// taken in double, as torch computes the Python scalar.
+OptStep make_opt_step(const char* op, OptKind kind, long long n, double lr, double beta1, double beta2, double eps,
+                      double momentum, int step, bool first, double grad_scale, double wd,
+                      const std::vector<int64_t>& wd_starts, const std::vector<double>& wd_values, double ema_decay,
+                      bool ema_first);
+
+// Fused optimizer over flat arenas of n elements (n % 4 == 0): reads grad (fp32 g32, local, or bf16 g16,
+// the reduced wire), updates the fp32 master p and the state (Adam: moments m and v; SGD: momentum
+// buffer m, v null), writes the bf16 shadow and clears gzero when given.  With `ema`, the same pass
+// also updates the weights' moving average from the new p.
+void optimizer_fused(const OptStep& o, float* p, float* m, float* v, const float* g32, const bf16* g16,
+                     bf16* shadow, float* gzero, float* ema, long long n, cudaStream_t s);
 // The EMA update of the optimizers alone, for weights no optimizer launch covers (frozen layers):
 // ema[i] = decay * ema[i] + (1 - decay) * p[i] with each operation rounded to fp32, or p[i] when `first`.
 // n elements, any n >= 0; p and ema 16-byte aligned.
@@ -262,13 +282,11 @@ void allreduce_fused(const CommCtx& ctx, const float* grad_f32, float* grad_out_
 int allreduce_grid(long long n, int world, int max_ctas, bool wire_fp32);
 // EXPERIMENTAL: ZeRO-1 step of arena range [start, start+n) in one kernel -- reduce-scatter, Adam on
 // the cells this rank owns, all-gather of the new bf16 weights into every rank's shadow (allreduce.cu).
-// With `ema`, the owner also updates the moving average of its cells as adam_fused does.  `decoupled`:
-// AdamW with keep = fp32(1 - lr * wd) (weight_decay is then not used).
-void zero1_step(const CommCtx& ctx, float* grad_f32, float* p, float* m, float* v, bf16* shadow,
-                long long start, long long n, float inv_world, int algo, int slot, uint32_t epoch, int max_ctas,
-                float lr, float beta1, float beta2, float eps, float weight_decay, int step, cudaStream_t s,
-                float* ema = nullptr, double ema_decay = 0.0, bool ema_first = false, bool decoupled = false,
-                float keep = 1.f);
+// The update is optimizer_fused's at grad_scale 1: Adam or AdamW with one decay for the whole range.
+// With `ema`, the owner also updates the moving average of its cells.
+void zero1_step(const CommCtx& ctx, const OptStep& o, float* grad_f32, float* p, float* m, float* v, bf16* shadow,
+                float* ema, long long start, long long n, float inv_world, int algo, int slot, uint32_t epoch,
+                int max_ctas, cudaStream_t s);
 // Parameter broadcast rank `root` -> all through the wire buffer (K-BCAST).
 void broadcast_fused(const CommCtx& ctx, float* data_f32, long long n, int root, int slot,
                      uint32_t epoch, cudaStream_t s);

@@ -5,8 +5,11 @@
 // Average = sample-weighted loss mean (distributedUtil.py:55-58), torch.optim.Adam with default
 // betas/eps (distributedVggf.py:230).  The reference pays two host syncs per step for the metrics;
 // here they are three atomics into a device meter.
+#include <cmath>
 #include <cstdlib>
+#include <sstream>
 #include <stdexcept>
+#include <string>
 
 #include "adam.cuh"
 #include "api.h"
@@ -343,49 +346,90 @@ void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long l
   check_last("head_ce_fused");
 }
 
-// ---------------------------------------------------------------------------------------- Adam
-// The moving average of 4 new weights, streamed like every other optimizer operand.
-__device__ __forceinline__ void ema_store4(float* __restrict__ ema, long long i, const float (&pp)[4], float d, float a,
-                                           int first) {
-  float4 ev = __ldcs(reinterpret_cast<const float4*>(ema) + i);
-  ev.x = ema_update(ev.x, pp[0], d, a, first);
-  ev.y = ema_update(ev.y, pp[1], d, a, first);
-  ev.z = ema_update(ev.z, pp[2], d, a, first);
-  ev.w = ema_update(ev.w, pp[3], d, a, first);
-  __stcs(reinterpret_cast<float4*>(ema) + i, ev);
+// ---------------------------------------------------------------------------------- optimizers
+EmaCoef ema_coef(double decay, bool first) {
+  return EmaCoef{static_cast<float>(decay), static_cast<float>(1.0 - decay), first ? 1 : 0};
 }
 
-// One pass over the flat arena: read grad (fp32 local or bf16 reduced wire), update fp32 master
-// weight and both moments, emit the bf16 shadow used by the GEMMs, and zero the fp32 gradient so
+OptStep make_opt_step(const char* op, OptKind kind, long long n, double lr, double beta1, double beta2, double eps,
+                      double momentum, int step, bool first, double grad_scale, double wd,
+                      const std::vector<int64_t>& wd_starts, const std::vector<double>& wd_values, double ema_decay,
+                      bool ema_first) {
+  auto check = [op](bool ok, const auto&... msg) {
+    if (ok) return;
+    std::ostringstream s;
+    ((s << op) << ... << msg);
+    throw std::runtime_error(s.str());
+  };
+  OptStep o{};
+  o.kind = kind;
+  o.lr = static_cast<float>(lr);
+  o.beta1 = static_cast<float>(beta1);
+  o.beta2 = static_cast<float>(beta2);
+  o.eps = static_cast<float>(eps);
+  if (kind != OPT_SGD) {   // from the fp32 betas
+    o.bc1_inv = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(o.beta1), step)));
+    o.bc2_inv_sqrt = static_cast<float>(1.0 / sqrt(1.0 - pow(static_cast<double>(o.beta2), step)));
+  }
+  o.momentum = static_cast<float>(momentum);
+  o.first = first ? 1 : 0;
+  o.grad_scale = static_cast<float>(grad_scale);
+  o.ema = ema_coef(ema_decay, ema_first);
+  auto value = [&](double d) { return static_cast<float>(kind == OPT_ADAMW ? 1.0 - lr * d : d); };
+  WdSegments& s = o.wd;
+  if (wd_starts.empty()) {
+    check(wd_values.empty(), ": wd_starts and wd_values go together");
+    s.n = 1;
+    s.value[0] = value(wd);
+    return o;
+  }
+  check(wd_starts.size() == wd_values.size(), ": wd_starts and wd_values must have the same length");
+  check(wd_starts.size() <= static_cast<size_t>(WD_MAX_SEGMENTS), ": at most ", WD_MAX_SEGMENTS,
+        " weight-decay segments per launch, got ", wd_starts.size());
+  check(wd_starts[0] == 0, ": the first weight-decay segment must start at 0");
+  s.n = static_cast<int>(wd_starts.size());
+  for (int k = 0; k < s.n; ++k) {
+    const int64_t start = wd_starts[k];
+    const double d = wd_values[k];
+    check(k == 0 || start > wd_starts[k - 1], ": weight-decay segment starts must increase");
+    check(start % 4 == 0, ": weight-decay segment starts must be multiples of 4, got ", start);
+    check(start < n, ": weight-decay segment start ", start, " lies outside the range of ", n);
+    check(std::isfinite(d) && d >= 0.0, ": weight decays must be finite and >= 0, got ", d);
+    s.start4[k] = start / 4;
+    s.value[k] = value(d);
+  }
+  return o;
+}
+
+// One pass over the flat arena: read grad (fp32 local or bf16 reduced wire), update the fp32 master
+// weight and the optimizer state, emit the bf16 shadow used by the GEMMs, and zero the fp32 gradient so
 // the red.add wgrad epilogues of the next step start from zero.
 // Footprint (same reasoning as allreduce.cu): the update runs on the comm stream UNDER the persistent
 // conv kernels of backward.  256 threads x <= 40 registers and no shared memory co-reside with any of
-// them, and the grid is one CTA per SM -- a background stream of HBM traffic.  (Round 1 launched 8
-// CTAs per SM: at every conv-kernel boundary the high-priority stream filled the SMs with optimizer
-// CTAs and the next conv kernel's persistent CTAs started late; bench/step_timeline.py.)
+// them, and the grid is capped by optimizer_grid -- a background stream of HBM traffic.  (Round 1
+// launched 8 CTAs per SM: at every conv-kernel boundary the high-priority stream filled the SMs with
+// optimizer CTAs and the next conv kernel's persistent CTAs started late; bench/step_timeline.py.)
 // EMA: also update the weights' moving average `ema` from the new p while it is in registers (one
 // more fp32 stream, 8 B per parameter); the EMA = false instantiation is the plain optimizer.
-// DECOUPLED: AdamW (adamw_update), the segment values being keep factors instead of L2 decays.
-// `wd` (WdSegments, api.h) sits in the parameter bank: the thread walks it forward as its grid-stride
-// loop moves through the range, one compare per iteration for a uniform decay.
-template <bool EMA, bool DECOUPLED>
-__global__ void __launch_bounds__(256, 6) adam_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
-                            const float* __restrict__ g32, const bf16* __restrict__ g16,
-                            bf16* __restrict__ shadow, long long n4, float lr, float b1, float b2,
-                            float eps, float bc1_inv, float bc2_inv_sqrt, float gscale,
-                            float* __restrict__ gzero, float* __restrict__ ema, float ema_d, float ema_a,
-                            int ema_first, const __grid_constant__ WdSegments wd) {
+// The step `o` (with its WdSegments) sits in the parameter bank: the thread walks the segments forward
+// as its grid-stride loop moves through the range, one compare per iteration for a uniform decay.
+template <int KIND, bool EMA>
+__device__ __forceinline__ void optimizer_pass(const OptStep& o, float* __restrict__ p, float* __restrict__ m,
+                                               float* __restrict__ v, const float* __restrict__ g32,
+                                               const bf16* __restrict__ g16, bf16* __restrict__ shadow,
+                                               float* __restrict__ gzero, float* __restrict__ ema, long long n4) {
   int seg = 0;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    while (seg + 1 < wd.n && i >= wd.start4[seg + 1]) ++seg;
-    const float w = wd.value[seg];
+    while (seg + 1 < o.wd.n && i >= o.wd.start4[seg + 1]) ++seg;
+    const float w = o.wd.value[seg];
     // Every stream here is touched exactly once per step: cache-streaming (evict-first) loads and
     // stores, so that ~4 GB of optimizer traffic does not flush the conv kernels' L2-resident operand
     // tiles while it runs under backward (bench/step_timeline.py: +30 % on the 512-channel layers).
-    float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i);
-    float4 mv = __ldcs(reinterpret_cast<const float4*>(m) + i);
-    float4 vv = __ldcs(reinterpret_cast<const float4*>(v) + i);
+    const float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i);
+    const float4 mv = __ldcs(reinterpret_cast<const float4*>(m) + i);
+    float4 vv{};
+    if constexpr (KIND != OPT_SGD) vv = __ldcs(reinterpret_cast<const float4*>(v) + i);
     float g[4];
     if (g16) {
       const uint2 raw = __ldcs(reinterpret_cast<const uint2*>(g16 + i * 4));
@@ -399,170 +443,87 @@ __global__ void __launch_bounds__(256, 6) adam_kernel(float* __restrict__ p, flo
     float mm[4] = {mv.x, mv.y, mv.z, mv.w};
     float vs[4] = {vv.x, vv.y, vv.z, vv.w};
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if constexpr (DECOUPLED)
-        adamw_update(g[k], gscale, pp[k], mm[k], vs[k], lr * bc1_inv, b1, b2, eps, w, bc2_inv_sqrt);
-      else
-        adam_update(g[k], gscale, pp[k], mm[k], vs[k], lr * bc1_inv, b1, b2, eps, w, bc2_inv_sqrt);
-    }
+    for (int k = 0; k < 4; ++k) optimizer_update<KIND>(o, g[k], o.grad_scale, w, pp[k], mm[k], vs[k]);
     __stcs(reinterpret_cast<float4*>(p) + i, make_float4(pp[0], pp[1], pp[2], pp[3]));
     __stcs(reinterpret_cast<float4*>(m) + i, make_float4(mm[0], mm[1], mm[2], mm[3]));
-    __stcs(reinterpret_cast<float4*>(v) + i, make_float4(vs[0], vs[1], vs[2], vs[3]));
-    if constexpr (EMA) ema_store4(ema, i, pp, ema_d, ema_a, ema_first);
+    if constexpr (KIND != OPT_SGD) __stcs(reinterpret_cast<float4*>(v) + i, make_float4(vs[0], vs[1], vs[2], vs[3]));
+    if constexpr (EMA) ema_update4(ema + i * 4, pp, o.ema);
     if (shadow)
       __stcs(reinterpret_cast<uint2*>(shadow + i * 4), make_uint2(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3])));
     if (gzero) __stcs(reinterpret_cast<float4*>(gzero) + i, make_float4(0.f, 0.f, 0.f, 0.f));
   }
 }
 
+// DECOUPLED: AdamW, the segment values being keep factors instead of L2 decays.
 template <bool EMA, bool DECOUPLED>
-static void launch_adam(int blocks, cudaStream_t s, float* p, float* m, float* v, const float* g32, const bf16* g16,
-                        bf16* shadow, long long n4, float lr, float beta1, float beta2, float eps, float bc1_inv,
-                        float bc2_inv_sqrt, float grad_scale, float* gzero, float* ema, float ema_d, float ema_a,
-                        int ema_first, const WdSegments& wd) {
-  adam_kernel<EMA, DECOUPLED><<<blocks, 256, 0, s>>>(p, m, v, g32, g16, shadow, n4, lr, beta1, beta2, eps, bc1_inv,
-                                                     bc2_inv_sqrt, grad_scale, gzero, ema, ema_d, ema_a, ema_first, wd);
+__global__ void __launch_bounds__(256, 6) adam_kernel(const __grid_constant__ OptStep o, float* __restrict__ p,
+    float* __restrict__ m, float* __restrict__ v, const float* __restrict__ g32, const bf16* __restrict__ g16,
+    bf16* __restrict__ shadow, float* __restrict__ gzero, float* __restrict__ ema, long long n4) {
+  optimizer_pass<DECOUPLED ? OPT_ADAMW : OPT_ADAM, EMA>(o, p, m, v, g32, g16, shadow, gzero, ema, n4);
 }
 
-void adam_fused(float* p, float* m, float* v, const float* g32, const bf16* g16, bf16* shadow,
-                long long n, float lr, float beta1, float beta2, float eps, const WdSegments& wd,
-                int step, float grad_scale, bool, float* g32_to_zero, cudaStream_t s, float* ema,
-                double ema_decay, bool ema_first, bool decoupled) {
-  if (n % 4) throw std::runtime_error("[b200] adam_fused: n must be a multiple of 4");
-  if (wd.n < 1 || wd.n > WD_MAX_SEGMENTS || wd.start4[0] != 0)
-    throw std::runtime_error("[b200] adam_fused: bad weight-decay segment table");
-  const double bc1 = 1.0 - pow(static_cast<double>(beta1), step);
-  const double bc2 = 1.0 - pow(static_cast<double>(beta2), step);
-  const long long n4 = n / 4;
-  // Tunable without a rebuild: B200_ADAM_CTAS_PER_SM (default 4).
-  static const int per_sm = [] {
-    const char* e = getenv("B200_ADAM_CTAS_PER_SM");
-    const int v = e ? atoi(e) : 4;
-    return v >= 1 && v <= 16 ? v : 4;
-  }();
-  static const bool carve = [] {
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<false, false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<true, false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<false, true>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(adam_kernel<true, true>));
-    return true;
-  }();
-  (void)carve;
-  const long long cap = static_cast<long long>(sm_count()) * per_sm;
-  const int blocks = static_cast<int>(n4 / 256 + 1 < cap ? n4 / 256 + 1 : cap);
-  const float bc1_inv = static_cast<float>(1.0 / bc1), bc2_inv_sqrt = static_cast<float>(1.0 / sqrt(bc2));
-  const float ema_d = ema ? static_cast<float>(ema_decay) : 0.f;
-  const float ema_a = ema ? static_cast<float>(1.0 - ema_decay) : 0.f;
-  const int first = ema && ema_first ? 1 : 0;
-  auto* launch = ema ? (decoupled ? launch_adam<true, true> : launch_adam<true, false>)
-                     : (decoupled ? launch_adam<false, true> : launch_adam<false, false>);
-  launch(blocks, s, p, m, v, g32, g16, shadow, n4, lr, beta1, beta2, eps, bc1_inv, bc2_inv_sqrt, grad_scale,
-         g32_to_zero, ema, ema_d, ema_a, first, wd);
-  count_launch();
-  check_last("adam_fused");
-}
-
-// --------------------------------------------------------------------------------------- SGD
-// torch.optim.SGD(momentum) semantics: buf = g (first step) | momentum*buf + g ; p -= lr*buf.
-// EMA and the weight-decay segments `wd`: as adam_kernel.  SGD has no decoupled form in torch: wd is L2.
+// m is the momentum buffer; v is not used.  SGD has no decoupled form in torch: the decay is L2.
 template <bool EMA>
-__global__ void __launch_bounds__(256, 6) sgd_kernel(float* __restrict__ p, float* __restrict__ mom, const float* __restrict__ g32,
-                           const bf16* __restrict__ g16, bf16* __restrict__ shadow, long long n4, float lr,
-                           float momentum, int first, float gscale, float* __restrict__ gzero,
-                           float* __restrict__ ema, float ema_d, float ema_a, int ema_first,
-                           const __grid_constant__ WdSegments wd) {
-  int seg = 0;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    while (seg + 1 < wd.n && i >= wd.start4[seg + 1]) ++seg;
-    const float w = wd.value[seg];
-    float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i);       // streaming, see adam_kernel
-    float4 bv = __ldcs(reinterpret_cast<const float4*>(mom) + i);
-    float g[4];
-    if (g16) {
-      const uint2 raw = __ldcs(reinterpret_cast<const uint2*>(g16 + i * 4));
-      const float2 a = unpack_bf16x2(raw.x), b = unpack_bf16x2(raw.y);
-      g[0] = a.x; g[1] = a.y; g[2] = b.x; g[3] = b.y;
-    } else {
-      const float4 gv = __ldcs(reinterpret_cast<const float4*>(g32) + i);
-      g[0] = gv.x; g[1] = gv.y; g[2] = gv.z; g[3] = gv.w;
-    }
-    float pp[4] = {pv.x, pv.y, pv.z, pv.w};
-    float bb[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float gk = g[k] * gscale + w * pp[k];
-      bb[k] = first ? gk : momentum * bb[k] + gk;
-      pp[k] -= lr * bb[k];
-    }
-    __stcs(reinterpret_cast<float4*>(p) + i, make_float4(pp[0], pp[1], pp[2], pp[3]));
-    __stcs(reinterpret_cast<float4*>(mom) + i, make_float4(bb[0], bb[1], bb[2], bb[3]));
-    if constexpr (EMA) ema_store4(ema, i, pp, ema_d, ema_a, ema_first);
-    if (shadow)
-      __stcs(reinterpret_cast<uint2*>(shadow + i * 4), make_uint2(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3])));
-    if (gzero) __stcs(reinterpret_cast<float4*>(gzero) + i, make_float4(0.f, 0.f, 0.f, 0.f));
-  }
+__global__ void __launch_bounds__(256, 6) sgd_kernel(const __grid_constant__ OptStep o, float* __restrict__ p,
+    float* __restrict__ m, float* __restrict__ v, const float* __restrict__ g32, const bf16* __restrict__ g16,
+    bf16* __restrict__ shadow, float* __restrict__ gzero, float* __restrict__ ema, long long n4) {
+  optimizer_pass<OPT_SGD, EMA>(o, p, m, v, g32, g16, shadow, gzero, ema, n4);
 }
 
-void sgd_fused(float* p, float* mom, const float* g32, const bf16* g16, bf16* shadow, long long n,
-               float lr, float momentum, const WdSegments& wd, bool first_step, float grad_scale,
-               float* g32_to_zero, cudaStream_t s, float* ema, double ema_decay, bool ema_first) {
-  if (n % 4) throw std::runtime_error("[b200] sgd_fused: n must be a multiple of 4");
-  if (wd.n < 1 || wd.n > WD_MAX_SEGMENTS || wd.start4[0] != 0)
-    throw std::runtime_error("[b200] sgd_fused: bad weight-decay segment table");
-  const long long n4 = n / 4;
-  static const bool carve = [] {
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(sgd_kernel<false>));
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(sgd_kernel<true>));
-    return true;
-  }();
-  (void)carve;
-  const long long cap = static_cast<long long>(sm_count()) * 4;
-  const int blocks = static_cast<int>(n4 / 256 + 1 < cap ? n4 / 256 + 1 : cap);
-  if (ema)
-    sgd_kernel<true><<<blocks, 256, 0, s>>>(p, mom, g32, g16, shadow, n4, lr, momentum, first_step ? 1 : 0,
-                                            grad_scale, g32_to_zero, ema, static_cast<float>(ema_decay),
-                                            static_cast<float>(1.0 - ema_decay), ema_first ? 1 : 0, wd);
-  else
-    sgd_kernel<false><<<blocks, 256, 0, s>>>(p, mom, g32, g16, shadow, n4, lr, momentum, first_step ? 1 : 0,
-                                             grad_scale, g32_to_zero, nullptr, 0.f, 0.f, 0, wd);
-  count_launch();
-  check_last("sgd_fused");
-}
-
-// ------------------------------------------------------------------------- EMA without an update
 // The moving average of weights that no optimizer launch covers (--freeze-layers: the frozen suffix of
 // the arena, which AveragedModel still averages): ema_update of every element, the update and the
 // `first` rule of the optimizer kernels' EMA.  Same footprint as adam_kernel (256 threads, no shared
 // memory, evict-first streams, one grid-stride pass).  n need not be a multiple of 4: the last n % 4
 // elements go through thread 0 one by one.
 __global__ void __launch_bounds__(256, 6) ema_kernel(const float* __restrict__ p, float* __restrict__ ema, long long n,
-                                                      float d, float a, int first) {
+                                                      const EmaCoef c) {
   const long long n4 = n / 4;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i);
     const float pp[4] = {pv.x, pv.y, pv.z, pv.w};
-    ema_store4(ema, i, pp, d, a, first);
+    ema_update4(ema + i * 4, pp, c);
   }
   if (blockIdx.x == 0 && threadIdx.x == 0)
-    for (long long i = n4 * 4; i < n; ++i) ema[i] = ema_update(ema[i], p[i], d, a, first);
+    for (long long i = n4 * 4; i < n; ++i) ema[i] = ema_update(ema[i], p[i], c.d, c.a, c.first);
 }
 
+using OptKernel = void (*)(OptStep, float*, float*, float*, const float*, const bf16*, bf16*, float*, float*, long long);
+static const OptKernel OPT_KERNELS[3][2] = {   // [kind][ema]
+    {adam_kernel<false, false>, adam_kernel<true, false>},
+    {adam_kernel<false, true>, adam_kernel<true, true>},
+    {sgd_kernel<false>, sgd_kernel<true>}};
+
+// One 256-thread CTA per 1024 elements, at most 4 CTAs per SM (Adam and AdamW: B200_ADAM_CTAS_PER_SM,
+// tunable without a rebuild), so that the side-stream launches compete with the conv kernels no more than
+// that.  Also registers the maximum-shared carve-out of every kernel above, once.
+static int optimizer_grid(long long n4, bool adam) {
+  static const int adam_per_sm = [] {
+    for (const auto& kind : OPT_KERNELS)
+      for (OptKernel k : kind) prefer_max_shared_carveout(reinterpret_cast<const void*>(k));
+    prefer_max_shared_carveout(reinterpret_cast<const void*>(ema_kernel));
+    const char* e = getenv("B200_ADAM_CTAS_PER_SM");
+    const int v = e ? atoi(e) : 4;
+    return v >= 1 && v <= 16 ? v : 4;
+  }();
+  const long long cap = static_cast<long long>(sm_count()) * (adam ? adam_per_sm : 4);
+  return static_cast<int>(n4 / 256 + 1 < cap ? n4 / 256 + 1 : cap);
+}
+
+void optimizer_fused(const OptStep& o, float* p, float* m, float* v, const float* g32, const bf16* g16,
+                     bf16* shadow, float* gzero, float* ema, long long n, cudaStream_t s) {
+  const char* what = o.kind == OPT_SGD ? "sgd_fused" : "adam_fused";
+  if (n % 4) throw std::runtime_error(std::string("[b200] ") + what + ": n must be a multiple of 4");
+  const int blocks = optimizer_grid(n / 4, o.kind != OPT_SGD);
+  OPT_KERNELS[o.kind][ema != nullptr]<<<blocks, 256, 0, s>>>(o, p, m, v, g32, g16, shadow, gzero, ema, n / 4);
+  count_launch();
+  check_last(what);
+}
+
+// Runs once per EMA step; its cost in the step is measured by bench/freeze_bench.py.
 void ema_fused(const float* p, float* ema, long long n, double decay, bool first, cudaStream_t s) {
   if (n <= 0) return;
-  static const bool carve = [] {
-    prefer_max_shared_carveout(reinterpret_cast<const void*>(ema_kernel));
-    return true;
-  }();
-  (void)carve;
-  // The grid cap of the optimizer launches it shares the side stream with (adam_fused's default of 4 CTAs per
-  // SM, B200_ADAM_CTAS_PER_SM, and sgd_fused's fixed 4), so that it competes with the conv kernels no more
-  // than they do.  It runs once per EMA step; its cost in the step is measured by bench/freeze_bench.py.
-  const long long cap = static_cast<long long>(sm_count()) * 4;
-  const int blocks = static_cast<int>(n / 1024 + 1 < cap ? n / 1024 + 1 : cap);
-  ema_kernel<<<blocks, 256, 0, s>>>(p, ema, n, static_cast<float>(decay), static_cast<float>(1.0 - decay),
-                                    first ? 1 : 0);
+  ema_kernel<<<optimizer_grid(n / 4, false), 256, 0, s>>>(p, ema, n, ema_coef(decay, first));
   count_launch();
   check_last("ema_fused");
 }
