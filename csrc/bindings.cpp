@@ -98,6 +98,27 @@ static std::vector<int64_t> conv_pixel_box(int64_t N, int64_t H, int64_t W) {
 static int64_t conv_bn_choice(int64_t N, int64_t H, int64_t W, int64_t cn) {
   return b200::conv_bn_choice((int)N, (int)H, (int)W, (int)cn);
 }
+// conv_plan(kind, N, H, W, Cin, Cout, sms, bn=0): what a conv launch runs (pure host code, no GPU needed);
+// bn: the tile width a caller passes to the launcher (0: the launcher's own choice).
+static py::dict conv_plan(const std::string& kind, int64_t N, int64_t H, int64_t W, int64_t Cin, int64_t Cout,
+                          int64_t sms, int64_t bn) {
+  static const char* kinds[] = {"fprop", "fprop_pool", "dgrad", "wgrad", "wgrad_partial"};
+  static const char* paths[] = {"halo", "pow2", "fill", "wgrad_halo64", "wgrad"};
+  int k = -1;
+  for (int i = 0; i < 5; ++i)
+    if (kind == kinds[i]) k = i;
+  TORCH_CHECK(k >= 0, "conv_plan: kind must be fprop, fprop_pool, dgrad, wgrad or wgrad_partial, got ", kind);
+  const b200::ConvPlan p = b200::conv_plan(k, (int)N, (int)H, (int)W, (int)Cin, (int)Cout, (int)sms, (int)bn);
+  py::dict d;
+  d["path"] = paths[p.path];
+  d["bn"] = p.bn;
+  d["box"] = py::make_tuple(p.Wb, p.Hb, p.Nb);
+  d["tiles"] = p.tiles;
+  d["ksplit"] = p.ksplit;
+  d["tiles_per_split"] = p.tiles_per_split;
+  d["resident"] = bool(p.resident);
+  return d;
+}
 static void unpool(const at::Tensor& dp, const at::Tensor& mask, at::Tensor dz, c10::optional<at::Tensor> colsum) {
   c10::cuda::CUDAGuard g(dp.device());
   TORCH_CHECK(dp.dim() == 4 && dz.dim() == 4 && dp.is_contiguous() && dz.is_contiguous() && mask.is_contiguous() &&
@@ -862,6 +883,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv_fprop_pool", &conv_fprop_pool);
   m.def("conv_pool_fusable", &conv_pool_fusable);
   m.def("conv_pixel_box", &conv_pixel_box);
+  m.def("conv_plan", &conv_plan, py::arg("kind"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("Cin"),
+        py::arg("Cout"), py::arg("sms"), py::arg("bn") = 0);
   m.def("conv_bn_choice", &conv_bn_choice);
   m.def("unpool2x2", &unpool);
   m.def("conv_dgrad", &conv_dgrad);

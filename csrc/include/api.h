@@ -45,10 +45,33 @@ void conv3x3_fprop(const bf16* x, const bf16* w, const float* bias, bf16* y, int
 // argmax bit 1, max > 0, 0}; the un-pooled activation is never materialised.  unpool2x2 is the
 // matching backward (elementwise.cu).
 bool conv3x3_pool_fusable(int N, int H, int W);
-// The pixel box {Wb, Hb, Nb, fill} the fprop / dgrad launchers of the implicit-GEMM path choose (fill = 1:
-// a box of any sides that fills more of the 128-row tile than make_tile's power-of-two one).
+// What a 3x3 convolution launch runs, as the launchers choose it for `sms` SMs: pure host code, so it
+// can be asked where no GPU is present.  conv3x3_fprop / _fprop_pool / _dgrad / _wgrad / _wgrad_partial
+// with their default tile width and split take every choice from here.
+enum ConvKind { CONV_KIND_FPROP, CONV_KIND_FPROP_POOL, CONV_KIND_DGRAD, CONV_KIND_WGRAD, CONV_KIND_WGRAD_PARTIAL };
+enum ConvPath {
+  CONV_PATH_HALO,          // conv_halo_kernel: 8 x 16 pixel halos
+  CONV_PATH_POW2,          // implicit GEMM, make_tile's power-of-two pixel box
+  CONV_PATH_FILL,          // implicit GEMM, a box of any sides (conv_fill_tile; the FILL kernels)
+  CONV_PATH_WGRAD_HALO64,  // wgrad_halo64_kernel: 64 input channels, 8 x 8 pixel tiles
+  CONV_PATH_WGRAD,         // WgradPolicy: 64-pixel power-of-two boxes
+};
+struct ConvPlan {
+  int path;                // ConvPath
+  int bn;                  // channel-tile width (wgrad_halo64: 64)
+  int Wb, Hb, Nb;          // pixel box of one tile
+  long long tiles;         // pixel tiles: fprop / dgrad per channel tile, wgrad over the whole reduction
+  int ksplit;              // wgrad: splits of the pixel tiles (fprop / dgrad: 1)
+  int tiles_per_split;     // wgrad: pixel tiles of every split but possibly the last (fprop / dgrad: tiles)
+  int resident;            // halo: every weight tile stays in shared memory
+};
+// bn: a tile width the caller asks for (0: chosen here), as the launchers' bn argument; an explicit width
+// also takes a wgrad off the halo64 kernel, and its split is then chosen for that width.
+ConvPlan conv_plan(int kind, int N, int H, int W, int Cin, int Cout, int sms, int bn = 0);
+// Views of conv_plan at the device's own SM count: the fprop box {Wb, Hb, Nb, fill} (fill = 1: the FILL
+// path), and the fprop channel-tile width (64, 128 or 256) for cn output channels.  Both query the
+// device; where none is present, ask conv_plan with an explicit SM count.
 void conv_pixel_box(int N, int H, int W, int* box);
-// The channel-tile width (64, 128 or 256) fprop / dgrad pick for cn output channels at that shape.
 int conv_bn_choice(int N, int H, int W, int cn);
 void conv3x3_fprop_pool(const bf16* x, const bf16* w, const float* bias, bf16* pool_out, uint32_t* pool_mask,
                         int N, int H, int W, int Cin, int Cout, int bn, cudaStream_t stream);
@@ -68,7 +91,7 @@ void conv3x3_wgrad(const bf16* dz, const bf16* x, float* dw, int N, int H, int W
 // workspace (also where no GPU is present).  A launch refuses a workspace that is null, misaligned or
 // too small before anything is enqueued.
 inline long long workspace_slice(long long elems) { return (elems + 3) / 4 * 4; }   // slices start on float4s
-int conv_wgrad_splits(int N, int H, int W, int Cin, int Cout, int sms);
+int conv_wgrad_splits(int N, int H, int W, int Cin, int Cout, int sms);   // conv_plan(WGRAD_PARTIAL).ksplit
 int conv0_wgrad_splits(int N, int H, int W, int sms);      // 2 per CTA: one per consumer warpgroup
 int gemm_splits(int K, int ksplit);
 int colsum_partial_blocks(long long rows, int C, int sms);

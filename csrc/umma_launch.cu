@@ -229,7 +229,6 @@ static void conv_halo_launch(ConvParams& prm, const bf16* act, cudaStream_t stre
   prm.div_tm = make_fastdiv(prm.tiles_m);
   const int tiles_n = (prm.Cn + BN - 1) / BN;
   prm.num_tiles = prm.tiles_m * tiles_n;
-  prm.resident = (tiles_n == 1 && 9 * (prm.Ca / UMMA_BK) <= Cfg::NB) ? 1 : 0;
   map_nhwc_box(&prm.mapA, act, t.N, t.H, t.W, prm.Ca, HALO_PITCH, HALO_HT + 2, 1);
   constexpr int smem = Cfg::SMEM + ConvPolicy<BN, 1, DGRAD, POOL>::EPI_SMEM;
   static bool configured = false;
@@ -428,30 +427,130 @@ static void conv_launch(ConvParams& prm, cudaStream_t stream) {
 // per wave; H100 80GB HBM3, 700 W): 7/4.  It is taken where the number of waves over the SMs times
 // that cost is no worse than at 128 -- at batch 64 on 132 SMs every 56^2 and 28^2 layer, not the
 // 14^2 ones, whose 196 wide tiles take 2 waves x 7/4 against 392 narrow tiles in 3 waves x 1.
-static int conv_bn(int cn, long long tiles128, long long tiles256) {
+static int conv_bn(int cn, long long tiles128, long long tiles256, long long sms) {
   if (cn <= 64) return 64;
   if (cn < 256) return 128;
-  const long long sms = num_sms();
   return ((tiles256 + sms - 1) / sms) * 7 <= ((tiles128 + sms - 1) / sms) * 4 ? 256 : 128;
 }
-// The same for fprop / dgrad: the pixel tiles are the same at both widths.
-static int conv_bn_pixels(const ConvTile& t, int cn) {
-  const long long tiles_m = static_cast<long long>(t.tiles_w) * t.tiles_h * ((t.N + t.Nb - 1) / t.Nb);
-  return conv_bn(cn, tiles_m * ((cn + 127) / 128), tiles_m * ((cn + 255) / 256));
+
+// Pixel-tile splits of the halo wgrad: one work item per SM, none empty.
+static int wgrad_halo64_splits(int total_tiles, int tiles_n, int sms, int* tiles_per_split) {
+  int ksplit = sms / tiles_n;
+  if (ksplit < 1) ksplit = 1;
+  if (ksplit > total_tiles) ksplit = total_tiles;
+  *tiles_per_split = (total_tiles + ksplit - 1) / ksplit;
+  return (total_tiles + *tiles_per_split - 1) / *tiles_per_split;
+}
+static bool wgrad_halo64_applicable(int H, int W, int Cin) {
+  return Cin == 64 && H % WH_T == 0 && W % WH_T == 0 && W >= 16 && halo_enabled();
+}
+
+// Pixel-tile splits of the generic wgrad when every split stores a slice of partials that a second
+// kernel adds up.  A slice costs a write and a read of Cout*9*Cin floats, so the 4096-pixel work
+// items of the atomic path (196 splits, 115 MB of partials at 128 -> 128 channels, 112^2, batch 64)
+// are too fine.  Of the counts that give at most ~4 work items per SM, take the one with the least
+// modelled time: waves over the SMs x k-blocks per item, plus the slices' traffic in the same unit
+// (WS_ELEMS_PER_KBLOCK floats written and read back in the time one SM takes for a k-block:
+// ~0.5 us against ~2.5 TB/s; a model, see DESIGN 2.9 for what was measured).  Ties: fewer splits.
+constexpr long long WS_ELEMS_PER_KBLOCK = 160000;
+static int wgrad_partial_ksplit(int total_tiles, int base, long long slice_elems, int sms) {
+  int kmax = (4 * sms + base - 1) / base;
+  if (kmax > total_tiles) kmax = total_tiles;
+  int best = 1;
+  long long best_cost = -1;
+  for (int k = 1; k <= kmax; ++k) {
+    const long long waves = (static_cast<long long>(base) * k + sms - 1) / sms;
+    const long long depth = (total_tiles + k - 1) / k;
+    const long long cost = waves * depth * WS_ELEMS_PER_KBLOCK + k * slice_elems;
+    if (best_cost < 0 || cost < best_cost) { best = k; best_cost = cost; }
+  }
+  return best;
+}
+
+// conv_plan with the launchers' explicit choices: a tile width `bn` (0: chosen here) and a wgrad split
+// `ksplit` (<= 0: chosen here); either one takes the wgrad off the halo64 kernel.  `tile` (optional)
+// receives the pixel tile of the implicit-GEMM and generic wgrad paths.
+static ConvPlan plan_conv(int kind, int N, int H, int W, int Cin, int Cout, int sms, int bn, int ksplit,
+                          ConvTile* tile) {
+  ConvPlan p{};
+  if (kind == CONV_KIND_WGRAD || kind == CONV_KIND_WGRAD_PARTIAL) {
+    if (bn == 0 && ksplit <= 0 && wgrad_halo64_applicable(H, W, Cin)) {
+      p.path = CONV_PATH_WGRAD_HALO64;
+      p.bn = 64; p.Wb = WH_T; p.Hb = WH_T; p.Nb = 1;
+      p.tiles = static_cast<long long>(N) * (W / WH_T) * (H / WH_T);
+      p.ksplit = wgrad_halo64_splits(static_cast<int>(p.tiles), (Cout + 63) / 64, sms, &p.tiles_per_split);
+      return p;
+    }
+    const ConvTile t = make_tile(N, H, W, 64);
+    const int total = static_cast<int>(conv_tile_count(t));
+    // The split is chosen for the width asked for, or for the narrow tile when the width is chosen
+    // here; a 256-wide tile then keeps that split, so it has half as many work items of the same depth.
+    const int split_bn = bn ? bn : (Cin <= 64 ? 64 : 128);
+    if (ksplit <= 0) {     // work items of <= ~64 k-blocks (4096 pixels), and at least ~4 per SM
+      const int base = ((Cout + UMMA_BM - 1) / UMMA_BM) * ((Cin + split_bn - 1) / split_bn) * 9;
+      if (kind == CONV_KIND_WGRAD_PARTIAL) {
+        ksplit = wgrad_partial_ksplit(total, base, static_cast<long long>(Cout) * 9 * Cin, sms);
+      } else {
+        ksplit = (total + 63) / 64;
+        const int min_split = (4 * sms + base - 1) / base;
+        if (ksplit < min_split) ksplit = min_split;
+      }
+    }
+    if (ksplit > total) ksplit = total;
+    p.path = CONV_PATH_WGRAD;
+    p.Wb = t.Wb; p.Hb = t.Hb; p.Nb = t.Nb;
+    p.tiles = total;
+    p.tiles_per_split = (total + ksplit - 1) / ksplit;
+    p.ksplit = (total + p.tiles_per_split - 1) / p.tiles_per_split;
+    if (bn == 0) {
+      const long long items = static_cast<long long>((Cout + UMMA_BM - 1) / UMMA_BM) * 9 * p.ksplit;
+      bn = conv_bn(Cin, items * ((Cin + 127) / 128), items * ((Cin + 255) / 256), sms);
+    }
+    p.bn = bn;
+    if (tile) *tile = t;
+    return p;
+  }
+  const bool dgrad = kind == CONV_KIND_DGRAD;
+  const int cn = dgrad ? Cin : Cout;          // output channels (GEMM N)
+  const int ca = dgrad ? Cout : Cin;          // channels of the A activation (GEMM K per tap)
+  p.ksplit = 1;
+  if (halo_applicable(H, W)) {                // the halo kernel's own 8 x 16 x 1 tiles
+    p.path = CONV_PATH_HALO;
+    p.bn = bn ? bn : (cn <= 64 ? 64 : 128);
+    p.Wb = HALO_WT; p.Hb = HALO_HT; p.Nb = 1;
+    p.tiles = static_cast<long long>(W / HALO_WT) * (H / HALO_HT) * N;
+    p.tiles_per_split = static_cast<int>(p.tiles);
+    const int nb = p.bn == 64 ? HaloCfg<64>::NB : HaloCfg<128>::NB;
+    p.resident = ((cn + p.bn - 1) / p.bn == 1 && 9 * (ca / UMMA_BK) <= nb) ? 1 : 0;
+    return p;
+  }
+  ConvTile t = make_tile(N, H, W, UMMA_BM);
+  const bool fill = kind != CONV_KIND_FPROP_POOL && conv_fill_tile(N, H, W, &t);
+  p.path = fill ? CONV_PATH_FILL : CONV_PATH_POW2;
+  p.Wb = t.Wb; p.Hb = t.Hb; p.Nb = t.Nb;
+  p.tiles = conv_tile_count(t);
+  p.tiles_per_split = static_cast<int>(p.tiles);
+  // the pixel tiles are the same at both widths
+  p.bn = bn ? bn : conv_bn(cn, p.tiles * ((cn + 127) / 128), p.tiles * ((cn + 255) / 256), sms);
+  if (tile) *tile = t;
+  return p;
+}
+
+ConvPlan conv_plan(int kind, int N, int H, int W, int Cin, int Cout, int sms, int bn) {
+  if (kind < CONV_KIND_FPROP || kind > CONV_KIND_WGRAD_PARTIAL) throw std::runtime_error("[b200] conv_plan: unknown kind");
+  if (N < 1 || H < 1 || W < 1 || Cin < 1 || Cout < 1 || sms < 1)
+    throw std::runtime_error("[b200] conv_plan: extents and the SM count must be positive");
+  if (bn != 0 && bn != 64 && bn != 128 && bn != 256)
+    throw std::runtime_error("[b200] conv_plan: bn must be 0 (chosen), 64, 128 or 256");
+  return plan_conv(kind, N, H, W, Cin, Cout, sms, bn, 0, nullptr);
 }
 
 void conv_pixel_box(int N, int H, int W, int* box) {
-  ConvTile t = make_tile(N, H, W, UMMA_BM);
-  const bool fill = !halo_applicable(H, W) && conv_fill_tile(N, H, W, &t);
-  box[0] = t.Wb; box[1] = t.Hb; box[2] = t.Nb; box[3] = fill ? 1 : 0;
+  const ConvPlan p = conv_plan(CONV_KIND_FPROP, N, H, W, 64, 64, num_sms());
+  box[0] = p.Wb; box[1] = p.Hb; box[2] = p.Nb; box[3] = p.path == CONV_PATH_FILL ? 1 : 0;
 }
 
-int conv_bn_choice(int N, int H, int W, int cn) {
-  if (halo_applicable(H, W)) return cn <= 64 ? 64 : 128;
-  ConvTile t = make_tile(N, H, W, UMMA_BM);
-  conv_fill_tile(N, H, W, &t);
-  return conv_bn_pixels(t, cn);
-}
+int conv_bn_choice(int N, int H, int W, int cn) { return conv_plan(CONV_KIND_FPROP, N, H, W, 64, cn, num_sms()).bn; }
 
 static void fprop_impl(const bf16* x, const bf16* w, const float* bias, bf16* y, bf16* pool_out,
                        uint32_t* pool_mask, int N, int H, int W, int Cin, int Cout, bool relu, int bn,
@@ -460,29 +559,28 @@ static void fprop_impl(const bf16* x, const bf16* w, const float* bias, bf16* y,
   check_channels(Cout, "conv3x3_fprop Cout");
   // the epilogue stages the bias in a 512-float shared-memory scratch (ConvPolicy::EPI_MAXC)
   if (bias && Cout > 512) throw std::runtime_error("[b200] conv3x3_fprop: a bias supports Cout <= 512");
+  const bool pool = pool_out != nullptr;
   ConvParams prm;
-  prm.t = make_tile(N, H, W, UMMA_BM);
+  const ConvPlan plan = plan_conv(pool ? CONV_KIND_FPROP_POOL : CONV_KIND_FPROP, N, H, W, Cin, Cout, num_sms(), bn,
+                                  0, &prm.t);
+  bn = plan.bn;
+  prm.t.N = N; prm.t.H = H; prm.t.W = W;
   prm.Ca = Cin; prm.Cn = Cout; prm.wcols_per_tap = Cin;
   prm.out = y; prm.bias = bias; prm.mask_src = nullptr; prm.colsum = nullptr;
   prm.pool_out = pool_out; prm.pool_mask = pool_mask;
   prm.flags = (bias ? CONV_BIAS : 0) | (relu ? CONV_RELU : 0) | (pool_out ? CONV_POOL : 0);
-  const bool pool = pool_out != nullptr;
-  prm.resident = 0;
-  if (halo_applicable(H, W)) {
-    if (bn == 0) bn = Cout <= 64 ? 64 : 128;
-    map_2d(&prm.mapB, w, Cout, 9LL * Cin, 9LL * Cin, 64, bn);
+  prm.resident = plan.resident;
+  map_2d(&prm.mapB, w, Cout, 9LL * Cin, 9LL * Cin, 64, bn);
+  if (plan.path == CONV_PATH_HALO) {
     switch (bn) {
       case 64: pool ? conv_halo_launch<64, false, true>(prm, x, stream) : conv_halo_launch<64, false>(prm, x, stream); return;
       case 128: pool ? conv_halo_launch<128, false, true>(prm, x, stream) : conv_halo_launch<128, false>(prm, x, stream); return;
       default: throw std::runtime_error("[b200] conv3x3_fprop: bn must be 64 or 128");
     }
   }
-  const bool fill = !pool && conv_fill_tile(N, H, W, &prm.t);
-  if (fill) set_fill(prm);
-  if (bn == 0) bn = conv_bn_pixels(prm.t, Cout);
-  map_2d(&prm.mapB, w, Cout, 9LL * Cin, 9LL * Cin, 64, bn);
   map_nhwc(&prm.mapA, x, N, H, W, Cin, prm.t.Wb, prm.t.Hb, prm.t.Nb);
-  if (fill) {
+  if (plan.path == CONV_PATH_FILL) {
+    set_fill(prm);
     switch (bn) {
       case 64: conv_launch<64, false, false, true>(prm, stream); return;
       case 128: conv_launch<128, false, false, true>(prm, stream); return;
@@ -523,28 +621,27 @@ void conv3x3_dgrad(const bf16* dz, const bf16* w, const bf16* mask_src, bf16* dx
                    int H, int W, int Cin, int Cout, int bn, cudaStream_t stream) {
   check_channels(Cin, "conv3x3_dgrad Cin");
   check_channels(Cout, "conv3x3_dgrad Cout");
+  if (colsum && Cin > 512) throw std::runtime_error("[b200] conv3x3_dgrad: fused column sum supports Cin <= 512");
   ConvParams prm;
-  prm.t = make_tile(N, H, W, UMMA_BM);
+  const ConvPlan plan = plan_conv(CONV_KIND_DGRAD, N, H, W, Cin, Cout, num_sms(), bn, 0, &prm.t);
+  bn = plan.bn;
+  prm.t.N = N; prm.t.H = H; prm.t.W = W;
   prm.Ca = Cout; prm.Cn = Cin; prm.wcols_per_tap = Cin;
   prm.out = dx; prm.bias = nullptr; prm.mask_src = mask_src; prm.colsum = colsum;
   prm.pool_out = nullptr; prm.pool_mask = nullptr;
   prm.flags = (mask_src ? CONV_MASK : 0) | (colsum ? CONV_COLSUM : 0);
-  if (colsum && Cin > 512) throw std::runtime_error("[b200] conv3x3_dgrad: fused column sum supports Cin <= 512");
-  prm.resident = 0;
+  prm.resident = plan.resident;
   map_2d(&prm.mapB, w, Cout, 9LL * Cin, 9LL * Cin, 64, 64);   // MN-major: 64 ci x 64 co boxes
-  if (halo_applicable(H, W)) {
-    if (bn == 0) bn = Cin <= 64 ? 64 : 128;
+  if (plan.path == CONV_PATH_HALO) {
     switch (bn) {
       case 64: conv_halo_launch<64, true>(prm, dz, stream); return;
       case 128: conv_halo_launch<128, true>(prm, dz, stream); return;
       default: throw std::runtime_error("[b200] conv3x3_dgrad: bn must be 64 or 128");
     }
   }
-  const bool fill = conv_fill_tile(N, H, W, &prm.t);
-  if (fill) set_fill(prm);
-  if (bn == 0) bn = conv_bn_pixels(prm.t, Cin);
   map_nhwc(&prm.mapA, dz, N, H, W, Cout, prm.t.Wb, prm.t.Hb, prm.t.Nb);
-  if (fill) {
+  if (plan.path == CONV_PATH_FILL) {
+    set_fill(prm);
     switch (bn) {
       case 64: conv_launch<64, true, false, true>(prm, stream); return;
       case 128: conv_launch<128, true, false, true>(prm, stream); return;
@@ -569,29 +666,17 @@ static void wgrad_launch(WgradParams& prm, cudaStream_t stream) {
   launch<P>(prm, stream);
 }
 
-// Pixel-tile splits of the halo wgrad: one work item per SM, none empty.
-static int wgrad_halo64_splits(int total_tiles, int tiles_n, int sms, int* tiles_per_split) {
-  int ksplit = sms / tiles_n;
-  if (ksplit < 1) ksplit = 1;
-  if (ksplit > total_tiles) ksplit = total_tiles;
-  *tiles_per_split = (total_tiles + ksplit - 1) / ksplit;
-  return (total_tiles + *tiles_per_split - 1) / *tiles_per_split;
-}
-static bool wgrad_halo64_applicable(int H, int W, int Cin) {
-  return Cin == 64 && H % WH_T == 0 && W % WH_T == 0 && W >= 16 && halo_enabled();
-}
-
 // 64-input-channel layers on 8-divisible maps: nine tap views of one X halo per pixel tile.
 template <bool PARTIAL = false>
-static int wgrad_halo64_launch(const bf16* dz, const bf16* x, float* dw, long long ws_elems, int N, int H, int W,
-                               int Cout, float scale, cudaStream_t stream) {
+static int wgrad_halo64_launch(const ConvPlan& plan, const bf16* dz, const bf16* x, float* dw, long long ws_elems,
+                               int N, int H, int W, int Cout, float scale, cudaStream_t stream) {
   WgradHaloParams prm;
   prm.tiles_n = (Cout + 63) / 64;
   prm.tiles_w = W / WH_T; prm.tiles_h = H / WH_T;
-  prm.total_tiles = N * prm.tiles_w * prm.tiles_h;
-  const int ksplit = wgrad_halo64_splits(prm.total_tiles, prm.tiles_n, num_sms(), &prm.tiles_per_split);
-  if (PARTIAL) check_workspace("conv3x3_wgrad_partial", dw, ws_elems, ksplit, static_cast<long long>(Cout) * 9 * 64);
-  prm.num_items = prm.tiles_n * ksplit;
+  prm.total_tiles = static_cast<int>(plan.tiles);
+  prm.tiles_per_split = plan.tiles_per_split;
+  if (PARTIAL) check_workspace("conv3x3_wgrad_partial", dw, ws_elems, plan.ksplit, static_cast<long long>(Cout) * 9 * 64);
+  prm.num_items = prm.tiles_n * plan.ksplit;
   prm.Cout = Cout; prm.dW = dw; prm.scale = scale;
   map_nhwc(&prm.mapX, x, N, H, W, 64, WH_PITCH, WH_PITCH, 1);
   map_nhwc(&prm.mapZ, dz, N, H, W, Cout, WH_T, WH_T, 1);
@@ -606,85 +691,33 @@ static int wgrad_halo64_launch(const bf16* dz, const bf16* x, float* dw, long lo
   wgrad_halo64_kernel<PARTIAL><<<grid, WH_THREADS, WH_SMEM, stream>>>(prm);
   count_launch();
   check_last("wgrad_halo64_kernel launch");
-  return ksplit;
-}
-
-// Pixel-tile splits of the generic wgrad when every split stores a slice of partials that a second
-// kernel adds up.  A slice costs a write and a read of Cout*9*Cin floats, so the 4096-pixel work
-// items of the atomic path (196 splits, 115 MB of partials at 128 -> 128 channels, 112^2, batch 64)
-// are too fine.  Of the counts that give at most ~4 work items per SM, take the one with the least
-// modelled time: waves over the SMs x k-blocks per item, plus the slices' traffic in the same unit
-// (WS_ELEMS_PER_KBLOCK floats written and read back in the time one SM takes for a k-block:
-// ~0.5 us against ~2.5 TB/s; a model, see DESIGN 2.9 for what was measured).  Ties: fewer splits.
-constexpr long long WS_ELEMS_PER_KBLOCK = 160000;
-static int wgrad_partial_ksplit(int total_tiles, int base, long long slice_elems, int sms) {
-  int kmax = (4 * sms + base - 1) / base;
-  if (kmax > total_tiles) kmax = total_tiles;
-  int best = 1;
-  long long best_cost = -1;
-  for (int k = 1; k <= kmax; ++k) {
-    const long long waves = (static_cast<long long>(base) * k + sms - 1) / sms;
-    const long long depth = (total_tiles + k - 1) / k;
-    const long long cost = waves * depth * WS_ELEMS_PER_KBLOCK + k * slice_elems;
-    if (best_cost < 0 || cost < best_cost) { best = k; best_cost = cost; }
-  }
-  return best;
-}
-
-// Pixel tiles and split of the generic wgrad.  ksplit <= 0: chosen here.
-static void wgrad_split(WgradParams& prm, int N, int H, int W, int Cin, int Cout, int ksplit, int bn, int sms,
-                        bool partial) {
-  prm.t = make_tile(N, H, W, 64);
-  const int tiles_n = (N + prm.t.Nb - 1) / prm.t.Nb;
-  prm.Cout = Cout; prm.Cin = Cin;
-  prm.total_tiles = prm.t.tiles_w * prm.t.tiles_h * tiles_n;
-  // The split is chosen for the width asked for, or for the narrow tile when the width is chosen
-  // here; a 256-wide tile then keeps that split, so it has half as many work items of the same depth.
-  const int split_bn = bn ? bn : (Cin <= 64 ? 64 : 128);
-  if (ksplit <= 0) {     // work items of <= ~64 k-blocks (4096 pixels), and at least ~4 per SM
-    const int base = ((Cout + UMMA_BM - 1) / UMMA_BM) * ((Cin + split_bn - 1) / split_bn) * 9;
-    if (partial) {
-      ksplit = wgrad_partial_ksplit(prm.total_tiles, base, static_cast<long long>(Cout) * 9 * Cin, sms);
-    } else {
-      ksplit = (prm.total_tiles + 63) / 64;
-      const int min_split = (4 * sms + base - 1) / base;
-      if (ksplit < min_split) ksplit = min_split;
-    }
-  }
-  if (ksplit > prm.total_tiles) ksplit = prm.total_tiles;
-  prm.tiles_per_split = (prm.total_tiles + ksplit - 1) / ksplit;
-  prm.ksplit = (prm.total_tiles + prm.tiles_per_split - 1) / prm.tiles_per_split;
+  return plan.ksplit;
 }
 
 int conv_wgrad_splits(int N, int H, int W, int Cin, int Cout, int sms) {
-  if (wgrad_halo64_applicable(H, W, Cin)) {
-    int per_split;
-    return wgrad_halo64_splits(N * (W / WH_T) * (H / WH_T), (Cout + 63) / 64, sms, &per_split);
-  }
-  WgradParams prm;
-  wgrad_split(prm, N, H, W, Cin, Cout, 0, 0, sms, true);
-  return prm.ksplit;
+  return conv_plan(CONV_KIND_WGRAD_PARTIAL, N, H, W, Cin, Cout, sms).ksplit;
 }
 
 static int wgrad_impl(const bf16* dz, const bf16* x, float* dw, long long ws_elems, bool partial, int N, int H,
                       int W, int Cin, int Cout, float scale, int ksplit, int bn, cudaStream_t stream) {
   check_channels(Cin, "conv3x3_wgrad Cin");
   check_channels(Cout, "conv3x3_wgrad Cout");
-  if (wgrad_halo64_applicable(H, W, Cin) && bn == 0 && ksplit <= 0) {
-    if (partial) return wgrad_halo64_launch<true>(dz, x, dw, ws_elems, N, H, W, Cout, scale, stream);
-    return wgrad_halo64_launch(dz, x, dw, 0, N, H, W, Cout, scale, stream);
-  }
   WgradParams prm;
-  wgrad_split(prm, N, H, W, Cin, Cout, ksplit, bn, num_sms(), partial);
-  if (partial) check_workspace("conv3x3_wgrad_partial", dw, ws_elems, prm.ksplit, static_cast<long long>(Cout) * 9 * Cin);
-  if (bn == 0) {
-    const long long items = static_cast<long long>((Cout + UMMA_BM - 1) / UMMA_BM) * 9 * prm.ksplit;
-    bn = conv_bn(Cin, items * ((Cin + 127) / 128), items * ((Cin + 255) / 256));
+  const ConvPlan plan = plan_conv(partial ? CONV_KIND_WGRAD_PARTIAL : CONV_KIND_WGRAD, N, H, W, Cin, Cout, num_sms(),
+                                  bn, ksplit, &prm.t);
+  if (plan.path == CONV_PATH_WGRAD_HALO64) {
+    if (partial) return wgrad_halo64_launch<true>(plan, dz, x, dw, ws_elems, N, H, W, Cout, scale, stream);
+    return wgrad_halo64_launch(plan, dz, x, dw, 0, N, H, W, Cout, scale, stream);
   }
+  prm.Cout = Cout; prm.Cin = Cin;
+  prm.total_tiles = static_cast<int>(plan.tiles);
+  prm.tiles_per_split = plan.tiles_per_split;
+  prm.ksplit = plan.ksplit;
+  if (partial) check_workspace("conv3x3_wgrad_partial", dw, ws_elems, prm.ksplit, static_cast<long long>(Cout) * 9 * Cin);
   prm.dW = dw; prm.scale = scale;
   map_nhwc(&prm.mapA, dz, N, H, W, Cout, prm.t.Wb, prm.t.Hb, prm.t.Nb);
   map_nhwc(&prm.mapB, x, N, H, W, Cin, prm.t.Wb, prm.t.Hb, prm.t.Nb);
-  switch (bn) {
+  switch (plan.bn) {
     case 64: partial ? wgrad_launch<64, true>(prm, stream) : wgrad_launch<64>(prm, stream); break;
     case 128: partial ? wgrad_launch<128, true>(prm, stream) : wgrad_launch<128>(prm, stream); break;
     case 256: partial ? wgrad_launch<256, true>(prm, stream) : wgrad_launch<256>(prm, stream); break;

@@ -153,27 +153,18 @@ def conv_chain(depth_channels: int) -> int:
     return 9 * depth_channels // 16 + 2
 
 
-def _pow2_div(x: int, cap: int) -> int:
-    p = 1
-    while p * 2 <= cap and x % (p * 2) == 0:
-        p *= 2
-    return p
+def split_chain(tiles_per_split: int, ksplit: int) -> int:
+    """Split-K wgrad: k16 steps over one split's 64-pixel tiles + the splits added + the epilogue operation."""
+    return 4 * tiles_per_split + ksplit + 1
 
 
-def wgrad_chain(N: int, H: int, W: int, Cin: int, Cout: int, sms: int) -> int:
-    """conv3x3_wgrad with its default split: k16 steps over one split's pixel tiles + the splits."""
-    if Cin == 64 and H % 8 == 0 and W % 8 == 0 and W >= 16:          # wgrad_halo64: 8 x 8 pixel tiles
-        tiles = N * (H // 8) * (W // 8)
-        ks = max(1, min(sms // _cdiv(Cout, 64), tiles))
-    else:                                                            # WgradPolicy: 64-pixel boxes
-        wb = _pow2_div(W, 32)
-        hb = _pow2_div(H, 64 // wb)
-        nb = 64 // (wb * hb)
-        tiles = _cdiv(W, wb) * _cdiv(H, hb) * _cdiv(N, nb)
-        base = _cdiv(Cout, 128) * _cdiv(Cin, 64 if Cin <= 64 else 128) * 9
-        ks = min(max(_cdiv(tiles, 64), _cdiv(4 * sms, base)), tiles)
-    per = _cdiv(tiles, ks)
-    return 4 * per + _cdiv(tiles, per) + 1
+def wgrad_chain(N: int, H: int, W: int, Cin: int, Cout: int, sms: int, kind: str = "wgrad", bn: int = 0) -> int:
+    """conv3x3_wgrad (``kind`` "wgrad_partial": conv3x3_wgrad_partial + the reduce) with its default split, at
+    tile width ``bn`` (0: the launcher's own), as the launcher plans it (conv_plan: needs the extension)."""
+    from distributed_vgg_f_b200 import ops
+
+    p = ops.require().conv_plan(kind, N, H, W, Cin, Cout, sms, bn)
+    return split_chain(p["tiles_per_split"], p["ksplit"])
 
 
 def conv0_wgrad_chain(pixels: int, sms: int) -> int:
@@ -183,10 +174,12 @@ def conv0_wgrad_chain(pixels: int, sms: int) -> int:
     return 4 * _cdiv(tiles, grid) + 2 * grid
 
 
-def conv_colsum_chain(pixels: int, channels: int, sms: int) -> int:
+def conv_colsum_chain(pixels: int, channels: int, sms: int, tiles: int = None) -> int:
     """Fused column sum of conv dgrad: a 5-level warp reduction, at most four warp sums per tile into
-    the CTA's shared-memory sums, one global atomic per CTA."""
-    tiles = _cdiv(pixels, 128) * _cdiv(channels, 64)
+    the CTA's shared-memory sums, one global atomic per CTA.  ``tiles``: the launch's pixel tiles times
+    its 64-channel blocks, where the pixel box does not fill the 128-row tile (default: full tiles)."""
+    if tiles is None:
+        tiles = _cdiv(pixels, 128) * _cdiv(channels, 64)
     return 5 + 4 * _cdiv(tiles, min(tiles, sms)) + sms
 
 

@@ -10,6 +10,7 @@ import torch
 import torch.nn.functional as F
 
 import kernel_check as KC
+from distributed_vgg_f_b200 import ops
 from distributed_vgg_f_b200.ops import ref as R
 
 MODES = ["exact", "gauss"]
@@ -215,7 +216,7 @@ def test_wgrad_criterion_catches_a_missing_pixel_block(mode):
     # emulation: the pixel reduction in 64-pixel k-blocks per tap, fp32
     A = dz.reshape(P, C)
     taps = list(R._taps(x))
-    chain = KC.wgrad_chain(N, H, W, C, C, sms=132)
+    chain = KC.split_chain(1, 8)     # wgrad_halo64 at 132 SMs: 8 pixel tiles, one per split (next test)
 
     def emu(drop=None):
         out = torch.zeros(C, 3, 3, C)
@@ -226,6 +227,14 @@ def test_wgrad_criterion_catches_a_missing_pixel_block(mode):
 
     KC.check(emu(), ref, mag, chain=chain, exact=exact)
     _rejects(lambda: KC.check(emu(drop=3), ref, mag, chain=chain, exact=exact))
+
+
+@pytest.mark.skipif(not ops.available(), reason="needs the built extension (host code only)")
+def test_wgrad_chain_is_the_planned_split():
+    """The split the criterion above assumes is the one the launcher plans for that shape."""
+    p = ops.require().conv_plan("wgrad", 4, 8, 16, 64, 64, 132)
+    assert (p["path"], p["tiles_per_split"], p["ksplit"]) == ("wgrad_halo64", 1, 8)
+    assert KC.wgrad_chain(4, 8, 16, 64, 64, 132) == KC.split_chain(1, 8)
 
 
 @pytest.mark.parametrize("mode", MODES)

@@ -35,19 +35,6 @@ def _case(N, H, W, Cin, Cout, seed, mode):
     return x, w, b, g
 
 
-def _wgrad_chain_bn(N, H, W, Cin, Cout, sms, bn):
-    """conv3x3_wgrad's fp32 addition chain with an explicit tile width: the default split is chosen
-    for that width (WgradPolicy, 64-pixel boxes)."""
-    wb = KC._pow2_div(W, 32)
-    hb = KC._pow2_div(H, 64 // wb)
-    nb = 64 // (wb * hb)
-    tiles = KC._cdiv(W, wb) * KC._cdiv(H, hb) * KC._cdiv(N, nb)
-    base = KC._cdiv(Cout, 128) * KC._cdiv(Cin, bn) * 9
-    ks = min(max(KC._cdiv(tiles, 64), KC._cdiv(4 * sms, base)), tiles)
-    per = KC._cdiv(tiles, ks)
-    return 4 * per + KC._cdiv(tiles, per) + 1
-
-
 @pytest.mark.parametrize("mode", MODES)
 @WIDE
 def test_wide_fprop(N, H, W, Cin, Cout, mode):
@@ -110,5 +97,5 @@ def test_wide_wgrad(N, H, W, Cin, Cout, mode):
     dw = torch.zeros(Cout, 3, 3, Cin, device=DEV)
     ops.conv3x3_wgrad(dz, x, dw, bn=256)
     ref, mag = R.conv3x3_wgrad64(dz, x)
-    KC.check(dw, ref, mag, chain=_wgrad_chain_bn(N, H, W, Cin, Cout, KC.sm_count(), 256), exact=mode == "exact",
+    KC.check(dw, ref, mag, chain=KC.wgrad_chain(N, H, W, Cin, Cout, KC.sm_count(), bn=256), exact=mode == "exact",
              family="conv_wgrad", what="bn=256")
