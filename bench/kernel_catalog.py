@@ -30,6 +30,8 @@ ROLE = [   # (regex on the demangled name, role, what it replaces in the referen
     (r"im2col3x3_c3_kernel|nchw_f32_to_nhwc_bf16_kernel", "input layout conversion for float inputs (tests, `forward_logits`)", "—"),
     (r"adam_kernel", "fused Adam over a bucket: grad (fp32 arena or bf16 wire) → fp32 master, moments, bf16 shadow, gradient range re-zeroed; evict-first streams", "`torch.optim.Adam` foreach kernels + `zero_grad` — `:230`, `:170-172`"),
     (r"sgd_kernel", "fused SGD + momentum (the reference's vestigial constants)", "—"),
+    (r"layerwise_norms_kernel", "LAMB / LARS phase 1 over a bucket: LAMB's moments, and per-CTA partial sums of ‖p‖² and ‖u‖² (LAMB) or ‖g‖² (LARS) at host-assigned slots, one tensor per CTA", "timm `Lamb` / `Lars`: per-tensor `norm` — not in the reference"),
+    (r"layerwise_update_kernel", "LAMB / LARS phase 2 over the tensors a bucket completes: trust ratio from the slots in a fixed order, the update, bf16 shadow, EMA, (LARS) gradient re-zeroed", "timm `Lamb` / `Lars` `step` — not in the reference"),
     (r"allreduce_kernel<0", "K-AR one-shot: every rank sums all peers' chunk over peer memory (no-multicast fallback)", "c10d Reducer + gloo all-reduce — `:225`, `:171`"),
     (r"allreduce_kernel<1", "K-AR two-shot: reduce-scatter + all-gather by peer loads / stores in one pass", "same"),
     (r"allreduce_kernel<2", "K-AR NVLS: pack fp32→bf16·1/ws, handshake, `multimem.ld_reduce` (switch adds, fp32 accumulate) + `multimem.st`, handshake", "same"),

@@ -412,6 +412,69 @@ static void sgd(at::Tensor p, at::Tensor mom, c10::optional<at::Tensor> g32, c10
                         shadow.has_value() ? bfp_mut(*shadow) : nullptr, f32p_opt(gzero), f32p_opt(ema), p.numel(),
                         cur_stream());
 }
+// LAMB / LARS, one phase of one launch over p's n elements (loss_optim.cu).  The segment table comes as six
+// equal-length lists; the workspace must hold every slot the table names, the ratio array every tensor.
+static void layerwise(int64_t phase, const std::string& kind, at::Tensor p, at::Tensor m, c10::optional<at::Tensor> v,
+                      c10::optional<at::Tensor> g32, c10::optional<at::Tensor> g16, c10::optional<at::Tensor> shadow,
+                      c10::optional<at::Tensor> gzero, c10::optional<at::Tensor> ema, at::Tensor ws,
+                      c10::optional<at::Tensor> ratio, double lr, double b1, double b2, double eps, double momentum,
+                      int64_t step, bool first, double grad_scale, double ema_decay, bool ema_first,
+                      const std::vector<int64_t>& starts, const std::vector<int64_t>& ctas,
+                      const std::vector<int64_t>& slots, const std::vector<int64_t>& nslots,
+                      const std::vector<int64_t>& tensors, const std::vector<double>& wds, double trust_coeff,
+                      double trust_eps) {
+  c10::cuda::CUDAGuard g(p.device());
+  TORCH_CHECK(phase == 1 || phase == 2, "layerwise: phase must be 1 or 2");
+  TORCH_CHECK(kind == "lamb" || kind == "lars", "layerwise: kind must be lamb or lars, got ", kind);
+  const bool lamb = kind == "lamb";
+  const char* op = phase == 1 ? "layerwise_phase1" : "layerwise_phase2";
+  TORCH_CHECK(!lamb || v.has_value(), op, ": LAMB needs v");
+  const bool reads_grad = phase == 1 || !lamb;
+  TORCH_CHECK(!reads_grad || g32.has_value() != g16.has_value(), op, ": exactly one of g32 and g16");
+  TORCH_CHECK(reads_grad || (!g32.has_value() && !g16.has_value() && !gzero.has_value()), op,
+              ": LAMB's phase 2 reads no gradient");
+  TORCH_CHECK(phase == 2 || (!shadow.has_value() && !ema.has_value() && !ratio.has_value()), op,
+              ": phase 1 writes no shadow, EMA or ratio");
+  TORCH_CHECK(!(phase == 1 && !lamb && gzero.has_value()), op, ": LARS clears the gradient in phase 2");
+  const int64_t n = p.numel();
+  for (const at::Tensor* t : {&p, &m}) check_vec(*t, at::kFloat, 16, op, "p and m");
+  if (lamb) check_vec(*v, at::kFloat, 16, op, "v");
+  check_ema(ema, n, ema_decay, op);
+  if (g32.has_value()) check_vec(*g32, at::kFloat, 16, op, "g32");
+  if (gzero.has_value()) check_vec(*gzero, at::kFloat, 16, op, "gzero");
+  if (g16.has_value()) check_vec(*g16, at::kBFloat16, 8, op, "g16");
+  if (shadow.has_value()) check_vec(*shadow, at::kBFloat16, 8, op, "shadow");
+  for (const auto* t : {&g32, &g16, &shadow, &gzero})
+    TORCH_CHECK(!t->has_value() || (*t)->numel() == n, op, ": every tensor has p's size");
+  TORCH_CHECK(m.numel() == n && (!lamb || v->numel() == n), op, ": every tensor has p's size");
+  check_vec(ws, at::kFloat, 16, op, "ws");
+  const b200::LayerwiseLaunch L =
+      b200::make_layerwise_launch(op, p.numel(), starts, ctas, slots, nslots, tensors, wds, trust_coeff, trust_eps,
+                                  b200::layerwise_max_grid());
+  int64_t need = 0, tmax = -1;
+  for (size_t k = 0; k < starts.size(); ++k) {
+    need = std::max<int64_t>(need, slots[k] + (phase == 1 ? ctas[k] : nslots[k]));
+    tmax = std::max<int64_t>(tmax, tensors[k]);
+    TORCH_CHECK(phase == 1 || nslots[k] >= 1, op, ": every tensor has at least one slot");
+  }
+  TORCH_CHECK(ws.numel() >= 2 * need, op, ": ws must hold 2 x ", need, " floats, got ", ws.numel());
+  if (ratio.has_value()) {
+    check_vec(*ratio, at::kFloat, 4, op, "ratio");
+    TORCH_CHECK(ratio->numel() > tmax, op, ": ratio must hold tensor ", tmax);
+  }
+  const b200::OptStep o = b200::make_opt_step(op, lamb ? b200::OPT_LAMB : b200::OPT_LARS, p.numel(), lr,
+                                              lamb ? b1 : 0.0, lamb ? b2 : 0.0, lamb ? eps : 0.0, momentum,
+                                              lamb ? (int)step : 0, first, grad_scale, 0.0, {}, {}, ema_decay,
+                                              ema_first);
+  float* vp = lamb ? f32p(*v) : nullptr;
+  if (phase == 1)
+    b200::layerwise_phase1(o, L, f32p(p), f32p(m), vp, f32p_opt(g32), bfp_opt(g16), f32p_opt(gzero), f32p(ws),
+                           cur_stream());
+  else
+    b200::layerwise_phase2(o, L, f32p(p), f32p(m), vp, f32p_opt(g32), bfp_opt(g16),
+                           shadow.has_value() ? bfp_mut(*shadow) : nullptr, f32p_opt(gzero), f32p_opt(ema), f32p(ws),
+                           f32p_opt(ratio), cur_stream());
+}
 static void ema_update(const at::Tensor& p, at::Tensor ema, double decay, bool first) {
   c10::cuda::CUDAGuard g(p.device());
   check_vec(p, at::kFloat, 16, "ema_update", "p");
@@ -966,6 +1029,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0, py::arg("ema_first") = false,
         py::arg("wd_starts") = std::vector<int64_t>(), py::arg("wd_values") = std::vector<double>());
   m.def("ema_update", &ema_update, py::arg("p"), py::arg("ema"), py::arg("decay"), py::arg("first"));
+  m.def("layerwise", &layerwise, py::arg("phase"), py::arg("kind"), py::arg("p"), py::arg("m"), py::arg("v"),
+        py::arg("g32"), py::arg("g16"), py::arg("shadow"), py::arg("gzero"), py::arg("ema"), py::arg("ws"),
+        py::arg("ratio"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("momentum"),
+        py::arg("step"), py::arg("first"), py::arg("grad_scale"), py::arg("ema_decay"), py::arg("ema_first"),
+        py::arg("starts"), py::arg("ctas"), py::arg("slots"), py::arg("nslots"), py::arg("tensors"), py::arg("wds"),
+        py::arg("trust_coeff"), py::arg("trust_eps"));
+  m.def("layerwise_max_segments", [] { return b200::LW_MAX_SEGMENTS; });
   m.def("psgd_project", &psgd_project, py::arg("g"), py::arg("e"), py::arg("q"), py::arg("p"), py::arg("n"),
         py::arg("m"), py::arg("rank"), py::arg("scale"));
   m.def("psgd_backproject", &psgd_backproject, py::arg("M"), py::arg("p"), py::arg("q"), py::arg("ws"), py::arg("n"),

@@ -63,6 +63,43 @@ __device__ __forceinline__ void sgd_update(float g, float gscale, float& p, floa
   p = __fmaf_rn(-lr, buf, p);
 }
 
+// LAMB's moments from the scaled gradient gk = g * gscale (no decay term: LAMB adds it to the update),
+// rounded as adam_moments_step rounds them.
+__device__ __forceinline__ void lamb_moments(float gk, float& m, float& v, float b1, float b2) {
+  m = __fmaf_rn(b1, m, __fmul_rn(1.f - b1, gk));
+  v = __fmaf_rn(b2, v, __fmul_rn(__fmul_rn(1.f - b2, gk), gk));
+}
+
+// LAMB's update direction u = (m bc1_inv) / (sqrt(v) bc2_inv_sqrt + eps) + wd p.  Phase 1 takes the norm of
+// this u and phase 2 applies it, both through this function, so the norm is the norm of what is applied.
+__device__ __forceinline__ float lamb_direction(float m, float v, float p, float bc1_inv, float bc2_inv_sqrt,
+                                                float eps, float wd) {
+  const float denom = __fmaf_rn(__fsqrt_rn(v), bc2_inv_sqrt, eps);
+  return __fmaf_rn(wd, p, __fdiv_rn(__fmul_rn(m, bc1_inv), denom));
+}
+
+// Trust ratios from the whole tensor's sums of squares (timm's Lamb / Lars with trust_clip and always_adapt
+// off): a tensor without decay, or with a zero norm, is not adapted.
+__device__ __forceinline__ float lamb_ratio(float sum_p2, float sum_u2, float wd) {
+  const float pn = __fsqrt_rn(sum_p2), un = __fsqrt_rn(sum_u2);
+  return (wd != 0.f && pn > 0.f && un > 0.f) ? __fdiv_rn(pn, un) : 1.f;
+}
+__device__ __forceinline__ float lars_ratio(float sum_p2, float sum_g2, float wd, float coeff, float eps) {
+  const float pn = __fsqrt_rn(sum_p2), gn = __fsqrt_rn(sum_g2);
+  return (wd != 0.f && pn > 0.f && gn > 0.f)
+             ? __fdiv_rn(__fmul_rn(coeff, pn), __fadd_rn(__fadd_rn(gn, __fmul_rn(wd, pn)), eps))
+             : 1.f;
+}
+
+// One LARS step of an element: d = r (g gscale + wd p), buf = d (first step) or momentum buf + d,
+// p -= lr buf.
+__device__ __forceinline__ void lars_update(float g, float gscale, float& p, float& buf, float lr, float momentum,
+                                            float wd, float r, bool first) {
+  const float d = __fmul_rn(r, __fmaf_rn(wd, p, __fmul_rn(g, gscale)));
+  buf = first ? d : __fmaf_rn(momentum, buf, d);
+  p = __fmaf_rn(-lr, buf, p);
+}
+
 // The update of one element for the optimizer KIND (OptKind) of the step `o`, with decay value w (an L2
 // decay, or AdamW's keep factor).  m is SGD's momentum buffer; SGD leaves v alone.
 template <int KIND>

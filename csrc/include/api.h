@@ -198,7 +198,7 @@ EmaCoef ema_coef(double decay, bool first);
 // The scalars of one optimizer launch, in the form the kernels consume.  Built by make_opt_step only.
 // The field order matters to the kernels' register allocation: in some orders nvcc loads neighbouring
 // fields as pairs, which costs adam_kernel spills at its 40-register cap.
-enum OptKind : int { OPT_ADAM = 0, OPT_ADAMW = 1, OPT_SGD = 2 };
+enum OptKind : int { OPT_ADAM = 0, OPT_ADAMW = 1, OPT_SGD = 2, OPT_LAMB = 3, OPT_LARS = 4 };
 struct OptStep {
   float lr, beta1, beta2, eps;   // beta1, beta2, eps: Adam / AdamW
   float bc1_inv, bc2_inv_sqrt;   // 1 / (1 - beta1^step), 1 / sqrt(1 - beta2^step): double, rounded once
@@ -229,6 +229,48 @@ void optimizer_fused(const OptStep& o, float* p, float* m, float* v, const float
 // ema[i] = decay * ema[i] + (1 - decay) * p[i] with each operation rounded to fp32, or p[i] when `first`.
 // n elements, any n >= 0; p and ema 16-byte aligned.
 void ema_fused(const float* p, float* ema, long long n, double decay, bool first, cudaStream_t s);
+
+// ---- layer-wise adaptive optimizers: LAMB and LARS (loss_optim.cu) -----------------------------
+// The trust ratio of a tensor needs norms over the whole tensor, which the gradient buckets cut apart, so
+// each step of these optimizers takes two passes.  Phase 1 runs per bucket once its gradient is final
+// (LAMB: moments, and the partial sums of p^2 and u^2; LARS: the partial sums of p^2 and (g gscale)^2) and
+// stores one pair of partial sums per CTA at a slot the host assigned.  Phase 2 runs once per group of
+// tensors whose last piece that bucket held: it adds each tensor's partials in a fixed order, forms the
+// ratio and applies the update, the bf16 shadow, the EMA and (LARS) the gradient zeroing.  No atomics:
+// a ratio is the same bits on every run and every rank.
+//
+// One launch covers a range of n4 float4s cut into segments, segment k being float4s [start4[k],
+// start4[k + 1]) of one tensor and CTAs [cta0[k], cta0[k + 1]).  Phase 1: the segment's CTA j stores its
+// partials at ws[2 (slot[k] + j)], ws[2 (slot[k] + j) + 1].  Phase 2: the tensor's partials are slots
+// [slot[k], slot[k] + nslots[k]); its ratio goes to ratio[tensor[k]] when `ratio` is given.
+constexpr int LW_MAX_SEGMENTS = 16;
+struct LayerwiseLaunch {
+  int n;                                   // segments
+  int cta0[LW_MAX_SEGMENTS + 1];           // cta0[0] = 0, increasing; cta0[n] = the grid
+  long long start4[LW_MAX_SEGMENTS + 1];   // start4[0] = 0, increasing; start4[n] = the range's float4s
+  int slot[LW_MAX_SEGMENTS];
+  int nslots[LW_MAX_SEGMENTS];             // phase 2
+  int tensor[LW_MAX_SEGMENTS];             // phase 2
+  float wd[LW_MAX_SEGMENTS];               // the tensor's decay; 0 leaves it unadapted (ratio 1)
+  float trust_coeff, trust_eps;            // LARS: ratio = coeff |p| / (|g| + wd |p| + eps)
+};
+// Validates the table (naming `op`) and fills a LayerwiseLaunch: starts in elements of the range
+// (multiples of 4, the first 0, increasing, inside n), CTAs per segment >= 1 and at most `max_grid` in all.
+LayerwiseLaunch make_layerwise_launch(const char* op, long long n, const std::vector<int64_t>& starts,
+                                      const std::vector<int64_t>& ctas, const std::vector<int64_t>& slots,
+                                      const std::vector<int64_t>& nslots, const std::vector<int64_t>& tensors,
+                                      const std::vector<double>& wds, double trust_coeff, double trust_eps,
+                                      long long max_grid);
+// CTAs a layer-wise launch may use in all: the optimizer launches' cap, 4 per SM.
+long long layerwise_max_grid();
+// o.kind OPT_LAMB (m, v: the moments) or OPT_LARS (m: the momentum buffer, v unused).  Exactly one of g32
+// and g16.  Phase 1 of LAMB clears gzero when given; phase 1 of LARS only reads.
+void layerwise_phase1(const OptStep& o, const LayerwiseLaunch& L, float* p, float* m, float* v, const float* g32,
+                      const bf16* g16, float* gzero, float* ws, cudaStream_t s);
+// LAMB reads no gradient (g32 = g16 = null); LARS reads it and clears gzero when given.
+void layerwise_phase2(const OptStep& o, const LayerwiseLaunch& L, float* p, float* m, float* v, const float* g32,
+                      const bf16* g16, bf16* shadow, float* gzero, float* ema, const float* ws, float* ratio,
+                      cudaStream_t s);
 
 // ---- PowerSGD gradient compression (powersgd.cu) ----------------------------------------------
 // A compressed tensor is an n x m row-major fp32 matrix (m % 4 == 0); P is [n][rank], Q is [m][rank],

@@ -513,6 +513,8 @@ static int optimizer_grid(long long n4, bool adam) {
 void optimizer_fused(const OptStep& o, float* p, float* m, float* v, const float* g32, const bf16* g16,
                      bf16* shadow, float* gzero, float* ema, long long n, cudaStream_t s) {
   const char* what = o.kind == OPT_SGD ? "sgd_fused" : "adam_fused";
+  if (o.kind != OPT_ADAM && o.kind != OPT_ADAMW && o.kind != OPT_SGD)
+    throw std::runtime_error("[b200] optimizer_fused: LAMB and LARS run as layerwise_phase1 / layerwise_phase2");
   if (n % 4) throw std::runtime_error(std::string("[b200] ") + what + ": n must be a multiple of 4");
   const int blocks = optimizer_grid(n / 4, o.kind != OPT_SGD);
   OPT_KERNELS[o.kind][ema != nullptr]<<<blocks, 256, 0, s>>>(o, p, m, v, g32, g16, shadow, gzero, ema, n / 4);
@@ -526,6 +528,232 @@ void ema_fused(const float* p, float* ema, long long n, double decay, bool first
   ema_kernel<<<optimizer_grid(n / 4, false), 256, 0, s>>>(p, ema, n, ema_coef(decay, first));
   count_launch();
   check_last("ema_fused");
+}
+
+// ------------------------------------------------------------------ layer-wise adaptive (LAMB, LARS)
+// Same footprint as adam_kernel (256 threads, at most 4 CTAs per SM in all, evict-first streams, the
+// maximum-shared carve-out), plus 72 bytes of static shared memory for the block reduction.  Every CTA
+// works inside one segment (one tensor): it finds its segment from the CTA table and grid-strides over
+// the segment alone, so that its partial sums belong to one tensor.
+
+// The segment of this CTA: the last k with cta0[k] <= blockIdx.x.
+__device__ __forceinline__ int lw_segment(const LayerwiseLaunch& L) {
+  int k = 0;
+  while (k + 1 < L.n && static_cast<int>(blockIdx.x) >= L.cta0[k + 1]) ++k;
+  return k;
+}
+
+// Sum over the block of (a, b) in a fixed order: a butterfly within each warp, then thread 0 adds the
+// eight warp sums in warp order.  The result is valid in thread 0.
+__device__ __forceinline__ float2 lw_block_sum(float a, float b, float2* red) {
+  for (int o = 16; o; o >>= 1) {
+    a = __fadd_rn(a, __shfl_xor_sync(0xffffffffu, a, o));
+    b = __fadd_rn(b, __shfl_xor_sync(0xffffffffu, b, o));
+  }
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = make_float2(a, b);
+  __syncthreads();
+  float2 t = make_float2(0.f, 0.f);
+  if (threadIdx.x == 0)
+    for (int w = 0; w < 8; ++w) t = make_float2(__fadd_rn(t.x, red[w].x), __fadd_rn(t.y, red[w].y));
+  return t;
+}
+
+__device__ __forceinline__ void lw_load_grad(const float* __restrict__ g32, const bf16* __restrict__ g16, long long i,
+                                             float* g) {
+  if (g16) {
+    const uint2 raw = __ldcs(reinterpret_cast<const uint2*>(g16 + i * 4));
+    const float2 a = unpack_bf16x2(raw.x), b = unpack_bf16x2(raw.y);
+    g[0] = a.x; g[1] = a.y; g[2] = b.x; g[3] = b.y;
+  } else {
+    const float4 gv = __ldcs(reinterpret_cast<const float4*>(g32) + i);
+    g[0] = gv.x; g[1] = gv.y; g[2] = gv.z; g[3] = gv.w;
+  }
+}
+
+// Phase 1.  LAMB: m, v updated from g * gscale, partials (sum p^2, sum u^2), gzero cleared.
+// LARS: partials (sum p^2, sum (g * gscale)^2); nothing written but the partials.
+template <int KIND>
+__global__ void __launch_bounds__(256, 6) layerwise_norms_kernel(const __grid_constant__ OptStep o,
+    const __grid_constant__ LayerwiseLaunch L, const float* __restrict__ p, float* __restrict__ m,
+    float* __restrict__ v, const float* __restrict__ g32, const bf16* __restrict__ g16, float* __restrict__ gzero,
+    float* __restrict__ ws) {
+  __shared__ float2 red[8];
+  const int k = lw_segment(L);
+  const int j = static_cast<int>(blockIdx.x) - L.cta0[k];
+  const long long stride = static_cast<long long>(L.cta0[k + 1] - L.cta0[k]) * blockDim.x;
+  const float wd = L.wd[k];
+  float sp = 0.f, sq = 0.f;
+  for (long long i = L.start4[k] + static_cast<long long>(j) * blockDim.x + threadIdx.x; i < L.start4[k + 1];
+       i += stride) {
+    const float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i);
+    const float pp[4] = {pv.x, pv.y, pv.z, pv.w};
+    float g[4];
+    lw_load_grad(g32, g16, i, g);
+    if constexpr (KIND == OPT_LAMB) {
+      const float4 mv = __ldcs(reinterpret_cast<const float4*>(m) + i);
+      const float4 vv = __ldcs(reinterpret_cast<const float4*>(v) + i);
+      float mm[4] = {mv.x, mv.y, mv.z, mv.w}, vs[4] = {vv.x, vv.y, vv.z, vv.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        lamb_moments(__fmul_rn(g[e], o.grad_scale), mm[e], vs[e], o.beta1, o.beta2);
+        const float u = lamb_direction(mm[e], vs[e], pp[e], o.bc1_inv, o.bc2_inv_sqrt, o.eps, wd);
+        sp = __fmaf_rn(pp[e], pp[e], sp);
+        sq = __fmaf_rn(u, u, sq);
+      }
+      __stcs(reinterpret_cast<float4*>(m) + i, make_float4(mm[0], mm[1], mm[2], mm[3]));
+      __stcs(reinterpret_cast<float4*>(v) + i, make_float4(vs[0], vs[1], vs[2], vs[3]));
+      if (gzero) __stcs(reinterpret_cast<float4*>(gzero) + i, make_float4(0.f, 0.f, 0.f, 0.f));
+    } else {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float gk = __fmul_rn(g[e], o.grad_scale);
+        sp = __fmaf_rn(pp[e], pp[e], sp);
+        sq = __fmaf_rn(gk, gk, sq);
+      }
+    }
+  }
+  const float2 t = lw_block_sum(sp, sq, red);
+  if (threadIdx.x == 0) reinterpret_cast<float2*>(ws)[L.slot[k] + j] = t;
+}
+
+// Phase 2: the tensor's ratio from its partials (every CTA of the segment adds the same slots in the same
+// order), then LAMB: p -= lr (r u) with u recomputed from the stored moments; LARS: lars_update on the
+// gradient.  Then the shadow, the EMA and (LARS) the gradient zeroing.
+template <int KIND, bool EMA>
+__global__ void __launch_bounds__(256, 6) layerwise_update_kernel(const __grid_constant__ OptStep o,
+    const __grid_constant__ LayerwiseLaunch L, float* __restrict__ p, float* __restrict__ m,
+    const float* __restrict__ v, const float* __restrict__ g32, const bf16* __restrict__ g16,
+    bf16* __restrict__ shadow, float* __restrict__ gzero, float* __restrict__ ema, const float* __restrict__ ws,
+    float* __restrict__ ratio) {
+  __shared__ float2 red[8];
+  __shared__ float s_ratio;
+  const int k = lw_segment(L);
+  float a = 0.f, b = 0.f;
+  for (int s = threadIdx.x; s < L.nslots[k]; s += blockDim.x) {
+    const float2 w = reinterpret_cast<const float2*>(ws)[L.slot[k] + s];
+    a = __fadd_rn(a, w.x);
+    b = __fadd_rn(b, w.y);
+  }
+  const float2 t = lw_block_sum(a, b, red);
+  const float wd = L.wd[k];
+  if (threadIdx.x == 0) {
+    const float r = KIND == OPT_LAMB ? lamb_ratio(t.x, t.y, wd) : lars_ratio(t.x, t.y, wd, L.trust_coeff, L.trust_eps);
+    s_ratio = r;
+    if (ratio && static_cast<int>(blockIdx.x) == L.cta0[k]) ratio[L.tensor[k]] = r;
+  }
+  __syncthreads();
+  const float r = s_ratio;
+  const int j = static_cast<int>(blockIdx.x) - L.cta0[k];
+  const long long stride = static_cast<long long>(L.cta0[k + 1] - L.cta0[k]) * blockDim.x;
+  for (long long i = L.start4[k] + static_cast<long long>(j) * blockDim.x + threadIdx.x; i < L.start4[k + 1];
+       i += stride) {
+    const float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i);
+    const float4 mv = __ldcs(reinterpret_cast<const float4*>(m) + i);
+    float pp[4] = {pv.x, pv.y, pv.z, pv.w}, mm[4] = {mv.x, mv.y, mv.z, mv.w};
+    if constexpr (KIND == OPT_LAMB) {
+      const float4 vv = __ldcs(reinterpret_cast<const float4*>(v) + i);
+      const float vs[4] = {vv.x, vv.y, vv.z, vv.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float u = lamb_direction(mm[e], vs[e], pp[e], o.bc1_inv, o.bc2_inv_sqrt, o.eps, wd);
+        pp[e] = __fmaf_rn(-o.lr, __fmul_rn(r, u), pp[e]);
+      }
+    } else {
+      float g[4];
+      lw_load_grad(g32, g16, i, g);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) lars_update(g[e], o.grad_scale, pp[e], mm[e], o.lr, o.momentum, wd, r, o.first);
+      __stcs(reinterpret_cast<float4*>(m) + i, make_float4(mm[0], mm[1], mm[2], mm[3]));
+      if (gzero) __stcs(reinterpret_cast<float4*>(gzero) + i, make_float4(0.f, 0.f, 0.f, 0.f));
+    }
+    __stcs(reinterpret_cast<float4*>(p) + i, make_float4(pp[0], pp[1], pp[2], pp[3]));
+    if constexpr (EMA) ema_update4(ema + i * 4, pp, o.ema);
+    if (shadow)
+      __stcs(reinterpret_cast<uint2*>(shadow + i * 4), make_uint2(pack_bf16x2(pp[0], pp[1]), pack_bf16x2(pp[2], pp[3])));
+  }
+}
+
+using LwNormsKernel = void (*)(OptStep, LayerwiseLaunch, const float*, float*, float*, const float*, const bf16*,
+                               float*, float*);
+using LwUpdateKernel = void (*)(OptStep, LayerwiseLaunch, float*, float*, const float*, const float*, const bf16*,
+                                bf16*, float*, float*, const float*, float*);
+static const LwNormsKernel LW_NORMS[2] = {layerwise_norms_kernel<OPT_LAMB>, layerwise_norms_kernel<OPT_LARS>};
+static const LwUpdateKernel LW_UPDATE[2][2] = {   // [lars][ema]
+    {layerwise_update_kernel<OPT_LAMB, false>, layerwise_update_kernel<OPT_LAMB, true>},
+    {layerwise_update_kernel<OPT_LARS, false>, layerwise_update_kernel<OPT_LARS, true>}};
+
+long long layerwise_max_grid() {
+  static const bool once = [] {
+    for (auto k : LW_NORMS) prefer_max_shared_carveout(reinterpret_cast<const void*>(k));
+    for (const auto& kind : LW_UPDATE)
+      for (auto k : kind) prefer_max_shared_carveout(reinterpret_cast<const void*>(k));
+    return true;
+  }();
+  (void)once;
+  return static_cast<long long>(sm_count()) * 4;
+}
+
+LayerwiseLaunch make_layerwise_launch(const char* op, long long n, const std::vector<int64_t>& starts,
+                                      const std::vector<int64_t>& ctas, const std::vector<int64_t>& slots,
+                                      const std::vector<int64_t>& nslots, const std::vector<int64_t>& tensors,
+                                      const std::vector<double>& wds, double trust_coeff, double trust_eps,
+                                      long long max_grid) {
+  auto check = [op](bool ok, const auto&... msg) {
+    if (ok) return;
+    std::ostringstream s;
+    ((s << op) << ... << msg);
+    throw std::runtime_error(s.str());
+  };
+  const size_t ns = starts.size();
+  check(ns >= 1 && ns <= static_cast<size_t>(LW_MAX_SEGMENTS), ": 1 to ", LW_MAX_SEGMENTS, " segments per launch, got ",
+        ns);
+  check(ctas.size() == ns && slots.size() == ns && nslots.size() == ns && tensors.size() == ns && wds.size() == ns,
+        ": starts, ctas, slots, nslots, tensors and wds must have the same length");
+  check(n > 0 && n % 4 == 0, ": n must be a positive multiple of 4, got ", n);
+  LayerwiseLaunch L{};
+  L.n = static_cast<int>(ns);
+  L.trust_coeff = static_cast<float>(trust_coeff);
+  L.trust_eps = static_cast<float>(trust_eps);
+  long long grid = 0;
+  for (size_t k = 0; k < ns; ++k) {
+    check(k > 0 || starts[0] == 0, ": the first segment must start at 0");
+    check(k == 0 || starts[k] > starts[k - 1], ": segment starts must increase");
+    check(starts[k] % 4 == 0 && starts[k] < n, ": segment start ", starts[k], " is not a multiple of 4 inside ", n);
+    check(ctas[k] >= 1, ": every segment needs a CTA");
+    check(slots[k] >= 0 && nslots[k] >= 0 && tensors[k] >= 0, ": slots, slot counts and tensors must be >= 0");
+    check(std::isfinite(wds[k]) && wds[k] >= 0.0, ": weight decays must be finite and >= 0, got ", wds[k]);
+    L.cta0[k] = static_cast<int>(grid);
+    L.start4[k] = starts[k] / 4;
+    L.slot[k] = static_cast<int>(slots[k]);
+    L.nslots[k] = static_cast<int>(nslots[k]);
+    L.tensor[k] = static_cast<int>(tensors[k]);
+    L.wd[k] = static_cast<float>(wds[k]);
+    grid += ctas[k];
+  }
+  check(grid <= max_grid, ": ", grid, " CTAs exceed the cap of ", max_grid);
+  L.cta0[ns] = static_cast<int>(grid);
+  L.start4[ns] = n / 4;
+  return L;
+}
+
+void layerwise_phase1(const OptStep& o, const LayerwiseLaunch& L, float* p, float* m, float* v, const float* g32,
+                      const bf16* g16, float* gzero, float* ws, cudaStream_t s) {
+  if (o.kind != OPT_LAMB && o.kind != OPT_LARS) throw std::runtime_error("[b200] layerwise_phase1: LAMB or LARS");
+  layerwise_max_grid();
+  LW_NORMS[o.kind == OPT_LARS]<<<L.cta0[L.n], 256, 0, s>>>(o, L, p, m, v, g32, g16, gzero, ws);
+  count_launch();
+  check_last("layerwise_phase1");
+}
+
+void layerwise_phase2(const OptStep& o, const LayerwiseLaunch& L, float* p, float* m, float* v, const float* g32,
+                      const bf16* g16, bf16* shadow, float* gzero, float* ema, const float* ws, float* ratio,
+                      cudaStream_t s) {
+  if (o.kind != OPT_LAMB && o.kind != OPT_LARS) throw std::runtime_error("[b200] layerwise_phase2: LAMB or LARS");
+  layerwise_max_grid();
+  LW_UPDATE[o.kind == OPT_LARS][ema != nullptr]<<<L.cta0[L.n], 256, 0, s>>>(o, L, p, m, v, g32, g16, shadow, gzero,
+                                                                              ema, ws, ratio);
+  count_launch();
+  check_last("layerwise_phase2");
 }
 
 }  // namespace b200

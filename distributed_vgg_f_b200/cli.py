@@ -75,9 +75,13 @@ def build_parser() -> argparse.ArgumentParser:
                      help="bf16: the sm_90a engine (bf16 activations / weights / wire, fp32 master weights, moments and "
                           "accumulators).  fp32: the reference's arithmetic on the torch-op engine (the native kernels "
                           "have no tf32 path yet)")
-    ext.add_argument("--optimizer", default="adam", choices=["adam", "adamw", "sgd"],
+    ext.add_argument("--optimizer", default="adam", choices=["adam", "adamw", "sgd", "lamb", "lars"],
                      help="adam / sgd: L2 weight decay (torch.optim.Adam / SGD); adamw: decoupled weight decay "
-                          "(torch.optim.AdamW)")
+                          "(torch.optim.AdamW); lamb / lars: layer-wise trust ratio |w| / |update| per tensor for large "
+                          "global batches (timm's Lamb with eps 1e-6, and Lars with trust coefficient 1e-3 and "
+                          "--momentum).  Only tensors with a nonzero decay are adapted, so lamb / lars need "
+                          "--weight-decay > 0 (--bias-weight-decay 0 keeps the biases unadapted), and --zero1 on is "
+                          "refused with them at world size > 1")
     ext.add_argument("--momentum", type=float, default=TRAIN.momentum)
     ext.add_argument("--weight-decay", type=float, default=0.0,
                      help="weight decay of every parameter, >= 0 (default 0 = none, as the reference)")
@@ -227,6 +231,15 @@ def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
         build_parser().error("--model-ema-decay must lie in [0, 1)")
     if not args.weight_decay >= 0.0 or (args.bias_weight_decay is not None and not args.bias_weight_decay >= 0.0):
         build_parser().error("--weight-decay and --bias-weight-decay must be >= 0")
+    if args.optimizer in ("lamb", "lars"):
+        from .utils.optim import check_layerwise_decay
+        try:
+            check_layerwise_decay(args.optimizer, args.weight_decay)
+        except ValueError as e:
+            build_parser().error(str(e))
+        if args.zero1 == "on" and args.world_size > 1:
+            build_parser().error("--optimizer %s with --zero1 on: ZeRO-1 shards a tensor across ranks, and its trust "
+                                 "ratio needs the whole tensor's norms; use --zero1 off (or auto)" % args.optimizer)
     if args.lr_warmup_epochs < 0:
         build_parser().error("--lr-warmup-epochs must be >= 0")
     if args.lr_scheduler == "cosine" and args.lr_warmup_epochs >= args.epochs:

@@ -24,6 +24,13 @@ class TrainDefaults:
     adam_beta1: float = 0.9
     adam_beta2: float = 0.999
     adam_eps: float = 1e-8
+    # LAMB and LARS (--optimizer lamb|lars) as timm's Lamb / Lars with their defaults: bias correction on,
+    # no trust clipping, only tensors with a nonzero decay adapted.
+    lamb_beta1: float = 0.9
+    lamb_beta2: float = 0.999
+    lamb_eps: float = 1e-6
+    lars_trust_coeff: float = 1e-3
+    lars_eps: float = 1e-8
 
 
 @dataclasses.dataclass(frozen=True)

@@ -33,10 +33,12 @@ from ..config import DATA, TRAIN
 from ..data.loader import FusedBatch, RaggedBatch
 from ..models import layout as L
 from ..models.vggf import VGGSpec, build_oracle
+from ..parallel import layerwise as lw
 from ..parallel import powersgd as psgd
 from ..parallel.buckets import Bucket, BucketPlan, engine_bucket_plan
 from ..parallel.process_group import distributed_is_initialized
 from ..utils.metrics import DeviceMeter
+from ..utils.optim import LAYERWISE, check_layerwise_decay
 
 BF16 = torch.bfloat16
 F32 = torch.float32
@@ -171,11 +173,12 @@ class NativeEngine:
         if spec.convs[0].cout % 64 or spec.convs[0].cin != 3:
             raise ValueError("first conv must be 3 -> multiple of 64 channels")
         self.spec, self.device, self.B = spec, torch.device(device), int(batch)
-        if optimizer not in ("adam", "adamw", "sgd"):
-            raise ValueError("optimizer must be adam, adamw or sgd (got %r)" % optimizer)
+        if optimizer not in ("adam", "adamw", "sgd", "lamb", "lars"):
+            raise ValueError("optimizer must be adam, adamw, sgd, lamb or lars (got %r)" % optimizer)
         for what, wd in (("weight_decay", weight_decay), ("bias_weight_decay", bias_weight_decay)):
             if wd is not None and not wd >= 0.0:
                 raise ValueError("%s must be >= 0 (got %r)" % (what, wd))
+        check_layerwise_decay(optimizer, weight_decay)
         self.lr, self.opt_name, self.momentum, self.weight_decay = lr, optimizer, momentum, weight_decay
         # torchvision's --bias-weight-decay: the biases' own decay (None: the biases take weight_decay)
         self.bias_weight_decay = bias_weight_decay
@@ -248,7 +251,7 @@ class NativeEngine:
         self.p32 = torch.zeros(n, dtype=F32, device=dev)
         self.g32 = torch.zeros(ng, dtype=F32, device=dev)
         self.m32 = torch.zeros(ng, dtype=F32, device=dev)
-        self.v32 = torch.zeros(ng, dtype=F32, device=dev) if optimizer in ("adam", "adamw") else None
+        self.v32 = torch.zeros(ng, dtype=F32, device=dev) if optimizer in ("adam", "adamw", "lamb") else None
         # each bucket's weight-decay segments [(start within the bucket, decay), ...], one entry when the
         # decay is uniform: biases and weights share buckets, and one launch per bucket stays one launch
         self._wd_segments = {bk.start: self.decay_segments(bk) for bk in self.plan.buckets}
@@ -342,6 +345,54 @@ class NativeEngine:
         self._psgd_now = False           # per train_step: this update compresses (update index > start iter)
         if self.powersgd_rank:
             self._powersgd_setup(ready, bucket_mb, conv_bucket_mb, tail_bucket_kb, wire_dtype)
+        self._layerwise_setup()
+
+    # ============================================================================ LAMB / LARS
+    def layerwise_plans(self) -> Dict[bool, "lw.LayerwisePlan"]:
+        """The phase-1 / phase-2 launch plans of --optimizer lamb|lars (parallel/layerwise.py), keyed by whether
+        the update compresses with PowerSGD: the plain buckets, and the buckets without the compressed tensors
+        plus one unit per compressed tensor."""
+        sms = ops.require().sm_count()
+        plans = {False: lw.layerwise_plan(self.plan, self.decay_of, sms)}
+        if self.powersgd_rank:
+            plan2 = self._psgd_tables[1][0]
+            plans[True] = lw.layerwise_plan(plan2, self.decay_of, sms, lw.update_units(plan2, list(self._psgd)))
+        return plans
+
+    def _layerwise_setup(self) -> None:
+        """LAMB / LARS only: the launch plans, the partial-sum workspace (a pair of fp32 per slot, one slot per
+        phase-1 CTA) and the per-tensor trust ratios of the last update."""
+        self.layerwise = self.opt_name in LAYERWISE
+        if not self.layerwise:
+            return
+        self._lw_plans = self.layerwise_plans()
+        self._lw_ws = torch.zeros(max(p.workspace_elems() for p in self._lw_plans.values()), dtype=F32,
+                                  device=self.device)
+        self.trust_ratio = torch.ones(len(self._lw_plans[False].tensors), dtype=F32, device=self.device)
+
+    def _layerwise_update(self, s: int, e: int, g16: Optional[torch.Tensor], zero: bool, grad_scale: float) -> None:
+        """The update of unit [s, e) under LAMB / LARS: its phase-1 launches, then the phase-2 launches of the
+        tensors whose last piece it holds.  Both on the caller's stream, after the unit's reduction."""
+        plan = self._lw_plans[self._psgd_now]
+        lamb, kind = self.opt_name == "lamb", self.opt_name
+        if lamb:
+            hyper = dict(beta1=TRAIN.lamb_beta1, beta2=TRAIN.lamb_beta2, eps=TRAIN.lamb_eps, step=self.step_count)
+        else:
+            hyper = dict(momentum=self.momentum, first=self.step_count == 1, trust_coeff=TRAIN.lars_trust_coeff,
+                         trust_eps=TRAIN.lars_eps)
+        for L in plan.phase1[s]:
+            a, b = L.start, L.end
+            grad = dict(g16=g16[a - s:b - s]) if g16 is not None else dict(g32=self.g32[a:b])
+            ops.layerwise_step(1, kind, self.p32[a:b], self.m32[a:b], self.v32[a:b] if lamb else None,
+                               zero=self.g32[a:b] if (zero and lamb) else None, ws=self._lw_ws, lr=self.lr,
+                               grad_scale=grad_scale, segments=L.segments, **grad, **hyper)
+        for L in plan.phase2[s]:
+            a, b = L.start, L.end
+            # LARS reads the reduced gradient again (always fp32 in g32: see _reduce_and_update) and clears it
+            grad = {} if lamb else dict(g32=self.g32[a:b], zero=self.g32[a:b])
+            ops.layerwise_step(2, kind, self.p32[a:b], self.m32[a:b], self.v32[a:b] if lamb else None,
+                               shadow=self.w16[a:b], ws=self._lw_ws, ratio=self.trust_ratio, lr=self.lr,
+                               grad_scale=grad_scale, segments=L.segments, **grad, **hyper, **self._ema_kw(a, b))
 
     # ============================================================================== PowerSGD
     def _plan_tables(self) -> tuple:
@@ -538,7 +589,7 @@ class NativeEngine:
             st["powersgd"] = {"rank": self.powersgd_rank, "start_iter": self.powersgd_start_iter}
         # state for the trainable tensors only: torch keeps none for parameters without a gradient
         names = self.trainable_names()
-        if self.opt_name in ("adam", "adamw"):
+        if self.opt_name in ("adam", "adamw", "lamb"):
             st["exp_avg"] = {n: L.to_torch(self.spec, n, self._view(self.m32, n)).cpu() for n in names}
             st["exp_avg_sq"] = {n: L.to_torch(self.spec, n, self._view(self.v32, n)).cpu() for n in names}
         else:
@@ -1082,6 +1133,9 @@ class NativeEngine:
 
     def _apply_update(self, s: int, e: int, g16: Optional[torch.Tensor], zero: bool = True,
                       grad_scale: float = 1.0) -> None:
+        if getattr(self, "layerwise", False):
+            self._layerwise_update(s, e, g16, zero, grad_scale)
+            return
         ranges = self._update_ranges(s, e)
         if len(ranges) == 1:
             self._launch_update(s, e, g16, zero, grad_scale, ranges[0][2])
@@ -1164,8 +1218,10 @@ class NativeEngine:
                     self._comm_events.append((zev0, zev1, (e - s) * self.arena.wire.element_size()))
                 self._mark("z1_%d end" % bi, "comm")
                 return
+            # LARS reads a tensor's gradient again in its phase 2, after later buckets reduced: in g32, whatever
+            # algorithm each bucket took
             to_f32 = (algo == "oneshot" or self.unpack_fp32 or self.arena.wire_dtype == F32
-                      or not self.apply_updates)
+                      or not self.apply_updates or self.opt_name == "lars")
             self._mark("ar%d start" % bi, "comm")
             ev0 = None
             if self._comm_events is not None:    # observability: device time of every reduction

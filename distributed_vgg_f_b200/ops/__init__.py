@@ -259,6 +259,21 @@ def sgd_step(p, mom, *, g32=None, g16=None, shadow=None, lr, momentum=0.9, weigh
     require().sgd(*args, ema, float(ema_decay), bool(ema_first), *_wd_args(wd_segments))
 
 
+def layerwise_step(phase: int, kind: str, p, m, v=None, *, g32=None, g16=None, shadow=None, zero=None, ema=None,
+                   ema_decay: float = 0.0, ema_first: bool = False, ws, ratio=None, lr: float, beta1: float = 0.9,
+                   beta2: float = 0.999, eps: float = 1e-6, momentum: float = 0.0, step: int = 0, first: bool = False,
+                   grad_scale: float = 1.0, segments, trust_coeff: float = 1e-3, trust_eps: float = 1e-8):
+    """One launch of LAMB or LARS (``kind``), phase 1 or 2 (parallel/layerwise.py), over the flat range of ``p``.
+    ``segments``: the launch's parallel.layerwise.Segment rows.  Phase 1 writes each CTA's partial sums into ``ws``;
+    phase 2 reads them, writes each tensor's ratio into ``ratio`` (when given) and updates ``p`` (+ ``shadow``,
+    ``ema``).  ``zero``: the gradient range to clear (LAMB: phase 1, LARS: phase 2)."""
+    cols = [[s.start for s in segments], [s.ctas for s in segments], [s.slot for s in segments],
+            [s.nslots for s in segments], [s.tensor for s in segments], [float(s.wd) for s in segments]]
+    require().layerwise(int(phase), kind, p, m, v, g32, g16, shadow, zero, ema, ws, ratio, float(lr), float(beta1),
+                        float(beta2), float(eps), float(momentum), int(step), bool(first), float(grad_scale),
+                        float(ema_decay), bool(ema_first), *cols, float(trust_coeff), float(trust_eps))
+
+
 def ema_update(p, ema, *, decay: float, first: bool = False):
     """ema = decay * ema + (1 - decay) * p (fp32, each operation rounded, no FMA), or ema = p with ``first``:
     the EMA update of ``adam_step`` / ``sgd_step`` for weights no optimizer launch covers (frozen layers)."""

@@ -104,6 +104,22 @@ def powersgd_table(model: str, num_classes: int, rank: int, freeze_layers: int =
     return 0
 
 
+def layerwise_table(model: str, num_classes: int, optimizer: str, sms: int, freeze_layers: int = 0,
+                    powersgd_rank: int = 0, bucket_mb: float = 32.0) -> int:
+    """The phase-1 / phase-2 launches of --optimizer lamb|lars over the buckets (parallel/layerwise.py)."""
+    from ..parallel.layerwise import describe as lw_describe, engine_layerwise_plans
+    spec = get_spec(model, num_classes)
+    plans = engine_layerwise_plans(spec, sms, freeze_layers=freeze_layers, powersgd_rank=powersgd_rank,
+                                   bucket_mb=bucket_mb)
+    for compressed, lwp in plans.items():
+        print("%s, %d classes, %d SMs%s%s:" % (model, num_classes, sms,
+                                               ", %d layers frozen" % freeze_layers if freeze_layers else "",
+                                               ", updates PowerSGD compresses" if compressed else ""))
+        for line in lw_describe(lwp, optimizer):
+            print(line)
+    return 0
+
+
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--model", default="vggf")
@@ -121,6 +137,9 @@ def main(argv=None) -> int:
                     help="plan for the first N layers frozen (the training option of the same name)")
     ap.add_argument("--powersgd-rank", type=int, default=0,
                     help="print which tensors PowerSGD at this rank compresses and the bytes per update, instead")
+    ap.add_argument("--optimizer", default=None, choices=[None, "lamb", "lars"],
+                    help="print the phase-1 / phase-2 launches of LAMB or LARS over the buckets (with --sms, "
+                         "--freeze-layers and --powersgd-rank), instead")
     a = ap.parse_args(argv)
     try:
         get_spec(a.model, a.num_classes).check_freeze_layers(a.freeze_layers)
@@ -129,6 +148,9 @@ def main(argv=None) -> int:
             check_config(a.powersgd_rank, 2)
     except ValueError as e:
         ap.error(str(e))
+    if a.optimizer:
+        return layerwise_table(a.model, a.num_classes, a.optimizer, a.sms, a.freeze_layers, a.powersgd_rank,
+                               a.bucket_mb)
     if a.powersgd_rank:
         return powersgd_table(a.model, a.num_classes, a.powersgd_rank, a.freeze_layers)
     if a.deterministic:

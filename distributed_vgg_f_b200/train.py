@@ -90,6 +90,12 @@ def build_optimizer(model_or_params, args):
         return torch.optim.SGD(params, lr=args.learning_rate, momentum=args.momentum, weight_decay=wd)
     if args.optimizer == "adamw":
         return torch.optim.AdamW(params, lr=args.learning_rate, weight_decay=wd)
+    if args.optimizer in ("lamb", "lars"):
+        from .utils.optim import Lamb, Lars, check_layerwise_decay
+        check_layerwise_decay(args.optimizer, wd)
+        if args.optimizer == "lamb":
+            return Lamb(params, lr=args.learning_rate, weight_decay=wd)
+        return Lars(params, lr=args.learning_rate, momentum=args.momentum, weight_decay=wd)
     return torch.optim.Adam(params, lr=args.learning_rate, weight_decay=wd)     # distributedVggf.py:230
 
 
