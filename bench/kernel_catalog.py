@@ -19,6 +19,8 @@ ROLE = [   # (regex on the demangled name, role, what it replaces in the referen
     (r"conv0_kernel<true>|conv0_kernel<1>", "first conv wgrad (same shared-memory operand, MN-major)", "cuDNN wgrad — `:171`"),
     (r"umma_kernel<b200::GemmPolicy", "FC GEMMs: swap-AB split-K forward / dgrad, wgrad with epilogue → fp32 arena or `bf16(dW/ws)` straight into the symmetric wire", "cuBLAS SGEMM under `nn.Linear` — `:162`, `:171`"),
     (r"head_ce_kernel", "K-FUN2+CE: last Linear + log-softmax / NLL + metrics + dlogits + the layer's dW, db, dX in one launch", "cuBLAS + ATen log_softmax / nll_loss + `Accuracy2` / `Average` — `:56`, `:168`, `distributedUtil.py:95-96`"),
+    (r"head_ce_kd_kernel", "K-FUN2+CE with knowledge distillation: head_ce_kernel's launch, the teacher's logits read too; loss (1 − α) CE + α T² KL and its dlogits", "`F.cross_entropy` + `F.kl_div` of a distillation script — not in the reference"),
+    (r"cross_entropy_kd_kernel", "cross-entropy with knowledge distillation for heads that do not fuse (C > 8, B > 256, VGG-16)", "`F.cross_entropy` + `F.kl_div` of a distillation script — not in the reference"),
     (r"cross_entropy_kernel", "cross-entropy fwd + bwd + metrics for wide heads (VGG-16/1000)", "`F.cross_entropy` — `:168`"),
     (r"fc_bias_act_kernel", "FC epilogue: bias + ReLU + Philox dropout → bf16 (mask never stored)", "ATen bias/relu/dropout — `:52-57`"),
     (r"fc_grad_act_kernel", "FC backward epilogue: ReLU / dropout mask regenerated from the activation", "ATen threshold_backward / dropout backward"),

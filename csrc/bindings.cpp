@@ -360,6 +360,69 @@ static void cross_entropy_soft(const at::Tensor& logits, const at::Tensor& targe
                            f32p_opt(class_weights), st, cur_stream());
 }
 
+static void check_head_ce(const char* what, const at::Tensor& h, const at::Tensor& W, const at::Tensor& bias,
+                          const at::Tensor& target, const at::Tensor& logits, const c10::optional<at::Tensor>& dlogits,
+                          int64_t ldd, const c10::optional<at::Tensor>& dW, const c10::optional<at::Tensor>& db,
+                          const c10::optional<at::Tensor>& dh, double drop_scale, bool relu,
+                          const c10::optional<at::Tensor>& meter, const c10::optional<at::Tensor>& loss_out,
+                          const c10::optional<at::Tensor>& class_weights) {
+  TORCH_CHECK(h.dim() == 2 && W.dim() == 2 && h.size(1) == W.size(1) && h.is_contiguous() && W.is_contiguous(),
+              what, ": h [B][K], W [C][K], contiguous");
+  TORCH_CHECK(target.scalar_type() == at::kLong && logits.is_contiguous() && logits.size(0) == h.size(0) &&
+              logits.size(1) == W.size(0), what, ": int64 targets, logits [B][C]");
+  TORCH_CHECK(dW.has_value() == db.has_value(), what, ": dW and db come together");
+  // dh keeps only the elements with h > 0: that is the dropout mask only after a ReLU
+  TORCH_CHECK(relu || drop_scale == 1.0, what, ": dropout without ReLU is not supported");
+  const int64_t B = h.size(0), C = W.size(0), K = h.size(1);
+  TORCH_CHECK(target.is_contiguous() && target.numel() >= B, what, ": contiguous targets of B = ", B);
+  TORCH_CHECK(bias.numel() >= C, what, ": bias must have C = ", C, " elements");
+  if (dlogits.has_value())
+    TORCH_CHECK(ldd >= C && dlogits->is_contiguous() && dlogits->numel() >= B * ldd,
+                what, ": dlogits must be contiguous, ldd >= C and at least B x ldd elements");
+  TORCH_CHECK(!dW.has_value() || (dW->is_contiguous() && dW->numel() >= C * K), what, ": contiguous dW of C x K");
+  TORCH_CHECK(!db.has_value() || db->numel() >= C, what, ": db must have C elements");
+  TORCH_CHECK(!dh.has_value() || (dh->is_contiguous() && dh->numel() >= B * K), what, ": contiguous dh of B x K");
+  TORCH_CHECK(!meter.has_value() || meter->numel() >= 3, what, ": meter must have 3 elements");
+  TORCH_CHECK(!loss_out.has_value() || loss_out->numel() >= 1, what, ": loss_out must have 1 element");
+  TORCH_CHECK(!class_weights.has_value() || class_weights->numel() >= C, what, ": class_weights of C = ", C);
+}
+
+// Distillation operands: teacher logits fp32 [B][C], contiguous, on the logits' device; 0 < alpha <= 1; T finite > 0.
+static b200::KdParams check_kd(const char* what, const at::Tensor& teacher, const at::Device& dev, int64_t B, int64_t C,
+                               double alpha, double temperature) {
+  TORCH_CHECK(teacher.device() == dev, what, ": teacher logits must be on ", dev, ", got ", teacher.device());
+  TORCH_CHECK(teacher.scalar_type() == at::kFloat && teacher.is_contiguous() && teacher.dim() == 2 &&
+              teacher.size(0) == B && teacher.size(1) == C,
+              what, ": teacher logits must be contiguous fp32 [", B, "][", C, "], got ", teacher.scalar_type(), " ",
+              teacher.sizes());
+  TORCH_CHECK(alpha > 0.0 && alpha <= 1.0, what, ": alpha must lie in (0, 1], got ", alpha);
+  TORCH_CHECK(std::isfinite(temperature) && temperature > 0.0, what, ": temperature must be finite and > 0, got ",
+              temperature);
+  return b200::kd_params(alpha, temperature, (int)B);
+}
+
+static b200::SoftTargets soft_list(const char* what, const c10::optional<std::vector<double>>& soft) {
+  TORCH_CHECK(!soft.has_value() || soft->size() == 3, what, ": soft is (eps, lam, mix)");
+  return soft.has_value() ? soft_targets(what, (*soft)[0], (*soft)[1], (*soft)[2] != 0.0) : b200::SoftTargets{};
+}
+
+// cross_entropy / cross_entropy_soft with the distillation loss; soft = (eps, lam, mix) or None (integer labels)
+static void cross_entropy_kd(const at::Tensor& logits, const at::Tensor& target, c10::optional<at::Tensor> dlogits,
+                             int64_t ldd, c10::optional<at::Tensor> meter, c10::optional<at::Tensor> loss_out,
+                             double grad_scale, c10::optional<at::Tensor> class_weights, const at::Tensor& teacher,
+                             double alpha, double temperature, c10::optional<std::vector<double>> soft) {
+  c10::cuda::CUDAGuard g(logits.device());
+  check_cross_entropy(logits, target, dlogits, ldd, meter, loss_out, class_weights);
+  TORCH_CHECK(logits.scalar_type() == at::kFloat, "cross_entropy_kd: fp32 logits");
+  const b200::KdParams kd = check_kd("cross_entropy_kd", teacher, logits.device(), logits.size(0), logits.size(1),
+                                     alpha, temperature);
+  const b200::SoftTargets st = soft_list("cross_entropy_kd", soft);
+  b200::cross_entropy_kd(f32p(logits), reinterpret_cast<const long long*>(target.data_ptr()),
+                         dlogits.has_value() ? bfp_mut(*dlogits) : nullptr, (int)ldd, f32p_opt(meter),
+                         f32p_opt(loss_out), (int)logits.size(0), (int)logits.size(1), (float)grad_scale,
+                         f32p_opt(class_weights), soft.has_value() ? &st : nullptr, f32p(teacher), kd, cur_stream());
+}
+
 // The optimizers' optional moving average of the weights: fp32, 16-byte aligned, p's size, decay in [0, 1].
 static void check_ema(const c10::optional<at::Tensor>& ema, int64_t n, double decay, const char* op) {
   if (!ema.has_value()) return;
@@ -977,6 +1040,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("cast_to_f32", &cast_to_f32);
   m.def("cross_entropy", &cross_entropy);
   m.def("cross_entropy_soft", &cross_entropy_soft);
+  m.def("cross_entropy_kd", &cross_entropy_kd, py::arg("logits"), py::arg("target"), py::arg("dlogits"), py::arg("ldd"),
+        py::arg("meter"), py::arg("loss_out"), py::arg("grad_scale"), py::arg("class_weights"), py::arg("teacher"),
+        py::arg("alpha"), py::arg("temperature"), py::arg("soft") = py::none());
   m.def("head_ce_supported", [](int64_t B, int64_t C, int64_t K) { return b200::head_ce_supported((int)B, (int)C, (int)K); });
   m.def("head_ce", [](const at::Tensor& h, const at::Tensor& W, const at::Tensor& bias, const at::Tensor& target,
                       at::Tensor logits, c10::optional<at::Tensor> dlogits, int64_t ldd, c10::optional<at::Tensor> dW,
@@ -985,25 +1051,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                       c10::optional<at::Tensor> class_weights, bool accumulate,
                       c10::optional<std::vector<double>> soft) {
     c10::cuda::CUDAGuard g(h.device());
-    TORCH_CHECK(h.dim() == 2 && W.dim() == 2 && h.size(1) == W.size(1) && h.is_contiguous() && W.is_contiguous(),
-                "head_ce: h [B][K], W [C][K], contiguous");
-    TORCH_CHECK(target.scalar_type() == at::kLong && logits.is_contiguous() && logits.size(0) == h.size(0) &&
-                logits.size(1) == W.size(0), "head_ce: int64 targets, logits [B][C]");
-    TORCH_CHECK(dW.has_value() == db.has_value(), "head_ce: dW and db come together");
-    // dh keeps only the elements with h > 0: that is the dropout mask only after a ReLU
-    TORCH_CHECK(relu || drop_scale == 1.0, "head_ce: dropout without ReLU is not supported");
-    const int64_t B = h.size(0), C = W.size(0), K = h.size(1);
-    TORCH_CHECK(target.is_contiguous() && target.numel() >= B, "head_ce: contiguous targets of B = ", B);
-    TORCH_CHECK(bias.numel() >= C, "head_ce: bias must have C = ", C, " elements");
-    if (dlogits.has_value())
-      TORCH_CHECK(ldd >= C && dlogits->is_contiguous() && dlogits->numel() >= B * ldd,
-                  "head_ce: dlogits must be contiguous, ldd >= C and at least B x ldd elements");
-    TORCH_CHECK(!dW.has_value() || (dW->is_contiguous() && dW->numel() >= C * K), "head_ce: contiguous dW of C x K");
-    TORCH_CHECK(!db.has_value() || db->numel() >= C, "head_ce: db must have C elements");
-    TORCH_CHECK(!dh.has_value() || (dh->is_contiguous() && dh->numel() >= B * K), "head_ce: contiguous dh of B x K");
-    TORCH_CHECK(!meter.has_value() || meter->numel() >= 3, "head_ce: meter must have 3 elements");
-    TORCH_CHECK(!loss_out.has_value() || loss_out->numel() >= 1, "head_ce: loss_out must have 1 element");
-    TORCH_CHECK(!class_weights.has_value() || class_weights->numel() >= C, "head_ce: class_weights of C = ", C);
+    check_head_ce("head_ce", h, W, bias, target, logits, dlogits, ldd, dW, db, dh, drop_scale, relu, meter, loss_out,
+                  class_weights);
     TORCH_CHECK(!soft.has_value() || soft->size() == 3, "head_ce: soft is (eps, lam, mix)");
     b200::SoftTargets st{};
     if (soft.has_value()) st = soft_targets("head_ce", (*soft)[0], (*soft)[1], (*soft)[2] != 0.0);
@@ -1019,6 +1068,30 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   py::arg("loss_out"), py::arg("class_weights"), py::arg("accumulate") = false,
   // soft = (eps, lam, mix): label smoothing and MixUp / CutMix targets (cross_entropy_soft); None: integer labels
   py::arg("soft") = py::none());
+  // head_ce with the distillation loss against teacher logits [B][C] fp32 (see cross_entropy_kd)
+  m.def("head_ce_kd", [](const at::Tensor& h, const at::Tensor& W, const at::Tensor& bias, const at::Tensor& target,
+                         at::Tensor logits, c10::optional<at::Tensor> dlogits, int64_t ldd, c10::optional<at::Tensor> dW,
+                         c10::optional<at::Tensor> db, c10::optional<at::Tensor> dh, double drop_scale, bool relu,
+                         c10::optional<at::Tensor> meter, c10::optional<at::Tensor> loss_out,
+                         c10::optional<at::Tensor> class_weights, bool accumulate,
+                         c10::optional<std::vector<double>> soft, const at::Tensor& teacher, double alpha,
+                         double temperature) {
+    c10::cuda::CUDAGuard g(h.device());
+    check_head_ce("head_ce_kd", h, W, bias, target, logits, dlogits, ldd, dW, db, dh, drop_scale, relu, meter, loss_out,
+                  class_weights);
+    const b200::KdParams kd = check_kd("head_ce_kd", teacher, h.device(), h.size(0), W.size(0), alpha, temperature);
+    const b200::SoftTargets st = soft_list("head_ce_kd", soft);
+    b200::head_ce_kd_fused(bfp(h), bfp(W), f32p(bias), reinterpret_cast<const long long*>(target.data_ptr()),
+                           f32p(logits), dlogits.has_value() ? bfp_mut(*dlogits) : nullptr, (int)ldd, f32p_opt(dW),
+                           f32p_opt(db), dh.has_value() ? bfp_mut(*dh) : nullptr, (float)drop_scale, relu,
+                           f32p_opt(meter), f32p_opt(loss_out), (int)h.size(0), (int)W.size(0), (int)h.size(1),
+                           f32p_opt(class_weights), accumulate, soft.has_value() ? &st : nullptr, f32p(teacher), kd,
+                           cur_stream());
+  },
+  py::arg("h"), py::arg("W"), py::arg("bias"), py::arg("target"), py::arg("logits"), py::arg("dlogits"), py::arg("ldd"),
+  py::arg("dW"), py::arg("db"), py::arg("dh"), py::arg("drop_scale"), py::arg("relu"), py::arg("meter"),
+  py::arg("loss_out"), py::arg("class_weights"), py::arg("accumulate"), py::arg("soft"), py::arg("teacher"),
+  py::arg("alpha"), py::arg("temperature"));
   m.def("adam", &adam, py::arg("p"), py::arg("m"), py::arg("v"), py::arg("g32"), py::arg("g16"), py::arg("shadow"),
         py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"), py::arg("wd"), py::arg("step"),
         py::arg("grad_scale"), py::arg("gzero"), py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0,

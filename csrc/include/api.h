@@ -164,6 +164,19 @@ void cross_entropy_soft(const float* logits, const long long* target, bf16* dlog
                         float* loss_out, int B, int C, float grad_scale, const float* class_weights,
                         const SoftTargets& st, cudaStream_t s);
 
+// Knowledge distillation against teacher logits u [B][C] fp32, weight alpha and temperature T:
+//   L = (1 - alpha) CE + alpha T^2 / B sum_r KL(softmax(u_r / T) || softmax(z_r / T))
+//   dL/dz[r][c] = (1 - alpha) (the cross-entropy gradient) + alpha T / B (softmax(z_r / T)_c - softmax(u_r / T)_c)
+// CE is the loss of cross_entropy_fused / cross_entropy_soft (class weights and soft targets apply to it alone);
+// meter / loss_out receive L.  kd_params(alpha, T, B) = {1 - alpha, alpha T / B, alpha T^2, 1 / T}.
+struct KdParams {
+  float ce, g, l, inv_t;
+};
+KdParams kd_params(double alpha, double temperature, int B);
+void cross_entropy_kd(const float* logits, const long long* target, bf16* dlogits, int ldd, float* meter,
+                      float* loss_out, int B, int C, float grad_scale, const float* class_weights,
+                      const SoftTargets* soft, const float* teacher, const KdParams& kd, cudaStream_t s);
+
 // K-FUN2+CE: last Linear(K -> C) + cross-entropy + metrics + the layer's whole backward in one launch
 // (C <= 8, K <= 1024, B <= 256).  h [B][K] bf16 (the previous FC layer's output), W [C][K] bf16.
 // Writes logits [B][C] fp32, meter / loss_out as cross_entropy_fused, optional dlogits (bf16, ld ldd);
@@ -174,6 +187,12 @@ void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long l
                    bf16* dlogits, int ldd, float* dW, float* db, bf16* dh, float drop_scale, bool relu, float* meter,
                    float* loss_out, int B, int C, int K, const float* class_weights, bool accumulate,
                    cudaStream_t s, const SoftTargets* soft = nullptr);
+// head_ce_fused with the distillation loss (see cross_entropy_kd): the dlogits it rounds to bf16 and feeds to the
+// layer's backward are those of L.
+void head_ce_kd_fused(const bf16* h, const bf16* W, const float* bias, const long long* target, float* logits,
+                      bf16* dlogits, int ldd, float* dW, float* db, bf16* dh, float drop_scale, bool relu, float* meter,
+                      float* loss_out, int B, int C, int K, const float* class_weights, bool accumulate,
+                      const SoftTargets* soft, const float* teacher, const KdParams& kd, cudaStream_t s);
 
 // Weight decay of one optimizer launch, per segment of its range: segment k covers the float4s
 // [start4[k], start4[k + 1]) (the last one runs to the end of the range) and takes value[k].  start4[0]

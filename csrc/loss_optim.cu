@@ -37,6 +37,30 @@ __device__ __forceinline__ void soft_row(const long long* __restrict__ target, i
   tmax = (tb != t && (lb > la || (lb == la && tb < t))) ? tb : t;
 }
 
+// Knowledge distillation (KdParams in api.h): for student logits z and teacher logits u of a row,
+// log ps = log_softmax(z / T), log pt = log_softmax(u / T); the row's KL term is sum_c pt_c (log pt_c - log ps_c)
+// and its gradient contribution kd.g (ps_c - pt_c).  Both log-softmaxes are taken from the row maxima.
+__device__ __forceinline__ void kd_logs(float z, float mz, float ls, float u, float mu, float lt, float inv_t,
+                                        float& lps, float& lpt) {
+  lps = (z - mz) * inv_t - ls;
+  lpt = (u - mu) * inv_t - lt;
+}
+
+// dlogit of class c: kd.ce * (the cross-entropy gradient g) + kd.g * (ps_c - pt_c).
+__device__ __forceinline__ float kd_grad(float g, float z, float mz, float ls, float u, float mu, float lt,
+                                         const KdParams& kd) {
+  float lps, lpt;
+  kd_logs(z, mz, ls, u, mu, lt, kd.inv_t, lps, lpt);
+  return fmaf(kd.g, __expf(lps) - __expf(lpt), kd.ce * g);
+}
+
+// The batch's loss: kd.ce * (cross-entropy mean) + kd.l * (sum of the warps' KL terms) / B.
+__device__ __forceinline__ float kd_loss(float ce_mean, const float* s_kl, int nwarps, int B, const KdParams& kd) {
+  float kl = 0.f;
+  for (int i = 0; i < nwarps; ++i) kl += s_kl[i];
+  return fmaf(kd.l, kl / static_cast<float>(B), kd.ce * ce_mean);
+}
+
 // One block, one warp per row (round-robin).  C is small (3) or moderate (1000).
 // SOFT: label smoothing and / or mixed targets (cross_entropy_soft); !SOFT is the integer-label loss.
 template <bool SOFT>
@@ -142,6 +166,145 @@ __global__ void cross_entropy_kernel(const float* __restrict__ logits, const lon
   }
 }
 
+// cross_entropy_kernel with the distillation loss (cross_entropy_kd): L = kd.ce * CE + kd.l * KL / B against the
+// teacher logits `tlog` [B][C], dlogits kd.ce * (the cross-entropy gradient) + kd.g * (ps - pt).  A kernel of its own
+// rather than a template parameter of cross_entropy_kernel, whose instantiations keep their code.
+template <bool SOFT>
+__global__ void __launch_bounds__(1024)
+cross_entropy_kd_kernel(const float* __restrict__ logits, const long long* __restrict__ target,
+                        bf16* __restrict__ dlogits, int ldd, float* __restrict__ meter,
+                        float* __restrict__ loss_out, int B, int C, float grad_scale,
+                        const float* __restrict__ cw, SoftTargets st,
+                        const float* __restrict__ tlog, KdParams kd) {
+  __shared__ float s_loss[32], s_correct[32], s_wsum[32];
+  float* s_kl = s_wsum;          // the warps' KL terms (s_wsum is free once pass 0 is over)
+  __shared__ float s_total_w;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+
+  // pass 0 (only with class weights): normaliser = sum_i w[target_i]
+  float wsum_local = 0.f;
+  if (cw) {
+    for (int r = threadIdx.x; r < B; r += blockDim.x) wsum_local += cw[target[r]];
+    for (int o = 16; o; o >>= 1) wsum_local += __shfl_xor_sync(0xffffffffu, wsum_local, o);
+    if (lane == 0) s_wsum[warp] = wsum_local;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float t = 0.f;
+      for (int i = 0; i < nwarps; ++i) t += s_wsum[i];
+      s_total_w = t;
+    }
+    __syncthreads();
+  }
+  // probability targets (mixed batches) are divided by B even with class weights, as torch does
+  const bool by_weight = cw && !(SOFT && st.mix);
+  const float norm = by_weight ? 1.f / s_total_w : grad_scale;   // grad_scale == 1/B for the mean
+  const float keep = 1.f - st.eps, eps_c = st.eps / static_cast<float>(C);
+
+  float loss_acc = 0.f, correct_acc = 0.f, kl_acc = 0.f;
+  for (int r = warp; r < B; r += nwarps) {
+    const float* row = logits + static_cast<long long>(r) * C;
+    int t = static_cast<int>(target[r]), tb = t, tmax = t;
+    float la = 1.f, lb = 0.f;
+    if constexpr (SOFT) soft_row(target, r, B, st, t, tb, la, lb, tmax);
+    float mx = -INFINITY;
+    int amax = 0x7fffffff;
+    for (int c = lane; c < C; c += 32) {
+      const float v = row[c];
+      if (v > mx) { mx = v; amax = c; }
+    }
+    for (int o = 16; o; o >>= 1) {
+      const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+      const int oa = __shfl_xor_sync(0xffffffffu, amax, o);
+      if (om > mx || (om == mx && oa < amax)) { mx = om; amax = oa; }
+    }
+    float se = 0.f;
+    for (int c = lane; c < C; c += 32) se += __expf(row[c] - mx);
+    for (int o = 16; o; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+    const float lse = mx + __logf(se);
+    // teacher row maximum, both log-normalisers at temperature T, and the row's KL term
+    float mu = -INFINITY, ls = 0.f, lt = 0.f;
+    {
+      const float* trow = tlog + static_cast<long long>(r) * C;
+      for (int c = lane; c < C; c += 32) mu = fmaxf(mu, trow[c]);
+      for (int o = 16; o; o >>= 1) mu = fmaxf(mu, __shfl_xor_sync(0xffffffffu, mu, o));
+      float ss = 0.f, su = 0.f;
+      for (int c = lane; c < C; c += 32) {
+        ss += __expf((row[c] - mx) * kd.inv_t);
+        su += __expf((trow[c] - mu) * kd.inv_t);
+      }
+      for (int o = 16; o; o >>= 1) {
+        ss += __shfl_xor_sync(0xffffffffu, ss, o);
+        su += __shfl_xor_sync(0xffffffffu, su, o);
+      }
+      ls = __logf(ss);
+      lt = __logf(su);
+      float kl = 0.f;
+      for (int c = lane; c < C; c += 32) {
+        float lps, lpt;
+        kd_logs(row[c], mx, ls, trow[c], mu, lt, kd.inv_t, lps, lpt);
+        kl += __expf(lpt) * (lpt - lps);
+      }
+      for (int o = 16; o; o >>= 1) kl += __shfl_xor_sync(0xffffffffu, kl, o);
+      if (lane == 0) kl_acc += kl;
+    }
+    if constexpr (SOFT) {
+      float qs = 0.f, ql = 0.f;          // sum_c q_c and the row's loss sum_c q_c (lse - z_c)
+      for (int c = lane; c < C; c += 32) {
+        const float q = soft_q(c, t, tb, la, lb, keep, eps_c, cw);
+        qs += q;
+        ql += q * (lse - row[c]);
+      }
+      for (int o = 16; o; o >>= 1) {
+        qs += __shfl_xor_sync(0xffffffffu, qs, o);
+        ql += __shfl_xor_sync(0xffffffffu, ql, o);
+      }
+      if (dlogits) {
+        for (int c = lane; c < ldd; c += 32) {
+          float g = 0.f;
+          if (c < C) g = (__expf(row[c] - lse) * qs - soft_q(c, t, tb, la, lb, keep, eps_c, cw)) * norm;
+          if (c < C) g = kd_grad(g, row[c], mx, ls, tlog[static_cast<long long>(r) * C + c], mu, lt, kd);
+          dlogits[static_cast<long long>(r) * ldd + c] = __float2bfloat16(g);
+        }
+      }
+      if (lane == 0) {
+        loss_acc += ql;
+        correct_acc += (amax == tmax) ? 1.f : 0.f;
+      }
+    } else {
+      const float w = cw ? cw[t] : 1.f;
+      if (dlogits) {
+        for (int c = lane; c < ldd; c += 32) {
+          float g = 0.f;
+          if (c < C) g = (__expf(row[c] - lse) - (c == t ? 1.f : 0.f)) * w * norm;
+          if (c < C) g = kd_grad(g, row[c], mx, ls, tlog[static_cast<long long>(r) * C + c], mu, lt, kd);
+          dlogits[static_cast<long long>(r) * ldd + c] = __float2bfloat16(g);
+        }
+      }
+      if (lane == 0) {
+        loss_acc += w * (lse - row[t]);
+        correct_acc += (amax == t) ? 1.f : 0.f;
+      }
+    }
+  }
+  if (lane == 0) { s_loss[warp] = loss_acc; s_correct[warp] = correct_acc; }
+  if (lane == 0) s_kl[warp] = kl_acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float tl = 0.f, tc = 0.f;
+    for (int i = 0; i < nwarps; ++i) { tl += s_loss[i]; tc += s_correct[i]; }
+    // batch loss as torch reports it: mean over the batch, or sum_i w_i nll_i / sum_i w_i with
+    // class weights; the meter accumulates loss * B like Average.update(loss.item(), B)
+    const float ce = by_weight ? tl / s_total_w : tl / static_cast<float>(B);
+    const float mean = kd_loss(ce, s_kl, nwarps, B, kd);
+    if (meter) {
+      atomicAdd(meter + 0, mean * static_cast<float>(B));
+      atomicAdd(meter + 1, tc);
+      atomicAdd(meter + 2, static_cast<float>(B));
+    }
+    if (loss_out) *loss_out = mean;
+  }
+}
+
 void cross_entropy_fused(const float* logits, const long long* target, bf16* dlogits, int ldd,
                          float* meter, float* loss_out, int B, int C, float grad_scale,
                          const float* class_weights, cudaStream_t s) {
@@ -160,6 +323,25 @@ void cross_entropy_soft(const float* logits, const long long* target, bf16* dlog
   check_last("cross_entropy_soft");
 }
 
+void cross_entropy_kd(const float* logits, const long long* target, bf16* dlogits, int ldd, float* meter,
+                      float* loss_out, int B, int C, float grad_scale, const float* class_weights,
+                      const SoftTargets* soft, const float* teacher, const KdParams& kd, cudaStream_t s) {
+  if (soft)
+    cross_entropy_kd_kernel<true><<<1, 1024, 0, s>>>(logits, target, dlogits, ldd, meter, loss_out, B, C, grad_scale,
+                                                     class_weights, *soft, teacher, kd);
+  else
+    cross_entropy_kd_kernel<false><<<1, 1024, 0, s>>>(logits, target, dlogits, ldd, meter, loss_out, B, C,
+                                                      grad_scale, class_weights, SoftTargets{0.f, 1.f, 0.f, 0},
+                                                      teacher, kd);
+  count_launch();
+  check_last("cross_entropy_kd");
+}
+
+KdParams kd_params(double alpha, double temperature, int B) {
+  return KdParams{static_cast<float>(1.0 - alpha), static_cast<float>(alpha * temperature / B),
+                  static_cast<float>(alpha * temperature * temperature), static_cast<float>(1.0 / temperature)};
+}
+
 // ------------------------------------------------------------- fused head: last Linear + CE + bwd
 // K-FUN2+CE (SURVEY 2.5): the funnel's Linear(512, C) (distributedVggf.py:56), cross_entropy (:168),
 // Accuracy2 / Average (distributedUtil.py:95-96, :55-58) and the whole backward of that layer in ONE
@@ -173,18 +355,22 @@ void cross_entropy_soft(const float* logits, const long long* target, bf16* dlog
 // Rounding points are those of the unfused path: dlogits are rounded to bf16 before they are used.
 constexpr int HEAD_MAXC = 8, HEAD_MAXK = 1024, HEAD_MAXB = 256, HEAD_THREADS = 512;
 
-// SOFT: soft targets as in cross_entropy_kernel<true>; the backward of the layer is unchanged.
-template <bool SOFT>
-__global__ void __launch_bounds__(HEAD_THREADS, 1)
-head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const float* __restrict__ bias,
-               const long long* __restrict__ target, float* __restrict__ logits, bf16* __restrict__ dlogits, int ldd,
-               float* __restrict__ dW, float* __restrict__ db, bf16* __restrict__ dh, float drop_scale, int relu,
-               float* __restrict__ meter, float* __restrict__ loss_out, int B, int C, int K,
-               const float* __restrict__ cw, int accumulate, SoftTargets st) {
+// SOFT: soft targets as in cross_entropy_kernel<true>; KD: the distillation loss of cross_entropy_kd_kernel, teacher
+// logits `tlog` [B][C].  The backward of the layer is unchanged: it takes whichever dlogits the loss made.
+template <bool SOFT, bool KD>
+__device__ __forceinline__ void head_ce_body(const bf16* __restrict__ h, const bf16* __restrict__ W,
+                                             const float* __restrict__ bias, const long long* __restrict__ target,
+                                             float* __restrict__ logits, bf16* __restrict__ dlogits, int ldd,
+                                             float* __restrict__ dW, float* __restrict__ db, bf16* __restrict__ dh,
+                                             float drop_scale, int relu, float* __restrict__ meter,
+                                             float* __restrict__ loss_out, int B, int C, int K,
+                                             const float* __restrict__ cw, int accumulate, const SoftTargets& st,
+                                             const float* __restrict__ tlog, const KdParams& kd) {
   __shared__ float sW[HEAD_MAXC * HEAD_MAXK];
   __shared__ float sdl[HEAD_MAXB * HEAD_MAXC];
   __shared__ float s_loss[32], s_correct[32], s_wsum[32];
   __shared__ float s_total_w;
+  float* s_kl = s_wsum;          // KD: the warps' KL terms (s_wsum is free once the normaliser is summed)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
   for (int i = threadIdx.x; i < C * K; i += blockDim.x) sW[i] = __bfloat162float(W[i]);
 
@@ -206,7 +392,7 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
   const float keep = 1.f - st.eps, eps_c = st.eps / static_cast<float>(C);
 
   // ---- forward + loss + dlogits ---------------------------------------------------------------
-  float loss_acc = 0.f, correct_acc = 0.f;
+  float loss_acc = 0.f, correct_acc = 0.f, kl_acc = 0.f;
   for (int r = warp; r < B; r += nwarps) {
     float acc[HEAD_MAXC];
 #pragma unroll
@@ -240,6 +426,33 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
         if (c == t) zt = acc[c];
       }
     const float lse = mx + __logf(se);
+    // KD: the teacher row, its maximum, both log-normalisers at temperature T and the row's KL term
+    float u[HEAD_MAXC], mu = -INFINITY, ls = 0.f, lt = 0.f;
+    if constexpr (KD) {
+      float ss = 0.f, su = 0.f, kl = 0.f;
+#pragma unroll
+      for (int c = 0; c < HEAD_MAXC; ++c)
+        if (c < C) {
+          u[c] = tlog[static_cast<long long>(r) * C + c];
+          mu = fmaxf(mu, u[c]);
+        }
+#pragma unroll
+      for (int c = 0; c < HEAD_MAXC; ++c)
+        if (c < C) {
+          ss += __expf((acc[c] - mx) * kd.inv_t);
+          su += __expf((u[c] - mu) * kd.inv_t);
+        }
+      ls = __logf(ss);
+      lt = __logf(su);
+#pragma unroll
+      for (int c = 0; c < HEAD_MAXC; ++c)
+        if (c < C) {
+          float lps, lpt;
+          kd_logs(acc[c], mx, ls, u[c], mu, lt, kd.inv_t, lps, lpt);
+          kl += __expf(lpt) * (lpt - lps);
+        }
+      if (lane == 0) kl_acc += kl;
+    }
     float w = cw ? cw[t] : 1.f;
     float qs = 0.f, ql = 0.f;        // SOFT: sum_c q_c and the row's loss sum_c q_c (lse - z_c)
     if constexpr (SOFT) {
@@ -262,6 +475,7 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
             g = (__expf(acc[c] - lse) * qs - soft_q(c, t, tb, la, lb, keep, eps_c, cw)) * norm;
           else
             g = (__expf(acc[c] - lse) - (c == t ? 1.f : 0.f)) * w * norm;
+          if constexpr (KD) g = kd_grad(g, acc[c], mx, ls, u[c], mu, lt, kd);
         }
       if (lane < C) {
         logits[static_cast<long long>(r) * C + lane] = z;
@@ -280,11 +494,14 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
     }
   }
   if (lane == 0) { s_loss[warp] = loss_acc; s_correct[warp] = correct_acc; }
+  if constexpr (KD)
+    if (lane == 0) s_kl[warp] = kl_acc;
   __syncthreads();
   if (threadIdx.x == 0) {
     float tl = 0.f, tc = 0.f;
     for (int i = 0; i < nwarps; ++i) { tl += s_loss[i]; tc += s_correct[i]; }
-    const float mean = by_weight ? tl / s_total_w : tl / static_cast<float>(B);
+    float mean = by_weight ? tl / s_total_w : tl / static_cast<float>(B);
+    if constexpr (KD) mean = kd_loss(mean, s_kl, nwarps, B, kd);
     if (meter) {
       atomicAdd(meter + 0, mean * static_cast<float>(B));
       atomicAdd(meter + 1, tc);
@@ -326,6 +543,29 @@ head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const flo
   }
 }
 
+template <bool SOFT>
+__global__ void __launch_bounds__(HEAD_THREADS, 1)
+head_ce_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const float* __restrict__ bias,
+               const long long* __restrict__ target, float* __restrict__ logits, bf16* __restrict__ dlogits, int ldd,
+               float* __restrict__ dW, float* __restrict__ db, bf16* __restrict__ dh, float drop_scale, int relu,
+               float* __restrict__ meter, float* __restrict__ loss_out, int B, int C, int K,
+               const float* __restrict__ cw, int accumulate, SoftTargets st) {
+  head_ce_body<SOFT, false>(h, W, bias, target, logits, dlogits, ldd, dW, db, dh, drop_scale, relu, meter, loss_out, B,
+                            C, K, cw, accumulate, st, nullptr, KdParams{});
+}
+
+template <bool SOFT>
+__global__ void __launch_bounds__(HEAD_THREADS, 1)
+head_ce_kd_kernel(const bf16* __restrict__ h, const bf16* __restrict__ W, const float* __restrict__ bias,
+                  const long long* __restrict__ target, float* __restrict__ logits, bf16* __restrict__ dlogits,
+                  int ldd, float* __restrict__ dW, float* __restrict__ db, bf16* __restrict__ dh, float drop_scale,
+                  int relu, float* __restrict__ meter, float* __restrict__ loss_out, int B, int C, int K,
+                  const float* __restrict__ cw, int accumulate, SoftTargets st, const float* __restrict__ teacher,
+                  KdParams kd) {
+  head_ce_body<SOFT, true>(h, W, bias, target, logits, dlogits, ldd, dW, db, dh, drop_scale, relu, meter, loss_out, B,
+                           C, K, cw, accumulate, st, teacher, kd);
+}
+
 bool head_ce_supported(int B, int C, int K) { return C <= HEAD_MAXC && K <= HEAD_MAXK && B <= HEAD_MAXB && B > 0; }
 
 void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long long* target, float* logits,
@@ -344,6 +584,25 @@ void head_ce_fused(const bf16* h, const bf16* W, const float* bias, const long l
                                                      accumulate ? 1 : 0, SoftTargets{0.f, 1.f, 0.f, 0});
   count_launch();
   check_last("head_ce_fused");
+}
+
+void head_ce_kd_fused(const bf16* h, const bf16* W, const float* bias, const long long* target, float* logits,
+                      bf16* dlogits, int ldd, float* dW, float* db, bf16* dh, float drop_scale, bool relu, float* meter,
+                      float* loss_out, int B, int C, int K, const float* class_weights, bool accumulate,
+                      const SoftTargets* soft, const float* teacher, const KdParams& kd, cudaStream_t s) {
+  if (!head_ce_supported(B, C, K)) throw std::runtime_error("[b200] head_ce_kd_fused: needs C <= 8, K <= 1024, B <= 256");
+  if (ldd > 32) throw std::runtime_error("[b200] head_ce_kd_fused: dlogits row stride must be <= 32");
+  if (soft)
+    head_ce_kd_kernel<true><<<1, HEAD_THREADS, 0, s>>>(h, W, bias, target, logits, dlogits, ldd, dW, db, dh, drop_scale,
+                                                       relu ? 1 : 0, meter, loss_out, B, C, K, class_weights,
+                                                       accumulate ? 1 : 0, *soft, teacher, kd);
+  else
+    head_ce_kd_kernel<false><<<1, HEAD_THREADS, 0, s>>>(h, W, bias, target, logits, dlogits, ldd, dW, db, dh,
+                                                        drop_scale, relu ? 1 : 0, meter, loss_out, B, C, K,
+                                                        class_weights, accumulate ? 1 : 0,
+                                                        SoftTargets{0.f, 1.f, 0.f, 0}, teacher, kd);
+  count_launch();
+  check_last("head_ce_kd_fused");
 }
 
 // ---------------------------------------------------------------------------------- optimizers

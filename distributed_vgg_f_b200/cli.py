@@ -17,6 +17,7 @@ Under ``torchrun`` the three required flags may be omitted: they default from
 from __future__ import annotations
 
 import argparse
+import math
 import os
 import sys
 from typing import Optional, Sequence
@@ -25,6 +26,7 @@ from .config import DATA, TRAIN
 
 # Below 32 the fifth 2x2 pool of VGG leaves an empty feature map.
 MIN_CROP = 32
+MODELS = ["vggf", "vgg16", "vgg11", "vgg13", "vgg19", "vggf11", "vggf13", "vggf19", "vggf-tiny", "vggf-mini"]
 
 
 def build_parser() -> argparse.ArgumentParser:
@@ -62,9 +64,7 @@ def build_parser() -> argparse.ArgumentParser:
                         help="Mini-batch size. The default value is {}".format(TRAIN.mini_batch))
 
     ext = parser.add_argument_group("extensions (not in the reference)")
-    ext.add_argument("--model", default="vggf",
-                     choices=["vggf", "vgg16", "vgg11", "vgg13", "vgg19", "vggf11", "vggf13", "vggf19",
-                              "vggf-tiny", "vggf-mini"],
+    ext.add_argument("--model", default="vggf", choices=MODELS,
                      help="vggf = the reference's network (VGG-16 + funnel head); vggNN = torchvision's plain "
                           "VGG-NN; vggfNN = VGG-NN + funnel head; -tiny / -mini are test-sized")
     ext.add_argument("--num-classes", type=int, default=None,
@@ -192,6 +192,19 @@ def build_parser() -> argparse.ArgumentParser:
     ext.add_argument("--model-ema-decay", type=float, default=0.99998,
                      help="EMA decay per image seen, 0 <= d < 1; the decay of one update is adjusted as torchvision "
                           "does: 1 - min(1, (1 - d) * world * mini_batch * accum_steps * model_ema_steps / epochs)")
+    ext.add_argument("--distill-teacher", default=None,
+                     help="knowledge distillation: train against the logits of this teacher as well as the labels.  A "
+                          "checkpoint of this project (--save) or a plain state dict with torchvision names, loaded "
+                          "whole (every tensor, right shapes, the student's class count).  The teacher runs in eval "
+                          "mode on the student's augmented input; the train loss is (1 - alpha) CE + alpha T^2 "
+                          "KL(softmax(teacher / T) || softmax(student / T)); the test loss stays plain cross-entropy "
+                          "(default: off)")
+    ext.add_argument("--distill-teacher-model", default=None, choices=MODELS,
+                     help="the teacher's layer table (default: the checkpoint's --model, else the student's)")
+    ext.add_argument("--distill-alpha", type=float, default=0.5,
+                     help="weight of the distillation term, 0 < alpha <= 1 (default 0.5)")
+    ext.add_argument("--distill-temperature", type=float, default=4.0,
+                     help="softmax temperature T of the distillation term, finite and > 0 (default 4.0)")
     return parser
 
 
@@ -251,6 +264,13 @@ def parse_command_line(argv: Optional[Sequence[str]] = None, init: bool = True):
     err = check_sizes(args)
     if err:
         build_parser().error(err)
+    if args.distill_teacher is not None:
+        if not 0.0 < args.distill_alpha <= 1.0:
+            build_parser().error("--distill-alpha must lie in (0, 1]")
+        if not (math.isfinite(args.distill_temperature) and args.distill_temperature > 0.0):
+            build_parser().error("--distill-temperature must be finite and > 0")
+        if args.eval_only:
+            build_parser().error("--distill-teacher trains a student; --eval-only scores a checkpoint (drop the teacher)")
     if args.freeze_layers:
         from .models.vggf import get_spec
         try:

@@ -149,6 +149,15 @@ class PhaseTimer:
         return {k: self.totals[k] / max(self.counts[k], 1) for k in self.totals}
 
 
+def check_native_spec(spec: VGGSpec) -> None:
+    """ValueError unless the native kernels run every convolution of ``spec``."""
+    for c in spec.convs[1:]:
+        if c.cin % 64 or c.cout % 64:
+            raise ValueError("native conv kernels need channel counts that are multiples of 64")
+    if spec.convs[0].cout % 64 or spec.convs[0].cin != 3:
+        raise ValueError("first conv must be 3 -> multiple of 64 channels")
+
+
 class NativeEngine:
     def __init__(self, spec: VGGSpec, device: torch.device, batch: int, lr: float = TRAIN.learning_rate,
                  optimizer: str = "adam", momentum: float = TRAIN.momentum, weight_decay: float = 0.0,
@@ -167,11 +176,7 @@ class NativeEngine:
         if compute_dtype != "bf16":
             raise NotImplementedError("the native engine computes in bf16 with fp32 master weights; "
                                       "use --engine oracle for fp32 numerics")
-        for c in spec.convs[1:]:
-            if c.cin % 64 or c.cout % 64:
-                raise ValueError("native conv kernels need channel counts that are multiples of 64")
-        if spec.convs[0].cout % 64 or spec.convs[0].cin != 3:
-            raise ValueError("first conv must be 3 -> multiple of 64 channels")
+        check_native_spec(spec)
         self.spec, self.device, self.B = spec, torch.device(device), int(batch)
         if optimizer not in ("adam", "adamw", "sgd", "lamb", "lars"):
             raise ValueError("optimizer must be adam, adamw, sgd, lamb or lars (got %r)" % optimizer)
@@ -208,6 +213,7 @@ class NativeEngine:
         self.apply_updates = True        # False: leave raw gradients in g32 (gradient inspection)
         self.meter: Optional[DeviceMeter] = None
         self.class_weights: Optional[torch.Tensor] = None
+        self.teacher: Optional["TeacherEngine"] = None       # knowledge distillation (set_distillation)
         self.timer = PhaseTimer(profile == "events", nvtx=(profile == "nvtx"))
         self._comm_events: Optional[list] = None     # [(start, end, wire bytes)] while comm timing is on
         self._tl: Optional[list] = None              # step timeline marks (timeline())
@@ -670,7 +676,9 @@ class NativeEngine:
         torch.cuda.synchronize(self.device)
 
     # ============================================================================== buffers
-    def _build_buffers(self) -> None:
+    def _build_buffers(self, backward: bool = True) -> None:
+        """Input staging, activations and the FC stack's buffers; with ``backward`` also the gradient buffers and,
+        under --deterministic, a workspace for every split-K launch of a training step (else for the forward's)."""
         spec, B, dev, HW = self.spec, self.B, self.device, self.HW
         # double-buffered device-side input staging, filled by a copy stream
         self.copy_stream = torch.cuda.Stream(device=dev)
@@ -741,8 +749,9 @@ class NativeEngine:
         self.fc_acc = [torch.zeros(B, f.fout, dtype=F32, device=dev) for f in spec.fcs]
         self.fc_y = [torch.empty(B, f.fout, dtype=BF16, device=dev) if i < len(spec.fcs) - 1 else None
                      for i, f in enumerate(spec.fcs)]
-        self.fc_dacc = [torch.zeros(B, f.fin, dtype=F32, device=dev) for f in spec.fcs]
-        self.fc_dz = [torch.zeros(B, _round_up(f.fout, 8), dtype=BF16, device=dev) for f in spec.fcs]
+        if backward:
+            self.fc_dacc = [torch.zeros(B, f.fin, dtype=F32, device=dev) for f in spec.fcs]
+            self.fc_dz = [torch.zeros(B, _round_up(f.fout, 8), dtype=BF16, device=dev) for f in spec.fcs]
         self.logits = torch.zeros(B, spec.num_classes, dtype=F32, device=dev)
         self.loss_buf = torch.zeros(1, dtype=F32, device=dev)
         self.scratch_meter = torch.zeros(4, dtype=F32, device=dev)
@@ -752,13 +761,16 @@ class NativeEngine:
         self.fused_head = (os.environ.get("B200_FUSED_HEAD", "1") == "1" and len(spec.fcs) >= 2
                            and bool(ops.require().head_ce_supported(B, lastf.fout, lastf.fin)))
         self._head_in = None
-        # backward activations-gradients: two ping-pong buffers big enough for the largest map
-        biggest = max(a.numel() for g in self._geo.values() for a in g["acts"])
-        self.dbuf = [torch.empty(biggest, dtype=BF16, device=dev) for _ in range(2)]
-        self.dfeat = torch.empty(B, ph, ph, cl, dtype=BF16, device=dev)
+        if backward:
+            # backward activations-gradients: two ping-pong buffers big enough for the largest map
+            biggest = max(a.numel() for g in self._geo.values() for a in g["acts"])
+            self.dbuf = [torch.empty(biggest, dtype=BF16, device=dev) for _ in range(2)]
+            self.dfeat = torch.empty(B, ph, ph, cl, dtype=BF16, device=dev)
         if self.deterministic:
             # one workspace for every split-K launch of the step: they all run on the compute stream
             plan = deterministic_plan(spec, B, HW, ops.require().sm_count(), self.fused_head, self.freeze_layers)
+            if not backward:
+                plan = [row for row in plan if row[1] == "fprop"] or [(None, "fprop", 1, 4)]
             self._ws = torch.empty(deterministic_workspace_elems(plan), dtype=F32, device=dev)
 
     def _set_hw(self, hw: int) -> None:
@@ -924,10 +936,17 @@ class NativeEngine:
         meter = self.meter.buf if self.meter is not None else self.scratch_meter
         # soft targets (label smoothing, MixUp / CutMix) shape the training loss only
         eps, mix = (self.label_smoothing, self._mix) if train else (0.0, None)
+        kd = train and self.teacher is not None
         if not self.fused_head:
-            ld = self.fc_dz[-1].shape[1]
+            ld = self.fc_dz[-1].shape[1] if train else 0
+            if kd:
+                ops.cross_entropy_kd(self.logits[:b], self.labels_dev[:b], self._teacher_logits, alpha=self.distill_alpha,
+                                     temperature=self.distill_temperature, dlogits=self.fc_dz[-1][:b], ldd=ld,
+                                     meter=meter, loss_out=self.loss_buf, class_weights=self.class_weights,
+                                     label_smoothing=eps, mix=mix)
+                return
             ops.cross_entropy(self.logits[:b], self.labels_dev[:b], self.fc_dz[-1][:b] if train else None,
-                              ld if train else 0, meter, self.loss_buf,
+                              ld, meter, self.loss_buf,
                               class_weights=self.class_weights if train else None,   # like the reference's loops
                               label_smoothing=eps, mix=mix)
             return
@@ -942,7 +961,10 @@ class NativeEngine:
                     self._grad(f.name + ".bias"), dh, 1.0 / (1.0 - p), bool(prev.relu), meter,
                     self.loss_buf, self.class_weights)
             soft = ops.soft_targets(eps, mix)
-            if soft is not None:
+            if kd:
+                C.head_ce_kd(*args, bool(self._accum), soft, self._teacher_logits, self.distill_alpha,
+                             self.distill_temperature)
+            elif soft is not None:
                 C.head_ce(*args, bool(self._accum), soft)
             elif self._accum:                # a later micro-batch of the group: dW += (db always accumulates)
                 C.head_ce(*args, True)
@@ -1257,6 +1279,26 @@ class NativeEngine:
     def set_meter(self, meter: Optional[DeviceMeter]) -> None:
         self.meter = meter
 
+    def set_distillation(self, teacher: Optional["TeacherEngine"], alpha: float = 0.5,
+                         temperature: float = 4.0) -> None:
+        """Train against ``teacher``'s logits as well as the labels (knowledge distillation): every train_step runs
+        the teacher's forward on the staged input, and the loss is (1 - alpha) CE + alpha T^2 KL(teacher || student)
+        at temperature T (ops.cross_entropy_kd).  None: plain cross-entropy again."""
+        if teacher is not None:
+            if not 0.0 < alpha <= 1.0:
+                raise ValueError("distillation alpha must lie in (0, 1] (got %r)" % alpha)
+            if not (math.isfinite(temperature) and temperature > 0.0):
+                raise ValueError("distillation temperature must be finite and > 0 (got %r)" % temperature)
+            if teacher.spec.num_classes != self.spec.num_classes:
+                raise ValueError("the teacher has %d classes, the student %d" % (teacher.spec.num_classes,
+                                                                                  self.spec.num_classes))
+            if (teacher.B, teacher.HW, teacher.device) != (self.B, self.HW, self.device):
+                raise ValueError("the teacher engine must be built for the student's batch, training crop and device")
+            if teacher.deterministic != self.deterministic:
+                raise ValueError("the teacher engine must follow the student's deterministic flag")
+        self.teacher = teacher
+        self.distill_alpha, self.distill_temperature = float(alpha), float(temperature)
+
     def set_class_weights(self, weights: Optional[torch.Tensor]) -> None:
         """Per-class loss weights (the reference's optional weighted cross-entropy)."""
         self.class_weights = None if weights is None else weights.to(self.device, F32).contiguous()
@@ -1286,6 +1328,11 @@ class NativeEngine:
         b = self._stage_input(batch)
         t.stop("input")
         self._mark("input")
+        if self.teacher is not None:
+            t.start("teacher")
+            self._teacher_logits = self.teacher.forward_teacher(self.x_nhwc, self.labels_dev, b)
+            t.stop("teacher")
+            self._mark("teacher")
         t.start("forward")
         self._forward(b, train=True)
         self._loss(b, train=True)
@@ -1410,3 +1457,68 @@ class NativeEngine:
 
     def eval(self) -> None:
         pass
+
+
+class TeacherEngine(NativeEngine):
+    """A NativeEngine that only runs forward, in evaluation mode (no dropout): the teacher of knowledge distillation.
+    It holds the weights (fp32 master for the biases, bf16 for the GEMMs), the input staging of an evaluation pass,
+    the activations at the training crop and the evaluation crop, and the logits.  No gradient, moment, EMA or wire
+    arena, no backward buffer and no comm or optimizer stream.  ``forward_teacher`` runs _forward and the fused
+    head's evaluation pass on the student's staged input; ``eval_step`` scores it like any engine."""
+
+    def __init__(self, spec: VGGSpec, device: torch.device, batch: int, state: Dict[str, torch.Tensor],
+                 input_hw: int = DATA.crop, eval_hw: Optional[int] = None, deterministic: bool = False) -> None:
+        ops.require()
+        check_native_spec(spec)
+        self.spec, self.device, self.B = spec, torch.device(device), int(batch)
+        self.HW = check_native_hw(input_hw, "input_hw")
+        self.eval_hw = self.HW if eval_hw is None else check_native_hw(eval_hw, "eval_hw")
+        self.deterministic, self._ws = bool(deterministic), None
+        self.world, self.rank, self.seed = 1, 0, 0            # each rank loads the same file: nothing to broadcast
+        self.freeze_layers, self._frozen = 0, set()
+        self.train_dropout, self.same_dropout_all_ranks, self.micro_count = False, False, 0
+        self.label_smoothing, self._mix, self._accum = 0.0, None, 0
+        self.meter, self.class_weights, self.teacher, self.ema32 = None, None, None, None
+        self.timer, self.nvtx, self._tl = PhaseTimer(False), False, None
+        self.plan = engine_bucket_plan(L.ready_order(spec), 32.0, 9.5, 2400.0)     # the arena offsets only
+        self.p32 = torch.zeros(self.plan.total, dtype=F32, device=self.device)
+        self.w16 = torch.zeros(self.plan.total, dtype=BF16, device=self.device)
+        self.import_state(state, sync=False)
+        self._wsrc, self._bsrc = self.w16, self.p32
+        self._build_buffers(backward=False)
+
+    def forward_teacher(self, x_nhwc: torch.Tensor, labels: torch.Tensor, b: int) -> torch.Tensor:
+        """Logits [b][C] fp32 of the network input ``x_nhwc`` staged by the student at the training crop (read in
+        place); ``labels`` only feed the fused head's metrics, which land in a scratch meter."""
+        self._set_hw(self.HW)
+        own = self.x_nhwc
+        self.x_nhwc, self.labels_dev = x_nhwc, labels
+        try:
+            self._forward(b, train=False)
+            if self.fused_head:          # the logits come out of the fused head kernel
+                self._loss(b, train=False)
+        finally:
+            self.x_nhwc = own
+        return self.logits[:b]
+
+    def device_bytes(self) -> int:
+        """Bytes of device memory the teacher's tensors take, from their shapes (views of one buffer counted once)."""
+        seen, total = set(), 0
+
+        def add(t) -> None:
+            nonlocal total
+            if isinstance(t, torch.Tensor):
+                st = t.untyped_storage()
+                if st.data_ptr() not in seen:
+                    seen.add(st.data_ptr())
+                    total += st.nbytes()
+            elif isinstance(t, (list, tuple)):
+                for u in t:
+                    add(u)
+            elif isinstance(t, dict):
+                for u in t.values():
+                    add(u)
+
+        for v in vars(self).values():
+            add(v)
+        return total

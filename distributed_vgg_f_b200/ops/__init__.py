@@ -216,6 +216,19 @@ def soft_targets(label_smoothing: float = 0.0, mix=None):
     return [float(label_smoothing), mix.lam if mix is not None else 1.0, 1.0 if mix is not None else 0.0]
 
 
+def cross_entropy_kd(logits, target, teacher, *, alpha: float, temperature: float, dlogits=None, ldd: int = 0,
+                     meter=None, loss_out=None, grad_scale: Optional[float] = None, class_weights=None,
+                     label_smoothing: float = 0.0, mix=None):
+    """``cross_entropy`` with knowledge distillation against fp32 ``teacher`` logits [B][C]: the loss is
+    (1 - alpha) CE + alpha T^2 KL(softmax(teacher / T) || softmax(logits / T)) / B with CE the loss ``cross_entropy``
+    computes (class weights, smoothing and mixing apply to it alone); meter and loss_out receive that loss."""
+    if grad_scale is None:
+        grad_scale = 1.0 / logits.shape[0]
+    require().cross_entropy_kd(logits, target, dlogits, ldd or logits.shape[1], meter, loss_out, grad_scale,
+                               class_weights, teacher, float(alpha), float(temperature),
+                               soft_targets(label_smoothing, mix))
+
+
 def _ema_args(ema, ema_decay: float, ema_first: bool) -> tuple:
     """Trailing arguments of the optimizer entries: none at all without a moving average."""
     return () if ema is None else (ema, float(ema_decay), bool(ema_first))

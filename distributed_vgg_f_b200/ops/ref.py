@@ -32,7 +32,8 @@ def pool_relu_bwd(y: torch.Tensor, dp: torch.Tensor) -> torch.Tensor:
 @torch.no_grad()
 def emulated_step(spec: VGGSpec, state: Dict[str, torch.Tensor], x: torch.Tensor, target: torch.Tensor,
                   dropout_masks: bool = False, return_intermediates: bool = False,
-                  override: dict = None, soft_target: torch.Tensor = None, label_smoothing: float = 0.0):
+                  override: dict = None, soft_target: torch.Tensor = None, label_smoothing: float = 0.0,
+                  teacher_logits: torch.Tensor = None, distill_alpha: float = 0.5, distill_temperature: float = 4.0):
     """Forward + backward of the network on fp32 torch ops with the engine's rounding points.
 
     state: torch-layout fp32 tensors (weights are rounded to bf16 here, biases stay fp32).
@@ -41,6 +42,10 @@ def emulated_step(spec: VGGSpec, state: Dict[str, torch.Tensor], x: torch.Tensor
     ``soft_target`` (probability targets [B][C], e.g. MixUp / CutMix) and ``label_smoothing``: the loss
     is F.cross_entropy(logits, soft_target or target, label_smoothing=) and its gradient
     (softmax - t) / B with t the smoothed target.
+
+    ``teacher_logits`` ([B][C], optional): knowledge distillation with weight ``distill_alpha`` and temperature
+    ``distill_temperature`` -- the loss is (1 - a) CE + a T^2 KL(softmax(u / T) || softmax(z / T)) / B and its
+    gradient (1 - a) (the CE gradient) + a T (softmax(z / T) - softmax(u / T)) / B, rounded to bf16 once.
 
     ``override`` (optional) pins the forward state to tensors observed elsewhere -- keys ``acts``
     (post-ReLU conv outputs, NCHW), ``feat`` (pooled feature map), ``fc_y`` (hidden FC outputs),
@@ -93,6 +98,14 @@ def emulated_step(spec: VGGSpec, state: Dict[str, torch.Tensor], x: torch.Tensor
         t = t * (1.0 - label_smoothing) + label_smoothing / logits.shape[1]
         loss = -(t * logp).sum(1).mean()
         dz = rb((torch.softmax(logits, 1) - t) / B)
+    if teacher_logits is not None:
+        a, T = float(distill_alpha), float(distill_temperature)
+        t = F.one_hot(target, logits.shape[1]).float() if soft_target is None else soft_target.float()
+        t = t * (1.0 - label_smoothing) + label_smoothing / logits.shape[1]
+        lps, lpt = torch.log_softmax(logits / T, 1), torch.log_softmax(teacher_logits.float() / T, 1)
+        kl = (lpt.exp() * (lpt - lps)).sum() / B
+        loss = (1.0 - a) * loss + a * T * T * kl
+        dz = rb((1.0 - a) * (torch.softmax(logits, 1) - t) / B + a * T * (lps.exp() - lpt.exp()) / B)
 
     grads: Dict[str, torch.Tensor] = {}
     inter = {"fc_dz": {}, "fc_y": {i: fc_in[i + 1] for i in range(last)}, "conv_dz": {}}
@@ -476,6 +489,40 @@ def cross_entropy64(logits: torch.Tensor, target: torch.Tensor, *, ldd: int = 0,
     dl = torch.zeros(B, max(ldd, C), dtype=torch.float64, device=z.device)
     dl[:, :C] = (torch.softmax(z, 1) - torch.nn.functional.one_hot(t, C).to(torch.float64)) * (w * norm)[:, None]
     correct = float((_first_argmax(z) == t).sum())
+    meter = torch.tensor([float(loss) * B, correct, float(B)], dtype=torch.float64)
+    return {"loss": loss, "dlogits": dl, "meter": meter}
+
+
+def kd_cross_entropy64(logits: torch.Tensor, teacher: torch.Tensor, target: torch.Tensor, *, alpha: float,
+                       temperature: float, class_weights=None, label_smoothing: float = 0.0, soft_target=None,
+                       ldd: int = 0):
+    """The distillation loss in float64, in closed form -> dict with
+    loss: (1 - alpha) CE + alpha T^2 sum_r KL(softmax(u_r / T) || softmax(z_r / T)) / B, where CE is
+    F.cross_entropy(z, soft_target or target, weight=class_weights, label_smoothing=);
+    dlogits [B][ldd]: (1 - alpha) dCE + alpha T (softmax(z / T) - softmax(u / T)) / B, columns >= C zero;
+    meter: (loss * B, count of first-maximum argmax == target (or the soft target's first maximum), B)."""
+    z, u = _f64(logits), _f64(teacher)
+    B, C = z.shape
+    t = target.to(torch.int64).view(-1)
+    a, T = float(alpha), float(temperature)
+    q = torch.nn.functional.one_hot(t, C).to(torch.float64) if soft_target is None else _f64(soft_target)
+    cls = t if soft_target is None else _first_argmax(_f64(soft_target))
+    q = q * (1.0 - label_smoothing) + label_smoothing / C
+    norm = 1.0 / B
+    if class_weights is not None:
+        cw = _f64(class_weights)
+        q = q * cw[None, :]
+        if soft_target is None:          # integer targets: torch divides by the targets' weights
+            norm = 1.0 / float(cw[t].sum())
+    logp = torch.log_softmax(z, 1)
+    ce = -(q * logp).sum() * norm
+    dce = (torch.softmax(z, 1) * q.sum(1, keepdim=True) - q) * norm
+    lps, lpt = torch.log_softmax(z / T, 1), torch.log_softmax(u / T, 1)
+    kl = (lpt.exp() * (lpt - lps)).sum() / B
+    loss = (1.0 - a) * ce + a * T * T * kl
+    dl = torch.zeros(B, max(ldd, C), dtype=torch.float64, device=z.device)
+    dl[:, :C] = (1.0 - a) * dce + a * T * (lps.exp() - lpt.exp()) / B
+    correct = float((_first_argmax(z) == cls).sum())
     meter = torch.tensor([float(loss) * B, correct, float(B)], dtype=torch.float64)
     return {"loss": loss, "dlogits": dl, "meter": meter}
 

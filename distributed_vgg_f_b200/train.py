@@ -199,6 +199,13 @@ def manage_training(args) -> Trainer:
         if ema_decay is not None:
             model_ema = build_model_ema(model.module if isinstance(model, FlatDDP) else model, ema_decay)
 
+    teacher, distill = None, None
+    if getattr(args, "distill_teacher", None):
+        teacher, distill = build_teacher(args, spec, device, native=optimizer is None, crop=sizes["train_crop_size"],
+                                         eval_crop=sizes["val_crop_size"])
+        if optimizer is None:
+            model.set_distillation(teacher, args.distill_alpha, args.distill_temperature)
+
     if getattr(args, "eval_only", False) and model_ema is not None and not args.resume:
         raise ValueError("--eval-only --model-ema scores a checkpoint's EMA: pass --resume <checkpoint>")
     start_epoch = 1
@@ -246,6 +253,8 @@ def manage_training(args) -> Trainer:
                 rec["lr"] = epoch_lr
             if hasattr(model, "phase_times"):
                 rec["phase_ms"] = model.phase_times()
+            if distill is not None:
+                rec.update(distill=distill, teacher_test_acc=teacher_acc.accuracy)
             for key in ("epoch_host_times", "epoch_allreduce"):       # set by Trainer for native engines
                 if getattr(trainer, key, None):
                     rec[key[len("epoch_"):]] = getattr(trainer, key)
@@ -261,7 +270,10 @@ def manage_training(args) -> Trainer:
                       on_epoch_end=on_epoch_end, shard_eval=getattr(args, "shard_eval", False),
                       accum_steps=getattr(args, "accum_steps", 1),
                       label_smoothing=getattr(args, "label_smoothing", 0.0), model_ema=model_ema,
-                      model_ema_steps=getattr(args, "model_ema_steps", 32))
+                      model_ema_steps=getattr(args, "model_ema_steps", 32),
+                      teacher=teacher if optimizer is not None else None,
+                      distill_alpha=getattr(args, "distill_alpha", 0.5),
+                      distill_temperature=getattr(args, "distill_temperature", 4.0))
     trainer.profile_timeline = getattr(args, "profile", None) == "timeline"
     if getattr(args, "eval_only", False):        # score a checkpoint: one validation pass, no training
         test_loss, test_acc = trainer._evaluate()
@@ -273,5 +285,35 @@ def manage_training(args) -> Trainer:
             rec.update(ema_test_loss=ema_loss.average, ema_test_acc=ema_acc.accuracy)
         trainer.history.append(rec)
         return trainer
+    if teacher is not None:
+        # a teacher trained on another class order scores near chance here
+        teacher_loss, teacher_acc = trainer._evaluate(model=teacher)
+        print("[Info] distillation: teacher {} from {} (alpha {}, temperature {}): test loss {}, test acc {}.".format(
+            distill["model"], distill["path"], distill["alpha"], distill["temperature"], teacher_loss, teacher_acc),
+            flush=True)
     trainer.fit(args.epochs, start_epoch=start_epoch)
     return trainer
+
+
+def build_teacher(args, spec, device: torch.device, native: bool, crop: int, eval_crop: int):
+    """The --distill-teacher model, loaded whole by this rank (every rank reads the same file, as --pretrained):
+    a forward-only ``TeacherEngine`` on the native engine, an eval-mode ``VGGOracle`` without gradients on the
+    torch-op engine (fp32).  Returns (teacher, the JSONL record's ``distill`` entry)."""
+    name, state = ckpt.load_teacher_state(args.distill_teacher, spec.num_classes,
+                                          getattr(args, "distill_teacher_model", None), args.model)
+    tspec = get_spec(name, spec.num_classes)
+    info = dict(path=args.distill_teacher, model=name, alpha=args.distill_alpha, temperature=args.distill_temperature)
+    if native:
+        from .engine.native_engine import TeacherEngine
+        try:
+            teacher = TeacherEngine(tspec, device, args.mini_batch, state, input_hw=crop, eval_hw=eval_crop,
+                                    deterministic=getattr(args, "deterministic", False))
+        except ValueError as e:
+            raise ValueError("--distill-teacher-model %s: the native engine cannot run it (%s)" % (name, e)) from None
+        print("[Info] distillation teacher: {} ({} parameters), {:.1f} MB of device memory, forward only".format(
+            name, tspec.num_params, teacher.device_bytes() / 1e6), flush=True)
+        return teacher, info
+    teacher = build_oracle(tspec, seed=0).to(device)       # its own generator: the global RNG stays untouched
+    teacher.load_state_dict(state)
+    teacher.eval().requires_grad_(False)
+    return teacher, info

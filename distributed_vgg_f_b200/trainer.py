@@ -23,6 +23,11 @@ mini-batches, and after the epoch's last one, so the last group of an epoch may 
 no group crosses an epoch boundary.  Each mini-batch's loss is its own mean; the update uses the sum of
 the group's gradients divided by k'.  Metrics count every mini-batch.
 
+``teacher`` (knowledge distillation, torch path; the native engine has its own, ``set_distillation``): an
+eval-mode module without gradients run under ``no_grad`` on the (mixed) training inputs; the training loss is
+(1 - a) CE + a T^2 F.kl_div(log_softmax(s / T), log_softmax(t / T), "batchmean", log_target=True) with CE as above,
+and the train meter accumulates it.  Accuracy and the test loss stay those of the labels.
+
 ``model_ema`` (torchvision's --model-ema): after the optimizer update whose 0-based index u within the
 epoch has u % model_ema_steps == 0, the moving average of the weights is updated -- by the native engine's
 optimizer kernels (``model_ema=True``, ``train_step(ema=True)``), or on the torch path by
@@ -65,6 +70,14 @@ def sys_stdout_flush() -> None:
     sys.stdout.flush()
 
 
+def distill_loss(student: torch.Tensor, teacher: torch.Tensor, ce: torch.Tensor, alpha: float,
+                 temperature: float) -> torch.Tensor:
+    """(1 - alpha) ce + alpha T^2 KL(softmax(teacher / T) || softmax(student / T)), the KL a batch mean."""
+    T = float(temperature)
+    kl = F.kl_div(F.log_softmax(student / T, 1), F.log_softmax(teacher / T, 1), reduction="batchmean", log_target=True)
+    return (1.0 - alpha) * ce + alpha * T * T * kl
+
+
 def _is_native(model) -> bool:
     return hasattr(model, "train_step") and hasattr(model, "eval_step")
 
@@ -73,7 +86,8 @@ class Trainer:
     def __init__(self, model, optimizer, train_loader, test_loader, device,
                  class_weights: Optional[torch.Tensor] = None, verbose_throughput: bool = True,
                  on_epoch_end=None, shard_eval: bool = False, accum_steps: int = 1,
-                 label_smoothing: float = 0.0, model_ema=None, model_ema_steps: int = 32) -> None:
+                 label_smoothing: float = 0.0, model_ema=None, model_ema_steps: int = 32, teacher=None,
+                 distill_alpha: float = 0.5, distill_temperature: float = 4.0) -> None:
         if accum_steps < 1:
             raise ValueError("accum_steps must be >= 1 (got %d)" % accum_steps)
         if accum_steps > 1 and not hasattr(train_loader, "__len__"):
@@ -87,6 +101,8 @@ class Trainer:
             raise ValueError("model_ema on the native engine needs NativeEngine(ema_decay=...)")
         self.model_ema = model_ema          # AveragedModel (torch path), True (native engine) or None
         self.model_ema_steps = int(model_ema_steps)
+        self.teacher = teacher              # torch path: the distillation teacher (an eval-mode module)
+        self.distill_alpha, self.distill_temperature = float(distill_alpha), float(distill_temperature)
         self.model = model
         self.optimizer = optimizer
         self.train_loader = train_loader
@@ -252,6 +268,10 @@ class Trainer:
             soft = None if mix is None else T.mixed_targets(targets, outputs.shape[1], mix)
             loss = F.cross_entropy(outputs, targets if soft is None else soft, weight=self.class_weights,
                                    label_smoothing=self.label_smoothing)
+            if self.teacher is not None:
+                with torch.no_grad():
+                    t_out = self.teacher(inputs)
+                loss = distill_loss(outputs, t_out, loss, self.distill_alpha, self.distill_temperature)
             if pending == 0:                             # zeroed once per group, before its first backward
                 if wrapper is not None:
                     wrapper.zero_grad()
@@ -275,7 +295,8 @@ class Trainer:
                 u += 1
                 pending = 0
             meter.add_reference(outputs.detach(), targets, self.class_weights, soft_target=soft,
-                                label_smoothing=self.label_smoothing)
+                                label_smoothing=self.label_smoothing,
+                                loss=loss.detach() if self.teacher is not None else None)
         return meter.snapshot()
 
     def _reduce_eval(self, meter: DeviceMeter):
@@ -286,22 +307,24 @@ class Trainer:
             dist.all_reduce(meter.buf)
         return meter.snapshot()
 
-    def _evaluate(self, ema: bool = False):
-        """One validation pass over the weights, or with ``ema`` over their moving average."""
+    def _evaluate(self, ema: bool = False, model=None):
+        """One validation pass over the weights, or with ``ema`` over their moving average, or over ``model`` (a
+        distillation teacher: an engine or module of the same kind)."""
         meter = DeviceMeter(self.device)
-        if _is_native(self.model):
-            self.model.set_meter(meter)
+        model = self.model if model is None else model
+        if _is_native(model):
+            model.set_meter(meter)
             if ema:
-                self.model.prepare_ema()             # collective under ZeRO-1: gathers the owned EMA cells
+                model.prepare_ema()             # collective under ZeRO-1: gathers the owned EMA cells
             for batch in self.test_loader:
                 if ema:
-                    self.model.eval_step(batch, ema=True)
+                    model.eval_step(batch, ema=True)
                 else:
-                    self.model.eval_step(batch)
-            self.model.sync()
+                    model.eval_step(batch)
+            model.sync()
             return self._reduce_eval(meter)
 
-        net = self.model_ema if ema else self.model
+        net = self.model_ema if ema else model
         net.eval()
         with torch.no_grad():
             for batch in self.test_loader:

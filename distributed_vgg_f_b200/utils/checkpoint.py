@@ -139,3 +139,36 @@ def load_checkpoint(path: str, model, optimizer=None, model_ema=None, ema_requir
         if optimizer is not None and opt and _check_frozen(path, opt, model):
             optimizer.load_state_dict({k: v for k, v in opt.items() if k != "frozen_layers"})
     return int(payload.get("epoch", 0))
+
+
+def load_teacher_state(path: str, num_classes: int, model: Optional[str] = None, student_model: str = "vggf"):
+    """The teacher of --distill-teacher: (model name, torch-layout fp32 state dict).  ``path`` holds a checkpoint of
+    this project (``{"model": {"module.<name>": ...}, "args": {...}}``) or a plain state dict with torchvision names.
+    The model is ``model`` when given, else the checkpoint's ``args["model"]``, else ``student_model``.  Unlike
+    --pretrained, the file must be the whole model: a missing, unexpected or misshapen tensor is refused, and so is
+    a class count other than ``num_classes``."""
+    from ..models.vggf import get_spec
+
+    if not os.path.isfile(path):
+        raise FileNotFoundError("--distill-teacher %s: no such file" % path)
+    payload = torch.load(path, map_location="cpu", weights_only=True)
+    if not isinstance(payload, dict):
+        raise ValueError("--distill-teacher %s: not a checkpoint or a state dict" % path)
+    ours = isinstance(payload.get("model"), dict)
+    state = strip_module_prefix(payload["model"] if ours else payload)
+    saved = payload.get("args") if ours and isinstance(payload.get("args"), dict) else {}
+    name = model or saved.get("model") or student_model
+    spec = get_spec(name, num_classes)
+    head = spec.fcs[-1].name + ".weight"
+    if head in state and state[head].dim() == 2 and state[head].shape[0] != num_classes:
+        raise ValueError("--distill-teacher %s: the teacher has %d classes, the student %d"
+                         % (path, state[head].shape[0], num_classes))
+    missing = [n for n in spec.param_names if n not in state]
+    unexpected = sorted(set(state) - set(spec.param_names))
+    wrong = [n for n in spec.param_names if n in state and tuple(state[n].shape) != tuple(spec.param_shape(n))]
+    if missing or unexpected or wrong:
+        raise ValueError("--distill-teacher %s does not hold a whole %s: missing %s, unexpected %s, wrong shape %s"
+                         % (path, name, missing[:4] or "none", unexpected[:4] or "none",
+                            ["%s %s (want %s)" % (n, tuple(state[n].shape), tuple(spec.param_shape(n)))
+                             for n in wrong[:4]] or "none"))
+    return name, {n: state[n].detach().to(torch.float32) for n in spec.param_names}

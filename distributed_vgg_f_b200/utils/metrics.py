@@ -69,14 +69,24 @@ class DeviceMeter:
         self.buf.zero_()
 
     def add_reference(self, logits: torch.Tensor, target: torch.Tensor, weight=None,
-                      soft_target: torch.Tensor = None, label_smoothing: float = 0.0) -> None:
+                      soft_target: torch.Tensor = None, label_smoothing: float = 0.0, loss=None) -> None:
         """Torch-op fallback used by the oracle path (same arithmetic as the kernel): accumulates
         ``loss * batch`` exactly like ``Average.update(loss.item(), batch)`` in the reference's loop,
         where ``loss`` is the (optionally class-weighted) mean torch reports.
 
         ``soft_target`` (probability targets [B][C], MixUp / CutMix) and ``label_smoothing``: the loss is
         F.cross_entropy's with them, and a sample is correct when argmax(logits) == argmax(soft_target)
-        (torchvision's classification reference, ``utils.accuracy`` on 2-D targets)."""
+        (torchvision's classification reference, ``utils.accuracy`` on 2-D targets).
+
+        ``loss`` (a scalar, e.g. the distillation objective): accumulated instead of the cross-entropy; the
+        accuracy is counted as without it."""
+        if loss is not None:
+            with torch.no_grad():
+                cls = soft_target.argmax(dim=1) if soft_target is not None else target
+                self.buf[0] += loss.float() * logits.shape[0]
+                self.buf[1] += logits.argmax(dim=1).eq(cls).sum()
+                self.buf[2] += logits.shape[0]
+            return
         if soft_target is not None or label_smoothing:
             with torch.no_grad():
                 tgt = soft_target if soft_target is not None else target
