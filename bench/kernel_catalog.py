@@ -20,6 +20,7 @@ ROLE = [   # (regex on the demangled name, role, what it replaces in the referen
     (r"umma_kernel<b200::GemmPolicy", "FC GEMMs: swap-AB split-K forward / dgrad, wgrad with epilogue → fp32 arena or `bf16(dW/ws)` straight into the symmetric wire", "cuBLAS SGEMM under `nn.Linear` — `:162`, `:171`"),
     (r"head_ce_kernel", "K-FUN2+CE: last Linear + log-softmax / NLL + metrics + dlogits + the layer's dW, db, dX in one launch", "cuBLAS + ATen log_softmax / nll_loss + `Accuracy2` / `Average` — `:56`, `:168`, `distributedUtil.py:95-96`"),
     (r"head_ce_kd_kernel", "K-FUN2+CE with knowledge distillation: head_ce_kernel's launch, the teacher's logits read too; loss (1 − α) CE + α T² KL and its dlogits", "`F.cross_entropy` + `F.kl_div` of a distillation script — not in the reference"),
+    (r"tta_accumulate_kernel", "--val-tta view-mean reduction: each view's softmax added into an fp32 [B][C] accumulator in view order; at the last view -log of the label's mean probability and its argmax into the meter", "the mean softmax of torchvision's `ten_crop` / `five_crop` views — not in the reference"),
     (r"cross_entropy_kd_kernel", "cross-entropy with knowledge distillation for heads that do not fuse (C > 8, B > 256, VGG-16)", "`F.cross_entropy` + `F.kl_div` of a distillation script — not in the reference"),
     (r"cross_entropy_kernel", "cross-entropy fwd + bwd + metrics for wide heads (VGG-16/1000)", "`F.cross_entropy` — `:168`"),
     (r"fc_bias_act_kernel", "FC epilogue: bias + ReLU + Philox dropout → bf16 (mask never stored)", "ATen bias/relu/dropout — `:52-57`"),
@@ -28,6 +29,9 @@ ROLE = [   # (regex on the demangled name, role, what it replaces in the referen
     (r"maxpool2x2_fwd_kernel|maxpool2x2_relu_bwd_kernel|maxpool2x2_relu_bwd_odd_kernel", "un-fused max-pool fwd / ReLU + pool bwd (tile shapes the epilogue cannot pool, odd maps in floor mode, `B200_FUSE_POOL=0`)", "cuDNN / ATen max_pool2d"),
     (r"unpool2x2_kernel", "backward of the epilogue-fused pool: pooled gradient + argmax bit masks → full-resolution dz, bias gradient fused", "max_pool2d_backward + threshold_backward"),
     (r"adaptive_avgpool", "AdaptiveAvgPool2d(7,7) fwd / bwd (elided when the map is already 7×7)", "ATen adaptive_avg_pool2d — torchvision VGG"),
+    (r"augment_view_nhwc_kernel", "--val-tta: one view (five-crop corner, centre, or mirror) of the fused transform: uint8 HWC → normalised bf16 NHWC4", "torchvision `FiveCrop` / `TenCrop` after `Resize` — not in the reference"),
+    (r"augment_ragged_views_h_kernel", "--val-tta, images of any size: Pillow's horizontal pass once over the union of the rows and columns every view reads", "PIL `Resize` before `TenCrop` — not in the reference"),
+    (r"augment_ragged_view_v_kernel", "--val-tta, images of any size: Pillow's vertical pass and the view's crop, per view", "PIL `Resize` + `TenCrop` — not in the reference"),
     (r"augment_nhwc_kernel|augment_im2col_kernel", "the six PIL transforms as one coordinate chain per output pixel: uint8 HWC → normalised bf16 NHWC4", "PIL / torchvision transforms — `:88-95`, `:103-108`"),
     (r"im2col3x3_c3_kernel|nchw_f32_to_nhwc_bf16_kernel", "input layout conversion for float inputs (tests, `forward_logits`)", "—"),
     (r"adam_kernel", "fused Adam over a bucket: grad (fp32 arena or bf16 wire) → fp32 master, moments, bf16 shadow, gradient range re-zeroed; evict-first streams", "`torch.optim.Adam` foreach kernels + `zero_grad` — `:230`, `:170-172`"),

@@ -718,6 +718,106 @@ static void augment_ragged_mixed(const at::Tensor& src, const at::Tensor& geom, 
   const b200::MixParams mix = mix_params("augment_ragged_mixed", kind, lam, box, OH, OW);
   augment_ragged_impl(src, geom, params, inter, out, geom_host, params_host, OH, OW, mean, stdv, &mix);
 }
+// A test-time augmentation view code (TtaPosition, or'ed with TtaFlip) whose OH x OW crop fits an RH x RW image.
+static void check_view(const char* what, int64_t view, int64_t RH, int64_t RW, int64_t OH, int64_t OW) {
+  TORCH_CHECK(view >= 0 && (view & ~(int64_t)b200::TtaFlip) <= b200::TtaCentreMirror, what, ": bad view code ", view);
+  TORCH_CHECK(OH <= RH && OW <= RW, what, ": a ", OH, " x ", OW, " view does not fit a ", RH, " x ", RW, " image");
+}
+
+static void augment_view(const at::Tensor& src, const at::Tensor& params, at::Tensor out, int64_t RH, int64_t RW,
+                         int64_t OH, int64_t OW, int64_t view, std::vector<double> mean, std::vector<double> stdv) {
+  c10::cuda::CUDAGuard g(src.device());
+  check_augment(src, params, out, OH, OW, 0, 4, mean, stdv);
+  check_view("augment_view", view, RH, RW, OH, OW);
+  float m[3] = {(float)mean[0], (float)mean[1], (float)mean[2]}, s[3] = {(float)stdv[0], (float)stdv[1], (float)stdv[2]};
+  b200::augment_view(src.data_ptr<uint8_t>(), f32p(params), bfp_mut(out), src.size(0), src.size(1), src.size(2),
+                     (int)RH, (int)RW, (int)OH, (int)OW, (int)view, m, s, cur_stream());
+}
+
+// augment_ragged for one view; `pass1`: the codes of every view of the batch, to run pass 1 for them first (empty:
+// inter already holds it).  Every operand is checked as augment_ragged checks it, and every view against every image.
+static void augment_ragged_view(const at::Tensor& src, const at::Tensor& geom, const at::Tensor& params,
+                                at::Tensor inter, at::Tensor out, const at::Tensor& geom_host,
+                                const at::Tensor& params_host, int64_t OH, int64_t OW, std::vector<double> mean,
+                                std::vector<double> stdv, int64_t view, std::vector<int64_t> pass1) {
+  c10::cuda::CUDAGuard g(src.device());
+  TORCH_CHECK(src.is_cuda() && src.scalar_type() == at::kByte && src.is_contiguous(),
+              "augment_ragged_view: src must be a contiguous CUDA uint8 tensor");
+  TORCH_CHECK(inter.is_cuda() && inter.scalar_type() == at::kByte && inter.is_contiguous(),
+              "augment_ragged_view: inter must be a contiguous CUDA uint8 tensor");
+  TORCH_CHECK(geom.is_cuda() && geom.scalar_type() == at::kLong && geom.is_contiguous() && geom.dim() == 2 &&
+                  geom.size(1) == 5, "augment_ragged_view: geom must be a contiguous CUDA int64 [N, 5] tensor");
+  const int64_t N = geom.size(0);
+  TORCH_CHECK(N > 0 && N <= 65535, "augment_ragged_view: 1 to 65535 images");
+  TORCH_CHECK(params.is_cuda() && params.scalar_type() == at::kFloat && params.is_contiguous() && params.dim() == 2 &&
+                  params.size(0) == N && params.size(1) == 8,
+              "augment_ragged_view: params must be a contiguous CUDA fp32 [N, 8] tensor");
+  TORCH_CHECK(!geom_host.is_cuda() && geom_host.scalar_type() == at::kLong && geom_host.is_contiguous() &&
+                  geom_host.sizes() == geom.sizes(), "augment_ragged_view: geom_host must be the CPU int64 copy of geom");
+  TORCH_CHECK(!params_host.is_cuda() && params_host.scalar_type() == at::kFloat && params_host.is_contiguous() &&
+                  params_host.sizes() == params.sizes(),
+              "augment_ragged_view: params_host must be the CPU fp32 copy of params");
+  TORCH_CHECK(OH > 0 && OW > 0 && mean.size() == 3 && stdv.size() == 3,
+              "augment_ragged_view: OH, OW > 0, 3 means and deviations");
+  TORCH_CHECK((int64_t)pass1.size() <= b200::kTtaMaxViews, "augment_ragged_view: at most ", b200::kTtaMaxViews,
+              " views");
+  check_vec(out, at::kBFloat16, 8, "augment_ragged_view", "out");
+  TORCH_CHECK(out.numel() >= N * OH * OW * 4, "augment_ragged_view: out must hold N x OH x OW x 4 elements");
+  const int64_t* gh = geom_host.data_ptr<int64_t>();
+  const float* ph = params_host.data_ptr<float>();
+  int64_t most = 1;
+  for (int64_t i = 0; i < N; ++i) {
+    const int64_t off = gh[i * 5], H = gh[i * 5 + 1], W = gh[i * 5 + 2], RH = gh[i * 5 + 3], RW = gh[i * 5 + 4];
+    TORCH_CHECK(H >= 1 && W >= 1 && H <= 65535 && W <= 65535 && off >= 0 && off + H * W * 3 <= src.numel(),
+                "augment_ragged_view: image ", i, " (offset ", off, ", ", H, " x ", W, ") lies outside src of ",
+                src.numel(), " bytes");
+    TORCH_CHECK(RH >= 1 && RW >= 1 && RH <= (1 << 24) && RW <= (1 << 24), "augment_ragged_view: image ", i,
+                " has a resized size of ", RH, " x ", RW);
+    const int64_t top = (int64_t)ph[i * 8], left = (int64_t)ph[i * 8 + 1];
+    const int64_t ch = (int64_t)ph[i * 8 + 2], cw = (int64_t)ph[i * 8 + 3];
+    TORCH_CHECK(top >= 0 && left >= 0 && ch >= 1 && cw >= 1 && top + ch <= H && left + cw <= W,
+                "augment_ragged_view: image ", i, " has a crop box (", top, ", ", left, ", ", ch, ", ", cw,
+                ") outside its ", H, " x ", W, " pixels");
+    check_view("augment_ragged_view", view, RH, RW, OH, OW);
+    for (int64_t v : pass1) check_view("augment_ragged_view", v, RH, RW, OH, OW);
+    most = std::max(most, H * RW);
+  }
+  const int64_t need = ragged_inter_bytes(geom_host);
+  TORCH_CHECK(inter.numel() >= need, "augment_ragged_view: inter must hold ", need, " bytes, got ", inter.numel());
+  const int64_t cap = std::max<int64_t>(1, 16 * b200::sm_count() / N);
+  const int grid_x = (int)std::min(cap, std::max((most + 255) / 256, (OH * OW + 255) / 256));
+  b200::TtaViews views{0ull, (int)pass1.size()};
+  for (size_t v = 0; v < pass1.size(); ++v) views.codes |= (unsigned long long)pass1[v] << (4 * v);
+  float m[3] = {(float)mean[0], (float)mean[1], (float)mean[2]}, s[3] = {(float)stdv[0], (float)stdv[1], (float)stdv[2]};
+  b200::augment_ragged_view(src.data_ptr<uint8_t>(), reinterpret_cast<const long long*>(geom.data_ptr<int64_t>()),
+                            f32p(params), inter.data_ptr<uint8_t>(), bfp_mut(out), (int)N, (int)OH, (int)OW, grid_x, m,
+                            s, (int)view, pass1.empty() ? nullptr : &views, cur_stream());
+}
+
+// One view's step of the view-mean reduction (tta_accumulate in api.h).
+static void tta_accumulate(const at::Tensor& logits, const at::Tensor& target, at::Tensor acc,
+                           c10::optional<at::Tensor> meter, c10::optional<at::Tensor> loss_out, int64_t view,
+                           int64_t views) {
+  c10::cuda::CUDAGuard g(logits.device());
+  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.is_contiguous() && logits.dim() == 2,
+              "tta_accumulate: logits must be a contiguous CUDA fp32 [B, C] tensor");
+  const int64_t B = logits.size(0), C = logits.size(1);
+  TORCH_CHECK(B >= 1 && C >= 1, "tta_accumulate: empty logits");
+  TORCH_CHECK(views >= 1 && views <= b200::kTtaMaxViews, "tta_accumulate: views must lie in [1, ",
+              b200::kTtaMaxViews, "], got ", views);
+  TORCH_CHECK(view >= 0 && view < views, "tta_accumulate: view ", view, " outside [0, ", views, ")");
+  TORCH_CHECK(target.is_cuda() && target.scalar_type() == at::kLong && target.is_contiguous() && target.numel() >= B,
+              "tta_accumulate: contiguous CUDA int64 targets of B = ", B);
+  TORCH_CHECK(acc.is_cuda() && acc.scalar_type() == at::kFloat && acc.is_contiguous() && acc.numel() >= B * C,
+              "tta_accumulate: acc must be a contiguous CUDA fp32 tensor of at least B x C elements");
+  TORCH_CHECK(!meter.has_value() || (meter->scalar_type() == at::kFloat && meter->numel() >= 3),
+              "tta_accumulate: meter must have 3 fp32 elements");
+  TORCH_CHECK(!loss_out.has_value() || (loss_out->scalar_type() == at::kFloat && loss_out->numel() >= 1),
+              "tta_accumulate: loss_out must have 1 fp32 element");
+  b200::tta_accumulate(f32p(logits), reinterpret_cast<const long long*>(target.data_ptr()), f32p(acc),
+                       f32p_opt(meter), f32p_opt(loss_out), (int)B, (int)C, (int)view, (int)views, cur_stream());
+}
+
 static void im2col_c3(const at::Tensor& x, at::Tensor out, int64_t kpad) {
   c10::cuda::CUDAGuard g(x.device());
   check_vec(x, at::kBFloat16, 8, "im2col_c3", "x");
@@ -1127,6 +1227,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("augment_ragged", &augment_ragged);
   m.def("augment_ragged_mixed", &augment_ragged_mixed);
   m.def("ragged_inter_bytes", &ragged_inter_bytes);
+  m.def("augment_view", &augment_view);
+  m.def("augment_ragged_view", &augment_ragged_view);
+  m.def("tta_accumulate", &tta_accumulate);
+  m.attr("TTA_FLIP") = (int)b200::TtaFlip;
   m.def("im2col_c3", &im2col_c3);
   m.def("nchw_to_nhwc", &nchw_to_nhwc);
   py::class_<PyPrefetcher>(m, "Prefetcher")

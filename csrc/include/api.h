@@ -336,6 +336,31 @@ void augment_mixed(const uint8_t* src, const float* params, bf16* out, int N, in
 void augment_ragged(const uint8_t* src, const long long* geom, const float* params, uint8_t* inter,
                     bf16* out, int N, int OH, int OW, int grid_x, const float* mean,
                     const float* stdv, cudaStream_t s, const MixParams* mix = nullptr);
+// ---- test-time augmentation views (--val-tta) --------------------------------------------------
+// A view is an OH x OW crop of the RH x RW resized image: its position (torchvision's five_crop order, then the
+// centre crop's mirror image), or'ed with TtaFlip to take the crop from the image's horizontal mirror.
+enum TtaPosition { TtaTopLeft = 0, TtaTopRight = 1, TtaBottomLeft = 2, TtaBottomRight = 3, TtaCentre = 4,
+                   TtaCentreMirror = 5 };
+constexpr int TtaFlip = 8;
+constexpr int kTtaMaxViews = 10;
+struct TtaViews {                 // view v's code in bits [4v, 4v + 4)
+  unsigned long long codes;
+  int n;
+};
+// augment_fused mode 0 (NHWC4) for one view; the view's flip is combined with each sample's flip bit.
+void augment_view(const uint8_t* src, const float* params, bf16* out, int N, int SH, int SW, int RH, int RW, int OH,
+                  int OW, int view, const float* mean, const float* stdv, cudaStream_t s);
+// augment_ragged for one view: with `pass1`, first pass 1 over the union of the columns and rows those views read
+// (the batch's other views then run pass 2 alone on the same inter); then pass 2 at `view`.
+void augment_ragged_view(const uint8_t* src, const long long* geom, const float* params, uint8_t* inter, bf16* out,
+                         int N, int OH, int OW, int grid_x, const float* mean, const float* stdv, int view,
+                         const TtaViews* pass1, cudaStream_t s);
+// The view-mean reduction of one view's fp32 logits [B][C] into acc [B][C]: acc = softmax at
+// view 0, acc += softmax at the later ones.  At view V - 1 it adds the batch's -log(acc[y] / V) sum, the count
+// of argmax(acc / V) == y (lowest index on ties) and B into meter, and writes the mean loss to loss_out.
+void tta_accumulate(const float* logits, const long long* target, float* acc, float* meter,
+                    float* loss_out, int B, int C, int view, int views, cudaStream_t s);
+
 // im2col of an NHWC(3, padded to cpad) bf16 image for layer 0 (used when the input is given as a
 // float tensor instead of uint8 + params).
 void im2col3x3_c3(const bf16* x, bf16* out, int N, int H, int W, int cpad, int kpad,

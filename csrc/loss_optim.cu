@@ -337,6 +337,74 @@ void cross_entropy_kd(const float* logits, const long long* target, bf16* dlogit
   check_last("cross_entropy_kd");
 }
 
+// Test-time augmentation (tta_accumulate): one block, one warp per row, as cross_entropy_kernel.  Each view adds its
+// softmax into acc in view order with plain stores (no atomics: the same bits on every run).  The last view also
+// scores the mean probability m = acc / V: loss -log m[y], argmax with the lowest index on ties.
+__global__ void __launch_bounds__(1024)
+tta_accumulate_kernel(const float* __restrict__ logits, const long long* __restrict__ target, float* __restrict__ acc,
+                      float* __restrict__ meter, float* __restrict__ loss_out, int B, int C, int view, int views) {
+  __shared__ float s_loss[32], s_correct[32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  const bool last = view == views - 1;
+  const float fv = static_cast<float>(views);
+  float loss_acc = 0.f, correct_acc = 0.f;
+  for (int r = warp; r < B; r += nwarps) {
+    const float* row = logits + static_cast<long long>(r) * C;
+    float* arow = acc + static_cast<long long>(r) * C;
+    float mx = -INFINITY;
+    for (int c = lane; c < C; c += 32) mx = fmaxf(mx, row[c]);
+    for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    float se = 0.f;
+    for (int c = lane; c < C; c += 32) se += expf(row[c] - mx);
+    for (int o = 16; o; o >>= 1) se += __shfl_xor_sync(0xffffffffu, se, o);
+    float best = -INFINITY;
+    int amax = 0x7fffffff;
+    for (int c = lane; c < C; c += 32) {
+      const float p = __fdiv_rn(expf(row[c] - mx), se);
+      const float a = view == 0 ? p : __fadd_rn(arow[c], p);
+      arow[c] = a;
+      if (last) {
+        const float m = __fdiv_rn(a, fv);
+        if (m > best) { best = m; amax = c; }
+      }
+    }
+    if (last) {
+      for (int o = 16; o; o >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oa = __shfl_xor_sync(0xffffffffu, amax, o);
+        if (ob > best || (ob == best && oa < amax)) { best = ob; amax = oa; }
+      }
+      __syncwarp();                  // the lane that stored acc[r][t] may be another one
+      if (lane == 0) {
+        const int t = static_cast<int>(target[r]);
+        loss_acc += -logf(__fdiv_rn(arow[t], fv));
+        correct_acc += (amax == t) ? 1.f : 0.f;
+      }
+    }
+  }
+  if (!last) return;
+  if (lane == 0) { s_loss[warp] = loss_acc; s_correct[warp] = correct_acc; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float tl = 0.f, tc = 0.f;
+    for (int i = 0; i < nwarps; ++i) { tl += s_loss[i]; tc += s_correct[i]; }
+    const float mean = tl / static_cast<float>(B);     // the meter takes loss * B, as cross_entropy_kernel's
+    if (meter) {
+      atomicAdd(meter + 0, mean * static_cast<float>(B));
+      atomicAdd(meter + 1, tc);
+      atomicAdd(meter + 2, static_cast<float>(B));
+    }
+    if (loss_out) *loss_out = mean;
+  }
+}
+
+void tta_accumulate(const float* logits, const long long* target, float* acc, float* meter, float* loss_out, int B,
+                    int C, int view, int views, cudaStream_t s) {
+  tta_accumulate_kernel<<<1, 1024, 0, s>>>(logits, target, acc, meter, loss_out, B, C, view, views);
+  count_launch();
+  check_last("tta_accumulate");
+}
+
 KdParams kd_params(double alpha, double temperature, int B) {
   return KdParams{static_cast<float>(1.0 - alpha), static_cast<float>(alpha * temperature / B),
                   static_cast<float>(alpha * temperature * temperature), static_cast<float>(1.0 / temperature)};

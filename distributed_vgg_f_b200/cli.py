@@ -189,6 +189,11 @@ def build_parser() -> argparse.ArgumentParser:
                      help="CenterCrop after it: the network's evaluation input, <= --val-resize-size (torchvision's "
                           "--val-crop-size; default %d).  Training and evaluation sizes may differ (FixRes: e.g. "
                           "--train-crop-size 176 --val-resize-size 232 --val-crop-size 224)" % DATA.crop)
+    ext.add_argument("--val-tta", default="none", choices=["none", "flip", "five-crop", "ten-crop"],
+                     help="test-time augmentation of every validation pass: several --val-crop-size views of the "
+                          "Resize(--val-resize-size) image, scored by the mean of their softmaxes.  flip: the centre "
+                          "crop and its mirror image; five-crop: torchvision's five_crop; ten-crop: its ten_crop "
+                          "(the five and those of the mirrored image).  Training does not change (default: none)")
     ext.add_argument("--model-ema-decay", type=float, default=0.99998,
                      help="EMA decay per image seen, 0 <= d < 1; the decay of one update is adjusted as torchvision "
                           "does: 1 - min(1, (1 - d) * world * mini_batch * accum_steps * model_ema_steps / epochs)")

@@ -48,9 +48,9 @@ class FusedBatch(NamedTuple):
     state: Optional[dict] = None    # consumer may set state["event"]: slot is reusable after it fires
     mix: Optional[T.MixDraw] = None     # MixUp / CutMix of this training batch
 
-    def to_float(self, device="cpu", out_hw: int = DATA.crop) -> Tuple[torch.Tensor, torch.Tensor]:
-        """Evaluate the fused transform with torch ops (CPU / oracle path), cut to ``out_hw``."""
-        x = T.augment_reference(self.images_u8.to(device), self.params, self.resized_hw, out_hw=out_hw)
+    def to_float(self, device="cpu", out_hw: int = DATA.crop, view: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Evaluate the fused transform with torch ops (CPU / oracle path), cut to ``out_hw`` (at TTA view ``view``)."""
+        x = T.augment_reference(self.images_u8.to(device), self.params, self.resized_hw, out_hw=out_hw, view=view)
         return x, self.labels.to(device)
 
 
@@ -64,9 +64,10 @@ class RaggedBatch(NamedTuple):
     state: Optional[dict] = None    # consumer may set state["event"]: slot is reusable after it fires
     mix: Optional[T.MixDraw] = None     # MixUp / CutMix of this training batch
 
-    def to_float(self, device="cpu", out_hw: int = DATA.crop) -> Tuple[torch.Tensor, torch.Tensor]:
-        """Evaluate the transform with Pillow's resampling on the CPU (CPU / oracle path), cut to ``out_hw``."""
-        x = T.ragged_reference(self.data_u8, self.geom, self.params, out_hw=out_hw)
+    def to_float(self, device="cpu", out_hw: int = DATA.crop, view: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Evaluate the transform with Pillow's resampling on the CPU (CPU / oracle path), cut to ``out_hw`` (at
+        TTA view ``view``)."""
+        x = T.ragged_reference(self.data_u8, self.geom, self.params, out_hw=out_hw, view=view)
         return x.to(device), self.labels.to(device)
 
 
@@ -345,12 +346,13 @@ class _ReferenceLoader:
 
     def __init__(self, samples, mb: int, train: bool, sampler: Optional[ShardedSampler],
                  shuffle: bool, seed: int, mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0,
-                 resize: int = DATA.resize, crop: int = DATA.crop) -> None:
+                 resize: int = DATA.resize, crop: int = DATA.crop, tta: str = "none") -> None:
         self.samples, self.mb, self.sampler = samples, mb, sampler
         self.crop = crop
         self.shuffle, self.seed, self.epoch = shuffle, seed, 0
         self.mixup_alpha, self.cutmix_alpha = (mixup_alpha, cutmix_alpha) if train else (0.0, 0.0)
-        self.tf = T.reference_transforms(train, resize, crop)
+        self.tf = T.reference_transforms(train, resize, crop) if tta == "none" else \
+            T.reference_transforms(train, resize, crop, tta)
 
     def __len__(self) -> int:
         n = len(self.sampler) if self.sampler is not None else len(self.samples)
@@ -393,12 +395,16 @@ class DataManager:
                  world_size: int = 1, rank: int = 0, pipeline: str = "fused", seed: int = 0,
                  reference_order: bool = False, decode_threads: int = 8, shard_eval: bool = False,
                  mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0, resize_size: int = DATA.resize,
-                 crop_size: int = DATA.crop) -> None:
+                 crop_size: int = DATA.crop, tta: str = "none") -> None:
         """``resize_size`` / ``crop_size``: the split's RandomResizedCrop (train) or Resize (val) size and
         the CenterCrop after it, the network's input (torchvision's --train-crop-size, --val-resize-size,
-        --val-crop-size)."""
+        --val-crop-size).  ``tta`` (validation, --val-tta): the reference pipeline yields every image's views,
+        float32 [mb, V, 3, crop, crop]; fused batches are the same for every mode (their consumer takes the views)."""
         if root_folder is None:
             raise ValueError("-rd/--root_dir is required")
+        T.tta_views(tta)
+        if train and tta != "none":
+            raise ValueError("test-time augmentation applies to validation splits only")
         self.root_folder, self.mb_size, self.train = root_folder, mini_batch, train
         self.resize_size, self.crop_size = int(resize_size), int(crop_size)
         self.path = os.path.join(root_folder, DATA.train_dir if train else DATA.val_dir)
@@ -431,7 +437,7 @@ class DataManager:
         elif pipeline == "reference":
             self.loader = _ReferenceLoader(self.samples, mini_batch, train, sampler, True, seed,
                                            mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha,
-                                           resize=self.resize_size, crop=self.crop_size)
+                                           resize=self.resize_size, crop=self.crop_size, tta=tta)
         else:
             raise ValueError("pipeline must be 'fused', 'reference' or 'auto'")
 

@@ -86,9 +86,50 @@ def resized_dims(train: bool, src_h: int, src_w: int, resize: int = DATA.resize)
     return max(int(resize * src_h / src_w), 1), resize
 
 
+# ------------------------------------------------------------------- test-time augmentation views
+# --val-tta: the views of an evaluation image, each an out_hw x out_hw crop of the Resize(R') image.  A view code
+# is a position (torchvision's five_crop order, then the centre crop's mirror image) or'ed with TTA_FLIP to take
+# the crop from the image's horizontal mirror; csrc/include/api.h (TtaPosition) uses the same codes.
+TTA_TOP_LEFT, TTA_TOP_RIGHT, TTA_BOTTOM_LEFT, TTA_BOTTOM_RIGHT, TTA_CENTRE, TTA_CENTRE_MIRROR = range(6)
+TTA_FLIP = 8
+_FIVE = (TTA_TOP_LEFT, TTA_TOP_RIGHT, TTA_BOTTOM_LEFT, TTA_BOTTOM_RIGHT, TTA_CENTRE)
+TTA_VIEWS = {
+    "none": (TTA_CENTRE,),
+    # the centre crop and its mirror image: hflip(center_crop(img)) is the crop of hflip(img) at the mirrored origin
+    "flip": (TTA_CENTRE, TTA_CENTRE_MIRROR | TTA_FLIP),
+    "five-crop": _FIVE,                                      # torchvision's five_crop
+    "ten-crop": _FIVE + tuple(v | TTA_FLIP for v in _FIVE),  # ten_crop(vertical_flip=False)
+}
+TTA_MODES = tuple(TTA_VIEWS)
+
+
+def tta_views(mode: str) -> Tuple[int, ...]:
+    """The view codes of a --val-tta mode, in the order their probabilities are added."""
+    if mode not in TTA_VIEWS:
+        raise ValueError("val_tta must be one of %s (got %r)" % (", ".join(TTA_MODES), mode))
+    return TTA_VIEWS[mode]
+
+
+def view_origin(view: int, RH: int, RW: int, OH: int, OW: int) -> Tuple[int, int, bool]:
+    """(top, left, mirrored) of view ``view``'s OH x OW crop of an RH x RW image; centre origins round half to
+    even, as torchvision's center_crop."""
+    pos = view & ~TTA_FLIP
+    if not 0 <= pos <= TTA_CENTRE_MIRROR or view < 0:
+        raise ValueError("bad view code %r" % view)
+    if OH > RH or OW > RW:
+        raise ValueError("a %d x %d view does not fit a %d x %d image" % (OH, OW, RH, RW))
+    cy, cx = int(round((RH - OH) / 2.0)), int(round((RW - OW) / 2.0))
+    y0 = {TTA_TOP_LEFT: 0, TTA_TOP_RIGHT: 0, TTA_BOTTOM_LEFT: RH - OH, TTA_BOTTOM_RIGHT: RH - OH}.get(pos, cy)
+    x0 = {TTA_TOP_LEFT: 0, TTA_BOTTOM_LEFT: 0, TTA_TOP_RIGHT: RW - OW, TTA_BOTTOM_RIGHT: RW - OW,
+          TTA_CENTRE_MIRROR: RW - OW - cx}.get(pos, cx)
+    return y0, x0, bool(view & TTA_FLIP)
+
+
 def augment_reference(src: torch.Tensor, params: torch.Tensor, resized_hw: Tuple[int, int],
-                      out_hw: int = DATA.crop, mean=DATA.mean, std=DATA.std) -> torch.Tensor:
-    """Torch evaluation of the fused transform.  src: uint8 [n,H,W,3] -> float32 [n,3,out,out]."""
+                      out_hw: int = DATA.crop, mean=DATA.mean, std=DATA.std, view: Optional[int] = None) -> torch.Tensor:
+    """Torch evaluation of the fused transform.  src: uint8 [n,H,W,3] -> float32 [n,3,out,out].
+    ``view`` (a TTA view code): that view's crop instead of the centre crop, its flip combined with each
+    sample's flip bit."""
     n, H, W, _ = src.shape
     RH, RW = resized_hw
     dev = src.device
@@ -98,9 +139,12 @@ def augment_reference(src: torch.Tensor, params: torch.Tensor, resized_hw: Tuple
     # undo CenterCrop(out_hw) on the RH x RW image (torchvision rounds the offset)
     off_y = int(round((RH - out_hw) / 2.0))
     off_x = int(round((RW - out_hw) / 2.0))
+    vflip = False
+    if view is not None:
+        off_y, off_x, vflip = view_origin(view, RH, RW, out_hw, out_hw)
     ay = (ys + off_y).expand(n, -1, -1)
     ax = (xs + off_x).expand(n, -1, -1)
-    flip = p[:, 6].view(n, 1, 1) > 0.5
+    flip = (p[:, 6].view(n, 1, 1) > 0.5) != vflip
     bx = torch.where(flip, (RW - 1) - ax, ax)
     by = ay
     # undo rotation: PIL affine, output pixel centre -> input coordinate, nearest = floor
@@ -204,12 +248,13 @@ def ragged_geometry(hw, train: bool, resize: int = DATA.resize) -> torch.Tensor:
 
 
 def ragged_reference(data_u8: torch.Tensor, geom: torch.Tensor, params: torch.Tensor,
-                     out_hw: int = DATA.crop, mean=DATA.mean, std=DATA.std) -> torch.Tensor:
+                     out_hw: int = DATA.crop, mean=DATA.mean, std=DATA.std, view: Optional[int] = None) -> torch.Tensor:
     """The reference chain for images of any size, with Pillow's resampling.  data_u8: the flat uint8
     buffer the geometry rows point into; params rows as ``sample_train_params`` / ``val_params``.
     Per image: crop box -> Pillow BILINEAR resize to (RH, RW) -> nearest rotation with zero fill ->
     flip -> centre crop -> normalise (float32, as ToTensor + Normalize).  Val rows (box = the whole
-    image, no rotation, no flip) are Resize + CenterCrop.  -> float32 [k, 3, out_hw, out_hw]."""
+    image, no rotation, no flip) are Resize + CenterCrop.  -> float32 [k, 3, out_hw, out_hw].
+    ``view``: as for ``augment_reference``."""
     n = int(geom.shape[0])
     data = data_u8.cpu()
     out = torch.empty(n, 3, out_hw, out_hw, dtype=torch.float32)
@@ -224,9 +269,12 @@ def ragged_reference(data_u8: torch.Tensor, geom: torch.Tensor, params: torch.Te
         img = data[off:off + H * W * 3].view(H, W, 3)[top:top + ch, left:left + cw]
         res = pil_resize_reference(img.contiguous(), RH, RW)                       # uint8 [RH, RW, 3]
         # the coordinate chain of augment_reference, evaluated in the same float32 operations
-        ay = ys + int(round((RH - out_hw) / 2.0))
-        ax = xs + int(round((RW - out_hw) / 2.0))
-        bx = (RW - 1) - ax if float(p[6]) > 0.5 else ax
+        y0, x0, vflip = int(round((RH - out_hw) / 2.0)), int(round((RW - out_hw) / 2.0)), False
+        if view is not None:
+            y0, x0, vflip = view_origin(view, RH, RW, out_hw, out_hw)
+        ay = ys + y0
+        ax = xs + x0
+        bx = (RW - 1) - ax if (float(p[6]) > 0.5) != vflip else ax
         dx, dy = bx + 0.5 - RW / 2.0, ay + 0.5 - RH / 2.0
         rx = torch.floor(p[4] * dx - p[5] * dy + RW / 2.0)
         ry = torch.floor(p[5] * dx + p[4] * dy + RH / 2.0)
@@ -304,9 +352,11 @@ def mixed_targets(labels: torch.Tensor, num_classes: int, mix: Optional[MixDraw]
     return t.transform(labels, params)
 
 
-def reference_transforms(train: bool, resize: int = DATA.resize, crop: int = DATA.crop):
+def reference_transforms(train: bool, resize: int = DATA.resize, crop: int = DATA.crop, tta: str = "none"):
     """The literal torchvision pipeline of the reference (distributedVggf.py:88-95 / :103-108), with
-    its 256 / 224 made ``resize`` / ``crop`` (--train-crop-size, --val-resize-size, --val-crop-size)."""
+    its 256 / 224 made ``resize`` / ``crop`` (--train-crop-size, --val-resize-size, --val-crop-size).
+    ``tta`` (validation only): Resize, then the mode's views with PIL's FiveCrop / TenCrop (``flip``: the centre
+    crop and its mirror image), each made a tensor and normalised: float32 [V, 3, crop, crop] per image."""
     from torchvision import transforms as T
 
     norm = T.Normalize(list(DATA.mean), list(DATA.std))
@@ -319,7 +369,16 @@ def reference_transforms(train: bool, resize: int = DATA.resize, crop: int = DAT
             T.ToTensor(),
             norm,
         ])
-    return T.Compose([T.Resize(size=resize), T.CenterCrop(size=crop), T.ToTensor(), norm])
+    if tta == "none":
+        return T.Compose([T.Resize(size=resize), T.CenterCrop(size=crop), T.ToTensor(), norm])
+    tta_views(tta)
+    if tta == "flip":
+        from torchvision.transforms import functional as TF
+        views = T.Compose([T.CenterCrop(size=crop), T.Lambda(lambda im: (im, TF.hflip(im)))])
+    else:
+        views = T.FiveCrop(size=crop) if tta == "five-crop" else T.TenCrop(size=crop)
+    return T.Compose([T.Resize(size=resize), views,
+                      T.Lambda(lambda ims: torch.stack([norm(T.functional.to_tensor(im)) for im in ims]))])
 
 
 def torchvision_chain_fixed(img_hwc_u8, params_row, resize: int = DATA.resize, crop: int = DATA.crop) -> torch.Tensor:

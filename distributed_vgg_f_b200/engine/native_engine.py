@@ -30,6 +30,7 @@ import torch.distributed as dist
 
 from .. import ops
 from ..config import DATA, TRAIN
+from ..data import transforms as T
 from ..data.loader import FusedBatch, RaggedBatch
 from ..models import layout as L
 from ..models.vggf import VGGSpec, build_oracle
@@ -159,6 +160,9 @@ def check_native_spec(spec: VGGSpec) -> None:
 
 
 class NativeEngine:
+    # --val-tta (set_val_tta): the views of every evaluation pass, and their [B][C] fp32 probability accumulator
+    val_tta, tta_acc = "none", None
+
     def __init__(self, spec: VGGSpec, device: torch.device, batch: int, lr: float = TRAIN.learning_rate,
                  optimizer: str = "adam", momentum: float = TRAIN.momentum, weight_decay: float = 0.0,
                  compute_dtype: str = "bf16", allreduce: str = "auto", wire_dtype: str = "bf16",
@@ -784,8 +788,9 @@ class NativeEngine:
         self._hw = hw
 
     # ================================================================================ inputs
-    def _stage_input(self, batch) -> int:
-        """Copy a batch to the device and produce the first conv's im2col rows.  Returns b."""
+    def _stage_input(self, batch, views=None) -> int:
+        """Copy a batch to the device and produce the first conv's im2col rows.  Returns b.  ``views`` (TTA view
+        codes): the input of the first view; ``_view_input`` makes the others from the same staged copy."""
         C = ops.require()
         HW = self._hw
         j = self._in_slot
@@ -810,6 +815,9 @@ class NativeEngine:
             if batch.state is not None:
                 batch.state["event"] = h2d          # the loader may refill the pinned slot after this
             cur.wait_event(h2d)
+            if views is not None:
+                self._staged = j
+                return self._view_input(batch, b, 0, views)
             # two passes: transform once per pixel into 8-byte NHWC4 pixels (25 MB at B=64, L2
             # resident), then expand to the first conv's im2col rows with coalesced 16-byte stores
             # MixUp / CutMix in the same pass (sample i with i-1 mod b); without a draw, the plain kernel
@@ -840,6 +848,9 @@ class NativeEngine:
             if batch.state is not None:
                 batch.state["event"] = h2d
             cur.wait_event(h2d)
+            if views is not None:
+                self._staged = j
+                return self._view_input(batch, b, 0, views)
             self._mix = batch.mix
             ops.augment_ragged(self._src_u8[j][:nbytes], self._geom_dev[j][:b], self._params_dev[j][:b],
                                self._inter_u8, self.x_nhwc[:b], batch.geom, batch.params, out_hw=HW,
@@ -852,9 +863,36 @@ class NativeEngine:
             self._mix = batch[2]
         b = int(y.shape[0])
         x = x.to(self.device, F32, non_blocking=True).contiguous()
+        if views is not None:        # the reference pipeline's views: [b][V][3][HW][HW]
+            assert x.dim() == 5 and x.shape[1] == len(views), "the batch does not carry the evaluation's views"
+            self.labels_dev[:b].copy_(y, non_blocking=True)
+            self._staged_x = x
+            return self._view_input(batch, b, 0, views)
         assert x.shape[2] == HW and x.shape[3] == HW, "input size differs from the pass's size (input_hw / eval_hw)"
         self.labels_dev[:b].copy_(y, non_blocking=True)
         C.nchw_to_nhwc(x, self.x_nhwc[:b])
+        if not self.fused_conv0:
+            C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
+        return b
+
+    def _view_input(self, batch, b: int, i: int, views) -> int:
+        """The network input of view ``i`` of ``views`` from the staged batch: one augment launch (a ragged batch's
+        first view also runs the horizontal pass for all of them), or the reference pipeline's view converted."""
+        C = ops.require()
+        HW = self._hw
+        if isinstance(batch, FusedBatch):
+            j = self._staged
+            ops.augment_view(self._src_u8[j][:b], self._params_dev[j][:b], self.x_nhwc[:b], batch.resized_hw,
+                             views[i], out_hw=HW)
+        elif isinstance(batch, RaggedBatch):
+            j, nbytes = self._staged, int(batch.data_u8.numel())
+            ops.augment_ragged_view(self._src_u8[j][:nbytes], self._geom_dev[j][:b], self._params_dev[j][:b],
+                                    self._inter_u8, self.x_nhwc[:b], batch.geom, batch.params, views[i], out_hw=HW,
+                                    pass1=views if i == 0 else ())
+        else:
+            x = self._staged_x[:, i]
+            assert x.shape[2] == HW and x.shape[3] == HW, "input size differs from the evaluation size (eval_hw)"
+            C.nchw_to_nhwc(x.contiguous(), self.x_nhwc[:b])
         if not self.fused_conv0:
             C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
         return b
@@ -1355,12 +1393,54 @@ class NativeEngine:
             torch.cuda.nvtx.range_pop()
         return self.loss_buf
 
+    def set_val_tta(self, mode: str) -> None:
+        """Evaluate with test-time augmentation (``data.transforms.TTA_VIEWS``): every eval_step runs each view of
+        the batch through the network and scores the mean of their softmaxes; forward_logits returns every view's
+        logits.  "none": the single centre crop, as without this call."""
+        T.tta_views(mode)
+        self.val_tta = mode
+        self.tta_acc = None if mode == "none" else torch.empty(self.B, self.spec.num_classes, dtype=F32,
+                                                               device=self.device)
+
+    def _view_logits(self, b: int) -> None:
+        """The forward of the staged view into self.logits[:b] (the fused head's evaluation pass writes them with
+        its metrics in the scratch meter)."""
+        self._forward(b, train=False)
+        if self.fused_head:
+            keep = self.meter
+            self.meter = None
+            self._loss(b, train=False)
+            self.meter = keep
+
+    def _tta_pass(self, batch, keep: Optional[list] = None) -> int:
+        """Stage the batch once, then per view: its augment launch, the forward at batch b and, without ``keep``,
+        the view's step of the reduction (into the meter at the last view).  ``keep``: collect each view's logits
+        instead of reducing them.  Views are looped rather than stacked into a larger batch, so every launch keeps
+        a shape the single-crop pass already makes."""
+        views = T.tta_views(self.val_tta)
+        meter = self.meter.buf if self.meter is not None else self.scratch_meter
+        b = self._stage_input(batch, views)
+        for i in range(len(views)):
+            if i:
+                self._view_input(batch, b, i, views)
+            self._view_logits(b)
+            if keep is not None:
+                keep.append(self.logits[:b].clone())
+            else:
+                ops.tta_accumulate(self.logits[:b], self.labels_dev[:b], self.tta_acc, view=i, views=len(views),
+                                   meter=meter, loss_out=self.loss_buf)
+        return b
+
     def eval_step(self, batch, ema: bool = False) -> torch.Tensor:
         """Evaluation forward, loss and metrics; ``ema``: with the moving average of the weights
-        (after prepare_ema())."""
+        (after prepare_ema()).  With a TTA mode (set_val_tta) the loss and metrics are those of the view mean."""
         self._use_weights(ema)
         self._set_hw(self.eval_hw)
         try:
+            if self.val_tta != "none":
+                self._tta_pass(batch)
+                self._release_input()
+                return self.loss_buf
             b = self._stage_input(batch)
             self._forward(b, train=False)
             self._loss(b, train=False)
@@ -1371,9 +1451,15 @@ class NativeEngine:
         return self.loss_buf
 
     def forward_logits(self, batch, ema: bool = False) -> torch.Tensor:
+        """Logits [b][C] fp32 of an evaluation pass; with a TTA mode (set_val_tta) every view's, [b][V][C]."""
         self._use_weights(ema)
         self._set_hw(self.eval_hw)
         try:
+            if self.val_tta != "none":
+                keep = []
+                self._tta_pass(batch, keep)
+                self._release_input()
+                return torch.stack(keep, 1)
             b = self._stage_input(batch)
             self._forward(b, train=False)
             if self.fused_head:          # the logits come out of the fused head kernel

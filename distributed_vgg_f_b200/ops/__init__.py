@@ -354,6 +354,28 @@ def augment_ragged(data_u8, geom, params, inter, out, geom_host, params_host, ou
     return out
 
 
+def augment_view(src_u8, params, out, resized_hw: Tuple[int, int], view: int, out_hw: int = DATA.crop):
+    """``augment`` (NHWC4) for one test-time augmentation view (``data.transforms.TTA_VIEWS``) of the resized image."""
+    require().augment_view(src_u8, params, out, resized_hw[0], resized_hw[1], out_hw, out_hw, int(view),
+                           list(DATA.mean), list(DATA.std))
+    return out
+
+
+def augment_ragged_view(data_u8, geom, params, inter, out, geom_host, params_host, view: int,
+                        out_hw: int = DATA.crop, pass1=()):
+    """``augment_ragged`` for one view.  ``pass1``: every view of the batch, to run the horizontal pass once for all
+    of them first (its rows and columns are the union of what they read); empty: ``inter`` already holds it."""
+    require().augment_ragged_view(data_u8, geom, params, inter, out, geom_host, params_host, out_hw, out_hw,
+                                  list(DATA.mean), list(DATA.std), int(view), [int(v) for v in pass1])
+    return out
+
+
+def tta_accumulate(logits, target, acc, *, view: int, views: int, meter=None, loss_out=None) -> None:
+    """Add view ``view`` of ``views`` to the view-mean reduction: acc[:B] = softmax(logits) at view 0, += at the
+    later ones; the last view adds (sum of -log(acc[y] / V), count of argmax(acc / V) == y, B) into ``meter``."""
+    require().tta_accumulate(logits, target, acc, meter, loss_out, int(view), int(views))
+
+
 def ragged_inter_bytes(geom_host) -> int:
     """Bytes of the intermediate ``augment_ragged`` needs for these geometry rows."""
     return int(require().ragged_inter_bytes(geom_host))

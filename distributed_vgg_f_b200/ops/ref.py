@@ -493,6 +493,20 @@ def cross_entropy64(logits: torch.Tensor, target: torch.Tensor, *, ldd: int = 0,
     return {"loss": loss, "dlogits": dl, "meter": meter}
 
 
+def tta_reduce64(view_logits: torch.Tensor, target: torch.Tensor):
+    """The --val-tta score of logits [V][B][C], one slice per view, in float64 -> dict with
+    probs [B][C]: mean over the views of softmax(logits); loss: the batch mean of -log probs[y];
+    meter: (loss * B, count of first-maximum argmax(probs) == target, B)."""
+    z = _f64(view_logits)
+    V, B, C = z.shape
+    t = target.to(torch.int64).view(-1)
+    probs = torch.softmax(z, 2).sum(0) / V
+    loss = -torch.log(probs.gather(1, t.view(-1, 1))).mean()
+    correct = float((_first_argmax(probs) == t).sum())
+    meter = torch.tensor([float(loss) * B, correct, float(B)], dtype=torch.float64)
+    return {"probs": probs, "loss": loss, "meter": meter}
+
+
 def kd_cross_entropy64(logits: torch.Tensor, teacher: torch.Tensor, target: torch.Tensor, *, alpha: float,
                        temperature: float, class_weights=None, label_smoothing: float = 0.0, soft_target=None,
                        ldd: int = 0):

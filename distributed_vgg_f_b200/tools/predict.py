@@ -9,6 +9,7 @@ line per image::
     python -m distributed_vgg_f_b200.tools.predict ck.pt --classes edible,other,toy img1.png img2.png
     python -m distributed_vgg_f_b200.tools.predict ck.pt --data-root /data/coil3 /data/coil3/ValidationData/toy
     python -m distributed_vgg_f_b200.tools.predict ck.pt --ema img1.png      # the weights' moving average
+    python -m distributed_vgg_f_b200.tools.predict ck.pt --tta ten-crop img1.png   # mean softmax of ten views
 
 ``--classes`` (or ``--data-root``, whose TrainData sub-folders define them) only names the outputs;
 directories are expanded to the image files inside.  Runs on the GPU through the native engine when
@@ -24,7 +25,7 @@ import torch
 
 from ..config import DATA
 from ..data.folder import IMG_EXTENSIONS, find_classes
-from ..data.transforms import reference_transforms
+from ..data.transforms import TTA_MODES, reference_transforms, tta_views
 from ..models.vggf import build_oracle, get_spec
 from ..utils.checkpoint import strip_module_prefix
 
@@ -66,9 +67,11 @@ def load_model(checkpoint: str, model: Optional[str] = None, num_classes: Option
 
 @torch.no_grad()
 def predict(checkpoint: str, images: Sequence[str], model: Optional[str] = None, engine: str = "auto",
-            batch: int = 32, ema: bool = False, resize: Optional[int] = None, crop: Optional[int] = None):
+            batch: int = 32, ema: bool = False, resize: Optional[int] = None, crop: Optional[int] = None,
+            tta: str = "none"):
     """Returns (logits [n, C] fp32 on the CPU, files).  ``resize`` / ``crop``: the validation transform's
-    sizes (default: the ones recorded in the checkpoint)."""
+    sizes (default: the ones recorded in the checkpoint).  ``tta`` (a --val-tta mode): every view's logits,
+    [n, V, C]."""
     from PIL import Image
 
     spec, state, saved = load_model(checkpoint, model, ema=ema, with_args=True)
@@ -77,7 +80,7 @@ def predict(checkpoint: str, images: Sequence[str], model: Optional[str] = None,
     resize, crop = resize or saved_resize, crop or saved_crop
     if crop > resize:
         raise ValueError("crop %d exceeds resize %d: the crop must lie inside the resized image" % (crop, resize))
-    tf = reference_transforms(False, resize, crop)
+    tf = reference_transforms(False, resize, crop) if tta == "none" else reference_transforms(False, resize, crop, tta)
     from ..engine.native_engine import check_native_hw
 
     def native_runs(hw):
@@ -95,6 +98,8 @@ def predict(checkpoint: str, images: Sequence[str], model: Optional[str] = None,
         from ..engine.native_engine import NativeEngine
         net = NativeEngine(spec, device=torch.device("cuda", 0), batch=batch, init_state=state, distributed=False,
                            input_hw=crop)
+        if tta != "none":
+            net.set_val_tta(tta)
     else:
         net = build_oracle(spec, seed=0).eval()
         net.load_state_dict(state)
@@ -103,9 +108,24 @@ def predict(checkpoint: str, images: Sequence[str], model: Optional[str] = None,
         x = torch.stack([tf(Image.open(f).convert("RGB")) for f in files[i:i + batch]])
         if use_native:
             out.append(net.forward_logits((x, torch.zeros(x.shape[0], dtype=torch.int64))).float().cpu())
+        elif tta != "none":                  # x: [b][V][3][crop][crop]
+            out.append(torch.stack([net(x[:, v]).float() for v in range(x.shape[1])], 1))
         else:
             out.append(net(x).float())
-    return (torch.cat(out) if out else torch.zeros(0, spec.num_classes)), files
+    empty = (0, spec.num_classes) if tta == "none" else (0, len(tta_views(tta)), spec.num_classes)
+    return (torch.cat(out) if out else torch.zeros(empty)), files
+
+
+def mean_probabilities(logits: torch.Tensor) -> torch.Tensor:
+    """Class probabilities of ``predict``'s logits: softmax, or with views ([n, V, C]) the mean of the views'
+    softmaxes added in view order, as --val-tta scores them."""
+    if logits.dim() == 2:
+        return torch.softmax(logits, dim=1)
+    acc = None
+    for v in range(logits.shape[1]):
+        p = torch.softmax(logits[:, v], dim=1)
+        acc = p if acc is None else acc + p
+    return acc / logits.shape[1]
 
 
 def main(argv=None) -> int:
@@ -122,13 +142,16 @@ def main(argv=None) -> int:
                     help="Resize of the shorter side (default: the checkpoint's --val-resize-size, else %d)" % DATA.resize)
     ap.add_argument("--crop", type=int, default=None,
                     help="CenterCrop, the network's input (default: the checkpoint's --val-crop-size, else %d)" % DATA.crop)
+    ap.add_argument("--tta", default="none", choices=list(TTA_MODES),
+                    help="test-time augmentation: classify by the mean softmax of the mode's views, as --val-tta "
+                         "(default: none, the centre crop)")
     a = ap.parse_args(argv)
     logits, files = predict(a.checkpoint, a.images, a.model, a.engine, a.batch, ema=a.ema, resize=a.resize,
-                            crop=a.crop)
+                            crop=a.crop, tta=a.tta)
     names = a.classes.split(",") if a.classes else None
     if names is None and a.data_root:
         names = find_classes(os.path.join(a.data_root, DATA.train_dir))[0]
-    prob = torch.softmax(logits, dim=1)
+    prob = mean_probabilities(logits)
     for f, p in zip(files, prob):
         k = int(p.argmax())
         print("%s\t%s\t%.4f" % (f, names[k] if names and k < len(names) else k, float(p[k])))

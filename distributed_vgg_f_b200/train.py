@@ -131,9 +131,11 @@ def manage_training(args) -> Trainer:
                                   mixup_alpha=getattr(args, "mixup_alpha", 0.0),
                                   cutmix_alpha=getattr(args, "cutmix_alpha", 0.0),
                                   resize_size=sizes["train_resize_size"], crop_size=sizes["train_crop_size"], **dm_kw)
+    val_tta = getattr(args, "val_tta", "none")
     valid_data_mngr = DataManager(args.root_dir, args.mini_batch, train=False,
                                   shard_eval=getattr(args, "shard_eval", False),
-                                  resize_size=sizes["val_resize_size"], crop_size=sizes["val_crop_size"], **dm_kw)
+                                  resize_size=sizes["val_resize_size"], crop_size=sizes["val_crop_size"],
+                                  **dm_kw, **({} if val_tta == "none" else dict(tta=val_tta)))
     train_loader, valid_loader = train_data_mngr.get_loader(), valid_data_mngr.get_loader()
 
     num_classes = args.num_classes or train_data_mngr.number_classes
@@ -143,6 +145,10 @@ def manage_training(args) -> Trainer:
     if sizes != input_sizes(None):
         print("[Info] input sizes: train RandomResizedCrop {} -> crop {}, eval Resize {} -> crop {}".format(
             sizes["train_resize_size"], sizes["train_crop_size"], sizes["val_resize_size"], sizes["val_crop_size"]))
+    if val_tta != "none":
+        from .data.transforms import tta_views
+        print("[Info] test-time augmentation: {} ({} views per image, mean of their softmaxes)".format(
+            val_tta, len(tta_views(val_tta))))
 
     spec = get_spec(args.model, num_classes)
     pretrained = torch.load(args.pretrained, map_location="cpu") if args.pretrained else None
@@ -205,6 +211,8 @@ def manage_training(args) -> Trainer:
                                          eval_crop=sizes["val_crop_size"])
         if optimizer is None:
             model.set_distillation(teacher, args.distill_alpha, args.distill_temperature)
+            if val_tta != "none":
+                teacher.set_val_tta(val_tta)          # its one-time score is taken like the student's
 
     if getattr(args, "eval_only", False) and model_ema is not None and not args.resume:
         raise ValueError("--eval-only --model-ema scores a checkpoint's EMA: pass --resume <checkpoint>")
@@ -249,6 +257,8 @@ def manage_training(args) -> Trainer:
             rec = dict(trainer.history[-1], time=time.time(), world_size=args.world_size)
             if sizes != input_sizes(None):
                 rec["input_sizes"] = sizes
+            if val_tta != "none":
+                rec["val_tta"] = val_tta
             if not schedule.constant:
                 rec["lr"] = epoch_lr
             if hasattr(model, "phase_times"):
@@ -273,12 +283,14 @@ def manage_training(args) -> Trainer:
                       model_ema_steps=getattr(args, "model_ema_steps", 32),
                       teacher=teacher if optimizer is not None else None,
                       distill_alpha=getattr(args, "distill_alpha", 0.5),
-                      distill_temperature=getattr(args, "distill_temperature", 4.0))
+                      distill_temperature=getattr(args, "distill_temperature", 4.0), val_tta=val_tta)
     trainer.profile_timeline = getattr(args, "profile", None) == "timeline"
     if getattr(args, "eval_only", False):        # score a checkpoint: one validation pass, no training
         test_loss, test_acc = trainer._evaluate()
         print("[Info] Evaluation: test loss: {}, test acc: {}.".format(test_loss, test_acc), flush=True)
         rec = dict(epoch=start_epoch - 1, test_loss=test_loss.average, test_acc=test_acc.accuracy)
+        if val_tta != "none":
+            rec["val_tta"] = val_tta
         if model_ema is not None:
             ema_loss, ema_acc = trainer._evaluate(ema=True)
             print("[Info] Evaluation: EMA test loss: {}, EMA test acc: {}.".format(ema_loss, ema_acc), flush=True)

@@ -87,7 +87,7 @@ class Trainer:
                  class_weights: Optional[torch.Tensor] = None, verbose_throughput: bool = True,
                  on_epoch_end=None, shard_eval: bool = False, accum_steps: int = 1,
                  label_smoothing: float = 0.0, model_ema=None, model_ema_steps: int = 32, teacher=None,
-                 distill_alpha: float = 0.5, distill_temperature: float = 4.0) -> None:
+                 distill_alpha: float = 0.5, distill_temperature: float = 4.0, val_tta: str = "none") -> None:
         if accum_steps < 1:
             raise ValueError("accum_steps must be >= 1 (got %d)" % accum_steps)
         if accum_steps > 1 and not hasattr(train_loader, "__len__"):
@@ -115,6 +115,12 @@ class Trainer:
         self.shard_eval = shard_eval
         if self.class_weights is not None and _is_native(model):
             model.set_class_weights(self.class_weights)
+        # --val-tta: every validation pass scores the mean softmax of the mode's views (the native engine loops them
+        # itself once told; the torch path below); training is untouched
+        T.tta_views(val_tta)
+        self.val_tta = val_tta
+        if val_tta != "none" and _is_native(model):
+            model.set_val_tta(val_tta)
         self.history = []
 
     # ------------------------------------------------------------------------------------------
@@ -328,7 +334,24 @@ class Trainer:
         net.eval()
         with torch.no_grad():
             for batch in self.test_loader:
+                if self.val_tta != "none":
+                    meter.add_tta(*self._views_forward(net, batch))
+                    continue
                 inputs, targets = self._to_device(batch, self.test_loader)
                 outputs = net(inputs)
                 meter.add_reference(outputs, targets)
         return self._reduce_eval(meter)
+
+    def _views_forward(self, net, batch):
+        """([logits of each --val-tta view], targets) of a validation batch on the torch path: a fused batch is
+        evaluated at each view, the reference pipeline's [b][V][3][H][W] batch is cut into its views."""
+        views = T.tta_views(self.val_tta)
+        if isinstance(batch, (FusedBatch, RaggedBatch)):
+            crop = getattr(self.test_loader, "crop", DATA.crop)
+            targets = batch.labels.to(self.device)
+            return [net(batch.to_float(self.device, out_hw=crop, view=v)[0]) for v in views], targets
+        x, targets = batch[0].to(self.device, non_blocking=True), batch[1].to(self.device, non_blocking=True)
+        if x.dim() != 5 or x.shape[1] != len(views):
+            raise ValueError("the validation batches do not carry the %s views: build the validation DataManager "
+                             "with tta=%r" % (self.val_tta, self.val_tta))
+        return [net(x[:, i]) for i in range(len(views))], targets

@@ -108,6 +108,20 @@ class DeviceMeter:
             self.buf[1] += logits.argmax(dim=1).eq(target).sum()
             self.buf[2] += logits.shape[0]
 
+    def add_tta(self, view_logits, target: torch.Tensor) -> None:
+        """Torch-op form of the --val-tta reduction (the native engine's tta_accumulate): logits of each view of the
+        batch ([b][C] each, in view order) -> the mean of their fp32 softmaxes, added in view order; a sample's loss
+        is -log of its label's mean probability, and it is correct when the first maximum of the mean is its label."""
+        with torch.no_grad():
+            acc = None
+            for z in view_logits:
+                p = torch.softmax(z.float(), dim=1)
+                acc = p if acc is None else acc + p
+            mean = acc / len(view_logits)
+            self.buf[0] += -torch.log(mean.gather(1, target.view(-1, 1))).sum()
+            self.buf[1] += mean.argmax(dim=1).eq(target).sum()
+            self.buf[2] += mean.shape[0]
+
     def snapshot(self):
         loss_sum, correct, count, _ = self.buf.tolist()
         avg, acc = Average(), Accuracy2()
