@@ -32,6 +32,8 @@ ROLE = [   # (regex on the demangled name, role, what it replaces in the referen
     (r"augment_view_nhwc_kernel", "--val-tta: one view (five-crop corner, centre, or mirror) of the fused transform: uint8 HWC → normalised bf16 NHWC4", "torchvision `FiveCrop` / `TenCrop` after `Resize` — not in the reference"),
     (r"augment_ragged_views_h_kernel", "--val-tta, images of any size: Pillow's horizontal pass once over the union of the rows and columns every view reads", "PIL `Resize` before `TenCrop` — not in the reference"),
     (r"augment_ragged_view_v_kernel", "--val-tta, images of any size: Pillow's vertical pass and the view's crop, per view", "PIL `Resize` + `TenCrop` — not in the reference"),
+    (r"jpeg_idct_kernel", "--pipeline stream: dequantise + JDCT_ISLOW IDCT of every 8×8 coefficient block of the batch into uint8 sample planes, libjpeg's range-limit table", "PIL `Image.open` (libjpeg-turbo IDCT) — `:88-95`, `:103-108`"),
+    (r"jpeg_color_kernel", "--pipeline stream: libjpeg's fancy chroma upsampling and fixed-point YCbCr → RGB, each image at its geometry offset; raw members copied", "PIL `convert(\"RGB\")` (libjpeg-turbo upsampling and colour conversion)"),
     (r"augment_nhwc_kernel|augment_im2col_kernel", "the six PIL transforms as one coordinate chain per output pixel: uint8 HWC → normalised bf16 NHWC4", "PIL / torchvision transforms — `:88-95`, `:103-108`"),
     (r"im2col3x3_c3_kernel|nchw_f32_to_nhwc_bf16_kernel", "input layout conversion for float inputs (tests, `forward_logits`)", "—"),
     (r"adam_kernel", "fused Adam over a bucket: grad (fp32 arena or bf16 wire) → fp32 master, moments, bf16 shadow, gradient range re-zeroed; evict-first streams", "`torch.optim.Adam` foreach kernels + `zero_grad` — `:230`, `:170-172`"),

@@ -8,6 +8,7 @@
 #include <torch/extension.h>
 
 #include "api.h"
+#include "jpeg.h"
 
 namespace py = pybind11;
 using b200::bf16;
@@ -845,7 +846,22 @@ struct PngImage {
 void decode_png_files(const std::vector<std::string>& paths, int threads, std::vector<PngImage>& out);
 void decode_png_files_into(const std::vector<std::string>& paths, int threads, uint8_t* dst, const int64_t* offsets,
                            const int64_t* hw, uint8_t* ok);
+void check_png_files(const std::vector<std::string>& paths, int threads, const int64_t* hw, uint8_t* ok);
 }  // namespace b200
+
+// bool [N]: which files the native PNG decoder takes at their size hw[i] = (H, W) (the stream pipeline's start-up
+// check; the rest go to PIL).
+static at::Tensor png_decodable(const std::vector<std::string>& paths, const at::Tensor& hw, int64_t threads) {
+  const int64_t N = (int64_t)paths.size();
+  TORCH_CHECK(!hw.is_cuda() && hw.scalar_type() == at::kLong && hw.is_contiguous() && hw.numel() == 2 * N,
+              "png_decodable: hw must be a CPU int64 [N, 2] tensor");
+  at::Tensor ok = at::zeros({N}, at::kBool);
+  {
+    py::gil_scoped_release nogil;
+    b200::check_png_files(paths, (int)threads, hw.data_ptr<int64_t>(), reinterpret_cast<uint8_t*>(ok.data_ptr<bool>()));
+  }
+  return ok;
+}
 
 // Ragged splits: decode each file into flat[offsets[i] :] when it is a plain 8-bit PNG of size hw[i].
 // Returns a bool [N] tensor of the files written; the caller decodes the rest with PIL.
@@ -893,6 +909,7 @@ static at::Tensor decode_pngs(const std::vector<std::string>& paths, int64_t thr
 
 // ------------------------------------------------------------------------------- batch prefetcher
 namespace b200 {
+struct StreamConfig;
 struct PrefetchConfig {
   const uint8_t* cache;
   const int64_t* labels;
@@ -907,6 +924,7 @@ struct PrefetchConfig {
   int64_t* ring_geom = nullptr;
   int64_t slot_bytes = 0;
   int resize = 256;
+  const StreamConfig* stream = nullptr;
 };
 class BatchPrefetcher;
 BatchPrefetcher* prefetcher_create(const PrefetchConfig& c);
@@ -1001,6 +1019,248 @@ struct PyPrefetcher {
     b200::prefetcher_stop(p);
   }
 };
+
+// ---------------------------------------------------------------------------------- streaming JPEG input
+namespace b200 {
+struct StreamConfig {
+  std::vector<std::string> paths;
+  std::vector<ImageHeader> headers;
+  const uint8_t* other = nullptr;
+  const int64_t* other_off = nullptr;
+  int16_t* ring_coef = nullptr;
+  int64_t coef_cap = 0;
+  int32_t* ring_quant = nullptr;
+  uint8_t* ring_raw = nullptr;
+  int64_t raw_cap = 0;
+  int32_t* ring_desc = nullptr;
+  int threads = 8;
+};
+}  // namespace b200
+
+// Header rows as jpeg_scan returns them: kind, H, W, sof, ncomp, h0, v0, h1, v1, h2, v2, blocks.
+constexpr int kHeaderCols = 12;
+static void header_row(const b200::ImageHeader& h, int64_t* r) {
+  const int64_t v[kHeaderCols] = {h.kind, h.H, h.W, h.sof, h.ncomp, h.h[0], h.v[0], h.h[1], h.v[1], h.h[2], h.v[2],
+                                  h.blocks};
+  std::copy(v, v + kHeaderCols, r);
+}
+static b200::ImageHeader header_from_row(const int64_t* r) {
+  b200::ImageHeader h;
+  h.kind = (int)r[0]; h.H = (int)r[1]; h.W = (int)r[2]; h.sof = (int)r[3]; h.ncomp = (int)r[4];
+  for (int c = 0; c < 3; ++c) { h.h[c] = (int)r[5 + 2 * c]; h.v[c] = (int)r[6 + 2 * c]; }
+  h.blocks = r[11];
+  return h;
+}
+
+static at::Tensor jpeg_scan(const std::vector<std::string>& paths, int64_t threads) {
+  std::vector<b200::ImageHeader> hs;
+  {
+    py::gil_scoped_release nogil;
+    b200::scan_image_headers(paths, (int)threads, hs);
+  }
+  at::Tensor out = at::empty({(int64_t)paths.size(), kHeaderCols}, at::kLong);
+  for (size_t i = 0; i < hs.size(); ++i) header_row(hs[i], out.data_ptr<int64_t>() + i * kHeaderCols);
+  return out;
+}
+
+static void check_header_rows(const at::Tensor& headers, int64_t N, const char* op) {
+  TORCH_CHECK(!headers.is_cuda() && headers.scalar_type() == at::kLong && headers.is_contiguous() &&
+                  headers.dim() == 2 && headers.size(0) == N && headers.size(1) == kHeaderCols,
+              op, ": headers must be jpeg_scan's CPU int64 [N, ", kHeaderCols, "] rows");
+}
+
+// One stream-JPEG file's quantised coefficients int16 [blocks, 64] and its components' tables int32 [ncomp, 64].
+static std::tuple<at::Tensor, at::Tensor> jpeg_entropy_decode(const std::string& path, const at::Tensor& header) {
+  check_header_rows(header.view({1, -1}), 1, "jpeg_entropy_decode");
+  const b200::ImageHeader h = header_from_row(header.data_ptr<int64_t>());
+  TORCH_CHECK(h.kind == b200::kFileJpeg, "jpeg_entropy_decode: ", path, " is not a file the stream decoder takes");
+  at::Tensor coef = at::empty({h.blocks, 64}, at::kShort);
+  at::Tensor quant = at::zeros({h.ncomp, 64}, at::kInt);
+  {
+    py::gil_scoped_release nogil;
+    b200::jpeg_entropy_decode(path, h, coef.data_ptr<int16_t>(), quant.data_ptr<int32_t>());
+  }
+  return {coef, quant};
+}
+
+// The stream pipeline's prefetcher: BatchPrefetcher over a split that is never cached.  Its ring: ring_geom,
+// ring_par, ring_lab as for a ragged split, and per slot ring_coef int16 [coef_cap], ring_quant int32
+// [mb * 3][64], ring_raw uint8 [raw_cap] and ring_desc int32 [mb][kJpegDesc].  `other` holds the RGB of the
+// files PIL decoded at start-up, file i at other_off[i] (-1 for the files decoded per batch).
+struct PyStreamPrefetcher {
+  b200::BatchPrefetcher* p = nullptr;
+  b200::StreamConfig sc;
+  at::Tensor labels, hw, other, other_off, ring_coef, ring_quant, ring_raw, ring_desc, ring_geom, ring_par, ring_lab;
+  PyStreamPrefetcher(std::vector<std::string> paths, const at::Tensor& headers, at::Tensor labels_, at::Tensor hw_,
+                     at::Tensor other_, at::Tensor other_off_, at::Tensor ring_coef_, at::Tensor ring_quant_,
+                     at::Tensor ring_raw_, at::Tensor ring_desc_, at::Tensor ring_geom_, at::Tensor ring_par_,
+                     at::Tensor ring_lab_, bool train, double scale_lo, double scale_hi, double ratio_lo,
+                     double ratio_hi, double degrees, int64_t resize, int64_t threads)
+      : labels(labels_), hw(hw_), other(other_), other_off(other_off_), ring_coef(ring_coef_), ring_quant(ring_quant_),
+        ring_raw(ring_raw_), ring_desc(ring_desc_), ring_geom(ring_geom_), ring_par(ring_par_), ring_lab(ring_lab_) {
+    const int64_t N = (int64_t)paths.size();
+    check_header_rows(headers, N, "StreamPrefetcher");
+    auto cpu = [](const at::Tensor& t, at::ScalarType dt) { return !t.is_cuda() && t.scalar_type() == dt && t.is_contiguous(); };
+    TORCH_CHECK(cpu(labels, at::kLong) && labels.numel() == N && cpu(hw, at::kLong) && hw.numel() == 2 * N &&
+                    cpu(other, at::kByte) && cpu(other_off, at::kLong) && other_off.numel() == N,
+                "StreamPrefetcher: labels int64 [N], hw int64 [N, 2], other uint8, other_off int64 [N]");
+    TORCH_CHECK(cpu(ring_par, at::kFloat) && ring_par.dim() == 3 && ring_par.size(2) == 8 && cpu(ring_lab, at::kLong) &&
+                    ring_lab.dim() == 2 && ring_lab.sizes() == ring_par.sizes().slice(0, 2),
+                "StreamPrefetcher: ring_par [slots][mb][8] and ring_lab [slots][mb]");
+    const int64_t slots = ring_par.size(0), mb = ring_par.size(1);
+    TORCH_CHECK(cpu(ring_geom, at::kLong) && ring_geom.dim() == 3 && ring_geom.size(0) == slots &&
+                    ring_geom.size(1) == mb && ring_geom.size(2) == 5, "StreamPrefetcher: ring_geom int64 [slots][mb][5]");
+    TORCH_CHECK(cpu(ring_coef, at::kShort) && ring_coef.dim() == 2 && ring_coef.size(0) == slots &&
+                    cpu(ring_raw, at::kByte) && ring_raw.dim() == 2 && ring_raw.size(0) == slots &&
+                    cpu(ring_quant, at::kInt) && ring_quant.dim() == 3 && ring_quant.size(0) == slots &&
+                    ring_quant.size(1) == mb * 3 && ring_quant.size(2) == 64 && cpu(ring_desc, at::kInt) &&
+                    ring_desc.dim() == 3 && ring_desc.size(0) == slots && ring_desc.size(1) == mb &&
+                    ring_desc.size(2) == b200::kJpegDesc,
+                "StreamPrefetcher: ring_coef int16 [slots][cap], ring_raw uint8 [slots][cap], ring_quant int32 "
+                "[slots][mb*3][64], ring_desc int32 [slots][mb][", b200::kJpegDesc, "]");
+    const int64_t* hr = headers.data_ptr<int64_t>();
+    const int64_t* s = hw.data_ptr<int64_t>();
+    const int64_t* oo = other_off.data_ptr<int64_t>();
+    std::vector<int64_t> coef_sizes, raw_sizes;
+    sc.paths = std::move(paths);
+    sc.headers.resize(N);
+    for (int64_t i = 0; i < N; ++i) {
+      const b200::ImageHeader h = header_from_row(hr + i * kHeaderCols);
+      sc.headers[i] = h;
+      const int64_t H = s[2 * i], W = s[2 * i + 1];
+      TORCH_CHECK(H >= 1 && W >= 1 && H <= 65535 && W <= 65535, "StreamPrefetcher: image ", i, " has size ", H, " x ", W);
+      if (h.kind == b200::kFileOther) {
+        TORCH_CHECK(oo[i] >= 0 && oo[i] + H * W * 3 <= other.numel(), "StreamPrefetcher: image ", i,
+                    " lies outside the start-up cache");
+      } else {
+        TORCH_CHECK(h.H == H && h.W == W, "StreamPrefetcher: image ", i, "'s size differs from its header");
+      }
+      if (h.kind == b200::kFileJpeg) {
+        int64_t want = 0;
+        for (int c = 0; c < h.ncomp; ++c) {
+          int bw, bh;
+          b200::jpeg_block_grid(h, c, bw, bh);
+          want += (int64_t)bw * bh;
+        }
+        TORCH_CHECK(h.blocks == want && (h.ncomp == 1 || h.ncomp == 3), "StreamPrefetcher: image ", i,
+                    " has an inconsistent header row");
+        coef_sizes.push_back(h.blocks * 64);
+      } else {
+        raw_sizes.push_back(H * W * 3);
+      }
+    }
+    // a slot must hold any batch: the coefficients of the mb largest JPEGs and the RGB of the mb largest others
+    for (auto* v : {&coef_sizes, &raw_sizes}) std::sort(v->begin(), v->end(), std::greater<int64_t>());
+    int64_t coef_need = 0, raw_need = 0, blocks_need = 0;
+    for (int64_t i = 0; i < std::min<int64_t>(mb, coef_sizes.size()); ++i) coef_need += coef_sizes[i];
+    for (int64_t i = 0; i < std::min<int64_t>(mb, raw_sizes.size()); ++i) raw_need += raw_sizes[i];
+    blocks_need = coef_need / 64;
+    TORCH_CHECK(ring_coef.size(1) >= coef_need && ring_raw.size(1) >= raw_need && blocks_need < (1ll << 31) &&
+                    raw_need < (1ll << 31), "StreamPrefetcher: a slot of ", ring_coef.size(1), " coefficients and ",
+                ring_raw.size(1), " raw bytes cannot hold ", coef_need, " and ", raw_need);
+    sc.other = other.data_ptr<uint8_t>(); sc.other_off = oo;
+    sc.ring_coef = ring_coef.data_ptr<int16_t>(); sc.coef_cap = ring_coef.size(1);
+    sc.ring_quant = ring_quant.data_ptr<int32_t>();
+    sc.ring_raw = ring_raw.data_ptr<uint8_t>(); sc.raw_cap = ring_raw.size(1);
+    sc.ring_desc = ring_desc.data_ptr<int32_t>();
+    sc.threads = (int)std::max<int64_t>(1, threads);
+    b200::PrefetchConfig c;
+    c.cache = nullptr; c.labels = labels.data_ptr<int64_t>();
+    c.H = 0; c.W = 0; c.mb = (int)mb; c.slots = (int)slots;
+    c.ring_img = nullptr; c.ring_par = ring_par.data_ptr<float>(); c.ring_lab = ring_lab.data_ptr<int64_t>();
+    c.train = train; c.scale_lo = (float)scale_lo; c.scale_hi = (float)scale_hi;
+    c.ratio_lo = (float)ratio_lo; c.ratio_hi = (float)ratio_hi; c.degrees = (float)degrees;
+    c.hw = s; c.ring_geom = ring_geom.data_ptr<int64_t>(); c.resize = (int)resize;
+    c.stream = &sc;
+    p = b200::prefetcher_create(c);
+  }
+  ~PyStreamPrefetcher() { if (p) b200::prefetcher_destroy(p); }
+  void start(std::vector<int64_t> idx, uint64_t seed) {
+    for (int64_t i : idx) TORCH_CHECK(i >= 0 && i < (int64_t)sc.paths.size(), "StreamPrefetcher: index ", i, " out of range");
+    py::gil_scoped_release nogil;
+    b200::prefetcher_start(p, std::move(idx), seed);
+  }
+  py::object next() {
+    int slot = -1, count = 0;
+    bool ok;
+    {
+      py::gil_scoped_release nogil;
+      ok = b200::prefetcher_next(p, slot, count);
+    }
+    if (!ok) return py::none();
+    return py::make_tuple(slot, count);
+  }
+  void release(int64_t slot, uint64_t ev) { b200::prefetcher_release(p, (int)slot, ev); }
+  void stop() {
+    py::gil_scoped_release nogil;
+    b200::prefetcher_stop(p);
+  }
+};
+
+// The device decode of a stream batch.  The kernels read desc and geom on the device; the host copies they were
+// made from are checked here, so that no row can send a launch outside coef, quant, raw, planes or out.
+static void jpeg_decode(const at::Tensor& coef, const at::Tensor& quant, const at::Tensor& desc, const at::Tensor& geom,
+                        const at::Tensor& raw, at::Tensor planes, at::Tensor out, const at::Tensor& desc_host,
+                        const at::Tensor& geom_host) {
+  c10::cuda::CUDAGuard g(out.device());
+  auto dev = [](const at::Tensor& t, at::ScalarType dt) { return t.is_cuda() && t.scalar_type() == dt && t.is_contiguous(); };
+  TORCH_CHECK(dev(desc, at::kInt) && desc.dim() == 2 && desc.size(1) == b200::kJpegDesc,
+              "jpeg_decode: desc must be a contiguous CUDA int32 [k, ", b200::kJpegDesc, "] tensor");
+  const int64_t k = desc.size(0);
+  TORCH_CHECK(k >= 1 && k <= 65535, "jpeg_decode: 1 to 65535 images");
+  TORCH_CHECK(dev(geom, at::kLong) && geom.dim() == 2 && geom.size(0) == k && geom.size(1) == 5,
+              "jpeg_decode: geom must be a contiguous CUDA int64 [k, 5] tensor");
+  TORCH_CHECK(!desc_host.is_cuda() && desc_host.scalar_type() == at::kInt && desc_host.is_contiguous() &&
+                  desc_host.sizes() == desc.sizes(), "jpeg_decode: desc_host must be the CPU int32 copy of desc");
+  TORCH_CHECK(!geom_host.is_cuda() && geom_host.scalar_type() == at::kLong && geom_host.is_contiguous() &&
+                  geom_host.sizes() == geom.sizes(), "jpeg_decode: geom_host must be the CPU int64 copy of geom");
+  TORCH_CHECK(dev(coef, at::kShort) && dev(quant, at::kInt) && quant.dim() == 2 && quant.size(1) == 64 &&
+                  dev(raw, at::kByte) && dev(planes, at::kByte) && dev(out, at::kByte),
+              "jpeg_decode: coef int16, quant int32 [rows, 64], raw, planes and out uint8, all contiguous CUDA tensors");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(planes.data_ptr()) % 8 == 0, "jpeg_decode: planes must be 8-byte aligned");
+  for (const at::Tensor* t : std::initializer_list<const at::Tensor*>{&coef, &quant, &desc, &geom, &raw, &planes})
+    TORCH_CHECK(t->device() == out.device(), "jpeg_decode: every operand on out's device");
+  const int32_t* d = desc_host.data_ptr<int32_t>();
+  const int64_t* gh = geom_host.data_ptr<int64_t>();
+  int64_t blocks = 0, most = 1;
+  for (int64_t i = 0; i < k; ++i) {
+    const int32_t* r = d + i * b200::kJpegDesc;
+    const int64_t off = gh[i * 5], H = gh[i * 5 + 1], W = gh[i * 5 + 2];
+    TORCH_CHECK(H >= 1 && W >= 1 && H <= 65535 && W <= 65535 && off >= 0 && off + H * W * 3 <= out.numel(),
+                "jpeg_decode: image ", i, " (offset ", off, ", ", H, " x ", W, ") lies outside out of ", out.numel(),
+                " bytes");
+    TORCH_CHECK(r[3] == blocks, "jpeg_decode: image ", i, " starts at block ", r[3], ", the batch is at ", blocks);
+    most = std::max(most, H * W);
+    const int n = r[0];
+    if (n == 0) {
+      TORCH_CHECK(r[4] >= 0 && r[4] + H * W * 3 <= raw.numel(), "jpeg_decode: image ", i, " lies outside raw");
+      continue;
+    }
+    b200::ImageHeader h;
+    h.H = (int)H; h.W = (int)W; h.ncomp = n;
+    h.h[0] = r[1]; h.v[0] = r[2]; h.h[1] = h.v[1] = h.h[2] = h.v[2] = 1;
+    const bool sampling = n == 1 ? r[1] == 1 && r[2] == 1
+                                 : (r[1] == 1 && r[2] == 1) || (r[1] == 2 && r[2] == 1) || (r[1] == 2 && r[2] == 2);
+    TORCH_CHECK((n == 1 || n == 3) && sampling, "jpeg_decode: image ", i, " has ", n, " components sampled ", r[1],
+                "x", r[2]);
+    for (int c = 0; c < n; ++c) {
+      int bw, bh;
+      b200::jpeg_block_grid(h, c, bw, bh);
+      TORCH_CHECK(r[5 + c] == bw && r[8 + c] == bh, "jpeg_decode: image ", i, " component ", c, " has a ", r[5 + c],
+                  " x ", r[8 + c], " block grid, its geometry needs ", bw, " x ", bh);
+      TORCH_CHECK(r[11 + c] >= 0 && r[11 + c] < quant.size(0), "jpeg_decode: image ", i, " component ", c,
+                  " reads quantisation row ", r[11 + c], " of ", quant.size(0));
+      blocks += (int64_t)bw * bh;
+    }
+  }
+  TORCH_CHECK(blocks * 64 <= coef.numel() && blocks * 64 <= planes.numel(), "jpeg_decode: ", blocks,
+              " blocks do not fit coef (", coef.numel(), ") or planes (", planes.numel(), ")");
+  const int64_t cap = std::max<int64_t>(1, 16 * b200::sm_count() / k);
+  const int grid_x = (int)std::min(cap, (most + 255) / 256);
+  b200::jpeg_decode(coef.data_ptr<int16_t>(), quant.data_ptr<int32_t>(), desc.data_ptr<int32_t>(),
+                    reinterpret_cast<const long long*>(geom.data_ptr<int64_t>()), raw.data_ptr<uint8_t>(),
+                    planes.data_ptr<uint8_t>(), out.data_ptr<uint8_t>(), (int)k, blocks, grid_x, cur_stream());
+}
 
 // ------------------------------------------------------------------------------------------- comm
 // The collectives write into every peer's wire buffer and signal pad: a range past the wire or a slot
@@ -1244,6 +1504,25 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("next", &PyPrefetcher::next)
       .def("release", &PyPrefetcher::release)
       .def("stop", &PyPrefetcher::stop);
+  m.def("jpeg_scan", &jpeg_scan, py::arg("paths"), py::arg("threads"));
+  m.def("png_decodable", &png_decodable, py::arg("paths"), py::arg("hw"), py::arg("threads"));
+  m.def("jpeg_entropy_decode", &jpeg_entropy_decode, py::arg("path"), py::arg("header"));
+  m.def("jpeg_decode", &jpeg_decode, py::arg("coef"), py::arg("quant"), py::arg("desc"), py::arg("geom"), py::arg("raw"),
+        py::arg("planes"), py::arg("out"), py::arg("desc_host"), py::arg("geom_host"));
+  m.attr("JPEG_DESC") = b200::kJpegDesc;
+  py::class_<PyStreamPrefetcher>(m, "StreamPrefetcher")
+      .def(py::init<std::vector<std::string>, const at::Tensor&, at::Tensor, at::Tensor, at::Tensor, at::Tensor,
+                    at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, at::Tensor, bool, double,
+                    double, double, double, double, int64_t, int64_t>(),
+           py::arg("paths"), py::arg("headers"), py::arg("labels"), py::arg("hw"), py::arg("other"),
+           py::arg("other_off"), py::arg("ring_coef"), py::arg("ring_quant"), py::arg("ring_raw"),
+           py::arg("ring_desc"), py::arg("ring_geom"), py::arg("ring_par"), py::arg("ring_lab"), py::arg("train"),
+           py::arg("scale_lo"), py::arg("scale_hi"), py::arg("ratio_lo"), py::arg("ratio_hi"), py::arg("degrees"),
+           py::arg("resize"), py::arg("threads"))
+      .def("start", &PyStreamPrefetcher::start)
+      .def("next", &PyStreamPrefetcher::next)
+      .def("release", &PyStreamPrefetcher::release)
+      .def("stop", &PyStreamPrefetcher::stop);
   py::class_<PyComm>(m, "Comm");
   m.def("probe_background", [](at::Tensor buf, int64_t mode, int64_t ctas, int64_t reps, at::Tensor sink) {
     b200::probe_background(f32p(buf), buf.numel(), (int)mode, (int)ctas, (int)reps, f32p(sink), cur_stream());

@@ -360,6 +360,12 @@ void augment_ragged_view(const uint8_t* src, const long long* geom, const float*
 // of argmax(acc / V) == y (lowest index on ties) and B into meter, and writes the mean loss to loss_out.
 void tta_accumulate(const float* logits, const long long* target, float* acc, float* meter,
                     float* loss_out, int B, int C, int view, int views, cudaStream_t s);
+// ---- streaming JPEG decode (jpeg.cu, --pipeline stream) ------------------------------------------
+// A batch of k images described by desc [k][kJpegDesc] (jpeg.h) and geom [k][5] rows as augment_ragged's:
+// dequantise + IDCT the total_blocks coefficient blocks into planes (total_blocks x 64 bytes), then write each
+// image's RGB at out + geom offset (raw members copied from raw).  grid_x: blocks per image of the second launch.
+void jpeg_decode(const int16_t* coef, const int* quant, const int* desc, const long long* geom, const uint8_t* raw,
+                 uint8_t* planes, uint8_t* out, int k, long long total_blocks, int grid_x, cudaStream_t s);
 
 // im2col of an NHWC(3, padded to cpad) bf16 image for layer 0 (used when the input is given as a
 // float tensor instead of uint8 + params).

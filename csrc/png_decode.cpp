@@ -117,6 +117,14 @@ static bool decode_one(const std::string& path, PngImage& out) {
   return true;
 }
 
+bool decode_png_file(const std::string& path, PngImage& out) {
+  try {
+    return decode_one(path, out);
+  } catch (...) {            // e.g. bad_alloc on a corrupt header
+    return false;
+  }
+}
+
 // Decode all files with `threads` workers.  Returns false for files this decoder does not handle.
 void decode_png_files(const std::vector<std::string>& paths, int threads, std::vector<PngImage>& out) {
   out.assign(paths.size(), PngImage());
@@ -156,6 +164,23 @@ void decode_png_files_into(const std::vector<std::string>& paths, int threads, u
         }
       } catch (...) {            // not handled here: PIL decodes this file
       }
+    }
+  };
+  if (threads < 1) threads = 1;
+  std::vector<std::thread> pool;
+  for (int t = 0; t < threads; ++t) pool.emplace_back(work);
+  for (auto& t : pool) t.join();
+}
+
+// ok[i]: file i is a PNG this decoder takes, of size hw[i] = (H, W).  Each file is decoded and dropped.
+void check_png_files(const std::vector<std::string>& paths, int threads, const int64_t* hw, uint8_t* ok) {
+  std::atomic<size_t> next{0};
+  auto work = [&]() {
+    for (;;) {
+      const size_t i = next.fetch_add(1);
+      if (i >= paths.size()) return;
+      PngImage img;
+      ok[i] = decode_png_file(paths[i], img) && img.h == hw[i * 2] && img.w == hw[i * 2 + 1];
     }
   };
   if (threads < 1) threads = 1;

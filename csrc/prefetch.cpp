@@ -5,6 +5,11 @@
 // thread that launches the training step (a Python producer thread does: with the GIL's 5 ms switch
 // interval the launch loop of a training step is held up).
 //
+// Stream splits (PrefetchConfig::stream): nothing is cached.  The worker lays each batch out in the slot (every
+// JPEG's coefficient blocks, every other image's raw RGB, one descriptor row each, csrc/include/jpeg.h) and a pool
+// of decode threads fills those fixed positions, so a slot's content does not depend on the thread count or on
+// timing.  A failed decode ends the epoch: next() raises the error once the batches before it are consumed.
+//
 // Slot life cycle:  free -> (worker fills) -> ready -> (consumer: next()) -> in use ->
 // (consumer: release(slot, cuda_event)) -> free; the worker cudaEventSynchronize()s the event the
 // consumer recorded after its host->device copy before it overwrites the slot.
@@ -16,12 +21,99 @@
 #include <cstring>
 #include <algorithm>
 #include <deque>
+#include <memory>
+#include <functional>
 #include <mutex>
 #include <random>
+#include <stdexcept>
+#include <string>
 #include <thread>
 #include <vector>
 
+#include "jpeg.h"
+
 namespace b200 {
+
+struct PngImage {
+  int w = 0, h = 0;
+  std::vector<uint8_t> rgb;
+  bool ok = false;
+};
+bool decode_png_file(const std::string& path, PngImage& out);
+
+// The files of a stream split and the slot arrays their batches are decoded into.
+struct StreamConfig {
+  std::vector<std::string> paths;
+  std::vector<ImageHeader> headers;
+  const uint8_t* other = nullptr;        // files PIL decoded at start-up: RGB at other + other_off[i]
+  const int64_t* other_off = nullptr;    // -1: not such a file
+  int16_t* ring_coef = nullptr;          // [slots][coef_cap]
+  int64_t coef_cap = 0;
+  int32_t* ring_quant = nullptr;         // [slots][mb * 3][64]
+  uint8_t* ring_raw = nullptr;           // [slots][raw_cap]
+  int64_t raw_cap = 0;
+  int32_t* ring_desc = nullptr;          // [slots][mb][kJpegDesc]
+  int threads = 8;
+};
+
+// fn(i) for i in [0, n) on a fixed set of threads; run() returns the first error's message ("" if none).
+class DecodePool {
+ public:
+  explicit DecodePool(int n) {
+    for (int t = 0; t < std::max(n, 1); ++t) threads_.emplace_back([this] { loop(); });
+  }
+  ~DecodePool() {
+    {
+      std::lock_guard<std::mutex> lk(mu_);
+      quit_ = true;
+    }
+    cv_work_.notify_all();
+    for (auto& t : threads_) t.join();
+  }
+  std::string run(int n, const std::function<void(int)>& fn) {
+    std::unique_lock<std::mutex> lk(mu_);
+    fn_ = &fn;
+    n_ = n;
+    next_ = done_ = 0;
+    err_.clear();
+    ++gen_;
+    cv_work_.notify_all();
+    cv_done_.wait(lk, [this] { return done_ == n_; });
+    return err_;
+  }
+
+ private:
+  void loop() {
+    uint64_t seen = 0;
+    std::unique_lock<std::mutex> lk(mu_);
+    for (;;) {
+      cv_work_.wait(lk, [&] { return quit_ || gen_ != seen; });
+      if (quit_) return;
+      seen = gen_;
+      while (next_ < n_) {
+        const int i = next_++;
+        lk.unlock();
+        std::string e;
+        try {
+          (*fn_)(i);
+        } catch (const std::exception& x) {
+          e = x.what();
+        }
+        lk.lock();
+        if (!e.empty() && err_.empty()) err_ = e;
+        if (++done_ == n_) cv_done_.notify_all();
+      }
+    }
+  }
+  std::vector<std::thread> threads_;
+  std::mutex mu_;
+  std::condition_variable cv_work_, cv_done_;
+  const std::function<void(int)>* fn_ = nullptr;
+  int n_ = 0, next_ = 0, done_ = 0;
+  uint64_t gen_ = 0;
+  bool quit_ = false;
+  std::string err_;
+};
 
 struct PrefetchConfig {
   const uint8_t* cache;      // [N][H][W][3]
@@ -40,6 +132,8 @@ struct PrefetchConfig {
   int64_t* ring_geom = nullptr;
   int64_t slot_bytes = 0;
   int resize = 256;
+  // stream splits: hw and ring_geom as above, no cache or offsets
+  const StreamConfig* stream = nullptr;
 };
 
 class BatchPrefetcher {
@@ -55,6 +149,7 @@ class BatchPrefetcher {
       std::lock_guard<std::mutex> lk(mu_);
       indices_ = std::move(indices);
       ready_.clear();
+      error_.clear();
       done_ = false;
       quit_ = false;
       free_.clear();
@@ -68,7 +163,10 @@ class BatchPrefetcher {
   bool next(int& slot, int& count) {
     std::unique_lock<std::mutex> lk(mu_);
     cv_ready_.wait(lk, [this] { return !ready_.empty() || done_; });
-    if (ready_.empty()) return false;
+    if (ready_.empty()) {
+      if (!error_.empty()) throw std::runtime_error(error_);
+      return false;
+    }
     slot = ready_.front().first;
     count = ready_.front().second;
     ready_.pop_front();
@@ -133,6 +231,8 @@ class BatchPrefetcher {
     const PrefetchConfig& c = cfg_;
     const size_t img_bytes = (size_t)c.H * c.W * 3;
     const size_t n = indices_.size();
+    std::unique_ptr<DecodePool> pool;
+    if (c.stream) pool.reset(new DecodePool(c.stream->threads));
     for (size_t b0 = 0; b0 < n; b0 += c.mb) {
       int slot;
       cudaEvent_t ev;
@@ -155,7 +255,7 @@ class BatchPrefetcher {
       uint8_t* img = c.ring_img + (size_t)slot * c.mb * img_bytes;
       float* par = c.ring_par + (size_t)slot * c.mb * 8;
       int64_t* lab = c.ring_lab + (size_t)slot * c.mb;
-      if (c.offsets) {
+      if (c.hw) {
         uint8_t* bytes = c.ring_img + (size_t)slot * c.slot_bytes;
         int64_t* geom = c.ring_geom + (size_t)slot * c.mb * 5;
         int64_t at = 0;
@@ -163,7 +263,7 @@ class BatchPrefetcher {
           const int64_t src = indices_[b0 + i];
           const int H = (int)c.hw[src * 2], W = (int)c.hw[src * 2 + 1];
           const size_t n = (size_t)H * W * 3;
-          std::memcpy(bytes + at, c.cache + c.offsets[src], n);
+          if (c.offsets) std::memcpy(bytes + at, c.cache + c.offsets[src], n);
           int64_t* g = geom + (size_t)i * 5;
           g[0] = at; g[1] = H; g[2] = W;
           if (c.train) { g[3] = c.resize; g[4] = c.resize; }         // data/transforms.py::resized_dims
@@ -172,6 +272,18 @@ class BatchPrefetcher {
           at += (int64_t)n;
           lab[i] = c.labels[src];
           sample_params(par + (size_t)i * 8, H, W);
+        }
+        if (c.stream) {
+          const std::string err = fill_stream(*pool, slot, &indices_[b0], k);
+          if (!err.empty()) {
+            {
+              std::lock_guard<std::mutex> lk(mu_);
+              error_ = err;
+              done_ = true;
+            }
+            cv_ready_.notify_all();
+            return;
+          }
         }
       } else {
         for (int i = 0; i < k; ++i) {
@@ -194,6 +306,54 @@ class BatchPrefetcher {
     cv_ready_.notify_all();
   }
 
+  // Lays the batch idx[0..k) out in the slot's stream arrays and decodes it on the pool.
+  std::string fill_stream(DecodePool& pool, int slot, const int64_t* idx, int k) {
+    const StreamConfig& s = *cfg_.stream;
+    const int mb = cfg_.mb;
+    int16_t* coef = s.ring_coef + (size_t)slot * s.coef_cap;
+    int32_t* quant = s.ring_quant + (size_t)slot * mb * 3 * 64;
+    uint8_t* raw = s.ring_raw + (size_t)slot * s.raw_cap;
+    int32_t* desc = s.ring_desc + (size_t)slot * mb * kJpegDesc;
+    int64_t blk = 0, at = 0;
+    for (int i = 0; i < k; ++i) {
+      const ImageHeader& h = s.headers[idx[i]];
+      int32_t* d = desc + (size_t)i * kJpegDesc;
+      std::fill(d, d + kJpegDesc, 0);
+      d[3] = (int32_t)blk;
+      if (h.kind == kFileJpeg) {
+        d[0] = h.ncomp;
+        d[1] = h.ncomp == 3 ? h.h[0] : 1;
+        d[2] = h.ncomp == 3 ? h.v[0] : 1;
+        for (int c = 0; c < h.ncomp; ++c) {
+          jpeg_block_grid(h, c, d[5 + c], d[8 + c]);
+          d[11 + c] = i * 3 + c;
+        }
+        blk += h.blocks;
+      } else {
+        const int64_t* hw = cfg_.hw + 2 * idx[i];
+        d[4] = (int32_t)at;
+        at += hw[0] * hw[1] * 3;
+      }
+    }
+    if (blk * 64 > s.coef_cap || at > s.raw_cap) return "stream prefetcher: a batch does not fit its slot";
+    return pool.run(k, [&](int i) {
+      const int64_t src = idx[i];
+      const ImageHeader& h = s.headers[src];
+      const int32_t* d = desc + (size_t)i * kJpegDesc;
+      const int64_t H = cfg_.hw[2 * src], W = cfg_.hw[2 * src + 1];
+      if (h.kind == kFileJpeg) {
+        jpeg_entropy_decode(s.paths[src], h, coef + (int64_t)d[3] * 64, quant + (size_t)i * 3 * 64);
+      } else if (h.kind == kFilePng) {
+        PngImage img;
+        if (!decode_png_file(s.paths[src], img) || img.h != H || img.w != W)
+          throw std::runtime_error(s.paths[src] + ": PNG decode failed or its size changed since the header scan");
+        std::memcpy(raw + d[4], img.rgb.data(), img.rgb.size());
+      } else {
+        std::memcpy(raw + d[4], s.other + s.other_off[src], (size_t)(H * W * 3));
+      }
+    });
+  }
+
   PrefetchConfig cfg_;
   std::vector<int64_t> indices_;
   std::deque<int> free_;
@@ -204,6 +364,7 @@ class BatchPrefetcher {
   std::thread worker_;
   std::mt19937_64 rng_;
   bool done_ = false, quit_ = false;
+  std::string error_;
 };
 
 BatchPrefetcher* prefetcher_create(const PrefetchConfig& c) { return new BatchPrefetcher(c); }

@@ -109,10 +109,15 @@ def build_parser() -> argparse.ArgumentParser:
                      help="gradient all-reduce algorithm (nccl = library baseline)")
     ext.add_argument("--wire-dtype", default="bf16", choices=["bf16", "fp32"])
     ext.add_argument("--bucket-mb", type=float, default=32.0)
-    ext.add_argument("--pipeline", default="auto", choices=["auto", "fused", "reference"],
+    ext.add_argument("--pipeline", default="auto", choices=["auto", "fused", "stream", "reference"],
                      help="input pipeline: fused GPU augment over a decoded uint8 cache (any image sizes, "
-                          "resampled as PIL does), the reference's per-sample PIL transforms, or auto "
-                          "(fused when the split has one image size and fits in host memory)")
+                          "resampled as PIL does), stream (no cache: each batch's JPEGs entropy-decoded on host "
+                          "threads, IDCT and colour conversion on the GPU, for splits larger than host memory), "
+                          "the reference's per-sample PIL transforms, or auto (fused when the split has one image "
+                          "size and fits in host memory)")
+    ext.add_argument("--decode-threads", type=int, default=8,
+                     help="host threads decoding images: the fused pipeline's cache build, the stream pipeline's "
+                          "per-batch decode")
     ext.add_argument("--pretrained", default=None,
                      help="path to a torchvision vgg16 state dict (offline pretrained=True)")
     ext.add_argument("--save", default=None, help="checkpoint path written by rank 0 every epoch")

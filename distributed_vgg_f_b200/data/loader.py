@@ -16,6 +16,11 @@ Same surface here, two pipelines:
     geometry row each, resampled on the device exactly as Pillow does.  The split must fit in host
     memory.  ``pipeline="auto"`` (the CLI default) switches to the reference pipeline for mixed
     image sizes or a split too big for host memory.
+  * ``pipeline="stream"`` -- nothing is cached: each batch's files are read when it is drawn.  Host
+    threads entropy-decode the JPEGs to quantised coefficients (csrc/jpeg_decode.cpp) and decode PNGs
+    to RGB; files neither decoder takes are decoded once by PIL at start-up.  Yields ``JpegBatch``,
+    which the device decodes (csrc/jpeg.cu) into exactly the ``RaggedBatch`` a ragged cache of the
+    split would yield: same indices, labels, parameters, geometry and MixUp / CutMix draws.
 Ragged final batches are preserved (``drop_last=False`` in the reference).
 
 With ``mixup_alpha`` / ``cutmix_alpha`` > 0 every training batch carries a MixUp or CutMix draw
@@ -69,6 +74,41 @@ class RaggedBatch(NamedTuple):
         TTA view ``view``)."""
         x = T.ragged_reference(self.data_u8, self.geom, self.params, out_hw=out_hw, view=view)
         return x.to(device), self.labels.to(device)
+
+
+class JpegBatch(NamedTuple):
+    """A stream batch before decoding: the JPEGs' quantised coefficients and tables, the other images' RGB, one
+    descriptor row per image (data/jpeg.py, csrc/include/jpeg.h), and ``geom`` rows of the decoded images back to
+    back, exactly as ``RaggedBatch``'s."""
+    coef: torch.Tensor          # int16 [blocks * 64]       (pinned when CUDA is present)
+    quant: torch.Tensor         # int32 [mb * 3, 64]        (same)
+    raw: torch.Tensor           # uint8 [bytes]             (same)
+    desc: torch.Tensor          # int32 [mb, 16]            (same)
+    geom: torch.Tensor          # int64 [mb, 5]             (same)
+    params: torch.Tensor        # float32 [mb, 8]           (same)
+    labels: torch.Tensor        # int64 [mb]                (same)
+    state: Optional[dict] = None    # consumer may set state["event"]: slot is reusable after it fires
+    mix: Optional[T.MixDraw] = None     # MixUp / CutMix of this training batch
+
+    @property
+    def nbytes(self) -> int:
+        """Bytes of the decoded images."""
+        g = self.geom[-1]
+        return int(g[0] + g[1] * g[2] * 3)
+
+    def decode(self) -> torch.Tensor:
+        """The decoded images back to back (uint8, a ``RaggedBatch``'s ``data_u8``), by the CPU reference."""
+        from .jpeg import decode_batch
+        return torch.from_numpy(decode_batch(self.coef.numpy(), self.quant.numpy(), self.raw.numpy(),
+                                             self.desc.numpy(), self.geom.numpy()))
+
+    def to_float(self, device="cpu", out_hw: int = DATA.crop, view: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Decode on the CPU, then evaluate the transform as ``RaggedBatch.to_float`` does."""
+        x = T.ragged_reference(self.decode(), self.geom, self.params, out_hw=out_hw, view=view)
+        return x.to(device), self.labels.to(device)
+
+
+DEVICE_BATCHES = (FusedBatch, RaggedBatch, JpegBatch)     # batches whose transform runs on the consumer's side
 
 
 def _decode(path: str) -> np.ndarray:
@@ -341,6 +381,103 @@ class _FusedLoader:
         th.join()
 
 
+class _StreamSplit(NamedTuple):
+    """What the stream loader knows of its split without decoding it: labels, sizes and header rows."""
+    labels: torch.Tensor        # int64 [N]
+    hw: torch.Tensor            # int64 [N, 2]
+    headers: torch.Tensor       # int64 [N, 12]: ops jpeg_scan rows
+
+
+class _StreamLoader(_FusedLoader):
+    """Batches for ``pipeline="stream"``: the ragged fused loader's batches, decoded from the files per batch.
+
+    A native worker (csrc/prefetch.cpp) draws each batch exactly as ``_FusedLoader`` does over a ragged cache and
+    lays it out in a pinned slot; ``threads`` decode threads fill the slot's fixed positions.  The slot holds the
+    coefficients of the ``mb`` largest JPEGs of the split and the RGB of its ``mb`` largest other images."""
+
+    def __init__(self, samples: List[Tuple[str, int]], mb: int, train: bool, sampler: Optional[ShardedSampler],
+                 shuffle: bool, seed: int, threads: int = 8, prefetch: int = 3, pin: Optional[bool] = None,
+                 mixup_alpha: float = 0.0, cutmix_alpha: float = 0.0, resize: int = DATA.resize,
+                 crop: int = DATA.crop, max_bytes: Optional[int] = None) -> None:
+        from .. import ops
+        C = ops.require()
+        self.mb, self.train, self.resize, self.crop = mb, train, resize, crop
+        self.mixup_alpha, self.cutmix_alpha = (mixup_alpha, cutmix_alpha) if train else (0.0, 0.0)
+        self.sampler, self.shuffle, self.seed = sampler, shuffle, seed
+        self.prefetch, self.epoch, self.ragged, self.resized_hw = prefetch, 0, True, None
+        self.pin = torch.cuda.is_available() if pin is None else pin
+        self.threads = threads
+        paths = [p for p, _ in samples]
+        headers = C.jpeg_scan(paths, threads)
+        # a PNG goes to the native decoder per batch only if that decoder takes it (the scan reads its IHDR alone)
+        png = (headers[:, 0] == 2).nonzero().flatten()
+        if len(png):
+            ok = C.png_decodable([paths[i] for i in png.tolist()], headers[png, 1:3].contiguous(), threads)
+            headers[png[~ok], 0] = 0
+        kind = headers[:, 0]
+        hw = headers[:, 1:3].clone()
+        # files neither native decoder takes: decoded once by PIL, kept as RGB.  Their size comes from the scan
+        # (JPEG frame, PNG IHDR) or PIL's header, and the budget is checked before anything is decoded.
+        other = (kind == 0).nonzero().flatten().tolist()
+        unsized = [i for i in other if hw[i, 0] < 1 or hw[i, 1] < 1]
+        with ThreadPoolExecutor(max_workers=threads) as ex:
+            for i, (h, w) in zip(unsized, ex.map(lambda i: _header_hw(paths[i]), unsized)):
+                hw[i, 0], hw[i, 1] = h, w
+        nbytes = (hw[other, 0] * hw[other, 1] * 3) if other else torch.zeros(0, dtype=torch.int64)
+        need = int(nbytes.sum())
+        budget = _cache_budget_bytes() if max_bytes is None else max_bytes
+        if need > budget:
+            raise CacheUnavailable("the %d files the stream decoders do not take need %.1f MB decoded, budget %.1f MB "
+                                   "(B200_MAX_CACHE_GB)" % (len(other), need / 2**20, budget / 2**20))
+        self.other_count, self.other_bytes = len(other), need
+        other_off = torch.full((len(paths),), -1, dtype=torch.int64)
+        if other:
+            other_off[other] = torch.cumsum(nbytes, 0) - nbytes
+        flat = torch.empty(max(need, 1), dtype=torch.uint8)
+
+        def pil(i: int) -> None:         # one decoded image per thread at a time
+            a = _decode(paths[i])
+            h, w = int(hw[i, 0]), int(hw[i, 1])
+            if a.shape != (h, w, 3):
+                raise ValueError("%s decodes to %s, its header says %dx%d" % (paths[i], a.shape, h, w))
+            off = int(other_off[i])
+            flat[off:off + h * w * 3].numpy()[...] = a.reshape(-1)
+
+        with ThreadPoolExecutor(max_workers=threads) as ex:
+            list(ex.map(pil, other))
+        self.cache = _StreamSplit(torch.tensor([l for _, l in samples], dtype=torch.int64), hw, headers)
+        jpeg = kind == 1
+        coef = (headers[jpeg, 11] * 64).sort(descending=True).values
+        rgb = (hw[~jpeg, 0] * hw[~jpeg, 1] * 3).sort(descending=True).values
+        slots = prefetch + 1
+        self._coef = self._buf((slots, max(int(coef[:mb].sum()), 64)), torch.int16)
+        self._raw = self._buf((slots, max(int(rgb[:mb].sum()), 1)), torch.uint8)
+        self._quant = self._buf((slots, mb * 3, 64), torch.int32)
+        self._desc = self._buf((slots, mb, C.JPEG_DESC), torch.int32)
+        self._geom = self._buf((slots, mb, T.GEOM_DIM), torch.int64)
+        self._par = self._buf((slots, mb, T.PARAM_DIM), torch.float32)
+        self._lab = self._buf((slots, mb), torch.int64)
+        self._state = [{} for _ in range(slots)]
+        self._pf = C.StreamPrefetcher(paths, headers, self.cache.labels, hw, flat, other_off, self._coef, self._quant,
+                                      self._raw, self._desc, self._geom, self._par, self._lab, train,
+                                      DATA.crop_scale[0], DATA.crop_scale[1], DATA.crop_ratio[0], DATA.crop_ratio[1],
+                                      DATA.rotation_deg, resize, threads)
+
+    def _batch(self, slot: int, k: int, index: int = 0) -> JpegBatch:
+        desc = self._desc[slot][:k]
+        d = desc.numpy()
+        blocks = int(d[-1, 3] + (d[-1, 5:8] * d[-1, 8:11]).sum())
+        raw = d[d[:, 0] == 0]
+        g = self._geom[slot][:k]
+        rows = g.numpy()[d[:, 0] == 0]
+        used = int((raw[:, 4] + rows[:, 1] * rows[:, 2] * 3).max()) if len(raw) else 0
+        return JpegBatch(self._coef[slot][:blocks * 64], self._quant[slot][:k * 3], self._raw[slot][:used], desc, g,
+                         self._par[slot][:k], self._lab[slot][:k], self._state[slot], self._draw(index))
+
+    def __iter__(self) -> Iterator[JpegBatch]:
+        return self._iter_native()
+
+
 class _ReferenceLoader:
     """Synchronous PIL + torchvision loader with the reference's exact semantics."""
 
@@ -417,6 +554,15 @@ class DataManager:
                                      reference_order=reference_order)
         elif shard_eval and world_size > 1:   # extension: exact partition, metrics all-reduced
             sampler = ShardedSampler(self.data_size, world_size, rank, shuffle=False, pad=False)
+        if pipeline == "stream":
+            self.loader = _StreamLoader(self.samples, mini_batch, train, sampler, True, seed, threads=decode_threads,
+                                        mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha,
+                                        resize=self.resize_size, crop=self.crop_size)
+            self.pipeline = pipeline
+            if self.loader.other_count:
+                print("[Info] stream pipeline: %d file(s) no stream decoder takes, decoded by PIL at start-up "
+                      "(%.1f MB)" % (self.loader.other_count, self.loader.other_bytes / 2**20), flush=True)
+            return
         if pipeline in ("fused", "auto"):
             try:
                 self.cache = DecodedCache(self.samples, decode_threads, allow_mixed=pipeline == "fused",
@@ -439,7 +585,7 @@ class DataManager:
                                            mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha,
                                            resize=self.resize_size, crop=self.crop_size, tta=tta)
         else:
-            raise ValueError("pipeline must be 'fused', 'reference' or 'auto'")
+            raise ValueError("pipeline must be 'fused', 'stream', 'reference' or 'auto'")
 
     def get_loader(self):
         return self.loader

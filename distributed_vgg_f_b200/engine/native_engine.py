@@ -31,7 +31,7 @@ import torch.distributed as dist
 from .. import ops
 from ..config import DATA, TRAIN
 from ..data import transforms as T
-from ..data.loader import FusedBatch, RaggedBatch
+from ..data.loader import FusedBatch, JpegBatch, RaggedBatch
 from ..models import layout as L
 from ..models.vggf import VGGSpec, build_oracle
 from ..parallel import layerwise as lw
@@ -692,6 +692,10 @@ class NativeEngine:
         self._labels_dev = [torch.zeros(B, dtype=torch.int64, device=dev) for _ in range(2)]
         self._geom_dev = [torch.zeros(B, 5, dtype=torch.int64, device=dev) for _ in range(2)]   # RaggedBatch rows
         self._inter_u8 = None        # RaggedBatch: horizontally filtered rows, written and read on one stream
+        # JpegBatch: coef, quant, raw and desc copied per slot on the copy stream (grown to the loader's slot
+        # capacity, as _src_u8); the IDCT's sample planes are written and read on one stream
+        self._jpeg_dev = [{} for _ in range(2)]
+        self._planes_u8 = None
         self._in_free = [None, None]           # event: the step that used this slot is done with it
         self.labels_dev = self._labels_dev[0]
         # first conv: fused kernels build the im2col operand in shared memory from NHWC4 pixels
@@ -827,19 +831,33 @@ class NativeEngine:
             if not self.fused_conv0:
                 C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
             return b
-        if isinstance(batch, RaggedBatch):
+        if isinstance(batch, (RaggedBatch, JpegBatch)):
+            jpeg = isinstance(batch, JpegBatch)
             b = int(batch.labels.shape[0])
-            nbytes = int(batch.data_u8.numel())
+            nbytes = batch.nbytes if jpeg else int(batch.data_u8.numel())
             if self._src_u8[j] is None or self._src_u8[j].dim() != 1 or self._src_u8[j].numel() < nbytes:
                 # grows to the loader's slot capacity (the mb largest images) and then stays
                 self._src_u8[j] = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
             need = ops.ragged_inter_bytes(batch.geom)
             if self._inter_u8 is None or self._inter_u8.numel() < need:
                 self._inter_u8 = torch.empty(need, dtype=torch.uint8, device=self.device)
+            if jpeg:
+                dev = self._jpeg_dev[j]
+                for name in ("coef", "quant", "raw", "desc"):
+                    t = getattr(batch, name)
+                    if name not in dev or dev[name].numel() < t.numel():
+                        dev[name] = torch.empty(max(t.numel(), 1), dtype=t.dtype, device=self.device)
+                if self._planes_u8 is None or self._planes_u8.numel() < batch.coef.numel():
+                    self._planes_u8 = torch.empty(max(batch.coef.numel(), 1), dtype=torch.uint8, device=self.device)
             with torch.cuda.stream(self.copy_stream):
                 if self._in_free[j] is not None:
                     self.copy_stream.wait_event(self._in_free[j])
-                self._src_u8[j][:nbytes].copy_(batch.data_u8, non_blocking=True)
+                if jpeg:
+                    for name in ("coef", "quant", "raw", "desc"):
+                        t = getattr(batch, name)
+                        dev[name][:t.numel()].copy_(t.view(-1), non_blocking=True)
+                else:
+                    self._src_u8[j][:nbytes].copy_(batch.data_u8, non_blocking=True)
                 self._geom_dev[j][:b].copy_(batch.geom, non_blocking=True)
                 self._params_dev[j][:b].copy_(batch.params, non_blocking=True)
                 self._labels_dev[j][:b].copy_(batch.labels, non_blocking=True)
@@ -848,6 +866,10 @@ class NativeEngine:
             if batch.state is not None:
                 batch.state["event"] = h2d
             cur.wait_event(h2d)
+            if jpeg:        # decode on the compute stream into the slot's image buffer, then as a RaggedBatch
+                C.jpeg_decode(dev["coef"], dev["quant"][:batch.quant.numel()].view(-1, 64),
+                              dev["desc"][:batch.desc.numel()].view(b, -1), self._geom_dev[j][:b], dev["raw"],
+                              self._planes_u8, self._src_u8[j][:nbytes], batch.desc, batch.geom)
             if views is not None:
                 self._staged = j
                 return self._view_input(batch, b, 0, views)
@@ -884,8 +906,9 @@ class NativeEngine:
             j = self._staged
             ops.augment_view(self._src_u8[j][:b], self._params_dev[j][:b], self.x_nhwc[:b], batch.resized_hw,
                              views[i], out_hw=HW)
-        elif isinstance(batch, RaggedBatch):
-            j, nbytes = self._staged, int(batch.data_u8.numel())
+        elif isinstance(batch, (RaggedBatch, JpegBatch)):
+            j = self._staged
+            nbytes = batch.nbytes if isinstance(batch, JpegBatch) else int(batch.data_u8.numel())
             ops.augment_ragged_view(self._src_u8[j][:nbytes], self._geom_dev[j][:b], self._params_dev[j][:b],
                                     self._inter_u8, self.x_nhwc[:b], batch.geom, batch.params, views[i], out_hw=HW,
                                     pass1=views if i == 0 else ())

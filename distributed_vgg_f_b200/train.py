@@ -125,7 +125,8 @@ def manage_training(args) -> Trainer:
             torch.distributed.barrier()
 
     dm_kw = dict(world_size=args.world_size, rank=args.rank, pipeline=args.pipeline,
-                 seed=args.seed, reference_order=args.reference_order)
+                 seed=args.seed, reference_order=args.reference_order,
+                 decode_threads=getattr(args, "decode_threads", 8))
     sizes = input_sizes(args)
     train_data_mngr = DataManager(args.root_dir, args.mini_batch, train=True,
                                   mixup_alpha=getattr(args, "mixup_alpha", 0.0),
@@ -145,6 +146,12 @@ def manage_training(args) -> Trainer:
     if sizes != input_sizes(None):
         print("[Info] input sizes: train RandomResizedCrop {} -> crop {}, eval Resize {} -> crop {}".format(
             sizes["train_resize_size"], sizes["train_crop_size"], sizes["val_resize_size"], sizes["val_crop_size"]))
+    stream = None
+    if train_data_mngr.pipeline == "stream":
+        stream = dict(pipeline="stream", decode_threads=train_loader.threads,
+                      stream_fallback=train_loader.other_count + valid_loader.other_count)
+        print("[Info] input pipeline: stream ({} decode threads, {} file(s) decoded by PIL at start-up)".format(
+            stream["decode_threads"], stream["stream_fallback"]))
     if val_tta != "none":
         from .data.transforms import tta_views
         print("[Info] test-time augmentation: {} ({} views per image, mean of their softmaxes)".format(
@@ -259,6 +266,8 @@ def manage_training(args) -> Trainer:
                 rec["input_sizes"] = sizes
             if val_tta != "none":
                 rec["val_tta"] = val_tta
+            if stream is not None:
+                rec.update(stream)
             if not schedule.constant:
                 rec["lr"] = epoch_lr
             if hasattr(model, "phase_times"):

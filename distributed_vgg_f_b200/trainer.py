@@ -44,7 +44,7 @@ import torch.nn.functional as F
 
 from .config import DATA
 from .data import transforms as T
-from .data.loader import FusedBatch, RaggedBatch
+from .data.loader import DEVICE_BATCHES
 from .utils.metrics import DeviceMeter
 
 
@@ -205,7 +205,7 @@ class Trainer:
 
     # ------------------------------------------------------------------------------------------
     def _to_device(self, batch, loader=None):
-        if isinstance(batch, (FusedBatch, RaggedBatch)):     # cut to the network input its loader is set to
+        if isinstance(batch, DEVICE_BATCHES):     # cut to the network input its loader is set to
             return batch.to_float(self.device, out_hw=getattr(loader, "crop", DATA.crop))
         inputs, targets = batch[0], batch[1]
         return inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
@@ -213,11 +213,11 @@ class Trainer:
     def _mixed_to_device(self, batch):
         """(inputs, integer targets, probability targets or None) of a training batch: the batch's
         MixUp / CutMix draw applied by torchvision (the reference pipeline has applied it already)."""
-        mix = batch.mix if isinstance(batch, (FusedBatch, RaggedBatch)) else (batch[2] if len(batch) > 2 else None)
+        mix = batch.mix if isinstance(batch, DEVICE_BATCHES) else (batch[2] if len(batch) > 2 else None)
         inputs, targets = self._to_device(batch, self.train_loader)
         if mix is None:
             return inputs, targets, None
-        if isinstance(batch, (FusedBatch, RaggedBatch)):
+        if isinstance(batch, DEVICE_BATCHES):
             inputs = T.apply_mix(inputs, targets, mix)
         return inputs, targets, mix
 
@@ -346,7 +346,7 @@ class Trainer:
         """([logits of each --val-tta view], targets) of a validation batch on the torch path: a fused batch is
         evaluated at each view, the reference pipeline's [b][V][3][H][W] batch is cut into its views."""
         views = T.tta_views(self.val_tta)
-        if isinstance(batch, (FusedBatch, RaggedBatch)):
+        if isinstance(batch, DEVICE_BATCHES):
             crop = getattr(self.test_loader, "crop", DATA.crop)
             targets = batch.labels.to(self.device)
             return [net(batch.to_float(self.device, out_hw=crop, view=v)[0]) for v in views], targets
