@@ -21,6 +21,7 @@ ROLE = [   # (regex on the demangled name, role, what it replaces in the referen
     (r"head_ce_kernel", "K-FUN2+CE: last Linear + log-softmax / NLL + metrics + dlogits + the layer's dW, db, dX in one launch", "cuBLAS + ATen log_softmax / nll_loss + `Accuracy2` / `Average` — `:56`, `:168`, `distributedUtil.py:95-96`"),
     (r"head_ce_kd_kernel", "K-FUN2+CE with knowledge distillation: head_ce_kernel's launch, the teacher's logits read too; loss (1 − α) CE + α T² KL and its dlogits", "`F.cross_entropy` + `F.kl_div` of a distillation script — not in the reference"),
     (r"tta_accumulate_kernel", "--val-tta view-mean reduction: each view's softmax added into an fp32 [B][C] accumulator in view order; at the last view -log of the label's mean probability and its argmax into the meter", "the mean softmax of torchvision's `ten_crop` / `five_crop` views — not in the reference"),
+    (r"class_metrics_kernel", "--val-metrics: per evaluation batch, int64 confusion-matrix counts of (label, first maximum of the logits or of the --val-tta view mean) and the count of labels ranked in the top 5; integer atomics", "scikit-learn `confusion_matrix` / torchvision's Acc@5 — not in the reference"),
     (r"cross_entropy_kd_kernel", "cross-entropy with knowledge distillation for heads that do not fuse (C > 8, B > 256, VGG-16)", "`F.cross_entropy` + `F.kl_div` of a distillation script — not in the reference"),
     (r"cross_entropy_kernel", "cross-entropy fwd + bwd + metrics for wide heads (VGG-16/1000)", "`F.cross_entropy` — `:168`"),
     (r"fc_bias_act_kernel", "FC epilogue: bias + ReLU + Philox dropout → bf16 (mask never stored)", "ATen bias/relu/dropout — `:52-57`"),

@@ -819,6 +819,32 @@ static void tta_accumulate(const at::Tensor& logits, const at::Tensor& target, a
                        f32p_opt(meter), f32p_opt(loss_out), (int)B, (int)C, (int)view, (int)views, cur_stream());
 }
 
+// Per-class evaluation counts of one batch (class_metrics in api.h).
+static void class_metrics(const at::Tensor& scores, const at::Tensor& target, at::Tensor confusion, at::Tensor top5,
+                          int64_t views) {
+  c10::cuda::CUDAGuard g(scores.device());
+  TORCH_CHECK(scores.is_cuda() && scores.scalar_type() == at::kFloat && scores.is_contiguous() && scores.dim() == 2,
+              "class_metrics: scores must be a contiguous CUDA fp32 [B, C] tensor");
+  const int64_t B = scores.size(0), C = scores.size(1);
+  TORCH_CHECK(B >= 1 && C >= 1, "class_metrics: empty scores");
+  TORCH_CHECK(views >= 1 && views <= b200::kTtaMaxViews, "class_metrics: views must lie in [1, ", b200::kTtaMaxViews,
+              "], got ", views);
+  TORCH_CHECK(target.device() == scores.device() && target.scalar_type() == at::kLong && target.is_contiguous() &&
+                  target.numel() >= B,
+              "class_metrics: contiguous int64 targets of B = ", B, " on the scores' device");
+  TORCH_CHECK(confusion.device() == scores.device() && confusion.scalar_type() == at::kLong &&
+                  confusion.is_contiguous(),
+              "class_metrics: confusion must be a contiguous int64 tensor on the scores' device");
+  TORCH_CHECK(confusion.dim() == 2 && confusion.size(0) == C && confusion.size(1) == C,
+              "class_metrics: confusion must be [", C, ", ", C, "] for scores of ", C, " classes, got ",
+              confusion.sizes());
+  TORCH_CHECK(top5.device() == scores.device() && top5.scalar_type() == at::kLong && top5.numel() >= 1,
+              "class_metrics: top5 must hold one int64 on the scores' device");
+  b200::class_metrics(f32p(scores), reinterpret_cast<const long long*>(target.data_ptr()),
+                      reinterpret_cast<long long*>(confusion.data_ptr()), reinterpret_cast<long long*>(top5.data_ptr()),
+                      (int)B, (int)C, (int)views, cur_stream());
+}
+
 static void im2col_c3(const at::Tensor& x, at::Tensor out, int64_t kpad) {
   c10::cuda::CUDAGuard g(x.device());
   check_vec(x, at::kBFloat16, 8, "im2col_c3", "x");
@@ -1490,6 +1516,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("augment_view", &augment_view);
   m.def("augment_ragged_view", &augment_ragged_view);
   m.def("tta_accumulate", &tta_accumulate);
+  m.def("class_metrics", &class_metrics);
   m.attr("TTA_FLIP") = (int)b200::TtaFlip;
   m.def("im2col_c3", &im2col_c3);
   m.def("nchw_to_nhwc", &nchw_to_nhwc);

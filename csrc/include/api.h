@@ -360,6 +360,12 @@ void augment_ragged_view(const uint8_t* src, const long long* geom, const float*
 // of argmax(acc / V) == y (lowest index on ties) and B into meter, and writes the mean loss to loss_out.
 void tta_accumulate(const float* logits, const long long* target, float* acc, float* meter,
                     float* loss_out, int B, int C, int view, int views, cudaStream_t s);
+// ---- per-class evaluation counts (--val-metrics) -------------------------------------------------
+// For each row of the fp32 scores [B][C] divided by `views` (logits: 1; tta_accumulate's acc: V), add 1 to
+// confusion[y][first maximum] (int64 [C][C], rows labels) and, when the label ranks among the first five
+// (#{c : s_c > s_y} + #{c < y : s_c == s_y} < 5), 1 to *top5.  Integer atomics only.
+void class_metrics(const float* scores, const long long* target, long long* confusion, long long* top5, int B, int C,
+                   int views, cudaStream_t s);
 // ---- streaming JPEG decode (jpeg.cu, --pipeline stream) ------------------------------------------
 // A batch of k images described by desc [k][kJpegDesc] (jpeg.h) and geom [k][5] rows as augment_ragged's:
 // dequantise + IDCT the total_blocks coefficient blocks into planes (total_blocks x 64 bytes), then write each

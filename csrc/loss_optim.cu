@@ -405,6 +405,73 @@ void tta_accumulate(const float* logits, const long long* target, float* acc, fl
   check_last("tta_accumulate");
 }
 
+// Per-class evaluation counts (class_metrics, --val-metrics): one warp per row, as tta_accumulate_kernel, eight rows
+// per block so that a batch's rows run on several SMs.  A row's scores are s_c = scores[r][c] / V with __fdiv_rn,
+// tta_accumulate's view mean (V = 1: the logits as they are, x / 1 being x).  The prediction is the first maximum
+// (v > max from -inf, lowest index on ties), the rule of the correct-counts of cross_entropy_kernel and
+// tta_accumulate_kernel, so the diagonal of M sums to their count.  The label's rank is
+// #{c : s_c > s_y} + #{c < y : s_c == s_y}; below 5 the row counts toward top-5.  A row without a maximum (every
+// score NaN or -inf) or with a label outside [0, C) is counted nowhere.  Integer atomics: the same counts every run.
+constexpr int CM_ROWS = 8, CM_UNROLL = 4;
+__global__ void __launch_bounds__(CM_ROWS * 32)
+class_metrics_kernel(const float* __restrict__ scores, const long long* __restrict__ target,
+                     unsigned long long* __restrict__ M, unsigned long long* __restrict__ top5, int B, int C, int views) {
+  __shared__ unsigned int s_top5[CM_ROWS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r = blockIdx.x * CM_ROWS + warp;
+  unsigned int hit = 0;
+  const long long t = r < B ? target[r] : -1;
+  if (t >= 0 && t < C) {                               // the same for every lane of the warp
+    const int y = static_cast<int>(t);
+    const float* row = scores + static_cast<long long>(r) * C;
+    const float fv = static_cast<float>(views);
+    const float sy = __fdiv_rn(row[y], fv);
+    float best = -INFINITY;
+    int amax = 0x7fffffff;
+    unsigned int ahead = 0;                            // classes ranked before the label
+    for (int c0 = lane; c0 < C; c0 += 32 * CM_UNROLL) {
+      float v[CM_UNROLL];                              // the loads first: CM_UNROLL in flight per lane
+#pragma unroll
+      for (int u = 0; u < CM_UNROLL; ++u) v[u] = c0 + 32 * u < C ? row[c0 + 32 * u] : 0.f;
+#pragma unroll
+      for (int u = 0; u < CM_UNROLL; ++u) {            // in increasing c, as one element per step would
+        const int c = c0 + 32 * u;
+        if (c < C) {
+          const float x = __fdiv_rn(v[u], fv);
+          if (x > best) { best = x; amax = c; }
+          ahead += (x > sy || (x == sy && c < y)) ? 1u : 0u;
+        }
+      }
+    }
+    for (int o = 16; o; o >>= 1) {
+      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+      const int oa = __shfl_xor_sync(0xffffffffu, amax, o);
+      if (ob > best || (ob == best && oa < amax)) { best = ob; amax = oa; }
+      ahead += __shfl_xor_sync(0xffffffffu, ahead, o);
+    }
+    if (lane == 0 && amax < C) {
+      atomicAdd(M + static_cast<long long>(y) * C + amax, 1ull);
+      hit = ahead < 5 ? 1u : 0u;
+    }
+  }
+  if (lane == 0) s_top5[warp] = hit;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long n = 0;
+    for (int i = 0; i < CM_ROWS; ++i) n += s_top5[i];
+    if (n) atomicAdd(top5, n);
+  }
+}
+
+void class_metrics(const float* scores, const long long* target, long long* confusion, long long* top5, int B, int C,
+                   int views, cudaStream_t s) {
+  class_metrics_kernel<<<(B + CM_ROWS - 1) / CM_ROWS, CM_ROWS * 32, 0, s>>>(
+      scores, target, reinterpret_cast<unsigned long long*>(confusion), reinterpret_cast<unsigned long long*>(top5), B,
+      C, views);
+  count_launch();
+  check_last("class_metrics");
+}
+
 KdParams kd_params(double alpha, double temperature, int B) {
   return KdParams{static_cast<float>(1.0 - alpha), static_cast<float>(alpha * temperature / B),
                   static_cast<float>(alpha * temperature * temperature), static_cast<float>(1.0 / temperature)};

@@ -199,6 +199,12 @@ def build_parser() -> argparse.ArgumentParser:
                           "Resize(--val-resize-size) image, scored by the mean of their softmaxes.  flip: the centre "
                           "crop and its mirror image; five-crop: torchvision's five_crop; ten-crop: its ten_crop "
                           "(the five and those of the mirrored image).  Training does not change (default: none)")
+    # SUPPRESS: without the flag the namespace (printed, and saved in checkpoints) is the one of earlier versions
+    ext.add_argument("--val-metrics", action="store_true", default=argparse.SUPPRESS,
+                     help="every validation pass also counts a confusion matrix (rows labels, columns predictions) and, "
+                          "with more than 5 classes, the top-5 hits on the GPU, and reports balanced accuracy, acc@5 "
+                          "and, up to 32 classes, per-class support, recall, precision and confusion row; the JSONL "
+                          "records get test_confusion, test_recall, ... (default: off)")
     ext.add_argument("--model-ema-decay", type=float, default=0.99998,
                      help="EMA decay per image seen, 0 <= d < 1; the decay of one update is adjusted as torchvision "
                           "does: 1 - min(1, (1 - d) * world * mini_batch * accum_steps * model_ema_steps / epochs)")

@@ -1456,17 +1456,25 @@ class NativeEngine:
 
     def eval_step(self, batch, ema: bool = False) -> torch.Tensor:
         """Evaluation forward, loss and metrics; ``ema``: with the moving average of the weights
-        (after prepare_ema()).  With a TTA mode (set_val_tta) the loss and metrics are those of the view mean."""
+        (after prepare_ema()).  With a TTA mode (set_val_tta) the loss and metrics are those of the view mean.
+        A meter with a confusion matrix (DeviceMeter(num_classes=)) also gets the batch's per-class counts: one
+        class_metrics launch on the logits, or on the view sums after the last view."""
         self._use_weights(ema)
         self._set_hw(self.eval_hw)
+        counts = self.meter is not None and self.meter.confusion is not None
         try:
             if self.val_tta != "none":
-                self._tta_pass(batch)
+                b = self._tta_pass(batch)
+                if counts:
+                    ops.class_metrics(self.tta_acc[:b], self.labels_dev[:b], self.meter.confusion, self.meter.top5,
+                                      views=len(T.tta_views(self.val_tta)))
                 self._release_input()
                 return self.loss_buf
             b = self._stage_input(batch)
             self._forward(b, train=False)
             self._loss(b, train=False)
+            if counts:
+                ops.class_metrics(self.logits[:b], self.labels_dev[:b], self.meter.confusion, self.meter.top5)
             self._release_input()
         finally:
             self._use_weights(False)

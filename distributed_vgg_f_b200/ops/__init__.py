@@ -376,6 +376,13 @@ def tta_accumulate(logits, target, acc, *, view: int, views: int, meter=None, lo
     require().tta_accumulate(logits, target, acc, meter, loss_out, int(view), int(views))
 
 
+def class_metrics(scores, target, confusion, top5, *, views: int = 1) -> None:
+    """Add one batch to the per-class evaluation counts: for each row of the fp32 ``scores`` [b][C] divided by ``views``
+    (logits: 1; tta_accumulate's acc: V), confusion[y][first maximum] += 1 (int64 [C][C], rows labels) and, when the
+    label ranks among the first five, top5 += 1 (``ref.class_metrics`` has the rule)."""
+    require().class_metrics(scores, target, confusion, top5, int(views))
+
+
 def ragged_inter_bytes(geom_host) -> int:
     """Bytes of the intermediate ``augment_ragged`` needs for these geometry rows."""
     return int(require().ragged_inter_bytes(geom_host))

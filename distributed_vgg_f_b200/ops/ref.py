@@ -507,6 +507,26 @@ def tta_reduce64(view_logits: torch.Tensor, target: torch.Tensor):
     return {"probs": probs, "loss": loss, "meter": meter}
 
 
+def class_metrics(scores: torch.Tensor, target: torch.Tensor, views: int = 1):
+    """The per-class evaluation counts of scores [B][C] (fp32 logits, or tta_accumulate's sums with ``views`` = V) ->
+    (confusion int64 [C][C], rows labels and columns predictions; top-5 count).  A row's scores are the fp32 quotient
+    s = scores / V, rounded to nearest as __fdiv_rn; its prediction is the first maximum, NaN never one; the label y
+    ranks #{c : s_c > s_y} + #{c < y : s_c == s_y} and counts toward top-5 below 5.  A row without a maximum (every
+    score NaN or -inf) or with a label outside [0, C) is counted nowhere."""
+    s = scores.detach().to("cpu", torch.float32) / float(views)
+    B, C = s.shape
+    t = target.detach().to("cpu", torch.int64).view(-1)[:B]
+    finite = torch.where(torch.isnan(s), torch.full_like(s, -float("inf")), s)
+    best, pred = _first_max(finite)
+    keep = (best > -float("inf")) & (t >= 0) & (t < C)
+    s, t, pred = s[keep], t[keep], pred[keep]
+    sy = s.gather(1, t.view(-1, 1))
+    pos = torch.arange(C)
+    rank = ((s > sy) | ((s == sy) & (pos < t.view(-1, 1)))).sum(1)
+    confusion = torch.bincount(t * C + pred, minlength=C * C).view(C, C)
+    return confusion, int((rank < 5).sum())
+
+
 def kd_cross_entropy64(logits: torch.Tensor, teacher: torch.Tensor, target: torch.Tensor, *, alpha: float,
                        temperature: float, class_weights=None, label_smoothing: float = 0.0, soft_target=None,
                        ldd: int = 0):

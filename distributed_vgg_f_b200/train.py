@@ -292,7 +292,9 @@ def manage_training(args) -> Trainer:
                       model_ema_steps=getattr(args, "model_ema_steps", 32),
                       teacher=teacher if optimizer is not None else None,
                       distill_alpha=getattr(args, "distill_alpha", 0.5),
-                      distill_temperature=getattr(args, "distill_temperature", 4.0), val_tta=val_tta)
+                      distill_temperature=getattr(args, "distill_temperature", 4.0), val_tta=val_tta,
+                      val_metrics=getattr(args, "val_metrics", False),
+                      class_names=val_class_names(valid_data_mngr.class_names, num_classes))
     trainer.profile_timeline = getattr(args, "profile", None) == "timeline"
     if getattr(args, "eval_only", False):        # score a checkpoint: one validation pass, no training
         test_loss, test_acc = trainer._evaluate()
@@ -300,10 +302,14 @@ def manage_training(args) -> Trainer:
         rec = dict(epoch=start_epoch - 1, test_loss=test_loss.average, test_acc=test_acc.accuracy)
         if val_tta != "none":
             rec["val_tta"] = val_tta
+        classes = {}
+        trainer.report_classes("Evaluation: ", "test", test_acc, classes, "test")
         if model_ema is not None:
             ema_loss, ema_acc = trainer._evaluate(ema=True)
             print("[Info] Evaluation: EMA test loss: {}, EMA test acc: {}.".format(ema_loss, ema_acc), flush=True)
             rec.update(ema_test_loss=ema_loss.average, ema_test_acc=ema_acc.accuracy)
+            trainer.report_classes("Evaluation: ", "EMA test", ema_acc, classes, "ema_test")
+        rec.update(classes)
         trainer.history.append(rec)
         return trainer
     if teacher is not None:
@@ -314,6 +320,13 @@ def manage_training(args) -> Trainer:
             flush=True)
     trainer.fit(args.epochs, start_epoch=start_epoch)
     return trainer
+
+
+def val_class_names(names, num_classes: int) -> list:
+    """The --val-metrics row names: the validation folder's classes (its order numbers the labels), by index past
+    them when --num-classes asks for more."""
+    names = list(names)[:num_classes]
+    return names + [str(c) for c in range(len(names), num_classes)]
 
 
 def build_teacher(args, spec, device: torch.device, native: bool, crop: int, eval_crop: int):

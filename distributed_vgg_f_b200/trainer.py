@@ -33,6 +33,11 @@ epoch has u % model_ema_steps == 0, the moving average of the weights is updated
 optimizer kernels (``model_ema=True``, ``train_step(ema=True)``), or on the torch path by
 ``model_ema.update_parameters`` (an ``AveragedModel``) after ``optimizer.step()``.  Every epoch the
 average is evaluated after the raw weights: ``[Info] Epoch: e/E, EMA test loss: .., EMA test acc: ..%.``
+
+``val_metrics`` (--val-metrics): the validation passes of the weights and of the EMA count a confusion matrix and
+the top-5 hits (``DeviceMeter(num_classes=)``), and each of their report lines is followed by the lines of
+``utils.metrics.class_report``; the history gets ``test_*`` / ``ema_test_*`` keys of ``utils.metrics.class_metrics``.
+``class_names`` name the rows (the validation folder's classes, which number the labels).
 """
 from __future__ import annotations
 
@@ -45,7 +50,7 @@ import torch.nn.functional as F
 from .config import DATA
 from .data import transforms as T
 from .data.loader import DEVICE_BATCHES
-from .utils.metrics import DeviceMeter
+from .utils.metrics import DeviceMeter, class_report
 
 
 def _bf16_peak() -> float:
@@ -87,7 +92,8 @@ class Trainer:
                  class_weights: Optional[torch.Tensor] = None, verbose_throughput: bool = True,
                  on_epoch_end=None, shard_eval: bool = False, accum_steps: int = 1,
                  label_smoothing: float = 0.0, model_ema=None, model_ema_steps: int = 32, teacher=None,
-                 distill_alpha: float = 0.5, distill_temperature: float = 4.0, val_tta: str = "none") -> None:
+                 distill_alpha: float = 0.5, distill_temperature: float = 4.0, val_tta: str = "none",
+                 val_metrics: bool = False, class_names=None) -> None:
         if accum_steps < 1:
             raise ValueError("accum_steps must be >= 1 (got %d)" % accum_steps)
         if accum_steps > 1 and not hasattr(train_loader, "__len__"):
@@ -121,7 +127,21 @@ class Trainer:
         self.val_tta = val_tta
         if val_tta != "none" and _is_native(model):
             model.set_val_tta(val_tta)
+        if val_metrics and not class_names:
+            raise ValueError("val_metrics needs the class names, one per class")
+        self.val_metrics = bool(val_metrics)
+        self.class_names = list(class_names) if class_names is not None else None
         self.history = []
+
+    def report_classes(self, head: str, what: str, acc, rec: dict, key: str) -> None:
+        """--val-metrics: print the per-class lines of an evaluation pass after its report line and add its
+        ``<key>_*`` entries to ``rec``."""
+        if acc.classes is None:
+            return
+        for line in class_report(head, what, acc.classes, self.class_names):
+            print(line)
+        sys_stdout_flush()
+        rec.update({key + "_" + k: v for k, v in acc.classes.items()})
 
     # ------------------------------------------------------------------------------------------
     def fit(self, epochs: int, start_epoch: int = 1) -> None:
@@ -139,12 +159,16 @@ class Trainer:
                 "test loss: {}, test acc: {}.".format(test_loss, test_acc),
                 flush=True,
             )
+            head = "Epoch: {}/{}, ".format(epoch, epochs)
+            classes = {}
+            self.report_classes(head, "test", test_acc, classes, "test")
             ema_s = 0.0
             if self.model_ema is not None:
                 te = time.perf_counter()
                 ema_loss, ema_acc = self._evaluate(ema=True)
                 print("[Info] Epoch: {}/{}, EMA test loss: {}, EMA test acc: {}.".format(epoch, epochs, ema_loss,
                                                                                       ema_acc), flush=True)
+                self.report_classes(head, "EMA test", ema_acc, classes, "ema_test")
                 ema_s = time.perf_counter() - te
             if self.verbose_throughput and train_loss.count:
                 print("[Perf] Epoch: {}/{}, train images/sec (this rank): {:.1f}{}{}".format(
@@ -161,6 +185,7 @@ class Trainer:
                                      test_acc=test_acc.accuracy))
             if self.model_ema is not None:
                 self.history[-1].update(ema_test_loss=ema_loss.average, ema_test_acc=ema_acc.accuracy)
+            self.history[-1].update(classes)
             if self.on_epoch_end is not None:
                 self.on_epoch_end(epoch, self)
 
@@ -311,12 +336,15 @@ class Trainer:
 
         if self.shard_eval and dist.is_available() and dist.is_initialized():
             dist.all_reduce(meter.buf)
+            if meter.counts is not None:
+                dist.all_reduce(meter.counts)
         return meter.snapshot()
 
     def _evaluate(self, ema: bool = False, model=None):
         """One validation pass over the weights, or with ``ema`` over their moving average, or over ``model`` (a
-        distillation teacher: an engine or module of the same kind)."""
-        meter = DeviceMeter(self.device)
+        distillation teacher: an engine or module of the same kind; its score is counted without --val-metrics)."""
+        counted = self.val_metrics and model is None
+        meter = DeviceMeter(self.device, len(self.class_names) if counted else None)
         model = self.model if model is None else model
         if _is_native(model):
             model.set_meter(meter)
