@@ -69,6 +69,11 @@ class RaggedBatch(NamedTuple):
     state: Optional[dict] = None    # consumer may set state["event"]: slot is reusable after it fires
     mix: Optional[T.MixDraw] = None     # MixUp / CutMix of this training batch
 
+    @property
+    def nbytes(self) -> int:
+        """Bytes of the images."""
+        return int(self.data_u8.numel())
+
     def to_float(self, device="cpu", out_hw: int = DATA.crop, view: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Evaluate the transform with Pillow's resampling on the CPU (CPU / oracle path), cut to ``out_hw`` (at
         TTA view ``view``)."""

@@ -20,6 +20,7 @@ Nothing synchronises with the host inside a step; loss / accuracy accumulate in 
 """
 from __future__ import annotations
 
+import contextlib
 import math
 import os
 
@@ -47,6 +48,14 @@ F32 = torch.float32
 
 def _round_up(x: int, m: int) -> int:
     return (x + m - 1) // m * m
+
+
+def _grown(buf: Optional[torch.Tensor], n: int, dtype: torch.dtype, device: torch.device) -> torch.Tensor:
+    """``buf`` when it is a 1-D buffer of at least ``n`` elements, else a new one of ``n``: the input slots' buffers
+    for batches of any image sizes grow to the largest batch the loader makes and then stay."""
+    if buf is None or buf.dim() != 1 or buf.numel() < n:
+        buf = torch.empty(n, dtype=dtype, device=device)
+    return buf
 
 
 def fc_ksplit(m_tiles: int, k_iters: int, target: int = 256) -> int:
@@ -793,131 +802,83 @@ class NativeEngine:
 
     # ================================================================================ inputs
     def _stage_input(self, batch, views=None) -> int:
-        """Copy a batch to the device and produce the first conv's im2col rows.  Returns b.  ``views`` (TTA view
-        codes): the input of the first view; ``_view_input`` makes the others from the same staged copy."""
-        C = ops.require()
-        HW = self._hw
-        j = self._in_slot
+        """Copy a batch to the device and produce the network input.  Returns b.  ``views`` (TTA view codes): the
+        input of the first view; ``_view_input`` makes the others from the same staged copy."""
+        j, HW = self._in_slot, self._hw
         self._in_slot ^= 1
         self.labels_dev = self._labels_dev[j]
-        self._mix = None
-        cur = torch.cuda.current_stream(self.device)
+        if isinstance(batch, (FusedBatch, RaggedBatch, JpegBatch)):
+            b, mix = self._copy_to_slot(batch, j), batch.mix
+        else:                            # the reference pipeline's (float batch, labels[, MixUp / CutMix draw])
+            b, mix = int(batch[1].shape[0]), batch[2] if len(batch) > 2 else None
+            x = self._staged_x = batch[0].to(self.device, F32, non_blocking=True).contiguous()
+            if views is not None:        # the reference pipeline's views: [b][V][3][HW][HW]
+                assert x.dim() == 5 and x.shape[1] == len(views), "the batch does not carry the evaluation's views"
+                assert x.shape[3] == HW and x.shape[4] == HW, "input size differs from the evaluation size (eval_hw)"
+            else:
+                assert x.shape[2] == HW and x.shape[3] == HW, \
+                    "input size differs from the pass's size (input_hw / eval_hw)"
+            self.labels_dev[:b].copy_(batch[1], non_blocking=True)
+        self._staged, self._mix = j, mix
+        return self._view_input(batch, b, 0, views)
+
+    def _copy_to_slot(self, batch, j: int) -> int:
+        """Copy a loader batch to input slot ``j`` (and decode a JpegBatch into the slot's image buffer).  Returns b."""
+        b, dev = int(batch.labels.shape[0]), self.device
         if isinstance(batch, FusedBatch):
-            b = int(batch.labels.shape[0])
-            src = batch.images_u8
-            if self._src_u8[j] is None or self._src_u8[j].shape[1:] != src.shape[1:]:
-                self._src_u8[j] = torch.empty((self.B,) + tuple(src.shape[1:]), dtype=torch.uint8,
-                                              device=self.device)
-            with torch.cuda.stream(self.copy_stream):
-                if self._in_free[j] is not None:
-                    self.copy_stream.wait_event(self._in_free[j])
-                self._src_u8[j][:b].copy_(src, non_blocking=True)
-                self._params_dev[j][:b].copy_(batch.params, non_blocking=True)
-                self._labels_dev[j][:b].copy_(batch.labels, non_blocking=True)
-                h2d = torch.cuda.Event()
-                h2d.record(self.copy_stream)
-            if batch.state is not None:
-                batch.state["event"] = h2d          # the loader may refill the pinned slot after this
-            cur.wait_event(h2d)
-            if views is not None:
-                self._staged = j
-                return self._view_input(batch, b, 0, views)
-            # two passes: transform once per pixel into 8-byte NHWC4 pixels (25 MB at B=64, L2
-            # resident), then expand to the first conv's im2col rows with coalesced 16-byte stores
-            # MixUp / CutMix in the same pass (sample i with i-1 mod b); without a draw, the plain kernel
-            self._mix = batch.mix
-            ops.augment(self._src_u8[j][:b], self._params_dev[j][:b], self.x_nhwc[:b], batch.resized_hw,
-                        out_hw=HW, mode="nhwc", pad=4, mix=self._mix)
-            if not self.fused_conv0:
-                C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
-            return b
-        if isinstance(batch, (RaggedBatch, JpegBatch)):
-            jpeg = isinstance(batch, JpegBatch)
-            b = int(batch.labels.shape[0])
-            nbytes = batch.nbytes if jpeg else int(batch.data_u8.numel())
-            if self._src_u8[j] is None or self._src_u8[j].dim() != 1 or self._src_u8[j].numel() < nbytes:
-                # grows to the loader's slot capacity (the mb largest images) and then stays
-                self._src_u8[j] = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            need = ops.ragged_inter_bytes(batch.geom)
-            if self._inter_u8 is None or self._inter_u8.numel() < need:
-                self._inter_u8 = torch.empty(need, dtype=torch.uint8, device=self.device)
-            if jpeg:
-                dev = self._jpeg_dev[j]
+            if self._src_u8[j] is None or self._src_u8[j].shape[1:] != batch.images_u8.shape[1:]:
+                self._src_u8[j] = torch.empty((self.B, *batch.images_u8.shape[1:]), dtype=torch.uint8, device=dev)
+            copies = [(self._src_u8[j][:b], batch.images_u8)]
+        else:
+            nbytes = batch.nbytes
+            self._src_u8[j] = _grown(self._src_u8[j], nbytes, torch.uint8, dev)
+            self._inter_u8 = _grown(self._inter_u8, ops.ragged_inter_bytes(batch.geom), torch.uint8, dev)
+            if isinstance(batch, JpegBatch):
+                jd, copies = self._jpeg_dev[j], []
                 for name in ("coef", "quant", "raw", "desc"):
                     t = getattr(batch, name)
-                    if name not in dev or dev[name].numel() < t.numel():
-                        dev[name] = torch.empty(max(t.numel(), 1), dtype=t.dtype, device=self.device)
-                if self._planes_u8 is None or self._planes_u8.numel() < batch.coef.numel():
-                    self._planes_u8 = torch.empty(max(batch.coef.numel(), 1), dtype=torch.uint8, device=self.device)
-            with torch.cuda.stream(self.copy_stream):
-                if self._in_free[j] is not None:
-                    self.copy_stream.wait_event(self._in_free[j])
-                if jpeg:
-                    for name in ("coef", "quant", "raw", "desc"):
-                        t = getattr(batch, name)
-                        dev[name][:t.numel()].copy_(t.view(-1), non_blocking=True)
-                else:
-                    self._src_u8[j][:nbytes].copy_(batch.data_u8, non_blocking=True)
-                self._geom_dev[j][:b].copy_(batch.geom, non_blocking=True)
-                self._params_dev[j][:b].copy_(batch.params, non_blocking=True)
-                self._labels_dev[j][:b].copy_(batch.labels, non_blocking=True)
-                h2d = torch.cuda.Event()
-                h2d.record(self.copy_stream)
-            if batch.state is not None:
-                batch.state["event"] = h2d
-            cur.wait_event(h2d)
-            if jpeg:        # decode on the compute stream into the slot's image buffer, then as a RaggedBatch
-                C.jpeg_decode(dev["coef"], dev["quant"][:batch.quant.numel()].view(-1, 64),
-                              dev["desc"][:batch.desc.numel()].view(b, -1), self._geom_dev[j][:b], dev["raw"],
-                              self._planes_u8, self._src_u8[j][:nbytes], batch.desc, batch.geom)
-            if views is not None:
-                self._staged = j
-                return self._view_input(batch, b, 0, views)
-            self._mix = batch.mix
-            ops.augment_ragged(self._src_u8[j][:nbytes], self._geom_dev[j][:b], self._params_dev[j][:b],
-                               self._inter_u8, self.x_nhwc[:b], batch.geom, batch.params, out_hw=HW,
-                               mix=self._mix)
-            if not self.fused_conv0:
-                C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
-            return b
-        x, y = batch[0], batch[1]
-        if len(batch) > 2:               # (mixed float batch, labels, draw) of the reference pipeline
-            self._mix = batch[2]
-        b = int(y.shape[0])
-        x = x.to(self.device, F32, non_blocking=True).contiguous()
-        if views is not None:        # the reference pipeline's views: [b][V][3][HW][HW]
-            assert x.dim() == 5 and x.shape[1] == len(views), "the batch does not carry the evaluation's views"
-            self.labels_dev[:b].copy_(y, non_blocking=True)
-            self._staged_x = x
-            return self._view_input(batch, b, 0, views)
-        assert x.shape[2] == HW and x.shape[3] == HW, "input size differs from the pass's size (input_hw / eval_hw)"
-        self.labels_dev[:b].copy_(y, non_blocking=True)
-        C.nchw_to_nhwc(x, self.x_nhwc[:b])
-        if not self.fused_conv0:
-            C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
+                    jd[name] = _grown(jd.get(name), max(t.numel(), 1), t.dtype, dev)
+                    copies.append((jd[name][:t.numel()], t.view(-1)))
+                self._planes_u8 = _grown(self._planes_u8, max(batch.coef.numel(), 1), torch.uint8, dev)
+            else:
+                copies = [(self._src_u8[j][:nbytes], batch.data_u8)]
+            copies.append((self._geom_dev[j][:b], batch.geom))
+        copies += [(self._params_dev[j][:b], batch.params), (self._labels_dev[j][:b], batch.labels)]
+        with torch.cuda.stream(self.copy_stream):
+            if self._in_free[j] is not None:
+                self.copy_stream.wait_event(self._in_free[j])
+            for dst, src in copies:
+                dst.copy_(src, non_blocking=True)
+            h2d = self.copy_stream.record_event()
+        if batch.state is not None:
+            batch.state["event"] = h2d          # the loader may refill the pinned slot after this
+        torch.cuda.current_stream(dev).wait_event(h2d)
+        if isinstance(batch, JpegBatch):
+            ops.require().jpeg_decode(jd["coef"], jd["quant"][:batch.quant.numel()].view(-1, 64),
+                                      jd["desc"][:batch.desc.numel()].view(b, -1), self._geom_dev[j][:b], jd["raw"],
+                                      self._planes_u8, self._src_u8[j][:nbytes], batch.desc, batch.geom)
         return b
 
     def _view_input(self, batch, b: int, i: int, views) -> int:
-        """The network input of view ``i`` of ``views`` from the staged batch: one augment launch (a ragged batch's
-        first view also runs the horizontal pass for all of them), or the reference pipeline's view converted."""
-        C = ops.require()
-        HW = self._hw
+        """The network input of the staged batch (with ``views``: of its view ``i``), and conv0's im2col rows if any."""
+        C, HW, j, x = ops.require(), self._hw, self._staged, self.x_nhwc[:b]
         if isinstance(batch, FusedBatch):
-            j = self._staged
-            ops.augment_view(self._src_u8[j][:b], self._params_dev[j][:b], self.x_nhwc[:b], batch.resized_hw,
-                             views[i], out_hw=HW)
-        elif isinstance(batch, (RaggedBatch, JpegBatch)):
-            j = self._staged
-            nbytes = batch.nbytes if isinstance(batch, JpegBatch) else int(batch.data_u8.numel())
-            ops.augment_ragged_view(self._src_u8[j][:nbytes], self._geom_dev[j][:b], self._params_dev[j][:b],
-                                    self._inter_u8, self.x_nhwc[:b], batch.geom, batch.params, views[i], out_hw=HW,
-                                    pass1=views if i == 0 else ())
-        else:
-            x = self._staged_x[:, i]
-            assert x.shape[2] == HW and x.shape[3] == HW, "input size differs from the evaluation size (eval_hw)"
-            C.nchw_to_nhwc(x.contiguous(), self.x_nhwc[:b])
-        if not self.fused_conv0:
-            C.im2col_c3(self.x_nhwc[:b], self.col0[:b * HW * HW], L.CONV0_K)
+            args = (self._src_u8[j][:b], self._params_dev[j][:b], x, batch.resized_hw)
+            if views is None:        # MixUp / CutMix in the same pass (sample i with i-1 mod b)
+                ops.augment(*args, out_hw=HW, mode="nhwc", pad=4, mix=self._mix)
+            else:
+                ops.augment_view(*args, views[i], out_hw=HW)
+        elif isinstance(batch, (RaggedBatch, JpegBatch)):     # view 0 also runs the horizontal pass of every view
+            args = (self._src_u8[j][:batch.nbytes], self._geom_dev[j][:b], self._params_dev[j][:b], self._inter_u8, x,
+                    batch.geom, batch.params)
+            if views is None:
+                ops.augment_ragged(*args, out_hw=HW, mix=self._mix)
+            else:
+                ops.augment_ragged_view(*args, views[i], out_hw=HW, pass1=views if i == 0 else ())
+        else:                            # the reference pipeline's float batch, or its view i
+            C.nchw_to_nhwc(self._staged_x if views is None else self._staged_x[:, i].contiguous(), x)
+        if not self.fused_conv0:         # a second pass expands the L2-resident NHWC4 pixels with 16-byte stores
+            C.im2col_c3(x, self.col0[:b * HW * HW], L.CONV0_K)
         return b
 
     def _release_input(self) -> None:
@@ -1426,8 +1387,8 @@ class NativeEngine:
                                                                device=self.device)
 
     def _view_logits(self, b: int) -> None:
-        """The forward of the staged view into self.logits[:b] (the fused head's evaluation pass writes them with
-        its metrics in the scratch meter)."""
+        """The evaluation forward of the network input into self.logits[:b] (the fused head's evaluation pass writes
+        them with its metrics in the scratch meter)."""
         self._forward(b, train=False)
         if self.fused_head:
             keep = self.meter
@@ -1459,10 +1420,8 @@ class NativeEngine:
         (after prepare_ema()).  With a TTA mode (set_val_tta) the loss and metrics are those of the view mean.
         A meter with a confusion matrix (DeviceMeter(num_classes=)) also gets the batch's per-class counts: one
         class_metrics launch on the logits, or on the view sums after the last view."""
-        self._use_weights(ema)
-        self._set_hw(self.eval_hw)
         counts = self.meter is not None and self.meter.confusion is not None
-        try:
+        with self._eval_pass(ema):
             if self.val_tta != "none":
                 b = self._tta_pass(batch)
                 if counts:
@@ -1476,33 +1435,32 @@ class NativeEngine:
             if counts:
                 ops.class_metrics(self.logits[:b], self.labels_dev[:b], self.meter.confusion, self.meter.top5)
             self._release_input()
-        finally:
-            self._use_weights(False)
-            self._set_hw(self.HW)
         return self.loss_buf
 
     def forward_logits(self, batch, ema: bool = False) -> torch.Tensor:
         """Logits [b][C] fp32 of an evaluation pass; with a TTA mode (set_val_tta) every view's, [b][V][C]."""
-        self._use_weights(ema)
-        self._set_hw(self.eval_hw)
-        try:
+        with self._eval_pass(ema):
             if self.val_tta != "none":
                 keep = []
                 self._tta_pass(batch, keep)
                 self._release_input()
                 return torch.stack(keep, 1)
             b = self._stage_input(batch)
-            self._forward(b, train=False)
-            if self.fused_head:          # the logits come out of the fused head kernel
-                keep = self.meter
-                self.meter = None
-                self._loss(b, train=False)
-                self.meter = keep
+            self._view_logits(b)
             self._release_input()
+        return self.logits[:b].clone()
+
+    @contextlib.contextmanager
+    def _eval_pass(self, ema: bool):
+        """An evaluation pass: the weights of ``_use_weights(ema)`` at the evaluation size, then the training
+        weights and size again."""
+        self._use_weights(ema)
+        self._set_hw(self.eval_hw)
+        try:
+            yield
         finally:
             self._use_weights(False)
             self._set_hw(self.HW)
-        return self.logits[:b].clone()
 
     def _use_weights(self, ema: bool) -> None:
         """Point the forward pass at the EMA arenas (ema16 weights, ema32 biases) or back at w16 / p32."""
@@ -1611,9 +1569,7 @@ class TeacherEngine(NativeEngine):
         own = self.x_nhwc
         self.x_nhwc, self.labels_dev = x_nhwc, labels
         try:
-            self._forward(b, train=False)
-            if self.fused_head:          # the logits come out of the fused head kernel
-                self._loss(b, train=False)
+            self._view_logits(b)
         finally:
             self.x_nhwc = own
         return self.logits[:b]
